@@ -1,14 +1,16 @@
 #!/usr/bin/env python
 """bench.py — contrast-loss fwd+bwd throughput on synthetic Cityscapes-shaped batches (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl engine|reference] [--workload s1|s2]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl engine|reference] [--workload s1|s2] [--dump-outputs DIR]
 
 Workload s1 = BASELINE configs[1]: HRNet-W48 pixel-contrast (no bank), 1024x512 input -> 256x128 embedding,
 19 classes, batch 8 PER GPU (weak scaling; the no-bank loss has no cross-rank exchange, SURVEY §8e).
 Workload s2 = configs[2] shape per rank (bank 19x(5000+5000)x256, one image per rank, bank merge allgather).
 A "step" = one pass of the hot path over one batch: label/argmax/key scan, anchor selection + gather, InfoNCE
 forward, InfoNCE backward and the dense embedding-gradient write (+ bank enqueue for s2).
-Prints ONE JSON line (rank 0).
+Prints ONE JSON line (rank 0).  --dump-outputs DIR writes what the last timed step returned to its caller (the loss, a
+fixed seeded sample of the dense embedding gradient, and for bank workloads of the queues) as DIR/<name>.npy; the inputs
+are seeded, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -40,12 +42,13 @@ def load_peaks():
         d = json.load(open(p))
         return dict(hbm_gbs=d["hbm_gbs"], bf16_tflops=d["bf16_tflops"],
                     bf16_tflops_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]), source="measured")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, source="fallback")
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 dense bf16 TFLOP/s
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_tflops_sustained=989.0, source="data sheet")
 
 
 def ncu_traffic(kernel):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed ncu --set full capture
-    (profiles/ncu_traffic.json, written by tools/ncu_traffic.py from a .ncu-rep); None if not captured."""
+    """dram__bytes_read.sum + dram__bytes_write.sum per launch from an ncu --set full capture summarised by
+    tools/ncu_traffic.py into profiles/ncu_traffic.json; None if not captured."""
     p = os.path.join(ROOT, "profiles", "ncu_traffic.json")
     if not os.path.exists(p):
         return None
@@ -141,7 +144,7 @@ def engine_configer(cfg, bank=False, precision="bf16"):
                       "max_views": cfg["max_views"], "loss_weight": 0.1, "use_rmi": False, "rng": "device",
                       "precision": precision}}
     if bank:
-        # bank sweeps run on the tcgen05 path (bf16 operands through the bank shadow)
+        # bank sweeps run on the tensor-core path (bf16 operands through the bank shadow)
         d["contrast"].update(with_memory=True, memory_size=cfg["M"], pixel_update_freq=cfg["F"])
     return cs.Configer(d)
 
@@ -398,7 +401,7 @@ def train_iter_bench(cfg, inp, dev, precision, iters=10):
     ms = e0.elapsed_time(e1) / iters
     ok = bool(torch.isfinite(loss).item())
     # The same iteration with the REFERENCE's loss step in place of the engine's (SURVEY 8(d): "the reference ATen path
-    # on the B200 itself"): the CPU port's torch ops follow their input's device, so on CUDA tensors they are the
+    # on the GPU itself"): the CPU port's torch ops follow their input's device, so on CUDA tensors they are the
     # reference's own op sequence (per-(image, class) nonzero/randperm/index loop, dense A x N temporaries, one
     # SelectBackward per pair).  A baseline leg like cpu_baseline: measured beside the engine, never part of it.
     ref_ms, ref_err = None, None
@@ -443,7 +446,7 @@ def train_iter_bench(cfg, inp, dev, precision, iters=10):
 # engine arm: every workload is measured through the public graphed-step API (GraphedContrastStep): ONE CUDA-graph replay
 # per step (bank steps on several ranks: two replays around the NCCL all_gather of the enqueue packet).
 # ---------------------------------------------------------------------------------------------------
-L2_BYTES = 126 << 20
+L2_BYTES = 50 << 20
 
 
 def working_set_bytes(cfg, bank):
@@ -503,7 +506,8 @@ class Workload:
 
     # ---- the step, two ways ----
     def replay(self, i):
-        return self.steps[i % self.R].replay()[0]
+        self.last = self.steps[i % self.R].replay()
+        return self.last[0]
 
     def eager(self, i):
         inp = self.inp[i % self.R]
@@ -513,7 +517,16 @@ class Workload:
         if self.bank:
             self.mbank.enqueue(e.detach(), inp["target"], network_stride=self.cfg["net_stride"], pixel_update_freq=self.cfg["F"])
         loss.backward()
+        self.last = (loss, e.grad)
         return loss
+
+    def outputs(self):
+        """Device copies of what the step last returned to its caller: loss, embedding gradient (+ the bank it wrote)."""
+        out = {"loss": self.last[0].detach().reshape(-1).clone(), "grad_embed": self.last[1].detach().clone()}
+        if self.bank:
+            out["segment_queue"] = self.mbank.segment_queue.detach().clone()
+            out["pixel_queue"] = self.mbank.pixel_queue.detach().clone()
+        return out
 
     def barrier(self):
         if self.world > 1:
@@ -526,9 +539,10 @@ class Workload:
             torch.distributed.all_reduce(t, op=torch.distributed.ReduceOp.MAX)
         return [float(v) for v in t.tolist()]
 
-    def time_loop(self, fn, steps, warmup, sampler=None):
+    def time_loop(self, fn, steps, warmup, sampler=None, snapshot=False):
         """K steps bracketed by barrier + synchronize, CUDA events on the launching stream, max over ranks.
-        Returns (device ms per step, host enqueue ms per step, clock window description)."""
+        Returns (device ms per step, host enqueue ms per step, clock window description).  snapshot: keep a copy of what
+        the last timed step returned (self.snap) before anything else runs."""
         for i in range(max(warmup, 3)):
             fn(i)
         self.barrier()
@@ -543,6 +557,8 @@ class Workload:
         ev[1].record()
         t_host = time.perf_counter() - t0               # host time to enqueue the K steps (no sync inside)
         self.barrier()
+        if snapshot:
+            self.snap = self.outputs()
         window = "timed region"
         if sampler is not None:
             # nvidia-smi samples every 200 ms; a short timed region would see no sample, so the SAME loop keeps running
@@ -646,7 +662,7 @@ class Workload:
         fn, mode = (self.replay, "graph") if self.steps else (self.eager, "eager")
         if not self.steps:
             out["graph_error"] = self.graph_error or "disabled (--no-graph)"
-        ms, host, window = self.time_loop(fn, a.steps, a.warmup, sampler)
+        ms, host, window = self.time_loop(fn, a.steps, a.warmup, sampler, snapshot=getattr(a, "dump_outputs", None) is not None)
         out.update(mode=mode, ms_per_step=ms, value=self.world * self.cfg["B"] / (ms / 1e3), host_ms_per_step=host,
                    clock_window=window, kernels_per_step=self.kernels_per_step())
         if with_e2e:
@@ -654,7 +670,7 @@ class Workload:
             ev, h2d = self.e2e(fn, e_steps)
             out["e2e"] = {"value": ev, "unit": "images/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 4, "steps": e_steps,
                           "h2d_gbs_per_gpu": h2d * ev / (self.world * self.cfg["B"]) / 1e9,
-                          "note": "PCIe-bound: pinned H2D copies reach 55 GB/s on this box (tools/h2d_probe.py), the step itself is 2 % of e2e"}
+                          "note": "host-to-device copies of the pinned inputs are part of every step"}
         if with_eager and self.steps:
             ems, ehost, _ = self.time_loop(self.eager, a.steps, a.warmup)
             out["eager"] = {"ms_per_step": ems, "value": self.world * self.cfg["B"] / (ems / 1e3), "host_ms_per_step": ehost}
@@ -704,6 +720,9 @@ def run_engine(args, cfg, bank, rank, world, dev):
     # ---- headline: the workload named on the command line (default s1 = BASELINE configs[1]), weak scaling ----
     head = Workload(args, args.workload, cfg, bank, rank, world, dev)
     hm = head.measure(sampler=sampler, with_eager=True)
+    if getattr(args, "dump_outputs", None) and rank == 0:
+        dump_outputs(head.snap, args.dump_outputs)
+    head.snap = None
     A_live = int(head.steps[0].ws.plan[2].item()) if head.steps else 0
     timeline = head.graph_timeline() if not os.environ.get("PCL_BENCH_TINY") else None
     inp0 = head.inp[0]
@@ -809,7 +828,7 @@ def run_engine(args, cfg, bank, rank, world, dev):
         # dominant kernel of the timed path: the engine's zero-fill of the dense gradient, timed INSIDE the graph replay
         fb = cfg["B"] * cfg["D"] * cfg["h"] * cfg["w"] * 4
         fa = fb / (fill["dur_us"] * 1e-6) / 1e9
-        roof = {"kernel": "k_fill_zero_excl (dense-gradient zero-fill on 116 SMs it owns, next to the InfoNCE kernel on the other 32; "
+        roof = {"kernel": "k_fill_zero_excl (dense-gradient zero-fill on the SMs it owns, next to the InfoNCE kernel on the other 32; "
                           "the HBM floor of the step; runs in the timed graph)",
                 "bound": "hbm", "achieved": fa, "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": fa / peaks["hbm_gbs"],
                 "traffic": ncu_traffic("k_fill_zero_excl"), "peak_source": peaks["source"], "algorithmic_bytes": fb,
@@ -824,7 +843,7 @@ def run_engine(args, cfg, bank, rank, world, dev):
     kps = hm["kernels_per_step"] or 0
     conf = dict(workload_config(cfg, bank),
                 step="one CUDA-graph replay per step (GraphedContrastStep)" if hm["mode"] == "graph" else "eager autograd call per step",
-                l2=("inputs larger than L2 (working set %.0f MB vs 126 MB)" % hm["working_set_mb"]) if hm["rotation_sets"] == 1
+                l2=("inputs larger than L2 (working set %.0f MB vs %d MB)" % (hm["working_set_mb"], L2_BYTES >> 20)) if hm["rotation_sets"] == 1
                 else f"rotating over {hm['rotation_sets']} input/gradient buffer sets ({hm['working_set_mb']:.0f} MB each) so that no step finds its inputs in L2")
     return {"metric": "contrast-loss fwd+bwd throughput", "value": hm["value"], "unit": "images/s", "n_gpus": world,
             "steps": args.steps, "warmup": max(args.warmup, 3), "ms_per_step": hm["ms_per_step"],
@@ -838,8 +857,28 @@ def run_engine(args, cfg, bank, rank, world, dev):
             "bank": blocks.get("bank"), "strong": blocks.get("strong"), "impl": "engine"}
 
 
+DUMP_SAMPLE = 1 << 22          # elements kept of an output larger than this (fixed seeded sample): <= 16 MB each
+
+
+def dump_outputs(arrays, out_dir):
+    """arrays: name -> tensor.  Writes out_dir/<name>.npy (float32; the loss in float64); an array of more than
+    DUMP_SAMPLE elements is replaced by a fixed seeded sample of its flattened elements (<name>_sample.npy, ascending
+    flat indices of torch.randperm(numel, Generator().manual_seed(20240601))[:DUMP_SAMPLE]) — the same elements in every
+    run, so two builds compare element for element."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        flat = t.reshape(-1)
+        if flat.numel() > DUMP_SAMPLE:
+            g = torch.Generator().manual_seed(20240601)
+            idx = torch.randperm(flat.numel(), generator=g)[:DUMP_SAMPLE].sort().values
+            flat, name = flat[idx.to(flat.device)], f"{name}_sample"
+        dt = torch.float64 if name == "loss" else torch.float32
+        np.save(os.path.join(out_dir, f"{name}.npy"), flat.to(dt).cpu().numpy())
+
+
 def tensor_sweep_roofline(dev, peaks, A=16384, N=65536, iters=5):
-    """The dense contraction alone (similarity + negative-sum sweep on tcgen05) at one S4 point (BASELINE configs[4]):
+    """The dense contraction alone (similarity + negative-sum sweep on wgmma) at one S4 point (BASELINE configs[4]):
     algorithmic FLOPs 2*A*N*D over the CUDA-event time, vs the measured bf16 peak."""
     from contrastiveseg_b200 import functional as Fn
     g = torch.Generator().manual_seed(7)
@@ -875,7 +914,7 @@ def tensor_sweep_roofline(dev, peaks, A=16384, N=65536, iters=5):
     out["backward"] = tb[len(tb) // 2]
     fl = 2.0 * A * N * 256
     ach = fl / (out["neg_sweep"] * 1e-3) / 1e12
-    return {"kernel": "k_tc_fwd<NEG> (anchor x bank similarity + negative-sum sweep, tcgen05)", "bound": "tensor",
+    return {"kernel": "k_tc_fwd<NEG> (anchor x bank similarity + negative-sum sweep, wgmma)", "bound": "tensor",
             "workload": f"S4 sweep point A={A} x N={N}, D=256, bf16 operands", "achieved": ach,
             "peak": peaks["bf16_tflops"], "unit": "TFLOP/s", "frac": ach / peaks["bf16_tflops"],
             "peak_source": peaks["source"], "traffic": None, "ms": out,
@@ -897,7 +936,10 @@ def main():
     ap.add_argument("--no-graph", action="store_true",
                     help="run GraphedContrastStep's launch sequence eagerly instead of as a captured CUDA graph")
     ap.add_argument("--precision", default="bf16", choices=["bf16", "fp32"],
-                    help="InfoNCE sweeps: bf16 operands on tcgen05 tensor cores (default) or the exact fp32 SIMT sweep")
+                    help="InfoNCE sweeps: bf16 operands on the tensor cores (default) or the exact fp32 SIMT sweep")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step returned (loss, seeded sample of the "
+                         "embedding gradient, bank queues) as DIR/<name>.npy")
     args = ap.parse_args()
     world = int(os.environ.get("WORLD_SIZE", "1"))
     rank = int(os.environ.get("RANK", "0"))

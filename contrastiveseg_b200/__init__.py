@@ -1,9 +1,9 @@
-"""B200-native pixel-contrast loss engine: drop-in for the loss path of tfzhou/ContrastiveSeg.
+"""H100-native pixel-contrast loss engine: drop-in for the loss path of tfzhou/ContrastiveSeg.
 
 Public surface mirrors the reference (SURVEY §8b): ``PixelContrastLoss``, ``ContrastCELoss``,
 ``ContrastAuxCELoss``, ``MemContrastCELoss`` (registry keys in ``SEG_LOSS_DICT``), ``MemoryBank`` /
 ``dequeue_and_enqueue``, ``ProjectionHead`` / ``l2_normalize`` and the trainer hook.  All arithmetic runs in
-hand-written sm_100a kernels (csrc/) behind the C ABI of include/pcl.h; there is no CPU or PyTorch fallback.
+hand-written sm_90a kernels (csrc/) behind the C ABI of include/pcl.h; there is no CPU or PyTorch fallback.
 """
 from .configer import Configer, cityscapes_contrast_config            # noqa: F401
 from .functional import ContrastOptions, l2_normalize, pixel_contrast_loss, upsample_cross_entropy   # noqa: F401

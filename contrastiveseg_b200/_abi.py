@@ -159,7 +159,7 @@ def load(build_if_missing: bool = False):
         if hasattr(lib, "pcl_emulated"):
             # tests/emu builds the SIMT kernel sources for host threads so that CPU-only test runs execute kernel logic;
             # that build is test infrastructure and must never serve the product (there is no CPU path)
-            raise PclError(f"{path} is the host-thread emulation build of the test suite, not the sm_100a library")
+            raise PclError(f"{path} is the host-thread emulation build of the test suite, not the sm_90a library")
         for name, (res, args) in SIGNATURES.items():
             fn = getattr(lib, name)            # AttributeError here = ABI mismatch: fail loudly
             fn.restype = res

@@ -64,7 +64,7 @@ class MemoryBank(nn.Module):
         if self.with_shadow:
             if self.shadow is None:
                 self.sync_shadow()
-            outputs["bank_shadow"] = self.shadow          # engine-only: bf16 copy for the tcgen05 sweep
+            outputs["bank_shadow"] = self.shadow          # engine-only: bf16 copy for the wgmma sweep
         return outputs
 
     def sync_shadow(self) -> torch.Tensor:
@@ -129,7 +129,7 @@ def enqueue_buffers(dev: torch.device, n_scratch: int, n_packet: int, world: int
     if bufs is None:
         # the packet is zero-filled ONCE: slots of absent (image, class) pairs carry only their count header, the rest of
         # their rows is never written — the all_gather ships the whole packet, so it must not be uninitialised memory
-        # (compute-sanitizer initcheck, profiles/r2_36_initcheck_packet_copy.log)
+        # (compute-sanitizer initcheck reports it otherwise)
         bufs = (torch.empty(n_scratch, dtype=torch.float32, device=dev),
                 torch.zeros(n_packet, dtype=torch.float32, device=dev),
                 torch.zeros((world, n_packet), dtype=torch.float32, device=dev) if world > 1 else None)

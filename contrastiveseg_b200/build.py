@@ -1,4 +1,4 @@
-"""In-tree build of libpcl_b200.so (sm_100a only) with plain nvcc — no torch headers, no JIT cache.
+"""In-tree build of libpcl_b200.so (sm_90a only) with plain nvcc — no torch headers, no JIT cache.
 
     python -m contrastiveseg_b200.build [--force]
 
@@ -19,7 +19,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 OBJDIR = os.path.join(LIBDIR, "obj")
 LIBNAME = "libpcl_b200.so"
-ARCH_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
               "-Xptxas", "-v"]
 

@@ -158,7 +158,7 @@ k_bank_rows(BankDims d, const float* __restrict__ keys, const int32_t* __restric
 // Q4: the pixel pointer advances by ONE per slot, so successive windows overlap and a later slot overwrites rows of an
 // earlier one).  Nothing reads the bank during the apply, so the result only depends on WHO WRITES LAST: thread 0 replays
 // the pointer arithmetic of all slots (integers only), then every row is copied once, in parallel, by its last writer.
-// (The sequential version took 9.6 us per packet: 77 us of the 8-GPU bank step, profiles/r2_20_bench_n8.json.)
+// (A sequential apply costs one dependent chain per packet, which grows with the number of ranks.)
 constexpr int APPLY_MAX_SLOTS = 1024;            // world * B slots of one class handled in shared memory
 
 __global__ void __launch_bounds__(256)
@@ -362,7 +362,7 @@ extern "C" int pcl_bank_shadow_rebuild(const float* segment_queue, const float* 
   cudaStream_t s = (cudaStream_t)stream;
   const int64_t rows = (int64_t)(K - 1) * 2 * M;
   const int64_t rows_pad = ceil_div64(rows > 0 ? rows : 1, 256) * 256;
-  k_shadow_rebuild<<<148 * 8, 256, 0, s>>>(segment_queue, pixel_queue, K, M, D, rows_pad, (__nv_bfloat16*)shadow_bf16);
+  k_shadow_rebuild<<<num_sms() * 8, 256, 0, s>>>(segment_queue, pixel_queue, K, M, D, rows_pad, (__nv_bfloat16*)shadow_bf16);
   PCL_LAUNCH_CHECK();
   return PCL_OK;
 }

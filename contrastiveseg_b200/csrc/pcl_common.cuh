@@ -1,4 +1,4 @@
-// Shared helpers for the pixel-contrast engine kernels (sm_100a).
+// Shared helpers for the pixel-contrast engine kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -89,7 +89,7 @@ static inline int smem_opt_in(SmemOptIn& st, F func, size_t max_bytes) {
     if (rc__ != PCL_OK) return rc__;                                        \
   } while (0)
 
-// SM count of the current device (cached per device; 148 when sizing on a host without one)
+// SM count of the current device (cached per device; 132 when sizing on a host without one)
 int num_sms();
 
 static inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }
@@ -133,6 +133,30 @@ __device__ __forceinline__ float warp_max(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
+}
+
+// wgmma accumulator fragment -> row view.  The tensor-core epilogues work on one row per thread and 32 consecutive
+// columns at a time, while the accumulator of an m64nN wgmma is spread over the warpgroup (layout: ptx_sm90.cuh).
+// frag_store_cols writes columns [8 i0, 8 (i0 + NI)) of warpgroup thread t's fragment to dst[row * pitch + column - 8 i0];
+// after a barrier of the warpgroup, load_row32 reads 32 consecutive columns of one row back.  A pitch of 4 (mod 32)
+// floats keeps the 16-byte row reads free of bank conflicts.
+template <int NI, int NF>
+__device__ __forceinline__ void frag_store_cols(const float (&d)[NF], int i0, float* dst, int pitch, int t) {
+  const int row = 16 * (t >> 5) + ((t & 31) >> 2), col = 2 * (t & 3);
+#pragma unroll
+  for (int i = 0; i < NI; ++i)
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      *reinterpret_cast<float2*>(dst + (row + 8 * h) * pitch + 8 * i + col) =
+          make_float2(d[4 * (i0 + i) + 2 * h], d[4 * (i0 + i) + 2 * h + 1]);
+}
+__device__ __forceinline__ void load_row32(const float* src, uint32_t (&v)[32]) {
+#pragma unroll
+  for (int q = 0; q < 8; ++q) {
+    const float4 x = reinterpret_cast<const float4*>(src)[q];
+    v[4 * q] = __float_as_uint(x.x); v[4 * q + 1] = __float_as_uint(x.y);
+    v[4 * q + 2] = __float_as_uint(x.z); v[4 * q + 3] = __float_as_uint(x.w);
+  }
 }
 
 // Class rank used for the sorted anchor layout: 1,2,...,K-1,0  (class 0 last: in bank mode its

@@ -9,7 +9,7 @@
 //   POS  per-row sum over positives of log-prob, of 1/(e+Neg), count -> partial per split
 //   BWD  recompute logits, form the gradient tile G (closed form), dA += G . C
 // Row statistics are combined in fixed split order, so results are bit-reproducible.
-// This is the exact path (fp32 FMA); the bf16 tcgen05 path lives in pcl_infonce_tc.cu.
+// This is the exact path (fp32 FMA); the bf16 wgmma path lives in pcl_infonce_tc.cu.
 #include "pcl_common.cuh"
 #include "pcl_sweep.cuh"
 #include "pcl_simt_tile.cuh"
@@ -311,10 +311,10 @@ int pcl::simt_make_args(const pcl_sweep_desc* d, SweepArgs* a) {
   a->row_tiles = ceil_div(d->a_rows, TM);
   a->a_pad = a->row_tiles * TM;
   a->col_tiles = (int)ceil_div64(a->n_cols > 0 ? a->n_cols : 1, TN);
-  int splits = 296 / a->row_tiles;
+  int splits = 2 * num_sms() / a->row_tiles;
   if (splits < 1) splits = 1;
   if (splits > a->col_tiles) splits = a->col_tiles;
-  if (splits > 148) splits = 148;
+  if (splits > num_sms()) splits = num_sms();
   a->splits = splits;
   return PCL_OK;
 }

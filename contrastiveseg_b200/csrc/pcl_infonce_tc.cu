@@ -1,20 +1,20 @@
-// Tensor-core InfoNCE sweep for sm_100a (SURVEY §8 row a6, north_star "anchor x memory-bank similarity as a dense
-// bf16 contraction on tcgen05 tensor cores fed by TMA staging").
+// Tensor-core InfoNCE sweep for sm_90a (SURVEY §8 row a6: "anchor x memory-bank similarity as a dense bf16
+// contraction on the tensor cores fed by TMA staging").
 //
 // One CTA = one 128-row anchor tile x a contiguous range of 256-column contrast tiles, D = 256 (K-major bf16):
-//   warp 0   TMA producer   : anchor tile once (4 x [128 x 64] boxes, 64 KB), then a 4-stage ring of [256 x 64]
-//                             contrast boxes (32 KB each), SWIZZLE_128B
-//   warp 1   MMA issuer     : tcgen05.mma cta_group::1 kind::f16, M=128 N=256 K=16, 16 MMAs per logit tile,
-//                             accumulators double-buffered in TMEM (2 x 256 columns = all 512)
-//   warps 2-9 epilogue      : tcgen05.ld 32x32b.x32 -> one FFMA + one ex2 per logit (scale 1/T and the row stabiliser
-//                             folded into the FFMA), class test only on tiles that straddle a class boundary,
-//                             row sums kept in registers; never materialises A x N
+//   warp 8       TMA producer : anchor tile once (4 x [128 x 64] boxes, 64 KB), then a 3-stage ring of [256 x 64]
+//                               contrast boxes (32 KB each), SWIZZLE_128B
+//   warps 0-7    two consumer warpgroups, 64 anchor rows each: wgmma m64n256k16 (16 per logit tile, fp32 accumulators
+//                in registers), then the epilogue on the same threads: the accumulator goes through a shared-memory
+//                staging buffer 32 columns at a time (one row per thread), one FFMA + one ex2 per logit (scale 1/T and
+//                the row stabiliser folded into the FFMA), class test only on tiles that straddle a class boundary,
+//                row sums kept in registers; never materialises A x N
 // Sweeps: NEG (sum over negatives of exp(l - m)), POS (log-prob sums over the positive column range).  The row
 // stabiliser is the Cauchy-Schwarz bound m_i = |a_i| * max|c| / T (exact in real arithmetic; no running max needed).
 // Partials per (split, row) are combined in fixed order by the shared row-statistic kernels (pcl_sweep.cuh).
 #include "pcl_common.cuh"
 #include "pcl_sweep.cuh"
-#include "ptx_sm100.cuh"
+#include "ptx_sm90.cuh"
 #include "pcl_topk.cuh"
 #include <stdlib.h>
 #include <mutex>
@@ -23,16 +23,21 @@ namespace pcl {
 int tc_make_tmap(CUtensorMap* m, const void* base, uint64_t rows, uint32_t box_rows);
 namespace tc {
 
-// Forward tile = 128 rows x 256 columns (one M128 x N256 x K16 UMMA per K step).  A 256-row x 128-column variant (two
-// M128 x N128 MMAs per contrast box, half the L2 traffic) measured 18 % SLOWER: N=128 MMAs read 128 B/clk of operands
-// from shared memory and starve the TMA fill (profiles/r1_sweep_variants_v3_fm256.jsonl).
+// Forward tile = 128 rows x 256 columns: each consumer warpgroup runs M64 x N256 x K16 wgmmas on its 64 rows, so both
+// read the same contrast box once per K step (the widest N wgmma has, the fewest operand bytes per MMA).
 constexpr int BM = 128, BN = 256, BK = 64, NKB = 4, DDIM = 256;
-constexpr int STAGES = 4;
+constexpr int STAGES = 3;
 constexpr int A_KB_BYTES = BM * BK * 2;          // 16 KB
 constexpr int B_STAGE_BYTES = BN * BK * 2;       // 32 KB
-constexpr int NUM_THREADS = 320;                 // warp 0 TMA, warp 1 MMA, warps 2..9 epilogue
-constexpr int EPI_THREADS = 256;
-constexpr uint32_t TMEM_COLS = 512;
+constexpr int WG_ROW_BYTES = 64 * 128;           // offset of warpgroup 1's 64 rows inside a [rows x 64] K-block
+constexpr int NUM_THREADS = 384;                 // warps 0-7: two consumer warpgroups, warps 8-11: producer warpgroup
+constexpr int PRODUCER_WARP = 8;                 // (its first warp issues the TMA loads)
+// Registers per thread after setmaxnreg: 2 x 128 x 232 + 128 x 40 fit the 64 K register file; the consumers hold the
+// wgmma accumulators (128 floats for an m64n256 tile).
+constexpr uint32_t CONSUMER_REGS = 232, PRODUCER_REGS = 40;
+constexpr int EPI_THREADS = 256;                 // the consumer warpgroups (named barrier 1; barriers 2, 3: one warpgroup)
+constexpr int CONSUMER_WARPS = 8;                // arrivals on an "empty" barrier: every consumer warp after its wgmma wait
+constexpr int SPITCH = 36;                       // staging row pitch in floats (32 columns + 4: conflict-free row reads)
 constexpr float LOG2E = 1.4426950408889634f, LN2 = 0.6931471805599453f;
 
 struct TcArgs {
@@ -56,8 +61,7 @@ struct TcArgs {
 };
 
 // n / R by multiplication (Granlund-Montgomery round-up method, exact for every 32-bit n): the bank-mode column label
-// n / R + 1 is evaluated per 32-column chunk by every epilogue thread, and the integer divide (about 25 instructions)
-// showed up as 11-17 % of all warp-stall samples of the POS and backward sweeps (profiles/r2_06_bank_source_top.txt).
+// n / R + 1 is evaluated per 32-column chunk by every epilogue thread, and the integer divide is about 25 instructions.
 __device__ __forceinline__ uint32_t div_R(const TcArgs& a, uint32_t n) {
   const uint32_t t = __umulhi(n, a.r_mul);
   return (t + ((n - t) >> 1)) >> a.r_sh;
@@ -75,10 +79,53 @@ static inline void make_div(uint32_t d, uint32_t* mul, uint32_t* sh) {
 struct SmemLayout {
   uint8_t a[NKB * A_KB_BYTES];
   uint8_t b[STAGES * B_STAGE_BYTES];
-  uint64_t full[STAGES], empty[STAGES], a_full, a_empty, tmem_full[2], tmem_empty[2];
-  uint32_t tmem_base;
+  float stage[2][2][64][SPITCH];                 // [warpgroup][column half][row]: one 32-column chunk of each half
+  uint64_t full[STAGES], empty[STAGES], a_full, a_empty;
   float comb[3][2][BM];
 };
+static_assert(sizeof(SmemLayout) + 1024 <= 227 * 1024, "shared memory of one H100 block");
+
+// The contrast ring, as the consumer warpgroups walk it: wait for a stage, issue its wgmmas, and release the stage
+// before once its wgmmas have retired (one wgmma group stays in flight behind the issue).
+struct Ring {
+  uint32_t stage = 0, phase = 0;
+  int prev = -1;
+  __device__ __forceinline__ void release_prev(uint64_t* empty, int lane) {
+    if (prev >= 0 && lane == 0) ptx::mbar_arrive(&empty[prev]);
+    prev = -1;
+  }
+};
+
+// acc = X . Y^T over D = 256 (4 K-blocks), both K-major: the operand that stays (`fixed`, one [rows x 64] box per
+// K-block at `fixed_kb_bytes`) and the one streamed through the ring (one K-block per stage).  RING_IS_A: the ring feeds
+// the M side (the transposed POS sweep), else the N side.
+template <int STAGES_, int RING_BYTES, bool RING_IS_A, int NF>
+__device__ __forceinline__ void ring_mma(float (&acc)[NF], uint32_t fixed_base, uint32_t fixed_kb_bytes, uint32_t ring_base,
+                                         uint64_t* full, uint64_t* empty, Ring& ring, int lane) {
+  ptx::wgmma_fence();
+#pragma unroll 1
+  for (int kb = 0; kb < NKB; ++kb) {
+    ptx::mbar_wait(&full[ring.stage], ring.phase);
+#pragma unroll
+    for (int k = 0; k < BK / 16; ++k) {
+      const uint64_t df = ptx::make_desc_kmajor_sw128(fixed_base + kb * fixed_kb_bytes + k * 32);
+      const uint64_t dr = ptx::make_desc_kmajor_sw128(ring_base + ring.stage * RING_BYTES + k * 32);
+      const uint64_t da = RING_IS_A ? dr : df, db = RING_IS_A ? df : dr;
+      if constexpr (NF == 128) ptx::wgmma_m64n256k16<0>(acc, da, db, (kb | k) != 0 ? 1u : 0u);
+      else ptx::wgmma_m64n64k16<0>(acc, da, db, (kb | k) != 0 ? 1u : 0u);
+    }
+    ptx::wgmma_commit();
+    if (kb > 0) {
+      ptx::wgmma_wait<1>();
+      ring.release_prev(empty, lane);
+    }
+    ring.prev = (int)ring.stage;
+    if (++ring.stage == STAGES_) { ring.stage = 0; ring.phase ^= 1; }
+  }
+  ptx::wgmma_wait<0>();
+  ring.release_prev(empty, lane);
+  ptx::fence_operands(acc);
+}
 
 __device__ __forceinline__ int col_label(const TcArgs& a, int n) {      // columns < 2^31
   return a.ccls ? a.ccls[n] : (a.mode == 1 ? (int)div_R(a, (uint32_t)n) + 1 : a.acls[n]);
@@ -87,8 +134,7 @@ __device__ __forceinline__ int col_label(const TcArgs& a, int n) {      // colum
 // First / last label of N consecutive 32-column chunks starting at column `base` (lo = -2 / hi = -3: chunk not complete
 // or test disabled).  Bank mode with class blocks of R >= 32 N rows: the N chunks meet at most ONE class boundary, so one
 // n / R for `base` and comparisons against the next block start replace 2 N multiply-shift divisions.  (Fewer
-// instructions, no measurable change of the sweep times: the label lines were 26 % of the NEG sweep's warp-stall samples,
-// profiles/r2_25_bank_source_top.txt, but they are evaluated one tile ahead, inside the wait for the accumulator.)
+// instructions; they are evaluated one tile ahead, inside the wait for the accumulator.)
 template <int N>
 __device__ __forceinline__ void chunk_labels(const TcArgs& a, int base, bool en, int64_t ncols, int (&lo)[N], int (&hi)[N]) {
   if (a.ccls == nullptr && a.mode == 1 && a.R >= 32 * N) {
@@ -254,24 +300,20 @@ k_tc_fwd(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtens
   }
 
   // ---- one-time setup ----
-  if (warp == 0 && lane == 0) {
+  if (warp == PRODUCER_WARP && lane == 0) {
     ptx::prefetch_tmap(&tmA);
     ptx::prefetch_tmap(&tmB);
-    for (int s = 0; s < STAGES; ++s) { ptx::mbar_init(&sm.full[s], 1); ptx::mbar_init(&sm.empty[s], 1); }
+    for (int s = 0; s < STAGES; ++s) { ptx::mbar_init(&sm.full[s], 1); ptx::mbar_init(&sm.empty[s], CONSUMER_WARPS); }
     ptx::mbar_init(&sm.a_full, 1);
-    ptx::mbar_init(&sm.a_empty, 1);
-    for (int i = 0; i < 2; ++i) { ptx::mbar_init(&sm.tmem_full[i], 1); ptx::mbar_init(&sm.tmem_empty[i], EPI_THREADS / 32); }
+    ptx::mbar_init(&sm.a_empty, CONSUMER_WARPS);
     ptx::fence_barrier_init();
   }
-  if (warp == 1) ptx::tmem_alloc<TMEM_COLS>(&sm.tmem_base);
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = sm.tmem_base;
 
-  if (warp == 0) {
+  if (warp >= PRODUCER_WARP) {
     // =========================== TMA producer ===========================
-    if (lane == 0) {
+    ptx::setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp == PRODUCER_WARP && lane == 0) {
       SegWalker w = w0;
       Seg sg;
       uint32_t stage = 0, phase = 0;
@@ -292,50 +334,17 @@ k_tc_fwd(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtens
         ++seg_idx;
       }
     }
-  } else if (warp == 1) {
-    // =========================== MMA issuer ===========================
-    if (lane == 0) {
-      constexpr uint32_t idesc = ptx::make_idesc_bf16(BM, BN, 0, 0);
-      const uint32_t a_base = ptx::smem_u32(sm.a), b_base = ptx::smem_u32(sm.b);
-      SegWalker w = w0;
-      Seg sg;
-      uint32_t stage = 0, phase = 0;
-      int seg_idx = 0, it = 0;
-      while (w.next(sg)) {
-        if (sg.ct1 <= sg.ct0) continue;
-        ptx::mbar_wait(&sm.a_full, seg_idx & 1);
-        ptx::tc_fence_after();
-        for (int ct = sg.ct0; ct < sg.ct1; ++ct, ++it) {
-          const uint32_t acc = it & 1, acc_phase = (it >> 1) & 1;
-          ptx::mbar_wait(&sm.tmem_empty[acc], acc_phase ^ 1);
-          ptx::tc_fence_after();
-          const uint32_t d_tmem = tmem_base + acc * BN;
-          for (int kb = 0; kb < NKB; ++kb) {
-            ptx::mbar_wait(&sm.full[stage], phase);
-            ptx::tc_fence_after();
-#pragma unroll
-            for (int k = 0; k < BK / 16; ++k) {
-              const uint64_t da = ptx::make_desc_kmajor_sw128(a_base + kb * A_KB_BYTES + k * 32);
-              const uint64_t db = ptx::make_desc_kmajor_sw128(b_base + stage * B_STAGE_BYTES + k * 32);
-              ptx::mma_f16_ss(d_tmem, da, db, idesc, (kb | k) != 0 ? 1u : 0u);
-            }
-            ptx::mma_commit(&sm.empty[stage]);          // smem slot free once these MMAs retire
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
-          }
-          ptx::mma_commit(&sm.tmem_full[acc]);          // accumulator ready for the epilogue
-        }
-        ptx::mma_commit(&sm.a_empty);                   // anchor tile may be overwritten
-        ++seg_idx;
-      }
-    }
   } else {
-    // =========================== epilogue warps ===========================
-    const int quarter = warp & 3;                     // TMEM lane quarter this warp may access
-    const int half = (warp - 2) >> 2;                 // which 128 columns of the 256-column tile
-    const int r_in = quarter * 32 + lane;
+    // =========================== consumer warpgroups: wgmma + epilogue ===========================
+    ptx::setmaxnreg_inc<CONSUMER_REGS>();
+    const int g = threadIdx.x >> 7, t = threadIdx.x & 127;
+    const int half = t >> 6;                          // which 128 columns of the 256-column tile
+    const int r_in = g * 64 + (t & 63);
+    const uint32_t a_base = ptx::smem_u32(sm.a) + g * WG_ROW_BYTES, b_base = ptx::smem_u32(sm.b);
+    Ring ring;
     SegWalker w = w0;
     Seg sg;
-    int it = 0;
+    int seg_idx = 0;
     while (w.next(sg)) {
       const int row = sg.r * BM + r_in;
       const bool valid = row < A;
@@ -380,8 +389,11 @@ k_tc_fwd(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtens
       float acc0 = 0.f, acc1 = 0.f, acc2 = 0.f, acc3 = 0.f;     // NEG: 4 partial sums; POS: possum2, s, cnt
       int nlab_lo[4], nlab_hi[4];                              // first / last label of the 4 chunks of the next tile
       chunk_labels<4>(a, sg.ct0 * BN + half * (BN / 2), sg.ct0 < sg.ct1 && a.sorted, ncols, nlab_lo, nlab_hi);
-      for (int ct = sg.ct0; ct < sg.ct1; ++ct, ++it) {
-        const uint32_t accb = it & 1, acc_phase = (it >> 1) & 1;
+      if (sg.ct1 > sg.ct0) ptx::mbar_wait(&sm.a_full, seg_idx & 1);
+      for (int ct = sg.ct0; ct < sg.ct1; ++ct) {
+        float acc[128];
+        ring_mma<STAGES, B_STAGE_BYTES, false>(acc, a_base, A_KB_BYTES, b_base, sm.full, sm.empty, ring, lane);
+        if (ct + 1 == sg.ct1 && lane == 0) ptx::mbar_arrive(&sm.a_empty);     // last MMA of the segment retired
         const int col0 = ct * BN + half * (BN / 2);
         // Per 32-column chunk: if the chunk is complete and of one class (sorted contrast set) every row treats it as
         // all-negative or all-positive without a per-element test.  Mixed chunks (a class boundary, the ragged end,
@@ -398,16 +410,15 @@ k_tc_fwd(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtens
         if (ct + 1 < sg.ct1) {
           chunk_labels<4>(a, (ct + 1) * BN + half * (BN / 2), a.sorted != 0, ncols, nlab_lo, nlab_hi);
         }
-        ptx::mbar_wait(&sm.tmem_full[accb], acc_phase);
-        ptx::tc_fence_after();
-        const uint32_t t_row = tmem_base + ((uint32_t)(quarter * 32) << 16) + accb * BN + half * (BN / 2);
-        uint32_t vbuf[2][32];
-        ptx::tmem_ld_32x32b_x32(t_row, vbuf[0]);
 #pragma unroll
         for (int ch = 0; ch < 4; ++ch) {
-          ptx::tmem_ld_wait();
-          if (ch < 3) ptx::tmem_ld_32x32b_x32(t_row + (ch + 1) * 32, vbuf[(ch + 1) & 1]);   // prefetch the next chunk
-          uint32_t(&v)[32] = vbuf[ch & 1];
+          // chunk ch of both column halves -> staging buffer -> this thread's row, 32 columns
+          frag_store_cols<4>(acc, 4 * ch, &sm.stage[g][0][0][0], SPITCH, t);
+          frag_store_cols<4>(acc, 16 + 4 * ch, &sm.stage[g][1][0][0], SPITCH, t);
+          ptx::bar_sync(2 + g, 128);
+          uint32_t v[32];
+          load_row32(&sm.stage[g][half][t & 63][0], v);
+          ptx::bar_sync(2 + g, 128);
           const int cb = col0 + ch * 32;
           const bool uniform = cuni[ch];
           const int ulab = clab[ch];
@@ -501,10 +512,8 @@ k_tc_fwd(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtens
             }
           }
         }
-        ptx::tc_fence_before();
-        __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(&sm.tmem_empty[accb]);
       }
+      if (sg.ct1 > sg.ct0) ++seg_idx;
       // ---- combine the two column halves, write the partials of this segment ----
       if (MODE != TC_DUMP && MODE != TC_H1 && MODE != TC_H2 && MODE != TC_H3) {
         if (MODE == TC_NEG || MODE == TC_NEGW) {
@@ -531,21 +540,16 @@ k_tc_fwd(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtens
       }
     }
   }
-
-  // ---- teardown ----
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) ptx::tmem_dealloc<TMEM_COLS>(tmem_base);
 }
 
 // =====================================================================================================
-// POS sweep of the bank mode for SMALL anchor sets, transposed: the bank's column tile is the M operand (TMEM lane =
-// bank column), a block of <= 64 anchors of ONE class the N operand.  The positives of an anchor are the R columns of
-// its class, so the work list is (class, anchor block, column split) and every element the epilogue touches is a
-// positive: all 128 lanes of all 4 schedulers work, whatever the class mix of the anchors.  (The row-tile POS sweep
-// above computes [128 anchors x 256 columns] tiles in which only the lanes of the tile's class do anything: with ~53
-// anchors per class — configs[2] — one or two of the eight epilogue warps carried a CTA, 53 us for 10 us of MUFU work,
-// profiles/r2_25_bank_source_top.txt.)  Per-anchor sums are reduced across the lanes once per work item.
+// POS sweep of the bank mode for SMALL anchor sets, transposed: the bank's column tile is the M operand (accumulator
+// row = bank column, 64 per consumer warpgroup), a block of <= 64 anchors of ONE class the N operand.  The positives of
+// an anchor are the R columns of its class, so the work list is (class, anchor block, column split) and every element
+// the epilogue touches is a positive: every consumer thread works, whatever the class mix of the anchors.  (The
+// row-tile POS sweep above computes [128 anchors x 256 columns] tiles in which only the rows of the tile's class do
+// anything: with ~53 anchors per class — configs[2] — one or two of the eight consumer warps would carry a CTA.)
+// Per-anchor sums are reduced across the bank columns once per work item.
 // Anchors must be in class-rank order (bank mode's contract, like the row-tile sweep's [rk_f, rk_l] range).
 // =====================================================================================================
 constexpr int PT_NB = 64;                          // anchors per block (N of the MMA)
@@ -553,6 +557,7 @@ constexpr int PT_BM = 128;                         // bank columns per tile (M o
 constexpr int PT_A_KB = PT_NB * BK * 2;            // 8 KB: [64 anchors x 64 K] box
 constexpr int PT_C_KB = PT_BM * BK * 2;            // 16 KB: [128 columns x 64 K] box
 constexpr int PT_STAGES = 8;                       // K-block stages of the bank stream (2 tiles in flight)
+static_assert(PT_BM == 2 * 64, "one M64 wgmma per consumer warpgroup");
 constexpr int PT_MAX_ROWS = 4096;                  // class-boundary scan of the prologue
 
 constexpr int PT_MAX_BLOCKS = PT_MAX_ROWS / PT_NB + PCL_MAX_CLASSES;      // blocks of <= 64 anchors of one class
@@ -560,24 +565,25 @@ constexpr int PT_MAX_BLOCKS = PT_MAX_ROWS / PT_NB + PCL_MAX_CLASSES;      // blo
 struct SmemPosT {
   uint8_t a[NKB * PT_A_KB];                        // 32 KB
   uint8_t c[PT_STAGES * PT_C_KB];                  // 128 KB
-  uint64_t full[PT_STAGES], empty[PT_STAGES], a_full, a_empty, tmem_full[2], tmem_empty[2];
-  uint32_t tmem_base;
+  float stage[2][64][PT_NB + 4];                   // [warpgroup][bank column][anchor]: the accumulator, row view
+  uint64_t full[PT_STAGES], empty[PT_STAGES], a_full, a_empty;
   int rk_first[PCL_MAX_CLASSES], rk_cnt[PCL_MAX_CLASSES];
   // work list: anchor blocks (first row, rows, class rank), exclusive prefix of their column tiles, blocks without tiles
   int blk_r0[PT_MAX_BLOCKS], blk_rk[PT_MAX_BLOCKS], tile_pref[PT_MAX_BLOCKS + 1], zlist[PT_MAX_BLOCKS];
   short blk_nv[PT_MAX_BLOCKS];
   int total_blocks, n_zero, P, U;
   float4 par[PT_NB];                               // per anchor of the block: m2, Neg, diag column (int bits), -
-  float comb[2][4][32][2];                         // [anchor half][lane quarter][anchor][possum2, s]
+  float comb[2][4][32][2];                         // [anchor half][column quarter][anchor][possum2, s]
 };
+static_assert(sizeof(SmemPosT) + 1024 <= 227 * 1024, "shared memory of one H100 block");
 
 // One segment = consecutive column tiles [t0, t1) of one anchor block; its partial sums go to slot `split`; the block
 // is covered by `nslots` segments (of consecutive CTAs).
 struct PosItem { int r0, nv, t0, t1, c_lo, c_hi, split, nslots; };
 
 // All tile units (block, tile) form one list of P entries; CTA k owns units [k U, (k+1) U) — a balanced walk whatever
-// the class mix (K = 171 classes: 171 blocks on 148 CTAs would otherwise make 23 CTAs do twice the work).  Every role
-// (TMA / MMA / epilogue) walks the same segments.  Blocks without tiles (class-0 anchors: their positives are the
+// the class mix (K = 171 classes: 171 blocks on 132 CTAs would otherwise make 39 CTAs do twice the work).  Every role
+// (TMA producer / consumer warpgroups) walks the same segments.  Blocks without tiles (class-0 anchors: their positives are the
 // analytic zero tail, k_finalize) are dealt round-robin and only write their rows.
 struct PosWalk {
   int u, u1, blk, z, k, G;
@@ -658,21 +664,17 @@ k_tc_pos_t(const __grid_constant__ CUtensorMap tmA64, const __grid_constant__ CU
     sm.U = max(1, max(U, u_slots));
     ptx::prefetch_tmap(&tmA64);
     ptx::prefetch_tmap(&tmC128);
-    for (int s = 0; s < PT_STAGES; ++s) { ptx::mbar_init(&sm.full[s], 1); ptx::mbar_init(&sm.empty[s], 1); }
+    for (int s = 0; s < PT_STAGES; ++s) { ptx::mbar_init(&sm.full[s], 1); ptx::mbar_init(&sm.empty[s], CONSUMER_WARPS); }
     ptx::mbar_init(&sm.a_full, 1);
-    ptx::mbar_init(&sm.a_empty, 1);
-    for (int i = 0; i < 2; ++i) { ptx::mbar_init(&sm.tmem_full[i], 1); ptx::mbar_init(&sm.tmem_empty[i], EPI_THREADS / 32); }
+    ptx::mbar_init(&sm.a_empty, CONSUMER_WARPS);
     ptx::fence_barrier_init();
   }
-  if (warp == 1) ptx::tmem_alloc<TMEM_COLS>(&sm.tmem_base);
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = sm.tmem_base;
 
-  if (warp == 0) {
+  if (warp >= PRODUCER_WARP) {
     // =========================== TMA producer ===========================
-    if (lane == 0) {
+    ptx::setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp == PRODUCER_WARP && lane == 0) {
       uint32_t stage = 0, phase = 0;
       int seq = 0;
       PosWalk w;
@@ -694,50 +696,17 @@ k_tc_pos_t(const __grid_constant__ CUtensorMap tmA64, const __grid_constant__ CU
         ++seq;
       }
     }
-  } else if (warp == 1) {
-    // =========================== MMA issuer ===========================
-    if (lane == 0) {
-      constexpr uint32_t idesc = ptx::make_idesc_bf16(PT_BM, PT_NB, 0, 0);
-      const uint32_t a_base = ptx::smem_u32(sm.a), c_base = ptx::smem_u32(sm.c);
-      uint32_t stage = 0, phase = 0;
-      int seq = 0, n = 0;
-      PosWalk w;
-      PosItem it;
-      w.init(sm, blockIdx.x, gridDim.x);
-      while (w.next(sm, a, it)) {
-        if (it.t1 <= it.t0) continue;
-        ptx::mbar_wait(&sm.a_full, seq & 1);
-        ptx::tc_fence_after();
-        for (int t = it.t0; t < it.t1; ++t, ++n) {
-          const uint32_t acc = n & 1, acc_phase = (n >> 1) & 1;
-          ptx::mbar_wait(&sm.tmem_empty[acc], acc_phase ^ 1);
-          ptx::tc_fence_after();
-          const uint32_t d_tmem = tmem_base + acc * PT_NB;
-          for (int kb = 0; kb < NKB; ++kb) {
-            ptx::mbar_wait(&sm.full[stage], phase);
-            ptx::tc_fence_after();
-#pragma unroll
-            for (int k = 0; k < BK / 16; ++k) {
-              const uint64_t dc = ptx::make_desc_kmajor_sw128(c_base + stage * PT_C_KB + k * 32);    // M side: bank columns
-              const uint64_t da = ptx::make_desc_kmajor_sw128(a_base + kb * PT_A_KB + k * 32);       // N side: anchors
-              ptx::mma_f16_ss(d_tmem, dc, da, idesc, (kb | k) != 0 ? 1u : 0u);
-            }
-            ptx::mma_commit(&sm.empty[stage]);
-            if (++stage == PT_STAGES) { stage = 0; phase ^= 1; }
-          }
-          ptx::mma_commit(&sm.tmem_full[acc]);
-        }
-        ptx::mma_commit(&sm.a_empty);
-        ++seq;
-      }
-    }
   } else {
-    // =========================== epilogue warps ===========================
-    const int quarter = warp & 3;                     // TMEM lane quarter this warp may access
-    const int ahalf = (warp - 2) >> 2;                // which 32 anchors of the block
-    const int et = threadIdx.x - 64;                  // 0..255 within the epilogue group
+    // =========================== consumer warpgroups: wgmma (M = 64 bank columns each, N = 64 anchors) + epilogue ====
+    ptx::setmaxnreg_inc<CONSUMER_REGS>();
+    const int g = threadIdx.x >> 7, t = threadIdx.x & 127;
+    const int quarter = g * 2 + ((t & 63) >> 5);      // which 32 bank columns of the 128-column tile
+    const int ahalf = t >> 6;                         // which 32 anchors of the block
+    const int et = threadIdx.x;                       // 0..255 within the consumer group
+    const uint32_t a_base = ptx::smem_u32(sm.a), c_base = ptx::smem_u32(sm.c) + g * WG_ROW_BYTES;
     const int64_t stride = (int64_t)a.slots * a.a_pad;
-    int n = 0;
+    Ring ring;
+    int seq = 0;
     PosWalk w;
     PosItem it;
     w.init(sm, blockIdx.x, gridDim.x);
@@ -772,18 +741,21 @@ k_tc_pos_t(const __grid_constant__ CUtensorMap tmA64, const __grid_constant__ CU
 #pragma unroll
       for (int i = 0; i < 32; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
       const int nvh = min(32, max(0, it.nv - ahalf * 32));                  // valid anchors of this warp's half
-      for (int t = it.t0; t < it.t1; ++t, ++n) {
-        const uint32_t accb = n & 1, acc_phase = (n >> 1) & 1;
-        const int col = t * PT_BM + quarter * 32 + lane;
-        const bool colkeep = col >= it.c_lo && col < it.c_hi;
-        ptx::mbar_wait(&sm.tmem_full[accb], acc_phase);
-        ptx::tc_fence_after();
+      if (it.t1 > it.t0) ptx::mbar_wait(&sm.a_full, seq & 1);
+      for (int tl = it.t0; tl < it.t1; ++tl) {
+        float acc[32];
+        ring_mma<PT_STAGES, PT_C_KB, true>(acc, a_base, PT_A_KB, c_base, sm.full, sm.empty, ring, lane);
+        if (tl + 1 == it.t1 && lane == 0) ptx::mbar_arrive(&sm.a_empty);     // last MMA of the block retired
+        frag_store_cols<8>(acc, 0, &sm.stage[g][0][0], PT_NB + 4, t);
+        ptx::bar_sync(2 + g, 128);
         uint32_t v[32];
-        ptx::tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(quarter * 32) << 16) + accb * PT_NB + ahalf * 32, v);
-        ptx::tmem_ld_wait();
+        load_row32(&sm.stage[g][t & 63][ahalf * 32], v);
+        ptx::bar_sync(2 + g, 128);
+        const int col = tl * PT_BM + quarter * 32 + lane;
+        const bool colkeep = col >= it.c_lo && col < it.c_hi;
         // groups of 8 anchors behind ONE warp-uniform test: inside a group the 8 LDS -> FMA -> EX2 -> LG2 / RCP chains
-        // are independent and interleave (a test per anchor made 32 basic blocks, i.e. 32 serial ~100-cycle chains per
-        // tile: 3000 cycles per tile instead of the ~1500 the MUFU pipe needs, profiles/r2_36 ncu: XU 20 %).  Anchors
+        // are independent and interleave (a test per anchor makes 32 basic blocks, i.e. 32 serial MUFU chains per
+        // tile).  Anchors
         // past the block's end inside a group carry neutral constants (m2 = 0, Neg = 1) and are never written.
 #pragma unroll
         for (int i0 = 0; i0 < 32; i0 += 8) {
@@ -799,10 +771,8 @@ k_tc_pos_t(const __grid_constant__ CUtensorMap tmA64, const __grid_constant__ CU
             }
           }
         }
-        ptx::tc_fence_before();
-        __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(&sm.tmem_empty[accb]);
       }
+      if (it.t1 > it.t0) ++seq;
       // ---- sum over the 128 lanes (columns): butterfly inside the warp, then the 4 quarters through shared memory ----
 #pragma unroll
       for (int i = 0; i < 32; ++i) {
@@ -836,33 +806,28 @@ k_tc_pos_t(const __grid_constant__ CUtensorMap tmA64, const __grid_constant__ CU
       asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");       // par / comb reusable by the next item
     }
   }
-
-  // ---- teardown ----
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) ptx::tmem_dealloc<TMEM_COLS>(tmem_base);
 }
 
 // =====================================================================================================
 // Backward: dA = G . C / T with G formed on the fly (closed form, SURVEY appendix A) — FlashAttention-backward
-// shaped: MMA1 S = A.C^T (128 x 128 tile, K = 256) -> epilogue turns S into the bf16 gradient tile G in shared
-// memory (128B-swizzled K-major) -> MMA2 dA(128 x 256, TMEM-resident across the whole column sweep) += G . C,
-// where the SAME shared-memory contrast tile is re-read as an MN-major B operand.
-// TMEM: S double buffer = columns [0,256), dA accumulator = columns [256,512).
+// shaped, per consumer warpgroup (64 anchor rows): wgmma 1 S = A.C^T (64 x 64 tile, K = 256) -> epilogue turns S into
+// the bf16 gradient tile G in shared memory (128B-swizzled K-major) -> wgmma 2 dA(64 x 256, registers, across the whole
+// column sweep) += G . C, where the SAME shared-memory contrast tile is re-read as an MN-major B operand.
 // =====================================================================================================
-constexpr int BNB = 128;                          // columns per tile in the backward sweep
-constexpr int C_KB_BYTES = BNB * BK * 2;          // 16 KB: one [128 x 64] box
-constexpr int C_STAGE_BYTES = NKB * C_KB_BYTES;   // 64 KB: the full [128 x 256] tile
-constexpr int G_BYTES = BM * BNB * 2;             // 32 KB
-constexpr int BWD_STAGES = 2;
+constexpr int BNB = 64;                           // columns per tile in the backward sweep
+constexpr int C_KB_BYTES = BNB * BK * 2;          // 8 KB: one [64 x 64] box
+constexpr int C_STAGE_BYTES = NKB * C_KB_BYTES;   // 32 KB: the full [64 x 256] tile
+constexpr int G_BYTES = BM * BNB * 2;             // 16 KB
+constexpr int BWD_STAGES = 3;
 
 struct SmemBwd {
   uint8_t a[NKB * A_KB_BYTES];                    // 64 KB
-  uint8_t c[BWD_STAGES * C_STAGE_BYTES];          // 128 KB
-  uint8_t g[G_BYTES];                             // 32 KB
-  uint64_t a_full, c_full[BWD_STAGES], c_empty[BWD_STAGES], s_full[2], s_empty[2], g_full, g_empty, da_full;
-  uint32_t tmem_base;
+  uint8_t c[BWD_STAGES * C_STAGE_BYTES];          // 96 KB
+  uint8_t g[G_BYTES];                             // 16 KB
+  float stage[2][64][BNB + 4];                    // [warpgroup][row][column]: S, row view
+  uint64_t a_full, c_full[BWD_STAGES], c_empty[BWD_STAGES];
 };
+static_assert(sizeof(SmemBwd) + 1024 <= 227 * 1024, "shared memory of one H100 block");
 
 struct TcBwdArgs {
   TcArgs t;
@@ -876,12 +841,8 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   return *reinterpret_cast<uint32_t*>(&v);
 }
 
-
-// EPI_W epilogue warps (8 or 16).  The epilogue (one ex2 + a few ALU ops per logit, then the bf16 gradient tile) is a chain
-// of dependent instructions per element; with 8 warps (2 per scheduler) the issue slots were 29 % busy and the tensor
-// pipe 49 % (profiles/r2_06_bank_source_top.txt): 16 warps halve the columns per thread and double the latency hiding.
-template <int EPI_W, bool TOPK>
-__global__ void __launch_bounds__(64 + 32 * EPI_W, 1)
+template <bool TOPK>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
 k_tc_bwd(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmC, TcBwdArgs ba,
          float* __restrict__ dpartials) {
   extern __shared__ uint8_t smem_raw[];
@@ -896,34 +857,26 @@ k_tc_bwd(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtens
   const int t_hi = (int)((ncols + BNB - 1) / BNB);
   // Column tiles are dealt round-robin to the splits (tile = split + it * splits): the tiles that hold a row tile's
   // positives (2 MUFU ops per logit, divergent rows) are spread over all its CTAs instead of landing on two or three
-  // of them (contiguous ranges left 30 % of the SM time idle behind the slowest CTAs: profiles/r1_s2_bwd_*).
+  // of them (contiguous ranges left 30 % of the SM time idle behind the slowest CTAs).
   const int my_lo = split, tstep = a.splits;
   const int ntiles = t_hi > split ? (t_hi - split + a.splits - 1) / a.splits : 0;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == PRODUCER_WARP && lane == 0) {
     ptx::prefetch_tmap(&tmA);
     ptx::prefetch_tmap(&tmC);
     ptx::mbar_init(&sm.a_full, 1);
-    for (int s = 0; s < BWD_STAGES; ++s) { ptx::mbar_init(&sm.c_full[s], 1); ptx::mbar_init(&sm.c_empty[s], 1); }
-    for (int i = 0; i < 2; ++i) { ptx::mbar_init(&sm.s_full[i], 1); ptx::mbar_init(&sm.s_empty[i], EPI_W); }
-    ptx::mbar_init(&sm.g_full, EPI_W);
-    ptx::mbar_init(&sm.g_empty, 1);
-    ptx::mbar_init(&sm.da_full, 1);
+    for (int s = 0; s < BWD_STAGES; ++s) { ptx::mbar_init(&sm.c_full[s], 1); ptx::mbar_init(&sm.c_empty[s], CONSUMER_WARPS); }
     ptx::fence_barrier_init();
   }
-  if (warp == 1) ptx::tmem_alloc<TMEM_COLS>(&sm.tmem_base);
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = sm.tmem_base;
-  const uint32_t tmem_dA = tmem_base + 2 * BNB;
 
-  if (warp == 0) {
-    if (lane == 0 && ntiles > 0) {
+  if (warp >= PRODUCER_WARP) {
+    ptx::setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp == PRODUCER_WARP && lane == 0 && ntiles > 0) {
       ptx::mbar_arrive_expect_tx(&sm.a_full, NKB * A_KB_BYTES);
       for (int kb = 0; kb < NKB; ++kb) ptx::tma_load_2d(sm.a + kb * A_KB_BYTES, &tmA, &sm.a_full, kb * BK, row0);
       for (int it = 0; it < ntiles; ++it) {
-        const int stage = it & 1, phase = (it >> 1) & 1;
+        const int stage = it % BWD_STAGES, phase = (it / BWD_STAGES) & 1;
         ptx::mbar_wait(&sm.c_empty[stage], phase ^ 1);
         ptx::mbar_arrive_expect_tx(&sm.c_full[stage], C_STAGE_BYTES);
         for (int kb = 0; kb < NKB; ++kb)
@@ -931,249 +884,184 @@ k_tc_bwd(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtens
                            (my_lo + it * tstep) * BNB);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0 && ntiles > 0) {
-      constexpr uint32_t idesc1 = ptx::make_idesc_bf16(BM, BNB, 0, 0);     // S = A . C^T   (both K-major)
-      constexpr uint32_t idesc2 = ptx::make_idesc_bf16(BM, DDIM, 0, 1);    // dA += G . C   (B operand MN-major)
-      const uint32_t a_base = ptx::smem_u32(sm.a), c_base = ptx::smem_u32(sm.c), g_base = ptx::smem_u32(sm.g);
-      ptx::mbar_wait(&sm.a_full, 0);
-      ptx::tc_fence_after();
-      auto mma2 = [&](int t) {                    // caller has observed g_full of tile t
-        const int stage = t & 1;
-        ptx::tc_fence_after();
+    return;
+  }
+  // =========================== consumer warpgroups: wgmma 1, epilogue, wgmma 2 ===========================
+  ptx::setmaxnreg_inc<CONSUMER_REGS>();
+  const int g = threadIdx.x >> 7, t = threadIdx.x & 127;
+  const int half = t >> 6;                        // which 32 columns of the 64-column tile
+  const int r_in = g * 64 + (t & 63);
+  const int row = row0 + r_in;
+  const bool valid = row < A;
+  const float* st = ba.rowstats;
+  const int rcls = valid ? a.acls[row] : -1;
+  const int rdiag = valid ? (a.mode == 0 ? row : (a.diag ? a.diag[row] : -1)) : -1;
+  const float m2 = valid ? a.row_m2[row] : 0.f;
+  const float neg_i = valid ? st[a.a_rows + row] : 1.f;
+  const float s_i = valid ? st[3 * a.a_rows + row] : 0.f;
+  float c_i = 0.f;
+  if (valid) {
+    const float np = st[4 * a.a_rows + row];
+    c_i = ba.rs_scale / ((float)A * np);
+    if (ba.nan_safe && !(np > 0.f)) c_i = 0.f;
+  }
+  const float cs_i = c_i * s_i;
+  const float cn_i = -c_i * neg_i;
+  // a10: selection weights on the negatives (tau key, tie weight; pcl_topk.cuh); key = rn(s * k1) as in the forward
+  uint32_t tk_tau = 0u;
+  float tk_tw = 1.f;
+  if (TOPK && valid) { tk_tau = a.tk_sel[row]; tk_tw = __uint_as_float(a.tk_sel[a.a_rows + row]); }
+  const uint32_t a_base = ptx::smem_u32(sm.a) + g * WG_ROW_BYTES, c_base = ptx::smem_u32(sm.c);
+  const uint32_t g_base = ptx::smem_u32(sm.g) + g * WG_ROW_BYTES;
+  uint8_t* g_row = sm.g + r_in * 128;             // + swizzled 16-byte chunk
+  float dacc[128];                                // dA of the warpgroup's 64 rows x 256 features
 #pragma unroll
-        for (int k = 0; k < BNB / 16; ++k) {
-          // A operand: G tile, K-major, K = column index j: 2 blocks of 64 j, 32 B per 16-element K step
-          const uint64_t dg = ptx::make_desc_kmajor_sw128(g_base + (k >> 2) * (BM * 128) + (k & 3) * 32);
-          // B operand: contrast tile read MN-major: N = feature d (4 chunks of 64 at 16 KB), K = j (16 rows = 2 KB per step)
-          const uint64_t dc = ptx::make_desc_mnmajor_sw128(c_base + stage * C_STAGE_BYTES + k * 2048, C_KB_BYTES, 1024);
-          ptx::mma_f16_ss(tmem_dA, dg, dc, idesc2, (t | k) != 0 ? 1u : 0u);
-        }
-        ptx::mma_commit(&sm.g_empty);
-        ptx::mma_commit(&sm.c_empty[stage]);
-      };
-      // Readiness-driven issue order: MMA1(n1) (needs a free S buffer and the contrast tile) and MMA2(n2) (needs the
-      // gradient tile G(n2) from the epilogue) are issued as soon as their inputs are ready, so a slow epilogue of
-      // tile n2 never delays the similarity MMA of the tiles behind it.
-      int n1 = 0, n2 = 0;
-      uint32_t idle = 0;
-      while (n2 < ntiles) {
-        bool progressed = false;
-        if (n1 < ntiles) {
-          const int stage = n1 & 1, phase = (n1 >> 1) & 1;
-          const uint32_t acc = n1 & 1;
-          if (ptx::mbar_try_wait(&sm.s_empty[acc], phase ^ 1) && ptx::mbar_try_wait(&sm.c_full[stage], phase)) {
-            ptx::tc_fence_after();
-            const uint32_t d_tmem = tmem_base + acc * BNB;
-#pragma unroll
-            for (int kb = 0; kb < NKB; ++kb) {
-#pragma unroll
-              for (int k = 0; k < BK / 16; ++k) {
-                const uint64_t da = ptx::make_desc_kmajor_sw128(a_base + kb * A_KB_BYTES + k * 32);
-                const uint64_t dc = ptx::make_desc_kmajor_sw128(c_base + stage * C_STAGE_BYTES + kb * C_KB_BYTES + k * 32);
-                ptx::mma_f16_ss(d_tmem, da, dc, idesc1, (kb | k) != 0 ? 1u : 0u);
-              }
-            }
-            ptx::mma_commit(&sm.s_full[acc]);
-            ++n1;
-            progressed = true;
-          }
-        }
-        if (n2 < n1 && ptx::mbar_try_wait(&sm.g_full, n2 & 1)) {
-          mma2(n2);
-          ++n2;
-          progressed = true;
-        }
-        if (progressed) idle = 0;
-        else if (++idle > (1u << 26)) {
-          printf("pcl: k_tc_bwd MMA issuer stuck block (%d,%d) n1=%d n2=%d of %d\n", blockIdx.x, blockIdx.y, n1, n2, ntiles);
-          __trap();
-        }
-      }
-      ptx::mma_commit(&sm.da_full);
+  for (int i = 0; i < 128; ++i) dacc[i] = 0.f;
+  int nlab_lo[1], nlab_hi[1];
+  chunk_labels<1>(a, my_lo * BNB + half * 32, ntiles > 0 && a.sorted && a.mode != 0, (int64_t)ncols, nlab_lo, nlab_hi);
+  if (ntiles > 0) ptx::mbar_wait(&sm.a_full, 0);
+  for (int it = 0; it < ntiles; ++it) {
+    const int ct = my_lo + it * tstep;
+    const int stage = it % BWD_STAGES, phase = (it / BWD_STAGES) & 1;
+    const int cb = ct * BNB + half * 32;
+    const int clab = nlab_lo[0];
+    const bool cuni = a.sorted && a.mode != 0 && cb + 32 <= (int)ncols && nlab_lo[0] == nlab_hi[0];
+    if (it + 1 < ntiles) {                         // labels of the next tile: loads fly while this tile is processed
+      chunk_labels<1>(a, (ct + tstep) * BNB + half * 32, a.sorted && a.mode != 0, (int64_t)ncols, nlab_lo, nlab_hi);
     }
-  } else {
-    constexpr int SLICES = EPI_W / 4;             // column slices of the 128-column tile (one per warp of a lane quarter)
-    constexpr int CPS = BNB / SLICES;             // columns per slice: 64 (8 warps) or 32 (16 warps)
-    constexpr int NCH = CPS / 32;                 // 32-column chunks per thread
-    const int quarter = warp & 3;
-    const int half = (warp - 2) >> 2;             // which column slice of the 128-column tile
-    const int r_in = quarter * 32 + lane;
-    const int row = row0 + r_in;
-    const bool valid = row < A;
-    const float* st = ba.rowstats;
-    const int rcls = valid ? a.acls[row] : -1;
-    const int rdiag = valid ? (a.mode == 0 ? row : (a.diag ? a.diag[row] : -1)) : -1;
-    const float m2 = valid ? a.row_m2[row] : 0.f;
-    const float neg_i = valid ? st[a.a_rows + row] : 1.f;
-    const float s_i = valid ? st[3 * a.a_rows + row] : 0.f;
-    float c_i = 0.f;
-    if (valid) {
-      const float np = st[4 * a.a_rows + row];
-      c_i = ba.rs_scale / ((float)A * np);
-      if (ba.nan_safe && !(np > 0.f)) c_i = 0.f;
-    }
-    const float cs_i = c_i * s_i;
-    const float cn_i = -c_i * neg_i;
-    // a10: selection weights on the negatives (tau key, tie weight; pcl_topk.cuh); key = rn(s * k1) as in the forward
-    uint32_t tk_tau = 0u;
-    float tk_tw = 1.f;
-    if (TOPK && valid) { tk_tau = a.tk_sel[row]; tk_tw = __uint_as_float(a.tk_sel[a.a_rows + row]); }
-    uint8_t* g_row = sm.g + r_in * 128;           // + kblock * 16 KB + swizzled 16-byte chunk
-    int nlab_lo[NCH], nlab_hi[NCH];
-    chunk_labels<NCH>(a, my_lo * BNB + half * CPS, ntiles > 0 && a.sorted && a.mode != 0, (int64_t)ncols, nlab_lo, nlab_hi);
-    for (int it = 0; it < ntiles; ++it) {
-      const int ct = my_lo + it * tstep;
-      const uint32_t acc = it & 1, phase = (it >> 1) & 1;
-      const int col0 = ct * BNB + half * CPS;
-      int clab[NCH];
-      bool cuni[NCH];
+    // ---- wgmma 1: S = A . C^T ----
+    ptx::mbar_wait(&sm.c_full[stage], phase);
+    const uint32_t c_stage = c_base + stage * C_STAGE_BYTES;
+    {
+      float sacc[32];
+      ptx::wgmma_fence();
 #pragma unroll
-      for (int ch = 0; ch < NCH; ++ch) {
-        const int cb = col0 + ch * 32;
-        clab[ch] = nlab_lo[ch];
-        cuni[ch] = a.sorted && a.mode != 0 && cb + 32 <= (int)ncols && nlab_lo[ch] == nlab_hi[ch];
-      }
-      if (it + 1 < ntiles) {                       // labels of the next tile: loads fly while this tile is processed
-        chunk_labels<NCH>(a, (ct + tstep) * BNB + half * CPS, a.sorted && a.mode != 0, (int64_t)ncols, nlab_lo, nlab_hi);
-      }
-      ptx::mbar_wait(&sm.s_full[acc], phase);
-      ptx::tc_fence_after();
-      const uint32_t t_row = tmem_base + ((uint32_t)(quarter * 32) << 16) + acc * BNB + half * CPS;
-      uint32_t packed[NCH][16];
-      uint32_t vbuf[NCH][32];
-      ptx::tmem_ld_32x32b_x32(t_row, vbuf[0]);
+      for (int kb = 0; kb < NKB; ++kb) {
 #pragma unroll
-      for (int ch = 0; ch < NCH; ++ch) {
-        ptx::tmem_ld_wait();
-        if (ch + 1 < NCH) ptx::tmem_ld_32x32b_x32(t_row + 32, vbuf[NCH - 1]);   // prefetch the second chunk
-        uint32_t(&v)[32] = vbuf[ch];
-        const int cb = col0 + ch * 32;
-        float gv[32];
-        if (cuni[ch] && clab[ch] != rcls) {
-          // all-negative chunk: G = c S e   (cs_i == 0 for rows beyond A)
-          if (TOPK) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              const float x = __fmul_rn(__uint_as_float(v[j]), a.k1);
-              gv[j] = cs_i * topk_weight(sortable_key(x), tk_tau, tk_tw) * ptx::ex2_approx(x - m2);
-            }
-          } else {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) gv[j] = cs_i * ptx::ex2_approx(fmaf(__uint_as_float(v[j]), a.k1, -m2));
-          }
-        } else if (cuni[ch]) {
-          // all-positive chunk: G = -c Neg / (e + Neg), zero on the masked (i,i) column
-          const bool has_diag = rdiag >= cb && rdiag < cb + 32;
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const float gpos = cn_i * ptx::rcp_approx(ptx::ex2_approx(fmaf(__uint_as_float(v[j]), a.k1, -m2)) + neg_i);
-            gv[j] = (has_diag && cb + j == rdiag) ? 0.f : gpos;
-          }
-        } else if (a.mode != 0) {
-          // mixed chunk: one label per lane, broadcast with shuffles
-          const int mylab = (cb + lane < (int)ncols) ? col_label(a, cb + lane) : -2;
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const int lj = __shfl_sync(0xffffffffu, mylab, j);
-            const float xq = __fmul_rn(__uint_as_float(v[j]), a.k1);
-            const float e = TOPK ? ptx::ex2_approx(xq - m2) : ptx::ex2_approx(fmaf(__uint_as_float(v[j]), a.k1, -m2));
-            const float gneg = TOPK ? cs_i * e * topk_weight(sortable_key(xq), tk_tau, tk_tw) : cs_i * e;
-            const float gpos = (cb + j == rdiag) ? 0.f : cn_i * ptx::rcp_approx(e + neg_i);
-            gv[j] = (!valid || lj == -2) ? 0.f : (lj == rcls ? gpos : gneg);
-          }
-        } else {
-          // self-contrast: every column is an anchor too -> H = G + G^T needs the column's statistics; lane L holds
-          // those of column cb + L and they are broadcast per element
-          const int cj = cb + lane;
-          const bool cok = cj < (int)ncols;
-          const int mylab = cok ? a.acls[cj] : -2;
-          float my_m2 = 0.f, my_neg = 1.f, my_cs = 0.f, my_cn = 0.f;
-          uint32_t my_tau = 0u;
-          float my_tw = 1.f;
-          if (TOPK && cok) { my_tau = a.tk_sel[cj]; my_tw = __uint_as_float(a.tk_sel[a.a_rows + cj]); }
-          if (cok) {
-            const float np_j = st[4 * a.a_rows + cj];
-            float c_j = ba.rs_scale / ((float)A * np_j);
-            if (ba.nan_safe && !(np_j > 0.f)) c_j = 0.f;
-            my_m2 = a.row_m2[cj];
-            my_neg = st[a.a_rows + cj];
-            my_cs = c_j * st[3 * a.a_rows + cj];
-            my_cn = -c_j * my_neg;
-          }
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const int lj = __shfl_sync(0xffffffffu, mylab, j);
-            const float m2j = __shfl_sync(0xffffffffu, my_m2, j);
-            const float negj = __shfl_sync(0xffffffffu, my_neg, j);
-            const float csj = __shfl_sync(0xffffffffu, my_cs, j);
-            const float cnj = __shfl_sync(0xffffffffu, my_cn, j);
-            const float x = __fmul_rn(__uint_as_float(v[j]), a.k1);
-            const float e = ptx::ex2_approx(x - m2);
-            const float e2 = ptx::ex2_approx(x - m2j);
-            const bool same = lj == rcls;
-            const bool diag = (cb + j == rdiag);
-            float wi = 1.f, wj = 1.f;
-            if (TOPK) {
-              const uint32_t key = sortable_key(x);
-              wi = topk_weight(key, tk_tau, tk_tw);
-              wj = topk_weight(key, __shfl_sync(0xffffffffu, my_tau, j), __shfl_sync(0xffffffffu, my_tw, j));
-            }
-            const float g_ij = same ? (diag ? 0.f : cn_i * ptx::rcp_approx(e + neg_i)) : cs_i * e * wi;
-            const float g_ji = same ? (diag ? 0.f : cnj * ptx::rcp_approx(e2 + negj)) : csj * e2 * wj;
-            gv[j] = (!valid || lj == -2) ? 0.f : (g_ij + g_ji);
-          }
-        }
-#pragma unroll
-        for (int j = 0; j < 16; ++j) packed[ch][j] = pack_bf16x2(gv[2 * j], gv[2 * j + 1]);
-      }
-      // S fully read: hand the accumulator back before waiting for the G buffer
-      ptx::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) ptx::mbar_arrive(&sm.s_empty[acc]);
-      // G buffer free once MMA2 of the previous tile retired
-      ptx::mbar_wait(&sm.g_empty, (it & 1) ^ 1);
-      // this thread's columns inside the G tile: K-block (64 columns) kb, 16-byte chunks 128B-swizzled by row
-#pragma unroll
-      for (int ch = 0; ch < NCH; ++ch) {
-        const int c0 = half * CPS + ch * 32;          // first column of the chunk inside the tile
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const int chunk = ((c0 & 63) >> 3) + q;
-          uint4 val = make_uint4(packed[ch][4 * q], packed[ch][4 * q + 1], packed[ch][4 * q + 2], packed[ch][4 * q + 3]);
-          *reinterpret_cast<uint4*>(g_row + (c0 >> 6) * (BM * 128) + ((chunk ^ (r_in & 7)) << 4)) = val;
+        for (int k = 0; k < BK / 16; ++k) {
+          const uint64_t da = ptx::make_desc_kmajor_sw128(a_base + kb * A_KB_BYTES + k * 32);
+          const uint64_t dc = ptx::make_desc_kmajor_sw128(c_stage + kb * C_KB_BYTES + k * 32);
+          ptx::wgmma_m64n64k16<0>(sacc, da, dc, (kb | k) != 0 ? 1u : 0u);
         }
       }
-      ptx::fence_proxy_async();                   // generic-proxy stores -> visible to the tensor core (async proxy)
-      __syncwarp();
-      if (lane == 0) ptx::mbar_arrive(&sm.g_full);
+      ptx::wgmma_commit();
+      ptx::wgmma_wait<0>();
+      ptx::fence_operands(sacc);
+      frag_store_cols<8>(sacc, 0, &sm.stage[g][0][0], BNB + 4, t);
     }
-    // ---- dA tile: TMEM -> global partial of this split ----
-    if (ntiles > 0) {
-      ptx::mbar_wait(&sm.da_full, 0);
-      ptx::tc_fence_after();
-    }
-    constexpr int DCOLS = DDIM / SLICES;           // dA columns this thread stores: 128 or 64
-    float* dst = dpartials + ((int64_t)split * a.a_pad + row) * DDIM + half * DCOLS;
-    const uint32_t t_da = tmem_dA + ((uint32_t)(quarter * 32) << 16) + half * DCOLS;
-#pragma unroll 1
-    for (int ch = 0; ch < DCOLS / 32; ++ch) {
-      uint32_t v[32];
-      if (ntiles > 0) {
-        ptx::tmem_ld_32x32b_x32(t_da + ch * 32, v);
-        ptx::tmem_ld_wait();
+    ptx::bar_sync(2 + g, 128);
+    uint32_t v[32];
+    load_row32(&sm.stage[g][t & 63][half * 32], v);
+    // ---- epilogue: the gradient tile G of this thread's row, 32 columns ----
+    float gv[32];
+    if (cuni && clab != rcls) {
+      // all-negative chunk: G = c S e   (cs_i == 0 for rows beyond A)
+      if (TOPK) {
+#pragma unroll
+        for (int j = 0; j < 32; ++j) {
+          const float x = __fmul_rn(__uint_as_float(v[j]), a.k1);
+          gv[j] = cs_i * topk_weight(sortable_key(x), tk_tau, tk_tw) * ptx::ex2_approx(x - m2);
+        }
       } else {
 #pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = 0u;
+        for (int j = 0; j < 32; ++j) gv[j] = cs_i * ptx::ex2_approx(fmaf(__uint_as_float(v[j]), a.k1, -m2));
+      }
+    } else if (cuni) {
+      // all-positive chunk: G = -c Neg / (e + Neg), zero on the masked (i,i) column
+      const bool has_diag = rdiag >= cb && rdiag < cb + 32;
+#pragma unroll
+      for (int j = 0; j < 32; ++j) {
+        const float gpos = cn_i * ptx::rcp_approx(ptx::ex2_approx(fmaf(__uint_as_float(v[j]), a.k1, -m2)) + neg_i);
+        gv[j] = (has_diag && cb + j == rdiag) ? 0.f : gpos;
+      }
+    } else if (a.mode != 0) {
+      // mixed chunk: one label per lane, broadcast with shuffles
+      const int mylab = (cb + lane < (int)ncols) ? col_label(a, cb + lane) : -2;
+#pragma unroll
+      for (int j = 0; j < 32; ++j) {
+        const int lj = __shfl_sync(0xffffffffu, mylab, j);
+        const float xq = __fmul_rn(__uint_as_float(v[j]), a.k1);
+        const float e = TOPK ? ptx::ex2_approx(xq - m2) : ptx::ex2_approx(fmaf(__uint_as_float(v[j]), a.k1, -m2));
+        const float gneg = TOPK ? cs_i * e * topk_weight(sortable_key(xq), tk_tau, tk_tw) : cs_i * e;
+        const float gpos = (cb + j == rdiag) ? 0.f : cn_i * ptx::rcp_approx(e + neg_i);
+        gv[j] = (!valid || lj == -2) ? 0.f : (lj == rcls ? gpos : gneg);
+      }
+    } else {
+      // self-contrast: every column is an anchor too -> H = G + G^T needs the column's statistics; lane L holds
+      // those of column cb + L and they are broadcast per element
+      const int cj = cb + lane;
+      const bool cok = cj < (int)ncols;
+      const int mylab = cok ? a.acls[cj] : -2;
+      float my_m2 = 0.f, my_neg = 1.f, my_cs = 0.f, my_cn = 0.f;
+      uint32_t my_tau = 0u;
+      float my_tw = 1.f;
+      if (TOPK && cok) { my_tau = a.tk_sel[cj]; my_tw = __uint_as_float(a.tk_sel[a.a_rows + cj]); }
+      if (cok) {
+        const float np_j = st[4 * a.a_rows + cj];
+        float c_j = ba.rs_scale / ((float)A * np_j);
+        if (ba.nan_safe && !(np_j > 0.f)) c_j = 0.f;
+        my_m2 = a.row_m2[cj];
+        my_neg = st[a.a_rows + cj];
+        my_cs = c_j * st[3 * a.a_rows + cj];
+        my_cn = -c_j * my_neg;
       }
 #pragma unroll
-      for (int j = 0; j < 32; j += 4)
-        *reinterpret_cast<uint4*>(dst + ch * 32 + j) = make_uint4(v[j], v[j + 1], v[j + 2], v[j + 3]);
+      for (int j = 0; j < 32; ++j) {
+        const int lj = __shfl_sync(0xffffffffu, mylab, j);
+        const float m2j = __shfl_sync(0xffffffffu, my_m2, j);
+        const float negj = __shfl_sync(0xffffffffu, my_neg, j);
+        const float csj = __shfl_sync(0xffffffffu, my_cs, j);
+        const float cnj = __shfl_sync(0xffffffffu, my_cn, j);
+        const float x = __fmul_rn(__uint_as_float(v[j]), a.k1);
+        const float e = ptx::ex2_approx(x - m2);
+        const float e2 = ptx::ex2_approx(x - m2j);
+        const bool same = lj == rcls;
+        const bool diag = (cb + j == rdiag);
+        float wi = 1.f, wj = 1.f;
+        if (TOPK) {
+          const uint32_t key = sortable_key(x);
+          wi = topk_weight(key, tk_tau, tk_tw);
+          wj = topk_weight(key, __shfl_sync(0xffffffffu, my_tau, j), __shfl_sync(0xffffffffu, my_tw, j));
+        }
+        const float g_ij = same ? (diag ? 0.f : cn_i * ptx::rcp_approx(e + neg_i)) : cs_i * e * wi;
+        const float g_ji = same ? (diag ? 0.f : cnj * ptx::rcp_approx(e2 + negj)) : csj * e2 * wj;
+        gv[j] = (!valid || lj == -2) ? 0.f : (g_ij + g_ji);
+      }
     }
+    // this thread's 32 columns = half of the G tile's 128-byte row: 4 chunks of 16 B, 128B-swizzled by row (the previous
+    // tile's wgmma 2 has retired: it was waited for before this tile began)
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const int chunk = half * 4 + q;
+      uint4 val = make_uint4(pack_bf16x2(gv[8 * q], gv[8 * q + 1]), pack_bf16x2(gv[8 * q + 2], gv[8 * q + 3]),
+                             pack_bf16x2(gv[8 * q + 4], gv[8 * q + 5]), pack_bf16x2(gv[8 * q + 6], gv[8 * q + 7]));
+      *reinterpret_cast<uint4*>(g_row + ((chunk ^ (r_in & 7)) << 4)) = val;
+    }
+    ptx::fence_proxy_async();                     // generic-proxy stores -> visible to the tensor core (async proxy)
+    ptx::bar_sync(2 + g, 128);                    // G rows of the warpgroup complete; staging buffer free again
+    // ---- wgmma 2: dA += G . C  (A operand: G, K-major, K = column j; B operand: the contrast tile read MN-major:
+    // N = feature d (4 chunks of 64 at C_KB_BYTES), K = j (16 rows = 2 KB per step)) ----
+    ptx::wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < BNB / 16; ++k) {
+      const uint64_t dg = ptx::make_desc_kmajor_sw128(g_base + k * 32);
+      const uint64_t dc = ptx::make_desc_mnmajor_sw128(c_stage + k * 2048, C_KB_BYTES, 1024);
+      ptx::wgmma_m64n256k16<1>(dacc, dg, dc, 1u);
+    }
+    ptx::wgmma_commit();
+    ptx::wgmma_wait<0>();
+    ptx::fence_operands(dacc);
+    if (lane == 0) ptx::mbar_arrive(&sm.c_empty[stage]);
   }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) ptx::tmem_dealloc<TMEM_COLS>(tmem_base);
+  // ---- dA of the warpgroup's rows -> global partial of this split (fragment layout, 8-byte stores) ----
+  const int fr = 16 * (t >> 5) + ((t & 31) >> 2), fc = 2 * (t & 3);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float* dst = dpartials + ((int64_t)split * a.a_pad + row0 + g * 64 + fr + 8 * h) * DDIM + fc;
+#pragma unroll
+    for (int i = 0; i < 32; ++i)
+      *reinterpret_cast<float2*>(dst + 8 * i) = make_float2(dacc[4 * i + 2 * h], dacc[4 * i + 2 * h + 1]);
+  }
 }
 
 // anchors fp32 -> bf16 rows (optional) and the per-row stabiliser m2 = |bf16(a)| * cbound * log2(e)/T
@@ -1269,7 +1157,7 @@ static int make_tmap(CUtensorMap* m, const void* base, uint64_t rows, uint32_t b
   if (!enc) { pcl::set_error_text("cuTensorMapEncodeTiled entry point not found"); return PCL_ERR_CUDA; }
   // cuTensorMapEncodeTiled is a DRIVER call: it needs a context current on THIS thread.  A thread that has not made a
   // runtime call yet (PyTorch's autograd worker on its first backward) has none -> CUDA_ERROR_INVALID_CONTEXT (201), seen
-  // in tools/dist_bank_check.py (profiles/r2_17_dist_bank_check_before_fix.log).  cudaFree(0) binds the primary context.
+  // in tools/dist_bank_check.py.  cudaFree(0) binds the primary context.
   (void)cudaFree(nullptr);
   cuuint64_t gdim[2] = {(cuuint64_t)tc::DDIM, rows};
   cuuint64_t gstride[1] = {(cuuint64_t)tc::DDIM * 2};
@@ -1304,8 +1192,8 @@ struct TcPlan {
 };
 
 // Tuning knobs for profiling runs (env PCL_TC_VARIANT, bit 0: polynomial exp2 for 1 in 4 logits, bit 1: 2-D grid
-// NEG sweep, bit 3: NEG sweep only).  Default 0 = the shipped configuration (all-MUFU exp2, persistent walk):
-// measured 1310 vs 1196 TFLOP/s with the polynomial share at 65536 x 131072 (profiles/r1_sweep_variants_v4.jsonl).
+// NEG sweep, bit 3: NEG sweep only, bit 4: row-tile POS sweep for small bank-mode anchor sets).  Default 0 = the
+// shipped configuration (all-MUFU exp2, persistent walk).
 static int tc_variant() {
   static int v = -1;
   if (v < 0) { const char* e = getenv("PCL_TC_VARIANT"); v = e ? atoi(e) : 0; }
@@ -1315,11 +1203,11 @@ static int tc_variant() {
 int pcl::num_sms() {
   static int cache[64] = {0};     // per device (a process may drive several GPUs)
   int dev = 0, v = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) { (void)cudaGetLastError(); return 148; }   // sizing on a host without a device
+  if (cudaGetDevice(&dev) != cudaSuccess) { (void)cudaGetLastError(); return 132; }   // sizing on a host without a device
   int& n = cache[dev & 63];
   if (n == 0) {
     if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && v > 0) n = v;
-    else { (void)cudaGetLastError(); return 148; }
+    else { (void)cudaGetLastError(); return 132; }
   }
   return n;
 }
@@ -1368,8 +1256,8 @@ static int make_tc_plan(const pcl_tc_desc* d, TcPlan* p) {
   if (slots_neg > col_tiles) slots_neg = col_tiles;
   if (slots_neg < 1) slots_neg = 1;
   a.slots = (int)(slots_neg > splits ? slots_neg : splits);
-  // backward sweeps 128-column tiles on a 2-D grid
-  const int col_tiles_b = (int)ceil_div64(a.n_cols > 0 ? a.n_cols : 1, 128);
+  // backward sweeps BNB-column tiles on a 2-D grid
+  const int col_tiles_b = (int)ceil_div64(a.n_cols > 0 ? a.n_cols : 1, tc::BNB);
   int sb = sms / p->row_tiles;
   if (sb < 1) sb = 1;
   if (sb > col_tiles_b) sb = col_tiles_b;
@@ -1403,7 +1291,7 @@ extern "C" int pcl_tc_sizes(const pcl_tc_desc* d, pcl_sweep_sizes_t* out) {
 
 extern "C" int pcl_to_bf16(const float* src, void* dst, int64_t n_real, int64_t n_total, void* stream) {
   PCL_REQUIRE(src && dst && n_total >= n_real && n_real >= 0);
-  tc::k_to_bf16<<<148 * 8, 256, 0, (cudaStream_t)stream>>>(src, (__nv_bfloat16*)dst, n_real, n_total);
+  tc::k_to_bf16<<<num_sms() * 8, 256, 0, (cudaStream_t)stream>>>(src, (__nv_bfloat16*)dst, n_real, n_total);
   PCL_LAUNCH_CHECK();
   return PCL_OK;
 }
@@ -1598,7 +1486,7 @@ int pcl::tc_bwd_ex(const pcl_tc_desc* d, const float* row_m2, const float* rowst
   ba.rowstats = rowstats;
   ba.rs_scale = d->temperature / d->base_temperature;
   ba.nan_safe = d->nan_safe;
-  const int splits = p.splits_bwd;       // the backward sweeps 128-column tiles on a 2-D grid
+  const int splits = p.splits_bwd;       // the backward sweeps BNB-column tiles on a 2-D grid
   ba.t.splits = splits;
   p.sw.splits = splits;
   CUtensorMap tmA, tmC;
@@ -1608,15 +1496,11 @@ int pcl::tc_bwd_ex(const pcl_tc_desc* d, const float* row_m2, const float* rowst
   else st = make_tmap(&tmC, d->contrast_bf16, (uint64_t)(d->contrast_rows_alloc > 0 ? d->contrast_rows_alloc : ba.t.n_cols), tc::BNB);
   if (st != PCL_OK) return st;
   const size_t smem = sizeof(tc::SmemBwd) + 1024;
-  PCL_SMEM_OPT_IN((tc::k_tc_bwd<8, false>), smem);
-  PCL_SMEM_OPT_IN((tc::k_tc_bwd<16, false>), smem);
-  PCL_SMEM_OPT_IN((tc::k_tc_bwd<16, true>), smem);
+  PCL_SMEM_OPT_IN((tc::k_tc_bwd<false>), smem);
+  PCL_SMEM_OPT_IN((tc::k_tc_bwd<true>), smem);
   dim3 grid(p.row_tiles, splits);
-  static int epi_w = 0;                        // PCL_TC_BWD_EPI=8|16 (tuning runs); default 16
-  if (epi_w == 0) { const char* e = getenv("PCL_TC_BWD_EPI"); epi_w = (e && atoi(e) == 8) ? 8 : 16; }
-  if (ba.t.tk_sel != nullptr) tc::k_tc_bwd<16, true><<<grid, 64 + 32 * 16, smem, s>>>(tmA, tmC, ba, dpartials);
-  else if (epi_w == 8)        tc::k_tc_bwd<8, false><<<grid, 64 + 32 * 8, smem, s>>>(tmA, tmC, ba, dpartials);
-  else                        tc::k_tc_bwd<16, false><<<grid, 64 + 32 * 16, smem, s>>>(tmA, tmC, ba, dpartials);
+  if (ba.t.tk_sel != nullptr) tc::k_tc_bwd<true><<<grid, tc::NUM_THREADS, smem, s>>>(tmA, tmC, ba, dpartials);
+  else                        tc::k_tc_bwd<false><<<grid, tc::NUM_THREADS, smem, s>>>(tmA, tmC, ba, dpartials);
   PCL_LAUNCH_CHECK();
   if (splits_out) *splits_out = splits;
   if (a_pad_out) *a_pad_out = ba.t.a_pad;

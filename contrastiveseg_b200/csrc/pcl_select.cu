@@ -39,8 +39,7 @@ k_keys(pcl_geom g, int nchunk, float scale_h, float scale_w, const int64_t* __re
     int key = NK;
     // K <= 32 (every configuration of the reference): the class-plane loads do not wait for the label — the label load
     // and the first 16 planes are one DRAM round trip, the remaining planes a second (was: label, then one round trip
-    // per group of 8 planes behind the label test; the scan is a chain of dependent round trips: 10.8 us for ONE image,
-    // profiles/r2_32_timeline_b1.log).  16 at a time: 1024 threads x 32 registers keeps two CTAs per SM.
+    // per group of 8 planes behind the label test; the scan is a chain of dependent round trips).  16 at a time: 1024 threads x 32 registers keeps two CTAs per SM.
     int pred32 = -1;
     if (seg != nullptr && K <= 32) {
       const float* sp = seg + (int64_t)b * K * HW + p;
@@ -106,8 +105,7 @@ k_keys(pcl_geom g, int nchunk, float scale_h, float scale_w, const int64_t* __re
   __syncthreads();
   if (!s_last) { tl_end(dbg, PCL_TL_KEYS); return; }
   // Totals: one warp per (image, key) row, one chunk per lane, FOUR rows per pass so that a warp has four loads in
-  // flight (a row-at-a-time loop cost one L2 round trip per row: 10 rows per warp = 7 of the scan's 21 us at B = 8,
-  // profiles/r2_35_timeline_full.log).  The totals also stay in shared memory for the plan (its loops re-read them).
+  // flight (a row-at-a-time loop costs one L2 round trip per row).  The totals also stay in shared memory for the plan (its loops re-read them).
   __shared__ int s_counts[4096];
   const int rows = g.B * NK;
   const bool in_smem = rows <= 4096;
@@ -532,8 +530,8 @@ k_scatter_reduce(pcl_geom g, const int32_t* __restrict__ plan, const int32_t* __
                  const float* __restrict__ grad_scale, float* __restrict__ grad, unsigned long long* step_counter,
                  unsigned int* dbg, int32_t* __restrict__ prev_rows) {
   // one BLOCK per anchor row, one thread per channel: the sum over the splits (up to 18 for the bank sweeps) is a chain
-  // of dependent adds per element, so the parallelism has to come from the elements (a warp per row left 7 warps per SM
-  // and took 42 us at 18 splits; profiles/r2_19_*)
+  // of dependent adds per element, so the parallelism has to come from the elements (a warp per row leaves few warps
+  // per SM)
   tl_begin(dbg, PCL_TL_SCATTER);
   struct TlEnd { unsigned int* d; __device__ ~TlEnd() { tl_end(d, PCL_TL_SCATTER); } } tl_guard{dbg};
   if (step_counter != nullptr && blockIdx.x == 0 && threadIdx.x == 0) *step_counter += 1ull;
@@ -572,8 +570,7 @@ k_fill_zero(uint4* __restrict__ p, uint64_t n16, unsigned int* dbg) {
 
 // The same fill as a few CTAs that OWN their SM (1024 threads + a dynamic shared-memory request no other kernel of the
 // step fits next to): a CTA of another kernel that shares an SM with fill warps queues its loads, shuffles and shared-
-// memory accesses behind the fill's stores and becomes the straggler of its kernel (12 fill CTAs of 256 threads — 10 % of
-// the HBM write rate — took the 256-CTA scan from 20 to 45 us, profiles/r2_27_fill_throttle.log).
+// memory accesses behind the fill's stores and becomes the straggler of its kernel.
 __global__ void __launch_bounds__(1024, 1)
 k_fill_zero_excl(uint4* __restrict__ p, uint64_t n16, unsigned int* dbg) {
   extern __shared__ uint8_t fill_smem_unused[];
@@ -600,7 +597,7 @@ int pcl::fill_zero(void* ptr, uint64_t bytes, void* stream, unsigned int* dbg, i
   uint64_t blocks = (n16 + 255) / 256;
   // CTAs per SM: the fill is a long-running branch that shares the SMs with the latency-bound kernels of the step; a
   // few resident warps per SM saturate the HBM write path (stores do not wait), more would only crowd the others out
-  // (1, 2, 4 or 8 CTAs per SM: the fill takes 43-47 us either way, profiles/r2_1*_probe.log).
+  // (the fill time does not depend on 1, 2, 4 or 8 CTAs per SM).
   // PCL_FILL_CTAS_PER_SM overrides (tuning runs).
   int per_sm = 1;
   if (const char* e = getenv("PCL_FILL_CTAS_PER_SM")) { int v = atoi(e); if (v >= 1 && v <= 8) per_sm = v; }

@@ -189,9 +189,9 @@ extern "C" int pcl_step_fused_fill(const pcl_step_desc* d, void* stream) {
   const uint64_t bytes = (uint64_t)d->g.B * d->g.D * d->g.h * d->g.w * sizeof(float);
   if ((bytes & 15) != 0 || ((uintptr_t)d->grad_embed & 15) != 0) return PCL_ERR_UNSUPPORTED;
   // The fill forks right before the fused InfoNCE kernel (at most 8 x 4 = 32 CTAs, one per SM).  Its CTAs OWN their SMs
-  // and leave 32 free: the InfoNCE kernel starts at once, next to the fill, instead of waiting ~32 us for fill CTAs to
-  // retire (its 320-thread, 168-register CTAs fit on no SM that holds fill warps) — the step went from 117 to 91 us
-  // (profiles/r2_31_fill_excl_late.log).  PCL_FILL_RESERVE_SMS overrides (tuning runs; 0 = the shared-SM fill).
+  // and leave 32 free: the InfoNCE kernel starts at once, next to the fill, instead of waiting for fill CTAs to retire
+  // (its 384-thread, register-heavy CTAs fit on no SM that holds fill warps).  PCL_FILL_RESERVE_SMS overrides (tuning
+  // runs; 0 = the shared-SM fill).
   int reserve = 32;
   if (const char* e = getenv("PCL_FILL_RESERVE_SMS")) reserve = atoi(e);
   return pcl::fill_zero(d->grad_embed, bytes, stream, d->sync, reserve);

@@ -30,7 +30,7 @@ class ContrastOptions:
     rng: str = "device"                    # "device" (no host sync) | "torch_cpu" (reference RNG stream)
     perm_fn: Optional[Callable[[int], torch.Tensor]] = None   # injected permutations (parity tests)
     seed: int = 304
-    precision: str = "fp32"                # "fp32" exact SIMT sweep | "bf16" tcgen05 sweep (bank / large problems)
+    precision: str = "fp32"                # "fp32" exact SIMT sweep | "bf16" wgmma sweep (bank / large problems)
     contrast_norm_bound: float = 1.0       # bound of the contrast rows' L2 norm (tensor path stabiliser; 1 = normalised)
     topk_negatives: Optional[int] = None   # a10 extension: keep only the k hardest negatives per anchor (None = reference)
 
@@ -94,6 +94,10 @@ class ContrastWorkspace:
             ts = _abi.SweepSizes()
             _abi.check(lib.pcl_tc_sizes(C.byref(td), C.byref(ts)), "pcl_tc_sizes")
             n_partial, n_dpartial = max(n_partial, ts.partial_f32), max(n_dpartial, ts.dpartial_f32)
+            if mode == 0 and ms <= 1024:     # the fused self-contrast kernel: one slot per 256-column tile
+                a_pad = -(-ms // 128) * 128
+                s_max = -(-a_pad // 256)
+                n_partial, n_dpartial = max(n_partial, s_max * a_pad), max(n_dpartial, s_max * a_pad * 256)
         i32 = dict(dtype=torch.int32, device=device)
         f32 = dict(dtype=torch.float32, device=device)
         self.keys = torch.empty(sizes.keys_u16, dtype=torch.int16, device=device)
@@ -253,7 +257,7 @@ def _step_tc_desc(ws, d) -> "_abi.TcDesc":
 
 def _topk_step_forward(lib, ws, d, opts, stream):
     """a10: selection + gather as usual, then the top-k InfoNCE sweep (exact fp32 path, or the tensor path: the radix
-    select then runs in the tcgen05 sweep's epilogue on the fp32-accumulated logits of the bf16 operands)."""
+    select then runs in the wgmma sweep's epilogue on the fp32-accumulated logits of the bf16 operands)."""
     k = int(opts.topk_negatives)
     if k < 1:
         raise _abi.PclError("topk_negatives must be >= 1 (None disables the selection)")
@@ -378,7 +382,7 @@ class _PixelContrastFn(torch.autograd.Function):
         shadow_c = None
         if opts.precision == "bf16":
             if not ws.tc_ok:
-                raise _abi.PclError("precision='bf16' (tcgen05 sweep) needs proj_dim == 256")
+                raise _abi.PclError("precision='bf16' (wgmma sweep) needs proj_dim == 256")
             d.precision = 1
             d.contrast_norm_bound = float(opts.contrast_norm_bound)
             if mode == 1:
@@ -608,7 +612,7 @@ def l2_normalize(x: torch.Tensor) -> torch.Tensor:
 
 
 # ------------------------------------------------------------------------------------------------
-# tensor-core (tcgen05) InfoNCE on explicit operands — D must be 256
+# tensor-core (wgmma) InfoNCE on explicit operands — D must be 256
 # ------------------------------------------------------------------------------------------------
 def to_bf16_rows(x: torch.Tensor, rows_alloc: int) -> torch.Tensor:
     """fp32 (n, 256) -> bf16 (rows_alloc, 256) zero-padded copy on the engine's conversion kernel."""
@@ -659,7 +663,7 @@ def infonce_tc_forward(anchors: torch.Tensor, anchor_cls: torch.Tensor, *, contr
                        diag_col: Optional[torch.Tensor] = None, temperature: float = 0.1, base_temperature: float = 0.07,
                        nan_safe: bool = False, sorted_cols: bool = True, norm_bound: float = 1.0, neg_only: bool = False,
                        topk: Optional[int] = None):
-    """bf16 tcgen05 sweep.  Returns (loss (1,), rowstats (6, A), state).  neg_only=True runs just the similarity +
+    """bf16 wgmma sweep.  Returns (loss (1,), rowstats (6, A), state).  neg_only=True runs just the similarity +
     negative-sum sweep (roofline measurement of the dense contraction).  topk=k: a10, the k hardest negatives per anchor
     (radix select in the sweep's epilogue)."""
     lib = _abi.load()
@@ -691,7 +695,7 @@ def infonce_tc_forward(anchors: torch.Tensor, anchor_cls: torch.Tensor, *, contr
 
 
 def tc_dump_logits(anchors: torch.Tensor, contrast_bf16: Optional[torch.Tensor], n_cols: int) -> torch.Tensor:
-    """Raw S = A.C^T from the TMA/tcgen05 pipeline (self-test of descriptors and barriers)."""
+    """Raw S = A.C^T from the TMA/wgmma pipeline (self-test of descriptors and barriers)."""
     lib = _abi.load()
     dev = anchors.device
     A = anchors.shape[0]
@@ -710,7 +714,7 @@ def tc_dump_logits(anchors: torch.Tensor, contrast_bf16: Optional[torch.Tensor],
 
 
 def infonce_tc_backward(state, rowstats: torch.Tensor, grad_loss: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """dA (A, 256) fp32 from the tcgen05 backward sweep (recompute S, G tile in shared memory, dA += G.C)."""
+    """dA (A, 256) fp32 from the wgmma backward sweep (recompute S, G tile in shared memory, dA += G.C)."""
     lib = _abi.load()
     d, ss, keep, row_m2 = state[:4]
     dev = row_m2.device

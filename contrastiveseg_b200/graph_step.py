@@ -109,7 +109,7 @@ class GraphedContrastStep:
         self.shadow = None
         if opts.precision == "bf16":
             if not self.ws.tc_ok:
-                raise _abi.PclError("precision='bf16' (tcgen05 sweep) needs proj_dim == 256")
+                raise _abi.PclError("precision='bf16' (wgmma sweep) needs proj_dim == 256")
             d.precision = 1
             d.contrast_norm_bound = float(opts.contrast_norm_bound)
             if mode == 1:

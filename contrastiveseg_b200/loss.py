@@ -1,7 +1,7 @@
 """Drop-in loss modules: same class names, constructor ``(configer)``, forward signatures and registry keys
 as the reference (lib/loss/loss_contrast.py, lib/loss/loss_contrast_mem.py, lib/loss/loss_manager.py:36-41).
 
-The contrast term runs on the B200 engine (functional.pixel_contrast_loss); the plain segmentation CE runs on
+The contrast term runs on the H100 engine (functional.pixel_contrast_loss); the plain segmentation CE runs on
 the fused up-sample + CE kernels (``contrast.fused_seg_ce``, default on).  Engine-only knobs are read from
 optional config keys under ``contrast``: ``rng`` ("device" | "torch_cpu"), ``nan_safe``, ``precision``
 ("fp32" | "bf16"), ``skip_warmup_contrast``, ``topk_negatives`` (a10 extension, default off).

@@ -1,5 +1,5 @@
 /*
- * pcl.h — C ABI of the B200 pixel-contrast loss engine (libpcl_b200.so).
+ * pcl.h — C ABI of the H100 pixel-contrast loss engine (libpcl_b200.so).
  *
  * The reference (tfzhou/ContrastiveSeg) has no FFI on this path: it is Python/ATen behind three
  * nn.Module classes and one trainer method (SURVEY.md §8b).  This header is the boundary a
@@ -261,7 +261,7 @@ int pcl_bank_shadow_rebuild(const float* segment_queue, const float* pixel_queue
                             int32_t D, void* shadow_bf16, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
- * a6 on the tensor cores (tcgen05 + TMA, bf16 operands, fp32 accumulate in TMEM), D must be 256.
+ * a6 on the tensor cores (wgmma + TMA, bf16 operands, fp32 accumulate), D must be 256.
  * Same semantics and row-statistic layout as pcl_infonce_fwd; operands are bf16 copies:
  *   anchors_bf16   (a_rows rounded up to 128, 256) bf16 — written here from anchors_f32 when that is non-NULL
  *   contrast_bf16  mode 1: the bank shadow ((K-1)*R rounded up to 256 rows, class-blocked, see pcl_bank_apply);
@@ -333,7 +333,7 @@ typedef struct {
   uint16_t* keys; int32_t* chunk_pref; int32_t* counts; int32_t* plan; int32_t* anchor_meta;
   float* anchors_f32; void* anchors_bf16; float* inv_norm; float* norm_max;
   float* partials; float* rowstats; float* dpartials; float* dA;
-  /* sweep selection: 0 = exact fp32 SIMT sweep (any D % 32 == 0, D <= 256); 1 = bf16 tcgen05 sweep (D == 256).
+  /* sweep selection: 0 = exact fp32 SIMT sweep (any D % 32 == 0, D <= 256); 1 = bf16 wgmma sweep (D == 256).
    * The tensor path reads the bank through its bf16 shadow (pcl_bank_apply / pcl_bank_shadow_rebuild). */
   int32_t precision;
   const void* shadow_bf16; int64_t shadow_rows;
@@ -382,8 +382,8 @@ int pcl_step_forward_ctr(const pcl_step_desc* d, uint64_t* step_counter, void* s
  *                           d->grad_embed; advances *step_counter.
  * The dense gradient d->grad_embed must be zero outside the A sampled columns.  Two ways:
  *   full fill     pcl_step_fused_fill before the scatter, e.g. on a second stream forked AFTER the selection: the 268 MB fill
- *                 saturates HBM and multiplies the latency of every DRAM read issued next to it (scan 22 -> 60 us, selection
- *                 13 -> 54 us, profiles/r2_07_*, r2_08_*), while the L2-resident InfoNCE kernel hides behind it;
+ *                 saturates HBM and multiplies the latency of every DRAM read issued next to it (scan, selection), while
+ *                 the L2-resident InfoNCE kernel hides behind it;
  *   sparse reset  prev_rows != NULL (1 + 2 * max_samples int32, zero before the first call, owned by the step): the buffer
  *                 persists between steps, zero-filled ONCE by the caller; the selection kernel clears exactly the entries
  *                 the previous step scattered and the scatter records its own.  The caller must not write the buffer.

@@ -5,8 +5,8 @@ Source rewriting (text level, the .cu files themselves are untouched):
   kernel<<<grid, block, smem, stream>>>(args)   ->  emu::cfg(grid, block, smem, stream).bind(kernel)(args)
   extern __shared__ [__align__(n)] T name[];     ->  T* name = reinterpret_cast<T*>(emu::dyn_smem());
   asm volatile("bar.sync id, %0;" :: "n"(N) ...) ->  emu::named_barrier(id, N);
-The tensor path (pcl_infonce_tc.cu) compiles against shim/ptx_sm100.cuh, a functional model of the mbarrier / TMA /
-tcgen05 primitives with the product header's names (found first on the include path).
+The tensor path (pcl_infonce_tc.cu, pcl_infonce_fused.cu) compiles against shim/ptx_sm90.cuh, a functional model of the
+mbarrier / TMA / wgmma primitives with the product header's names (found first on the include path).
 """
 from __future__ import annotations
 

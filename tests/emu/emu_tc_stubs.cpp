@@ -1,9 +1,9 @@
 // TEST INFRASTRUCTURE: the marker that keeps the emulation build out of the product, and the host-side model of
-// cuTensorMapEncodeTiled that pairs with the TMA model in shim/ptx_sm100.cuh.
+// cuTensorMapEncodeTiled that pairs with the TMA model in shim/ptx_sm90.cuh.
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <string.h>
-#include "ptx_sm100.cuh"
+#include "ptx_sm90.cuh"
 
 extern "C" int pcl_emulated(void) { return 1; }      // contrastiveseg_b200._abi.load refuses a library that exports this
 

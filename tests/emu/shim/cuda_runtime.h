@@ -3,8 +3,8 @@
 // Host-side execution model for the engine's SIMT kernels, so that CPU-only test runs (-m "not gpu") execute the REAL
 // kernel sources of contrastiveseg_b200/csrc (selection, sampling plan, exact fp32 sweeps, top-k select, bank update,
 // normalise, fused seg-CE, graph rank draw) instead of only their host wiring.  tests/emu/build_emu.py rewrites the
-// launch syntax and compiles those .cu files with g++ against this header; the tcgen05/TMA tensor path is inline PTX
-// and is NOT emulated (its entry points are stubs that return PCL_ERR_UNSUPPORTED).
+// launch syntax and compiles those .cu files with g++ against this header; the wgmma/TMA tensor path compiles against
+// the functional model in shim/ptx_sm90.cuh.
 //
 // Model: one CUDA block = a set of cooperative fibers (ucontext) inside one OS thread; __syncthreads and the warp
 // collectives (__shfl*_sync, __ballot_sync, __all_sync, __syncwarp) are scheduling points with CUDA's semantics for
@@ -28,6 +28,7 @@
 #define __host__
 #define __forceinline__ inline __attribute__((always_inline))
 #define __launch_bounds__(...)
+#define __maxnreg__(...)
 #define __shared__ static
 #define __align__(n) alignas(n)
 #define PCL_EMULATION 1
@@ -88,8 +89,7 @@ struct Block {
   uint3 bid{0, 0, 0}, bdim{1, 1, 1}, gdim{1, 1, 1};
   void* dyn = nullptr;
   size_t dyn_bytes = 0;
-  std::vector<float> tmem;           // tensor memory of the block: 128 lanes x 512 columns (tcgen05 model, ptx_sm100.cuh)
-  struct AsyncOp { int engine; std::function<void()> run; };   // engine 0 = TMA (may complete out of order), 1 = tensor pipe (in order)
+  struct AsyncOp { int engine; std::function<void()> run; };   // engine 0 = TMA (may complete out of order), 1 = in order
   std::deque<AsyncOp> async_q;       // issued-but-not-yet-executed asynchronous operations
   std::function<void()> body;
 };

@@ -283,7 +283,7 @@ def _bf(x):
 
 
 def fuzz_tensor_path(seed: int, n: int):
-    """tcgen05 sweeps (functional model) on explicit operands: self-contrast, explicit contrast set (sorted / unsorted
+    """wgmma sweeps (functional model) on explicit operands: self-contrast, explicit contrast set (sorted / unsorted
     labels), bank through the bf16 shadow; ragged A and N (not multiples of the 128 x 256 tile), few / many classes.
     Loss and positive counts against the float64 closed form on the bf16-rounded operands; gradient within the bf16
     tolerance of the path (max-abs 6e-3 * max|g|, relative Frobenius 5e-3)."""

@@ -1,4 +1,4 @@
-"""Generate golden vectors by running the UNMODIFIED reference (imported from /root/reference).
+"""Generate golden vectors by running the UNMODIFIED reference (located by oracle.ref_loader.reference_root()).
 
 Run in the build container only:  python tests/golden/make_golden.py
 Writes tests/golden/*.npz.  The reference is fp32 PyTorch; every torch.randperm it draws is
@@ -167,8 +167,59 @@ def enqueue_case(name, *, B, D, h, w, K, img_stride, net_stride, M, Fq, steps, s
     print(f"{name}: steps={steps} final seg ptr={sp.tolist()} pix ptr={pp.tolist()}")
 
 
+def random_seed_case(seed, mem):
+    """tests/test_oracle_vs_reference.py: the reference's loss and gradient on make_contrast_batch(seed) (inputs are
+    regenerated by the test), with the randperm draws it made."""
+    ref = load_reference()
+    K, D = 6, 32
+    data = make_contrast_batch(B=3, D=D, h=20, w=24, num_classes=K, img_stride=2, block=6, seed=seed, boost=1.5)
+    predict = data["seg"].argmax(1)
+    cfg = DictConfiger(cfg_dict(0.1, 0.07, 50, 7))
+    rec = PermRecorder(torch.Generator().manual_seed(seed))
+    embed = data["embed"].clone().requires_grad_(True)
+    with patched_randperm(rec):
+        if mem:
+            bank = make_bank(K, 15, D, seed)
+            loss = ref.mem.PixelContrastLoss(cfg)(embed, data["target"], predict,
+                                                  torch.cat((bank["segment_queue"], bank["pixel_queue"]), 1))
+        else:
+            loss = ref.nomem.PixelContrastLoss(cfg)(embed, data["target"], predict)
+    loss.backward()
+    flat, lens = pack_perms(rec.draws)
+    name = f"ref_seed{seed}_{'mem' if mem else 'nomem'}"
+    np.savez_compressed(os.path.join(HERE, name + ".npz"), perm_flat=flat, perm_lens=lens, loss=np.float64(loss.item()),
+                        grad_embed=embed.grad.numpy())
+    print(f"{name}: loss={loss.item():.7f}")
+
+
+def enqueue_random_case():
+    """tests/test_oracle_vs_reference.py::test_enqueue_random: the queues after five reference enqueues."""
+    ref = load_reference()
+    K, D, M, Fq = 5, 16, 6, 4
+    bank = make_bank(K, M, D, 3)
+    a = [bank[k].clone() for k in ("segment_queue", "segment_queue_ptr", "pixel_queue", "pixel_queue_ptr")]
+    me = types.SimpleNamespace(network_stride=2, memory_size=M, pixel_update_freq=Fq)
+    out = {}
+    for s in range(5):
+        data = make_contrast_batch(B=2, D=D, h=12, w=12, num_classes=K, img_stride=2, block=6, seed=50 + s)
+        rec = PermRecorder(torch.Generator().manual_seed(s))
+        with patched_randperm(rec):
+            ref.enqueue(me, data["embed"], data["target"], *a)
+        out[f"perm_flat{s}"], out[f"perm_lens{s}"] = pack_perms(rec.draws)
+        for k, x in zip(("sq", "sp", "pq", "pp"), a):
+            out[f"{k}{s + 1}"] = x.numpy().copy()
+    np.savez_compressed(os.path.join(HERE, "ref_enqueue_random.npz"), **out)
+    print("ref_enqueue_random: steps=5")
+
+
 if __name__ == "__main__":
     only = sys.argv[1:]
+    if only == ["random"]:           # the cases of tests/test_oracle_vs_reference.py
+        for seed in (31, 32, 33):
+            for mem in (False, True):
+                random_seed_case(seed, mem)
+        enqueue_random_case()
+        sys.exit(0)
     if only == ["aux"]:              # add the round-2 cases without touching the committed round-1 files
         torch.manual_seed(0)
         aux_wrapper_case("wrapper_aux_embed", with_embed=True)

@@ -1,5 +1,5 @@
 """CPU execution of the engine's REAL kernel sources (tests/emu: the .cu files compiled for host fibers; the tensor path
-against a functional model of mbarrier / TMA / tcgen05): the GPU tests of test_gpu_parity.py / test_gpu_topk.py /
+against a functional model of mbarrier / TMA / wgmma): the GPU tests of test_gpu_parity.py / test_gpu_topk.py /
 test_gpu_zpending.py are re-run here with DEV = "cpu", through the same Python layer and the same C ABI (all but the
 full-size ones).  This covers the kernel logic (indices,
 barriers, reductions, selection, sampling, bank update, top-k select, graph rank draw) on machines without a GPU; it
@@ -108,10 +108,11 @@ TENSOR = (
 
 @pytest.mark.parametrize("fn,kw", TENSOR)
 def test_tensor_path_on_the_functional_tcgen05_model(emu, fn, kw):
-    """csrc/pcl_infonce_tc.cu (TMA-fed tcgen05 sweeps) compiled against tests/emu/shim/ptx_sm100.cuh, a functional model
-    of mbarrier / TMA (SWIZZLE_128B) / tcgen05.mma (shared-memory descriptors, K- and MN-major) / tensor memory: the
-    warp-specialised pipelines, descriptor arithmetic, class tests and epilogues run on the CPU.  The kernels are the
-    ones verified on the B200, so a pass also confirms that the model reads descriptors the way the hardware does."""
+    """csrc/pcl_infonce_tc.cu (TMA-fed wgmma sweeps) compiled against tests/emu/shim/ptx_sm90.cuh, a functional model
+    of mbarrier / TMA (SWIZZLE_128B) / wgmma (shared-memory descriptors, K- and MN-major, accumulator fragments): the
+    warp-specialised pipelines, descriptor arithmetic, fragment staging, class tests and epilogues run on the CPU.  The
+    same cases pass on the H100 (test_gpu_parity.py), so a pass also confirms that the model reads descriptors and
+    fragments the way the hardware does."""
     fn(**kw)
 
 
@@ -133,7 +134,7 @@ def test_topk_inside_the_captured_step_on_emulation(emu, monkeypatch, precision,
 
 @pytest.mark.parametrize("geom", [dict(B=2, h=32, w=32, K=7, ms=128, mv=8), dict(B=3, h=32, w=48, K=9, ms=700, mv=40)])
 def test_fused_small_anchor_step_on_emulation(emu, monkeypatch, geom):
-    """csrc/pcl_infonce_fused.cu on the functional tcgen05 model (one phase per launch: the emulator runs the blocks of a
+    """csrc/pcl_infonce_fused.cu on the functional wgmma model (one phase per launch: the emulator runs the blocks of a
     grid one after another, so the two inter-CTA barriers become launch boundaries), the scan with the plan folded into
     its last block, the selection with the device-side seed counter and the reducing scatter."""
     from contrastiveseg_b200 import graph_step, _abi
@@ -160,7 +161,7 @@ def test_graphed_bank_step_on_emulation(emu, monkeypatch, precision):
 
 @pytest.mark.parametrize("K,M,A,seed", [(5, 300, 200, 1), (12, 70, 150, 3), (40, 130, 260, 5), (171, 8, 400, 6)])
 def test_tensor_path_bank_positives_by_class_blocks_on_emulation(emu, K, M, A, seed):
-    """k_tc_pos_t on the functional tcgen05 / TMA model: blocks cut into several partial slots, several blocks per class."""
+    """k_tc_pos_t on the functional wgmma / TMA model: blocks cut into several partial slots, several blocks per class."""
     G.test_tensor_path_bank_positives_by_class_blocks(K, M, A, seed)
 
 
@@ -234,7 +235,7 @@ def test_full_size_cityscapes_batch_on_emulation(emu):
 
 def test_results_do_not_depend_on_the_thread_schedule():
     """Between synchronisation points the GPU may run the threads of a block in any order; the emulator's default is
-    ascending.  Re-run a cross-section of the emulated cases (SIMT sweeps, selection, bank, top-k, the tcgen05 pipelines,
+    ascending.  Re-run a cross-section of the emulated cases (SIMT sweeps, selection, bank, top-k, the wgmma pipelines,
     the bit-exact graph/eager comparison) with a randomly permuted order: a failure here means a missing barrier."""
     import os
     import subprocess

@@ -1,4 +1,4 @@
-"""Full-size parity on the hardware (VERDICT r1 #6 / weak #8): the tensor (bf16 tcgen05) and the exact (fp32 SIMT) sweeps
+"""Full-size parity on the hardware (VERDICT r1 #6 / weak #8): the tensor (bf16 wgmma) and the exact (fp32 SIMT) sweeps
 at the contrast-set sizes of BASELINE configs[2] (K=19, M=5000: N = 190 000) and configs[3] (K=171, M=5000: N = 1.71 M,
 1.75 GB bank + 0.88 GB shadow) against a column-chunked float64 closed form (tests/helpers.bank_infonce_chunked, plain
 torch ops; itself pinned to oracle.ref_port.infonce_closed_form in tests/test_host_logic.py).  What changes at these

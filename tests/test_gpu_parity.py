@@ -353,7 +353,7 @@ def test_full_size_cityscapes_batch_properties():
 
 
 # ---------------------------------------------------------------------------------------------------
-# tensor-core (tcgen05) path.  Tolerances: loss <= 2e-5 relative to the float64 oracle on the bf16-ROUNDED
+# tensor-core (wgmma) path.  Tolerances: loss <= 2e-5 relative to the float64 oracle on the bf16-ROUNDED
 # operands (fp32 accumulate + ex2/lg2.approx), <= 1e-4 relative to the fp32-operand oracle (north_star bar).
 # ---------------------------------------------------------------------------------------------------
 def _bf(x):
@@ -589,7 +589,7 @@ def test_coco_stuff_shape_171_classes_with_bank(precision):
 
 def test_bank_tensor_path_workspace_sizes_cover_runtime_slots():
     """Regression: the step's partial buffers must be sized for the persistent sweep's slot count with a device-side
-    plan (148 slots), not the host-known case (a buffer overrun here corrupted neighbouring allocations)."""
+    plan (one slot per SM), not the host-known case (a buffer overrun here corrupted neighbouring allocations)."""
     from contrastiveseg_b200.synth import make_bank, make_contrast_batch
     K, D, M = 19, 256, 2000
     data = make_contrast_batch(B=1, D=D, h=64, w=64, num_classes=K, img_stride=4, block=16, seed=3)

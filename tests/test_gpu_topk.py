@@ -2,7 +2,7 @@
 sort-based definition.  a10 is not in the reference code, default off and excluded from the reference parity bar
 (SURVEY §8 a10); these tests pin the kernels to the oracle semantics.
 
-STATUS: strict since round 2 (all cases pass on the B200, profiles/r2_02_pytest_full.log); the same cases also run on
+STATUS: strict (all cases pass on the GPU); the same cases also run on
 the CPU emulator (tests/test_emu_kernels.py)."""
 import os
 
@@ -15,7 +15,7 @@ from contrastiveseg_b200 import functional as Fn
 from oracle import ref_port as P
 from helpers import load_golden, unpack_perms, rel_err
 
-pytestmark = [pytest.mark.gpu, pytest.mark.timeout(300)]      # strict: verified on the B200 (profiles/r2_01_*)
+pytestmark = [pytest.mark.gpu, pytest.mark.timeout(300)]
 DEV = "cuda:0"
 
 
@@ -178,7 +178,7 @@ def test_topk_inside_the_captured_step_equals_the_eager_step(precision, D):
 
 
 # ---------------------------------------------------------------------------------------------------
-# a10 on the tensor path: the radix select runs in the tcgen05 sweep's epilogue (csrc/pcl_infonce_tc.cu TC_H1..H3, TC_NEGW)
+# a10 on the tensor path: the radix select runs in the wgmma sweep's epilogue (csrc/pcl_infonce_tc.cu TC_H1..H3, TC_NEGW)
 # on the fp32-accumulated logits of the bf16 operands.  Dyadic operands (multiples of 1/4, |x| <= 3/4) are exact in bf16 and
 # their 256-term dot products exact in fp32, so selection state, loss and gradient must equal the oracle's like on the
 # exact path; the key is in log2 units (x = s * log2(e) / T), so tau is compared through the ordering, not bitwise.

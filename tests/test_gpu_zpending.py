@@ -1,7 +1,7 @@
 """GPU tests of the deferred bank write and the CUDA-graph step (the file sorts last among the GPU tests on purpose: it
-contains the CUDA-graph capture).  Strict since round 2.  The three fp32 cases failed in the round-1 driver run ONLY when
-they ran after tests/test_gpu_topk.py: a D=64 top-k call lowered the dynamic-shared-memory opt-in of k_sweep<POS> below
-the D=256 size (cudaErrorInvalidValue at the next D=256 launch; log: profiles/r2_02_pytest_full_before_fix.log) — fixed
+contains the CUDA-graph capture).  The three fp32 cases once failed ONLY when they ran after tests/test_gpu_topk.py: a
+D=64 top-k call lowered the dynamic-shared-memory opt-in of k_sweep<POS> below the D=256 size (cudaErrorInvalidValue at
+the next D=256 launch) — fixed
 by the per-device one-time opt-in to the kernel's maximum (PCL_SMEM_OPT_IN, csrc/pcl_common.cuh);
 `test_smem_opt_in_survives_a_smaller_launch` below pins it."""
 import os
@@ -13,7 +13,7 @@ import contrastiveseg_b200 as cs
 from contrastiveseg_b200 import functional as Fn
 from contrastiveseg_b200.synth import make_bank, make_contrast_batch
 
-pytestmark = [pytest.mark.gpu, pytest.mark.timeout(300)]      # strict: verified on the B200 (profiles/r2_01_*)
+pytestmark = [pytest.mark.gpu, pytest.mark.timeout(300)]
 DEV = "cuda:0"
 
 

@@ -175,7 +175,7 @@ def test_topk_step_call_sequence(rec):
 
 
 def test_topk_on_the_tensor_path_call_sequence_and_bad_k(rec):
-    """precision='bf16' + topk_negatives: selection, then the tensor-path top-k forward (radix select in the tcgen05 sweep's
+    """precision='bf16' + topk_negatives: selection, then the tensor-path top-k forward (radix select in the wgmma sweep's
     epilogue) and its backward with the SAME scratch (selection state)."""
     embed, labels, seg = _inputs(D=256)
     loss = cs.pixel_contrast_loss(embed, labels, seg=seg,
