@@ -376,7 +376,7 @@ int pcl_step_forward_ctr(const pcl_step_desc* d, uint64_t* step_counter, void* s
  *   pcl_step_stats          label/argmax scan + totals + plan in one launch (d->sync != NULL)
  *   pcl_step_fused_select   selection + gather; anchor ranks drawn from *step_counter (captured sequences), or from
  *                           d->seed / d->ranks when step_counter is NULL
- *   pcl_step_fused_loss     ONE kernel for the InfoNCE forward and backward (logits stay in tensor memory;
+ *   pcl_step_fused_loss     ONE kernel for the InfoNCE forward and backward (logits stay in registers;
  *                           csrc/pcl_infonce_fused.cu)
  *   pcl_step_fused_scatter  sum of the per-column-tile gradient partials + scatter of the A sampled rows into
  *                           d->grad_embed; advances *step_counter.
