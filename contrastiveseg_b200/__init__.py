@@ -6,7 +6,7 @@ Public surface mirrors the reference (SURVEY §8b): ``PixelContrastLoss``, ``Con
 hand-written sm_90a kernels (csrc/) behind the C ABI of include/pcl.h; there is no CPU or PyTorch fallback.
 """
 from .configer import Configer, cityscapes_contrast_config            # noqa: F401
-from .functional import ContrastOptions, l2_normalize, pixel_contrast_loss, upsample_cross_entropy   # noqa: F401
+from .functional import ContrastOptions, l2_normalize, pixel_contrast_loss, project_normalize, upsample_cross_entropy  # noqa: F401,E501
 from .loss import (ContrastAuxCELoss, ContrastCELoss, MemContrastCELoss, PixelContrastLoss, SEG_LOSS_DICT,  # noqa: F401
                    get_seg_loss)
 from .bank import MemoryBank, dequeue_and_enqueue, gather_packets      # noqa: F401

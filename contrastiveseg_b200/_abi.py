@@ -99,6 +99,10 @@ SIGNATURES = {
     "pcl_scatter_grad": (c_i32, [C.POINTER(Geom), c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_vp, c_vp]),
     "pcl_l2norm_fwd": (c_i32, [c_vp, c_vp, c_i32, c_i32, c_i64, c_vp]),
     "pcl_l2norm_bwd": (c_i32, [c_vp, c_vp, c_vp, c_i32, c_i32, c_i64, c_vp]),
+    "pcl_proj_workspace_bytes": (c_i64, [c_i32, c_i32, c_i64, c_i32]),
+    "pcl_proj_pack": (c_i32, [c_vp, c_i32, c_vp, c_vp]),
+    "pcl_proj_fwd": (c_i32, [c_vp, c_vp, c_vp, c_i32, c_i32, c_i64, c_vp, c_vp, c_vp]),
+    "pcl_proj_bwd": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "pcl_seg_ce_scratch_floats": (c_i64, [c_i32, c_i32, c_i32]),
     "pcl_seg_ce_fwd": (c_i32, [c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_vp, c_vp, c_vp]),
     "pcl_seg_ce_bwd": (c_i32, [c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_vp, c_vp, c_vp,

@@ -21,6 +21,7 @@
 
 namespace pcl {
 int tc_make_tmap(CUtensorMap* m, const void* base, uint64_t rows, uint32_t box_rows);
+int tc_make_tmap_cols(CUtensorMap* m, const void* base, uint64_t cols, uint64_t rows, uint32_t box_rows);
 namespace tc {
 
 // Forward tile = 128 rows x 256 columns: each consumer warpgroup runs M64 x N256 x K16 wgmmas on its 64 rows, so both
@@ -1138,29 +1139,47 @@ static PFN_tmapEncodeTiled get_encode() {
   return fn;
 }
 
-// bf16 row-major (rows, 256) matrix, box = 64 columns (128 B) x box_rows, 128-byte swizzle, OOB rows read as zero.
-// Encoding costs ~2 us of host time and the step re-uses the same few (pointer, rows, box) triples every call, so a
-// small read-mostly cache keeps them (a tensor map only describes addresses/shapes: no lifetime coupling).
-struct TmapKey { const void* base; uint64_t rows; uint32_t box_rows; };
+// Whether the calling thread has a current driver context (cuCtxGetCurrent; unknown -> false).
+typedef CUresult (*PFN_ctxGetCurrent)(void**);
+static bool has_current_context() {
+  static PFN_ctxGetCurrent fn = [] {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    const bool ok = cudaGetDriverEntryPoint("cuCtxGetCurrent", &p, cudaEnableDefault, &q) == cudaSuccess &&
+                    q == cudaDriverEntryPointSuccess;
+    return ok ? (PFN_ctxGetCurrent)p : (PFN_ctxGetCurrent) nullptr;
+  }();
+  void* ctx = nullptr;
+  return fn != nullptr && fn(&ctx) == CUDA_SUCCESS && ctx != nullptr;
+}
+
+// bf16 row-major (rows, cols) matrix (cols a multiple of 8), box = 64 columns (128 B) x box_rows, 128-byte swizzle, OOB
+// rows read as zero.  Encoding costs ~2 us of host time and the step re-uses the same few (pointer, shape, box) keys
+// every call, so a small read-mostly cache keeps them (a tensor map only describes addresses/shapes: no lifetime coupling).
+struct TmapKey { const void* base; uint64_t cols; uint64_t rows; uint32_t box_rows; };
 struct TmapEntry { TmapKey k; CUtensorMap m; bool used; };
 static TmapEntry g_tmaps[16];
 static unsigned g_tmap_next = 0;
 static std::mutex g_tmap_mu;
 
-static int make_tmap(CUtensorMap* m, const void* base, uint64_t rows, uint32_t box_rows) {
+static int make_tmap_cols(CUtensorMap* m, const void* base, uint64_t cols, uint64_t rows, uint32_t box_rows) {
   {
     std::lock_guard<std::mutex> lk(g_tmap_mu);
     for (auto& e : g_tmaps)
-      if (e.used && e.k.base == base && e.k.rows == rows && e.k.box_rows == box_rows) { *m = e.m; return PCL_OK; }
+      if (e.used && e.k.base == base && e.k.cols == cols && e.k.rows == rows && e.k.box_rows == box_rows) {
+        *m = e.m;
+        return PCL_OK;
+      }
   }
   PFN_tmapEncodeTiled enc = get_encode();
   if (!enc) { pcl::set_error_text("cuTensorMapEncodeTiled entry point not found"); return PCL_ERR_CUDA; }
   // cuTensorMapEncodeTiled is a DRIVER call: it needs a context current on THIS thread.  A thread that has not made a
   // runtime call yet (PyTorch's autograd worker on its first backward) has none -> CUDA_ERROR_INVALID_CONTEXT (201), seen
-  // in tools/dist_bank_check.py.  cudaFree(0) binds the primary context.
-  (void)cudaFree(nullptr);
-  cuuint64_t gdim[2] = {(cuuint64_t)tc::DDIM, rows};
-  cuuint64_t gstride[1] = {(cuuint64_t)tc::DDIM * 2};
+  // in tools/dist_bank_check.py.  cudaFree(0) binds the primary context.  Only then: during a stream capture (a thread
+  // that is capturing has a context) cudaFree is a prohibited call and would invalidate the capture.
+  if (!has_current_context()) (void)cudaFree(nullptr);
+  cuuint64_t gdim[2] = {(cuuint64_t)cols, rows};
+  cuuint64_t gstride[1] = {(cuuint64_t)cols * 2};
   cuuint32_t box[2] = {(cuuint32_t)tc::BK, box_rows};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), gdim, gstride, box, estr,
@@ -1175,14 +1194,21 @@ static int make_tmap(CUtensorMap* m, const void* base, uint64_t rows, uint32_t b
   }
   std::lock_guard<std::mutex> lk(g_tmap_mu);
   TmapEntry& e = g_tmaps[g_tmap_next++ % 16];
-  e.k = TmapKey{base, rows, box_rows};
+  e.k = TmapKey{base, cols, rows, box_rows};
   e.m = *m;
   e.used = true;
   return PCL_OK;
 }
 
+static int make_tmap(CUtensorMap* m, const void* base, uint64_t rows, uint32_t box_rows) {
+  return make_tmap_cols(m, base, tc::DDIM, rows, box_rows);
+}
+
 int pcl::tc_make_tmap(CUtensorMap* m, const void* base, uint64_t rows, uint32_t box_rows) {
   return make_tmap(m, base, rows, box_rows);
+}
+int pcl::tc_make_tmap_cols(CUtensorMap* m, const void* base, uint64_t cols, uint64_t rows, uint32_t box_rows) {
+  return make_tmap_cols(m, base, cols, rows, box_rows);
 }
 
 struct TcPlan {

@@ -612,6 +612,71 @@ def l2_normalize(x: torch.Tensor) -> torch.Tensor:
 
 
 # ------------------------------------------------------------------------------------------------
+# §8f row 2: projection head's last 1x1 conv + L2 normalise as one wgmma GEMM (lib/models/modules/projection.py:17-24)
+# ------------------------------------------------------------------------------------------------
+PROJ_DIM = 256
+
+
+def _proj_dims(x: torch.Tensor, weight: torch.Tensor):
+    if x.dim() != 4:
+        raise _abi.PclError(f"project_normalize: x must be (B, Cin, H, W), got {tuple(x.shape)}")
+    B, Cin, H, W = x.shape
+    if weight.shape[0] != PROJ_DIM or weight.numel() != PROJ_DIM * Cin:
+        raise _abi.PclError(f"project_normalize: weight must be ({PROJ_DIM}, {Cin}, 1, 1), got {tuple(weight.shape)}")
+    return B, Cin, H * W
+
+
+class _ProjNormFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, weight, bias):
+        lib = _abi.load()
+        _require_cuda(x, "x")
+        if x.dtype != torch.float32:
+            raise _abi.PclError(f"project_normalize: x must be float32, got {x.dtype}")
+        B, Cin, HW = _proj_dims(x, weight)
+        dev = x.device
+        xc = x.contiguous()
+        w = weight.detach().to(device=dev, dtype=torch.float32).reshape(PROJ_DIM, Cin).contiguous()
+        bc = None if bias is None else bias.detach().to(device=dev, dtype=torch.float32).contiguous()
+        wpack = torch.empty(lib.pcl_proj_workspace_bytes(B, Cin, HW, 0), dtype=torch.uint8, device=dev)
+        zn = torch.empty((B, PROJ_DIM) + tuple(x.shape[2:]), dtype=torch.float32, device=dev)
+        inv = torch.empty(B * HW, dtype=torch.float32, device=dev)
+        with _on_device(dev):
+            s = _stream_ptr(dev)
+            _abi.check(lib.pcl_proj_pack(w.data_ptr(), Cin, wpack.data_ptr(), s), "pcl_proj_pack")
+            _abi.check(lib.pcl_proj_fwd(xc.data_ptr(), wpack.data_ptr(), _abi.ptr(bc), B, Cin, HW, zn.data_ptr(),
+                                        inv.data_ptr(), s), "pcl_proj_fwd")
+        ctx.save_for_backward(xc, zn, inv, wpack)
+        ctx.dims = (B, Cin, HW, tuple(weight.shape), bias is not None)
+        return zn
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, gzn):
+        lib = _abi.load()
+        xc, zn, inv, wpack = ctx.saved_tensors
+        B, Cin, HW, wshape, has_bias = ctx.dims
+        dev = xc.device
+        g = gzn.to(device=dev, dtype=torch.float32).contiguous()
+        scratch = torch.empty(lib.pcl_proj_workspace_bytes(B, Cin, HW, 1), dtype=torch.uint8, device=dev)
+        gx = torch.empty_like(xc)
+        gw = torch.empty((PROJ_DIM, Cin), dtype=torch.float32, device=dev)
+        gb = torch.empty(PROJ_DIM, dtype=torch.float32, device=dev) if has_bias else None
+        with _on_device(dev):
+            _abi.check(lib.pcl_proj_bwd(xc.data_ptr(), zn.data_ptr(), inv.data_ptr(), g.data_ptr(), wpack.data_ptr(), B,
+                                        Cin, HW, scratch.data_ptr(), gx.data_ptr(), gw.data_ptr(), _abi.ptr(gb),
+                                        _stream_ptr(dev)), "pcl_proj_bwd")
+        return gx, gw.view(wshape), gb
+
+
+def project_normalize(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """F.normalize(F.conv2d(x, weight, bias), p=2, dim=1) for a 1x1 convolution to 256 channels, as one bf16 wgmma GEMM
+    with the normalise in its epilogue (fp32 accumulate; backward: gz in bf16, split-K weight gradient reduced in a
+    fixed order).  x (B, Cin, H, W) fp32 CUDA, weight (256, Cin, 1, 1), bias (256) or None."""
+    return _ProjNormFn.apply(x, weight, bias)
+
+
+# ------------------------------------------------------------------------------------------------
 # tensor-core (wgmma) InfoNCE on explicit operands — D must be 256
 # ------------------------------------------------------------------------------------------------
 def to_bf16_rows(x: torch.Tensor, rows_alloc: int) -> torch.Tensor:

@@ -198,6 +198,25 @@ int pcl_l2norm_fwd(const float* x, float* y, int32_t B, int32_t D, int64_t HW, v
 int pcl_l2norm_bwd(const float* x, const float* gy, float* gx, int32_t B, int32_t D, int64_t HW, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * §8f row 2: the projection head's last 1x1 convolution and its L2 normalise as one bf16 wgmma GEMM (fp32 accumulate),
+ * forward and backward.  Replaces lib/models/modules/projection.py:17-24 (the final nn.Conv2d(Cin, 256, 1) of the
+ * head, then F.normalize(p=2, dim=1)) and their autograd backward.  Output channels are fixed at 256.
+ *   x (B,Cin,HW) fp32 NCHW, weight (256,Cin) fp32, bias (256) fp32 or NULL, zn (B,256,HW) fp32, inv_norm (B*HW) fp32
+ *   (1 / max(|z|, 1e-12) per pixel; kept for the backward).
+ *   wpack    pcl_proj_workspace_bytes(B, Cin, HW, 0) bytes: bf16 copies of the weight written by pcl_proj_pack; pack
+ *            again whenever the weight changes.  Used by the forward and the backward.
+ *   scratch  pcl_proj_workspace_bytes(B, Cin, HW, 1) bytes: backward-only (bf16 gz, split-K weight-gradient partials).
+ *   pcl_proj_bwd writes gx (B,Cin,HW), gw (256,Cin) and gb (256, may be NULL); gw and gb are reduced in a fixed order
+ *   (bit-reproducible).  The size query returns a negative pcl_status for an unsupported shape.
+ * ----------------------------------------------------------------------------------------------*/
+int64_t pcl_proj_workspace_bytes(int32_t B, int32_t Cin, int64_t HW, int32_t which);
+int pcl_proj_pack(const float* weight, int32_t Cin, void* wpack, void* stream);
+int pcl_proj_fwd(const float* x, const void* wpack, const float* bias, int32_t B, int32_t Cin, int64_t HW, float* zn,
+                 float* inv_norm, void* stream);
+int pcl_proj_bwd(const float* x, const float* zn, const float* inv_norm, const float* gzn, const void* wpack, int32_t B,
+                 int32_t Cin, int64_t HW, void* scratch, float* gx, float* gw, float* gb, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * §8f row 1 (next row): the segmentation CE of ContrastCELoss.forward, fused.  Replaces
  * lib/loss/loss_contrast.py:180-181 (F.interpolate(seg, (Himg,Wimg), bilinear, align_corners=True)) +
  * lib/loss/loss_helper.py:169-212 (nn.CrossEntropyLoss(weight, ignore_index, reduction mean)) and their autograd
