@@ -17,6 +17,7 @@ PLAN_TC, PLAN_V, PLAN_A, PLAN_FLAGS = 0, 1, 2, 3
 FLAG_NO_CLASS, FLAG_ZERO_VIEWS, FLAG_SPLIT_ERROR = 1, 2, 4
 CHUNK = 1024
 MAX_CLASSES = 256
+DT_F32, DT_BF16, DT_F16 = 0, 1, 2          # element types of embed / seg / bank keys (pcl_step_desc.embed_dtype, ...)
 
 
 class PclError(RuntimeError):
@@ -72,7 +73,8 @@ class StepDesc(C.Structure):
                 ("partials", c_vp), ("rowstats", c_vp), ("dpartials", c_vp), ("dA", c_vp),
                 ("precision", c_i32), ("shadow_bf16", c_vp), ("shadow_rows", c_i64), ("contrast_norm_bound", c_f32),
                 ("row_m2", c_vp),
-                ("loss", c_vp), ("grad_embed", c_vp), ("sync", c_vp)]
+                ("loss", c_vp), ("grad_embed", c_vp), ("sync", c_vp),
+                ("embed_dtype", c_i32), ("seg_dtype", c_i32)]
 
 
 ABI_STRUCTS = (Geom, SelectSizes, SweepDesc, SweepSizes, BankGeom, TcDesc, StepDesc)   # pcl_abi_sizeof ids 0..6
@@ -111,6 +113,8 @@ SIGNATURES = {
     "pcl_bank_scratch_floats": (c_i64, [C.POINTER(BankGeom)]),
     "pcl_bank_packet": (c_i32, [C.POINTER(BankGeom), c_vp, c_vp, c_vp, c_u64, c_vp, c_vp, c_vp]),
     "pcl_bank_packet_dev": (c_i32, [C.POINTER(BankGeom), c_vp, c_vp, c_u64, c_vp, c_vp, c_vp, c_vp]),
+    "pcl_bank_packet_dt": (c_i32, [C.POINTER(BankGeom), c_vp, c_i32, c_vp, c_vp, c_u64, c_vp, c_vp, c_vp]),
+    "pcl_bank_packet_dev_dt": (c_i32, [C.POINTER(BankGeom), c_vp, c_i32, c_vp, c_u64, c_vp, c_vp, c_vp, c_vp]),
     "pcl_bank_apply": (c_i32, [C.POINTER(BankGeom), c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "pcl_bank_apply_ctr": (c_i32, [C.POINTER(BankGeom), c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "pcl_bank_shadow_rebuild": (c_i32, [c_vp, c_vp, c_i32, c_i32, c_i32, c_vp, c_vp]),

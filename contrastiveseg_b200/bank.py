@@ -156,7 +156,10 @@ def dequeue_and_enqueue(keys: torch.Tensor, labels: torch.Tensor, segment_queue:
     if not _is_cuda(keys):
         raise _abi.PclError("keys must be a CUDA tensor: the engine has no CPU path")
     dev = keys.device
-    keys_c = keys.detach().to(torch.float32).contiguous()
+    keys_c = keys.detach()
+    if keys_c.dtype not in _fn.DTYPE_CODES:              # bf16 / fp16 keys are read as they are (converted on load)
+        keys_c = keys_c.to(torch.float32)
+    keys_c = keys_c.contiguous()
     labels_c = labels.to(device=dev, dtype=torch.int64).contiguous()
     B, D, h, w = keys_c.shape
     K, M = segment_queue.shape[0], segment_queue.shape[1]
@@ -190,8 +193,13 @@ def dequeue_and_enqueue(keys: torch.Tensor, labels: torch.Tensor, segment_queue:
     _enqueue_counter[0] += 1
     s = (enqueue_seed(seed) + _enqueue_counter[0]) & 0xFFFFFFFFFFFFFFFF
     with _fn._on_device(dev):
-        _abi.check(lib.pcl_bank_packet(C.byref(g), keys_c.data_ptr(), labels_c.data_ptr(), _abi.ptr(ranks), s,
-                                       scratch.data_ptr(), packet.data_ptr(), _fn._stream_ptr(dev)), "pcl_bank_packet")
+        if keys_c.dtype == torch.float32:
+            _abi.check(lib.pcl_bank_packet(C.byref(g), keys_c.data_ptr(), labels_c.data_ptr(), _abi.ptr(ranks), s,
+                                           scratch.data_ptr(), packet.data_ptr(), _fn._stream_ptr(dev)), "pcl_bank_packet")
+        else:
+            _abi.check(lib.pcl_bank_packet_dt(C.byref(g), keys_c.data_ptr(), _fn.DTYPE_CODES[keys_c.dtype],
+                                              labels_c.data_ptr(), _abi.ptr(ranks), s, scratch.data_ptr(), packet.data_ptr(),
+                                              _fn._stream_ptr(dev)), "pcl_bank_packet_dt")
         packets = gather_packets(packet, group, out=recv) if distributed else packet.view(1, -1)
 
     def apply_packets():           # the in-place write (rows, pointers, bf16 shadow): ordered, rank-major

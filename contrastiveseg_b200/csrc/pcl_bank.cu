@@ -48,8 +48,9 @@ k_bank_counts(BankDims d, const int64_t* __restrict__ labels, int32_t* __restric
     if (s_cnt[i]) atomicAdd(&counts[b * d.g.K + i], s_cnt[i]);
 }
 
+template <typename T>       // element type of keys (converted on load: the sums equal those of the fp32 copy)
 __global__ void __launch_bounds__(256)
-k_bank_segsum(BankDims d, const float* __restrict__ keys, const int64_t* __restrict__ labels,
+k_bank_segsum(BankDims d, const T* __restrict__ keys, const int64_t* __restrict__ labels,
               unsigned long long* __restrict__ sums) {
   extern __shared__ unsigned long long s_bins[];      // [K][SEG_DG]
   const int b = blockIdx.z, d0 = blockIdx.y * SEG_DG, t0 = blockIdx.x * SEG_PX;
@@ -64,7 +65,7 @@ k_bank_segsum(BankDims d, const float* __restrict__ keys, const int64_t* __restr
     int t = t0 + u * 256 + threadIdx.x;
     cls[u] = t < d.T ? grid_label(d, lab_b, t) : -1;
   }
-  const float* kb = keys + (int64_t)b * D * d.HW;
+  const T* kb = keys + (int64_t)b * D * d.HW;
   // Label maps are blocky: most warps see a single class.  Accumulate the thread's own pixels in a register while
   // the class does not change, then reduce class-uniform warps with shuffles -> one shared-memory atomic per warp
   // instead of one per pixel (the per-pixel version serialised on a handful of hot bins: 145 us for one image).
@@ -72,13 +73,13 @@ k_bank_segsum(BankDims d, const float* __restrict__ keys, const int64_t* __restr
 #pragma unroll
   for (int dl = 0; dl < SEG_DG; ++dl) {
     if (d0 + dl >= D) break;
-    const float* row = kb + (int64_t)(d0 + dl) * d.HW;
+    const T* row = kb + (int64_t)(d0 + dl) * d.HW;
     long long acc = 0;
     int acc_cls = -1;
 #pragma unroll
     for (int u = 0; u < PER; ++u) {
       if (cls[u] > 0) {
-        const long long q = __float2ll_rn(row[t0 + u * 256 + threadIdx.x] * FIX_SCALE);
+        const long long q = __float2ll_rn(to_f32(row[t0 + u * 256 + threadIdx.x]) * FIX_SCALE);
         if (cls[u] != acc_cls) {
           if (acc_cls > 0) atomicAdd(&s_bins[acc_cls * SEG_DG + dl], (unsigned long long)acc);
           acc = 0;
@@ -106,8 +107,9 @@ k_bank_segsum(BankDims d, const float* __restrict__ keys, const int64_t* __restr
 }
 
 // one CTA per (image, class) slot
+template <typename T>
 __global__ void __launch_bounds__(256)
-k_bank_rows(BankDims d, const float* __restrict__ keys, const int32_t* __restrict__ counts,
+k_bank_rows(BankDims d, const T* __restrict__ keys, const int32_t* __restrict__ counts,
             const unsigned long long* __restrict__ sums, const int32_t* __restrict__ ranks, uint64_t seed,
             const unsigned long long* __restrict__ seed_offset, float* __restrict__ packet) {
   if (seed_offset != nullptr) seed += *seed_offset;          // captured sequence: per-replay part lives on the device
@@ -120,7 +122,7 @@ k_bank_rows(BankDims d, const float* __restrict__ keys, const int32_t* __restric
   if (threadIdx.x == 0) { out[0] = (float)n; out[1] = (float)kp; }
   if (n == 0) return;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarp = blockDim.x >> 5;
-  const float* kb = keys + (int64_t)b * D * d.HW;
+  const T* kb = keys + (int64_t)b * D * d.HW;
   for (int row = warp - 1 + 0; row < kp; row += nwarp) {
     // row == -1: segment mean; row >= 0: pixel row
     if (row < 0) {
@@ -143,13 +145,13 @@ k_bank_rows(BankDims d, const float* __restrict__ keys, const int32_t* __restric
       col = col < 0 ? 0 : (col >= n ? n - 1 : col);           // perm value used directly as the column (Q5)
       float ss = 0.f;
       for (int dd = lane; dd < D; dd += 32) {
-        float v = kb[(int64_t)dd * d.HW + col];
+        float v = to_f32(kb[(int64_t)dd * d.HW + col]);
         ss += v * v;
       }
       ss = warp_sum(ss);
       const float den = fmaxf(sqrtf(ss), 1e-12f);
       float* o = out + 2 + D + (int64_t)row * D;
-      for (int dd = lane; dd < D; dd += 32) o[dd] = kb[(int64_t)dd * d.HW + col] / den;
+      for (int dd = lane; dd < D; dd += 32) o[dd] = to_f32(kb[(int64_t)dd * d.HW + col]) / den;
     }
   }
 }
@@ -297,12 +299,13 @@ extern "C" int64_t pcl_bank_scratch_floats(const pcl_bank_geom* g) {
   return (int64_t)g->B * g->K + 2 * (int64_t)g->B * g->K * g->D + 2;
 }
 
-static int bank_packet_impl(const pcl_bank_geom* g, const float* keys, const int64_t* labels, const int32_t* ranks,
-                            uint64_t seed, const uint64_t* seed_offset, float* scratch, float* packet, void* stream) {
+static int bank_packet_impl(const pcl_bank_geom* g, const void* keys, int keys_dtype, const int64_t* labels,
+                            const int32_t* ranks, uint64_t seed, const uint64_t* seed_offset, float* scratch, float* packet,
+                            void* stream) {
   BankDims d;
   int st = make_dims(g, &d);
   if (st != PCL_OK) return st;
-  PCL_REQUIRE(keys && labels && scratch && packet);
+  PCL_REQUIRE(keys && labels && scratch && packet && dtype_ok(keys_dtype));
   cudaStream_t s = (cudaStream_t)stream;
   const int64_t slots = (int64_t)g->B * g->K;
   int32_t* counts = reinterpret_cast<int32_t*>(scratch);
@@ -312,23 +315,36 @@ static int bank_packet_impl(const pcl_bank_geom* g, const float* keys, const int
   const int chunks = ceil_div(d.T, SEG_PX);
   k_bank_counts<<<dim3(chunks, g->B), 256, g->K * sizeof(int), s>>>(d, labels, counts);
   PCL_LAUNCH_CHECK();
-  k_bank_segsum<<<dim3(chunks, ceil_div(g->D, SEG_DG), g->B), 256, (size_t)g->K * SEG_DG * sizeof(unsigned long long), s>>>(
-      d, keys, labels, sums);
+  PCL_DT_SWITCH(keys_dtype, T,
+    k_bank_segsum<T><<<dim3(chunks, ceil_div(g->D, SEG_DG), g->B), 256, (size_t)g->K * SEG_DG * sizeof(unsigned long long),
+                       s>>>(d, (const T*)keys, labels, sums);)
   PCL_LAUNCH_CHECK();
-  k_bank_rows<<<(unsigned)slots, 256, 0, s>>>(d, keys, counts, sums, ranks, seed,
-                                              reinterpret_cast<const unsigned long long*>(seed_offset), packet);
+  PCL_DT_SWITCH(keys_dtype, T,
+    k_bank_rows<T><<<(unsigned)slots, 256, 0, s>>>(d, (const T*)keys, counts, sums, ranks, seed,
+                                                   reinterpret_cast<const unsigned long long*>(seed_offset), packet);)
   PCL_LAUNCH_CHECK();
   return PCL_OK;
 }
 
 extern "C" int pcl_bank_packet(const pcl_bank_geom* g, const float* keys, const int64_t* labels, const int32_t* ranks,
                                uint64_t seed, float* scratch, float* packet, void* stream) {
-  return bank_packet_impl(g, keys, labels, ranks, seed, nullptr, scratch, packet, stream);
+  return bank_packet_impl(g, keys, PCL_DT_F32, labels, ranks, seed, nullptr, scratch, packet, stream);
 }
 
 extern "C" int pcl_bank_packet_dev(const pcl_bank_geom* g, const float* keys, const int64_t* labels, uint64_t seed,
                                    const uint64_t* seed_offset, float* scratch, float* packet, void* stream) {
-  return bank_packet_impl(g, keys, labels, nullptr, seed, seed_offset, scratch, packet, stream);
+  return bank_packet_impl(g, keys, PCL_DT_F32, labels, nullptr, seed, seed_offset, scratch, packet, stream);
+}
+
+extern "C" int pcl_bank_packet_dt(const pcl_bank_geom* g, const void* keys, int32_t keys_dtype, const int64_t* labels,
+                                  const int32_t* ranks, uint64_t seed, float* scratch, float* packet, void* stream) {
+  return bank_packet_impl(g, keys, keys_dtype, labels, ranks, seed, nullptr, scratch, packet, stream);
+}
+
+extern "C" int pcl_bank_packet_dev_dt(const pcl_bank_geom* g, const void* keys, int32_t keys_dtype, const int64_t* labels,
+                                      uint64_t seed, const uint64_t* seed_offset, float* scratch, float* packet,
+                                      void* stream) {
+  return bank_packet_impl(g, keys, keys_dtype, labels, nullptr, seed, seed_offset, scratch, packet, stream);
 }
 
 extern "C" int pcl_bank_apply(const pcl_bank_geom* g, const float* packets, int32_t world, float* segment_queue,

@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
@@ -35,13 +36,34 @@ void count_launch();
     if (!(cond)) return PCL_ERR_ARG;      \
   } while (0)
 
-// internal (not part of the C ABI): fused variants used by pcl_step_forward / pcl_step_backward
-int select_gather_ex(const pcl_geom* g, const float* embed, const uint16_t* keys, const int32_t* chunk_pref,
+// ---- input element types (PCL_DT_*) ----------------------------------------------------------------
+// Kernels that read the embedding, the logits or the bank keys, and the writers of the dense gradient, are templated
+// on the element type.  Loads convert to fp32 (exact); a half gradient is the fp32 value rounded once to nearest-even.
+__device__ __forceinline__ float to_f32(float x) { return x; }
+__device__ __forceinline__ float to_f32(__nv_bfloat16 x) { return __bfloat162float(x); }
+__device__ __forceinline__ float to_f32(__half x) { return __half2float(x); }
+template <typename T> __device__ __forceinline__ T from_f32(float x);
+template <> __device__ __forceinline__ float from_f32<float>(float x) { return x; }
+template <> __device__ __forceinline__ __nv_bfloat16 from_f32<__nv_bfloat16>(float x) { return __float2bfloat16(x); }
+template <> __device__ __forceinline__ __half from_f32<__half>(float x) { return __float2half_rn(x); }
+static inline bool dtype_ok(int dt) { return dt == PCL_DT_F32 || dt == PCL_DT_BF16 || dt == PCL_DT_F16; }
+static inline size_t dtype_size(int dt) { return dt == PCL_DT_F32 ? sizeof(float) : 2; }
+// Runs the statements that follow with the type name T bound to the element type of dtype code `dt` (fp32 for 0).
+#define PCL_DT_SWITCH(dt, T, ...)                                       \
+  switch (dt) {                                                         \
+    case PCL_DT_BF16: { using T = __nv_bfloat16; __VA_ARGS__ } break;   \
+    case PCL_DT_F16: { using T = __half; __VA_ARGS__ } break;           \
+    default: { using T = float; __VA_ARGS__ } break;                    \
+  }
+
+// internal (not part of the C ABI): fused variants used by pcl_step_forward / pcl_step_backward.  `embed_dtype` /
+// `seg_dtype` / `grad_dtype`: element type of embed and grad_clear / seg / grad_embed (PCL_DT_*).
+int select_gather_ex(const pcl_geom* g, const void* embed, const uint16_t* keys, const int32_t* chunk_pref,
                      const int32_t* plan, const int32_t* ranks, uint64_t seed, int normalize, int32_t* anchor_meta,
                      float* anchors_f32, void* anchors_bf16, float* inv_norm, float* norm_max, float* row_m2,
                      float m2_scale, float* partials, int64_t n_slot_rows, void* stream,
                      const unsigned long long* seed_ctr = nullptr, unsigned int* dbg = nullptr,
-                     const int32_t* prev_rows = nullptr, float* grad_clear = nullptr);
+                     const int32_t* prev_rows = nullptr, void* grad_clear = nullptr, int embed_dtype = PCL_DT_F32);
 int tc_fwd_ex(const pcl_tc_desc* d, float* row_m2, float* partials, float* rowstats, float* loss, void* stream,
               bool skip_prep, unsigned long long* step_counter = nullptr);
 int simt_fwd_ex(const pcl_sweep_desc* d, float* partials, float* rowstats, float* loss, void* stream,
@@ -52,19 +74,26 @@ int tc_query(const pcl_tc_desc* d, int64_t* n_slot_rows, float* m2_scale);
 int tc_bwd_ex(const pcl_tc_desc* d, const float* row_m2, const float* rowstats, const float* grad_loss, float* dpartials,
               float* dA, void* stream, int* splits_out, int* a_pad_out, const uint32_t* topk_scratch = nullptr);
 int zero_scatter_reduce(const pcl_geom* g, const int32_t* plan, const int32_t* anchor_meta, const float* dpartials,
-                        int splits, int a_pad, float inv_T, const float* grad_loss, float* grad_embed, void* stream);
+                        int splits, int a_pad, float inv_T, const float* grad_loss, void* grad_embed, void* stream,
+                        int grad_dtype = PCL_DT_F32);
 
 int self_fused_supported(const pcl_tc_desc* d);
 int self_fused(const pcl_tc_desc* d, const float* row_m2, float* partials, float* rowstats, float* loss, float* dpartials,
                unsigned int* sync, void* stream);
-int class_stats_plan(const pcl_geom* g, const int64_t* labels, const float* seg, const int64_t* predict, uint16_t* keys,
-                     int32_t* chunk_pref, int32_t* counts, int32_t* plan, unsigned int* done_ctr, void* stream);
+int class_stats(const pcl_geom* g, const int64_t* labels, const void* seg, const int64_t* predict, uint16_t* keys,
+                int32_t* chunk_pref, int32_t* counts, void* stream, int seg_dtype);
+int class_stats_plan(const pcl_geom* g, const int64_t* labels, const void* seg, const int64_t* predict, uint16_t* keys,
+                     int32_t* chunk_pref, int32_t* counts, int32_t* plan, unsigned int* done_ctr, void* stream,
+                     int seg_dtype = PCL_DT_F32);
 int scatter_reduce_rows(const pcl_geom* g, const int32_t* plan, const int32_t* anchor_meta, const float* dpartials, int splits,
-                        int split_cols, int a_pad, float inv_T, const float* grad_scale, float* grad_embed, unsigned long long* step_counter,
-                        void* stream, unsigned int* dbg = nullptr, int32_t* prev_rows = nullptr);
+                        int split_cols, int a_pad, float inv_T, const float* grad_scale, void* grad_embed, unsigned long long* step_counter,
+                        void* stream, unsigned int* dbg = nullptr, int32_t* prev_rows = nullptr, int grad_dtype = PCL_DT_F32);
 int fill_zero(void* ptr, uint64_t bytes, void* stream, unsigned int* dbg, int reserve_sms);
 int scatter_rows(const pcl_geom* g, const int32_t* plan, const int32_t* anchor_meta, const float* dA,
-                 const float* anchors_f32, const float* inv_norm, int normalize, float* grad_embed, void* stream);
+                 const float* anchors_f32, const float* inv_norm, int normalize, void* grad_embed, void* stream,
+                 int grad_dtype = PCL_DT_F32);
+int scatter_grad(const pcl_geom* g, const int32_t* plan, const int32_t* anchor_meta, const float* dA, const float* anchors_f32,
+                 const float* inv_norm, int normalize, void* grad_embed, void* stream, int grad_dtype);
 
 // ---- per-device kernel attributes ----------------------------------------------------------------
 // cudaFuncAttributeMaxDynamicSharedMemorySize is a property of (function, device) and SETS the limit (a later call with

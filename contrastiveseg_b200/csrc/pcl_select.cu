@@ -19,9 +19,10 @@ __device__ __forceinline__ void plan_body(const pcl_geom& g, const int32_t* coun
 // ------------------------------------------------------------------------------------------------
 // k_keys
 // ------------------------------------------------------------------------------------------------
+template <typename TS>      // element type of seg (the argmax compares the values converted to fp32)
 __global__ void __launch_bounds__(PCL_CHUNK, 2)
 k_keys(pcl_geom g, int nchunk, float scale_h, float scale_w, const int64_t* __restrict__ labels,
-       const float* __restrict__ seg, const int64_t* __restrict__ predict, uint16_t* __restrict__ keys,
+       const TS* __restrict__ seg, const int64_t* __restrict__ predict, uint16_t* __restrict__ keys,
        int32_t* chunk_hist, int32_t* counts, int32_t* plan, unsigned int* done_ctr) {
   extern __shared__ int s_hist[];                 // 2K+1 bins
   unsigned int* dbg = done_ctr ? done_ctr - 4 : nullptr;       // the step's sync buffer (timeline, diagnostics)
@@ -42,18 +43,21 @@ k_keys(pcl_geom g, int nchunk, float scale_h, float scale_w, const int64_t* __re
     // per group of 8 planes behind the label test; the scan is a chain of dependent round trips).  16 at a time: 1024 threads x 32 registers keeps two CTAs per SM.
     int pred32 = -1;
     if (seg != nullptr && K <= 32) {
-      const float* sp = seg + (int64_t)b * K * HW + p;
+      const TS* sp = seg + (int64_t)b * K * HW + p;
       float best = -CUDART_INF_F;
       pred32 = 0;
 #pragma unroll
       for (int c0 = 0; c0 < 32; c0 += 16) {
         if (c0 < K) {
-          float v[16];
+          // kept in the input type until the compare.  Under the 32-register cap of this launch bound every instantiation
+          // spills a little (ptxas, bytes stored / loaded): fp32 36 / 112 as before; bf16 and fp16 40 / 104 (52 / 132
+          // when converted at load time)
+          TS v[16];
 #pragma unroll
-          for (int u = 0; u < 16; ++u) v[u] = (c0 + u < K) ? __ldg(sp + (int64_t)(c0 + u) * HW) : -CUDART_INF_F;
+          for (int u = 0; u < 16; ++u) v[u] = (c0 + u < K) ? __ldg(sp + (int64_t)(c0 + u) * HW) : from_f32<TS>(-CUDART_INF_F);
 #pragma unroll
           for (int u = 0; u < 16; ++u)
-            if (v[u] > best) { best = v[u]; pred32 = c0 + u; }        // first maximum wins, like torch.max
+            if (to_f32(v[u]) > best) { best = to_f32(v[u]); pred32 = c0 + u; }    // first maximum wins, like torch.max
         }
       }
     }
@@ -62,13 +66,13 @@ k_keys(pcl_geom g, int nchunk, float scale_h, float scale_w, const int64_t* __re
       if (seg != nullptr && K <= 32) {
         pred = pred32;
       } else if (seg != nullptr) {
-        const float* sp = seg + (int64_t)b * K * HW + p;
+        const TS* sp = seg + (int64_t)b * K * HW + p;
         float best = -CUDART_INF_F;
         pred = 0;
         for (int c0 = 0; c0 < K; c0 += 8) {
           float v[8];
 #pragma unroll
-          for (int u = 0; u < 8; ++u) v[u] = (c0 + u < K) ? __ldg(sp + (int64_t)(c0 + u) * HW) : -CUDART_INF_F;
+          for (int u = 0; u < 8; ++u) v[u] = (c0 + u < K) ? to_f32(__ldg(sp + (int64_t)(c0 + u) * HW)) : -CUDART_INF_F;
 #pragma unroll
           for (int u = 0; u < 8; ++u)
             if (v[u] > best) { best = v[u]; pred = c0 + u; }       // first maximum wins, like torch.max
@@ -260,14 +264,15 @@ k_plan(pcl_geom g, int nchunk, const int32_t* __restrict__ counts, int32_t* __re
 // ------------------------------------------------------------------------------------------------
 // k_select: one warp per anchor row
 // ------------------------------------------------------------------------------------------------
+template <typename T>       // element type of embed and grad_clear
 __global__ void __launch_bounds__(256)
-k_select(pcl_geom g, int nchunk, const float* __restrict__ embed, const uint16_t* __restrict__ keys,
+k_select(pcl_geom g, int nchunk, const T* __restrict__ embed, const uint16_t* __restrict__ keys,
          const int32_t* __restrict__ chunk_pref, const int32_t* __restrict__ plan,
          const int32_t* __restrict__ ranks, uint64_t seed, int normalize, int32_t* __restrict__ meta,
          float* __restrict__ anchors, __nv_bfloat16* __restrict__ anchors_bf16, float* __restrict__ inv_norm,
          float* __restrict__ norm_max, float* __restrict__ row_m2, float m2_scale, float* __restrict__ partials,
          int64_t n_slot_rows, const unsigned long long* __restrict__ seed_ctr, unsigned int* dbg,
-         const int32_t* __restrict__ prev_rows, float* __restrict__ grad_clear) {
+         const int32_t* __restrict__ prev_rows, T* __restrict__ grad_clear) {
   tl_begin(dbg, PCL_TL_SELECT);
   struct TlEnd { unsigned int* d; __device__ ~TlEnd() { tl_end(d, PCL_TL_SELECT); } } tl_guard{dbg};
   // Sparse reset (persistent dense-gradient buffer of a captured step): instead of re-filling B*D*h*w zeros every step,
@@ -278,8 +283,8 @@ k_select(pcl_geom g, int nchunk, const float* __restrict__ embed, const uint16_t
     const int msp = g.max_samples;
     if (ip < min(prev_rows[0], msp)) {
       const int64_t HWp = (int64_t)g.h * g.w;
-      float* dstp = grad_clear + (int64_t)prev_rows[1 + msp + ip] * g.D * HWp + prev_rows[1 + ip];
-      for (int d = threadIdx.x & 31; d < g.D; d += 32) dstp[(int64_t)d * HWp] = 0.f;
+      T* dstp = grad_clear + (int64_t)prev_rows[1 + msp + ip] * g.D * HWp + prev_rows[1 + ip];
+      for (int d = threadIdx.x & 31; d < g.D; d += 32) dstp[(int64_t)d * HWp] = from_f32<T>(0.f);
     }
   }
   // captured launch sequences: the per-step part of the seed lives in device memory (same formula as pcl_step_ranks)
@@ -399,11 +404,11 @@ k_select(pcl_geom g, int nchunk, const float* __restrict__ embed, const uint16_t
 
   // gather the D channels of (b, pix)
   const int s = base + v;
-  const float* src = embed + (int64_t)b * D * HW + pix;
+  const T* src = embed + (int64_t)b * D * HW + pix;
   float* dst = anchors + (int64_t)s * D;
   float ss = 0.f;
   for (int d = lane; d < D; d += 32) {
-    float x = src[(int64_t)d * HW];
+    float x = to_f32(src[(int64_t)d * HW]);
     ss += x * x;
     dst[d] = x;
   }
@@ -438,10 +443,11 @@ k_select(pcl_geom g, int nchunk, const float* __restrict__ embed, const uint16_t
 // ------------------------------------------------------------------------------------------------
 // k_scatter: dA rows -> dense NCHW gradient (buffer is zeroed by a memset first)
 // ------------------------------------------------------------------------------------------------
+template <typename T>       // element type of grad: the fp32 value is rounded once
 __global__ void __launch_bounds__(256)
 k_scatter(pcl_geom g, const int32_t* __restrict__ plan, const int32_t* __restrict__ meta,
           const float* __restrict__ dA, const float* __restrict__ anchors, const float* __restrict__ inv_norm,
-          int normalize, float* __restrict__ grad) {
+          int normalize, T* __restrict__ grad) {
   const int lane = threadIdx.x & 31;
   const int s = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int A = plan[PCL_PLAN_A];
@@ -457,11 +463,11 @@ k_scatter(pcl_geom g, const int32_t* __restrict__ plan, const int32_t* __restric
     dot = warp_sum(dot);
     inv = inv_norm[s];
   }
-  float* dst = grad + (int64_t)b * D * HW + pix;
+  T* dst = grad + (int64_t)b * D * HW + pix;
   for (int d = lane; d < D; d += 32) {
     float v = ga[d];
     if (normalize) v = (v - anchors[(int64_t)s * D + d] * dot) * inv;
-    dst[(int64_t)d * HW] = v;
+    dst[(int64_t)d * HW] = from_f32<T>(v);
   }
 }
 
@@ -470,44 +476,48 @@ k_scatter(pcl_geom g, const int32_t* __restrict__ plan, const int32_t* __restric
 // it with 16-byte stores and then drops in the gradient entries of the anchors sampled from that image.
 // HBM-bound: writes B*D*h*w*4 bytes once (the floor of the backward: autograd needs the dense tensor).
 // ------------------------------------------------------------------------------------------------
+template <typename T>
 __global__ void __launch_bounds__(256)
 k_zero_scatter(pcl_geom g, const int32_t* __restrict__ plan, const int32_t* __restrict__ meta,
-               const float* __restrict__ dA, float* __restrict__ grad) {
+               const float* __restrict__ dA, T* __restrict__ grad) {
   const int plane = blockIdx.x;
   const int D = g.D, ms = g.max_samples;
   const int b = plane / D, d = plane - b * D;
   const int64_t HW = (int64_t)g.h * g.w;
-  float* dst = grad + (int64_t)plane * HW;
-  if ((HW & 3) == 0) {
-    float4* d4 = reinterpret_cast<float4*>(dst);
-    const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
-    for (int64_t i = threadIdx.x; i < HW / 4; i += blockDim.x) d4[i] = z;
+  T* dst = grad + (int64_t)plane * HW;
+  constexpr int E = 16 / sizeof(T);                // elements per 16-byte store
+  if (HW % E == 0) {
+    uint4* d4 = reinterpret_cast<uint4*>(dst);
+    const uint4 z = make_uint4(0u, 0u, 0u, 0u);
+    for (int64_t i = threadIdx.x; i < HW / E; i += blockDim.x) d4[i] = z;
   } else {
-    for (int64_t i = threadIdx.x; i < HW; i += blockDim.x) dst[i] = 0.f;
+    for (int64_t i = threadIdx.x; i < HW; i += blockDim.x) dst[i] = from_f32<T>(0.f);
   }
   __syncthreads();
   const int A = min(plan[PCL_PLAN_A], ms);
   for (int s = threadIdx.x; s < A; s += blockDim.x)
-    if (meta[ms + s] == b) dst[meta[s]] = dA[(int64_t)s * D + d];
+    if (meta[ms + s] == b) dst[meta[s]] = from_f32<T>(dA[(int64_t)s * D + d]);
 }
 
 // Same, with the reduction of the backward sweep's per-split partial gradients folded in (step path: the (A, D)
 // gradient matrix is never written): value = scale * sum_p dpartials[p][s][d].
+template <typename T>
 __global__ void __launch_bounds__(256)
 k_zero_scatter_reduce(pcl_geom g, const int32_t* __restrict__ plan, const int32_t* __restrict__ meta,
                       const float* __restrict__ dpartials, int splits, int a_pad, float inv_T,
-                      const float* __restrict__ grad_loss, float* __restrict__ grad) {
+                      const float* __restrict__ grad_loss, T* __restrict__ grad) {
   const int plane = blockIdx.x;
   const int D = g.D, ms = g.max_samples;
   const int b = plane / D, d = plane - b * D;
   const int64_t HW = (int64_t)g.h * g.w;
-  float* dst = grad + (int64_t)plane * HW;
-  if ((HW & 3) == 0) {
-    float4* d4 = reinterpret_cast<float4*>(dst);
-    const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
-    for (int64_t i = threadIdx.x; i < HW / 4; i += blockDim.x) d4[i] = z;
+  T* dst = grad + (int64_t)plane * HW;
+  constexpr int E = 16 / sizeof(T);                // elements per 16-byte store
+  if (HW % E == 0) {
+    uint4* d4 = reinterpret_cast<uint4*>(dst);
+    const uint4 z = make_uint4(0u, 0u, 0u, 0u);
+    for (int64_t i = threadIdx.x; i < HW / E; i += blockDim.x) d4[i] = z;
   } else {
-    for (int64_t i = threadIdx.x; i < HW; i += blockDim.x) dst[i] = 0.f;
+    for (int64_t i = threadIdx.x; i < HW; i += blockDim.x) dst[i] = from_f32<T>(0.f);
   }
   __syncthreads();
   const int A = min(plan[PCL_PLAN_A], ms);
@@ -516,7 +526,7 @@ k_zero_scatter_reduce(pcl_geom g, const int32_t* __restrict__ plan, const int32_
     if (meta[ms + s] == b) {
       float v = 0.f;
       for (int p = 0; p < splits; ++p) v += dpartials[((int64_t)p * a_pad + s) * D + d];    // fixed order
-      dst[meta[s]] = v * scale;
+      dst[meta[s]] = from_f32<T>(v * scale);
     }
   }
 }
@@ -524,10 +534,11 @@ k_zero_scatter_reduce(pcl_geom g, const int32_t* __restrict__ plan, const int32_
 // Scatter of the A gradient rows into an ALREADY zero-filled dense gradient, with the fixed-order sum of the per-split
 // (per-column-tile) partial rows folded in: one block per anchor row.  Also advances the step counter of a captured
 // sequence (last kernel of the step).
+template <typename T>
 __global__ void __launch_bounds__(256)
 k_scatter_reduce(pcl_geom g, const int32_t* __restrict__ plan, const int32_t* __restrict__ meta,
                  const float* __restrict__ dpartials, int splits, int split_cols, int a_pad, float inv_T,
-                 const float* __restrict__ grad_scale, float* __restrict__ grad, unsigned long long* step_counter,
+                 const float* __restrict__ grad_scale, T* __restrict__ grad, unsigned long long* step_counter,
                  unsigned int* dbg, int32_t* __restrict__ prev_rows) {
   // one BLOCK per anchor row, one thread per channel: the sum over the splits (up to 18 for the bank sweeps) is a chain
   // of dependent adds per element, so the parallelism has to come from the elements (a warp per row leaves few warps
@@ -546,11 +557,11 @@ k_scatter_reduce(pcl_geom g, const int32_t* __restrict__ plan, const int32_t* __
   const int pix = meta[s], b = meta[ms + s];
   if (prev_rows != nullptr && threadIdx.x == 0) { prev_rows[1 + s] = pix; prev_rows[1 + ms + s] = b; }
   const float scale = inv_T * (grad_scale ? grad_scale[0] : 1.f);
-  float* dst = grad + (int64_t)b * D * HW + pix;
+  T* dst = grad + (int64_t)b * D * HW + pix;
   for (int d = threadIdx.x; d < D; d += blockDim.x) {
     float v = 0.f;
     for (int p = 0; p < splits; ++p) v += dpartials[((int64_t)p * a_pad + s) * D + d];      // fixed order
-    dst[(int64_t)d * HW] = v * scale;
+    dst[(int64_t)d * HW] = from_f32<T>(v * scale);
   }
 }
 
@@ -625,20 +636,26 @@ int pcl::fill_zero(void* ptr, uint64_t bytes, void* stream, unsigned int* dbg, i
 }
 
 int pcl::scatter_reduce_rows(const pcl_geom* g, const int32_t* plan, const int32_t* anchor_meta, const float* dpartials,
-                             int splits, int split_cols, int a_pad, float inv_T, const float* grad_scale, float* grad_embed,
-                             unsigned long long* step_counter, void* stream, unsigned int* dbg, int32_t* prev_rows) {
-  if (!g || !plan || !anchor_meta || !dpartials || !grad_embed || splits < 1) return PCL_ERR_ARG;
-  k_scatter_reduce<<<g->max_samples, g->D <= 128 ? 128 : 256, 0, (cudaStream_t)stream>>>(
-      *g, plan, anchor_meta, dpartials, splits, split_cols, a_pad, inv_T, grad_scale, grad_embed, step_counter, dbg, prev_rows);
+                             int splits, int split_cols, int a_pad, float inv_T, const float* grad_scale, void* grad_embed,
+                             unsigned long long* step_counter, void* stream, unsigned int* dbg, int32_t* prev_rows,
+                             int grad_dtype) {
+  if (!g || !plan || !anchor_meta || !dpartials || !grad_embed || splits < 1 || !dtype_ok(grad_dtype)) return PCL_ERR_ARG;
+  PCL_DT_SWITCH(grad_dtype, T,
+    k_scatter_reduce<T><<<g->max_samples, g->D <= 128 ? 128 : 256, 0, (cudaStream_t)stream>>>(
+        *g, plan, anchor_meta, dpartials, splits, split_cols, a_pad, inv_T, grad_scale, (T*)grad_embed, step_counter, dbg,
+        prev_rows);)
   PCL_LAUNCH_CHECK();
   return PCL_OK;
 }
 
 int pcl::zero_scatter_reduce(const pcl_geom* g, const int32_t* plan, const int32_t* anchor_meta, const float* dpartials,
-                             int splits, int a_pad, float inv_T, const float* grad_loss, float* grad_embed, void* stream) {
-  if (!g || !plan || !anchor_meta || !dpartials || !grad_embed) return PCL_ERR_ARG;
-  k_zero_scatter_reduce<<<(unsigned)(g->B * g->D), 256, 0, (cudaStream_t)stream>>>(*g, plan, anchor_meta, dpartials, splits,
-                                                                                 a_pad, inv_T, grad_loss, grad_embed);
+                             int splits, int a_pad, float inv_T, const float* grad_loss, void* grad_embed, void* stream,
+                             int grad_dtype) {
+  if (!g || !plan || !anchor_meta || !dpartials || !grad_embed || !dtype_ok(grad_dtype)) return PCL_ERR_ARG;
+  PCL_DT_SWITCH(grad_dtype, T,
+    k_zero_scatter_reduce<T><<<(unsigned)(g->B * g->D), 256, 0, (cudaStream_t)stream>>>(*g, plan, anchor_meta, dpartials,
+                                                                                      splits, a_pad, inv_T, grad_loss,
+                                                                                      (T*)grad_embed);)
   PCL_LAUNCH_CHECK();
   return PCL_OK;
 }
@@ -646,12 +663,15 @@ int pcl::zero_scatter_reduce(const pcl_geom* g, const int32_t* plan, const int32
 // Scatter-only variant for callers that zero-fill the dense gradient themselves (e.g. overlapped with the forward on a
 // second stream): drops the A gradient rows into an already-zero (B,D,h,w) buffer.
 int pcl::scatter_rows(const pcl_geom* g, const int32_t* plan, const int32_t* anchor_meta, const float* dA,
-                      const float* anchors_f32, const float* inv_norm, int normalize, float* grad_embed, void* stream) {
-  if (!g || !plan || !anchor_meta || !dA || !grad_embed) return PCL_ERR_ARG;
+                      const float* anchors_f32, const float* inv_norm, int normalize, void* grad_embed, void* stream,
+                      int grad_dtype) {
+  if (!g || !plan || !anchor_meta || !dA || !grad_embed || !dtype_ok(grad_dtype)) return PCL_ERR_ARG;
   if (normalize && (!anchors_f32 || !inv_norm)) return PCL_ERR_ARG;
   const int warps = 8;
-  k_scatter<<<ceil_div(g->max_samples, warps), warps * 32, 0, (cudaStream_t)stream>>>(*g, plan, anchor_meta, dA, anchors_f32,
-                                                                                     inv_norm, normalize, grad_embed);
+  PCL_DT_SWITCH(grad_dtype, T,
+    k_scatter<T><<<ceil_div(g->max_samples, warps), warps * 32, 0, (cudaStream_t)stream>>>(*g, plan, anchor_meta, dA,
+                                                                                          anchors_f32, inv_norm, normalize,
+                                                                                          (T*)grad_embed);)
   PCL_LAUNCH_CHECK();
   return PCL_OK;
 }
@@ -684,9 +704,14 @@ extern "C" int pcl_select_sizes(const pcl_geom* g, pcl_select_sizes_t* out) {
 
 extern "C" int pcl_class_stats(const pcl_geom* g, const int64_t* labels, const float* seg, const int64_t* predict,
                                uint16_t* keys, int32_t* chunk_pref, int32_t* counts, void* stream) {
+  return pcl::class_stats(g, labels, seg, predict, keys, chunk_pref, counts, stream, PCL_DT_F32);
+}
+
+int pcl::class_stats(const pcl_geom* g, const int64_t* labels, const void* seg, const int64_t* predict, uint16_t* keys,
+                     int32_t* chunk_pref, int32_t* counts, void* stream, int seg_dtype) {
   int st = check_geom(g);
   if (st != PCL_OK) return st;
-  PCL_REQUIRE(labels && keys && chunk_pref && counts && (seg || predict));
+  PCL_REQUIRE(labels && keys && chunk_pref && counts && (seg || predict) && dtype_ok(seg_dtype));
   cudaStream_t s = (cudaStream_t)stream;
   const int64_t HW = (int64_t)g->h * g->w;
   const int nchunk = (int)ceil_div64(HW, PCL_CHUNK);
@@ -694,26 +719,29 @@ extern "C" int pcl_class_stats(const pcl_geom* g, const int64_t* labels, const f
   PCL_CUDA(cudaMemsetAsync(counts, 0, (size_t)g->B * 2 * g->K * sizeof(int32_t), s));
   dim3 grid(nchunk, g->B);
   size_t smem = (2 * g->K + 1) * sizeof(int);
-  k_keys<<<grid, PCL_CHUNK, smem, s>>>(*g, nchunk, scale_h, scale_w, labels, seg, predict, keys, chunk_pref, counts,
-                                       nullptr, nullptr);
+  PCL_DT_SWITCH(seg_dtype, T,
+    k_keys<T><<<grid, PCL_CHUNK, smem, s>>>(*g, nchunk, scale_h, scale_w, labels, (const T*)seg, predict, keys, chunk_pref,
+                                            counts, nullptr, nullptr);)
   PCL_LAUNCH_CHECK();
   return PCL_OK;
 }
 
 // Step path: scan + totals + plan in ONE launch (the last block to finish runs the plan; done_ctr: one zeroed word).
-int pcl::class_stats_plan(const pcl_geom* g, const int64_t* labels, const float* seg, const int64_t* predict, uint16_t* keys,
-                          int32_t* chunk_pref, int32_t* counts, int32_t* plan, unsigned int* done_ctr, void* stream) {
+int pcl::class_stats_plan(const pcl_geom* g, const int64_t* labels, const void* seg, const int64_t* predict, uint16_t* keys,
+                          int32_t* chunk_pref, int32_t* counts, int32_t* plan, unsigned int* done_ctr, void* stream,
+                          int seg_dtype) {
   int st = check_geom(g);
   if (st != PCL_OK) return st;
-  PCL_REQUIRE(labels && keys && chunk_pref && counts && plan && done_ctr && (seg || predict));
+  PCL_REQUIRE(labels && keys && chunk_pref && counts && plan && done_ctr && (seg || predict) && dtype_ok(seg_dtype));
   cudaStream_t s = (cudaStream_t)stream;
   const int64_t HW = (int64_t)g->h * g->w;
   const int nchunk = (int)ceil_div64(HW, PCL_CHUNK);
   const float scale_h = (float)g->Himg / (float)g->h, scale_w = (float)g->Wimg / (float)g->w;
   dim3 grid(nchunk, g->B);
   size_t smem = (2 * g->K + 1) * sizeof(int);
-  k_keys<<<grid, PCL_CHUNK, smem, s>>>(*g, nchunk, scale_h, scale_w, labels, seg, predict, keys, chunk_pref, counts, plan,
-                                       done_ctr);
+  PCL_DT_SWITCH(seg_dtype, T,
+    k_keys<T><<<grid, PCL_CHUNK, smem, s>>>(*g, nchunk, scale_h, scale_w, labels, (const T*)seg, predict, keys, chunk_pref,
+                                            counts, plan, done_ctr);)
   PCL_LAUNCH_CHECK();
   return PCL_OK;
 }
@@ -729,14 +757,15 @@ extern "C" int pcl_plan_anchors(const pcl_geom* g, const int32_t* counts, int32_
   return PCL_OK;
 }
 
-int pcl::select_gather_ex(const pcl_geom* g, const float* embed, const uint16_t* keys, const int32_t* chunk_pref,
+int pcl::select_gather_ex(const pcl_geom* g, const void* embed, const uint16_t* keys, const int32_t* chunk_pref,
                           const int32_t* plan, const int32_t* ranks, uint64_t seed, int normalize, int32_t* anchor_meta,
                           float* anchors_f32, void* anchors_bf16, float* inv_norm, float* norm_max, float* row_m2,
                           float m2_scale, float* partials, int64_t n_slot_rows, void* stream,
-                          const unsigned long long* seed_ctr, unsigned int* dbg, const int32_t* prev_rows, float* grad_clear) {
+                          const unsigned long long* seed_ctr, unsigned int* dbg, const int32_t* prev_rows, void* grad_clear,
+                          int embed_dtype) {
   int st = check_geom(g);
   if (st != PCL_OK) return st;
-  PCL_REQUIRE(embed && keys && chunk_pref && plan && anchor_meta && anchors_f32 && inv_norm);
+  PCL_REQUIRE(embed && keys && chunk_pref && plan && anchor_meta && anchors_f32 && inv_norm && dtype_ok(embed_dtype));
   cudaStream_t s = (cudaStream_t)stream;
   const int ms = g->max_samples;
   const int nchunk = (int)ceil_div64((int64_t)g->h * g->w, PCL_CHUNK);
@@ -745,10 +774,12 @@ int pcl::select_gather_ex(const pcl_geom* g, const float* embed, const uint16_t*
   // rows in [A, max_samples) are zero-filled by the kernel itself (no separate memsets); the bf16 copy is padded to
   // a multiple of 128 rows: cover those too
   const int rows = anchors_bf16 ? ceil_div(ms, 128) * 128 : ms;
-  k_select<<<ceil_div(rows, warps), warps * 32, 0, s>>>(*g, nchunk, embed, keys, chunk_pref, plan, ranks, seed,
-                                                       normalize, anchor_meta, anchors_f32,
-                                                       (__nv_bfloat16*)anchors_bf16, inv_norm, norm_max, row_m2, m2_scale,
-                                                       partials, n_slot_rows, seed_ctr, dbg, prev_rows, grad_clear);
+  PCL_DT_SWITCH(embed_dtype, T,
+    k_select<T><<<ceil_div(rows, warps), warps * 32, 0, s>>>(*g, nchunk, (const T*)embed, keys, chunk_pref, plan, ranks,
+                                                             seed, normalize, anchor_meta, anchors_f32,
+                                                             (__nv_bfloat16*)anchors_bf16, inv_norm, norm_max, row_m2,
+                                                             m2_scale, partials, n_slot_rows, seed_ctr, dbg, prev_rows,
+                                                             (T*)grad_clear);)
   PCL_LAUNCH_CHECK();
   return PCL_OK;
 }
@@ -764,21 +795,29 @@ extern "C" int pcl_select_gather(const pcl_geom* g, const float* embed, const ui
 extern "C" int pcl_scatter_grad(const pcl_geom* g, const int32_t* plan, const int32_t* anchor_meta, const float* dA,
                                 const float* anchors_f32, const float* inv_norm, int normalize, float* grad_embed,
                                 void* stream) {
+  return pcl::scatter_grad(g, plan, anchor_meta, dA, anchors_f32, inv_norm, normalize, grad_embed, stream, PCL_DT_F32);
+}
+
+int pcl::scatter_grad(const pcl_geom* g, const int32_t* plan, const int32_t* anchor_meta, const float* dA,
+                      const float* anchors_f32, const float* inv_norm, int normalize, void* grad_embed, void* stream,
+                      int grad_dtype) {
   int st = check_geom(g);
   if (st != PCL_OK) return st;
-  PCL_REQUIRE(plan && anchor_meta && dA && grad_embed);
+  PCL_REQUIRE(plan && anchor_meta && dA && grad_embed && dtype_ok(grad_dtype));
   if (normalize) PCL_REQUIRE(anchors_f32 && inv_norm);
   cudaStream_t s = (cudaStream_t)stream;
   if (!normalize) {
-    k_zero_scatter<<<(unsigned)(g->B * g->D), 256, 0, s>>>(*g, plan, anchor_meta, dA, grad_embed);
+    PCL_DT_SWITCH(grad_dtype, T,
+      k_zero_scatter<T><<<(unsigned)(g->B * g->D), 256, 0, s>>>(*g, plan, anchor_meta, dA, (T*)grad_embed);)
     PCL_LAUNCH_CHECK();
     return PCL_OK;
   }
-  size_t bytes = (size_t)g->B * g->D * g->h * g->w * sizeof(float);
+  size_t bytes = (size_t)g->B * g->D * g->h * g->w * dtype_size(grad_dtype);
   PCL_CUDA(cudaMemsetAsync(grad_embed, 0, bytes, s));
   const int warps = 8;
-  k_scatter<<<ceil_div(g->max_samples, warps), warps * 32, 0, s>>>(*g, plan, anchor_meta, dA, anchors_f32, inv_norm,
-                                                                  normalize, grad_embed);
+  PCL_DT_SWITCH(grad_dtype, T,
+    k_scatter<T><<<ceil_div(g->max_samples, warps), warps * 32, 0, s>>>(*g, plan, anchor_meta, dA, anchors_f32, inv_norm,
+                                                                       normalize, (T*)grad_embed);)
   PCL_LAUNCH_CHECK();
   return PCL_OK;
 }

@@ -44,8 +44,8 @@ extern "C" int pcl_step_stats(const pcl_step_desc* d, void* stream) {
   if (!d) return PCL_ERR_ARG;
   if (d->sync != nullptr)        // one launch: the scan's last block computes totals and plan (sync[4] = its counter)
     return pcl::class_stats_plan(&d->g, d->labels, d->seg, d->predict, d->keys, d->chunk_pref, d->counts, d->plan,
-                                 d->sync + 4, stream);
-  int st = pcl_class_stats(&d->g, d->labels, d->seg, d->predict, d->keys, d->chunk_pref, d->counts, stream);
+                                 d->sync + 4, stream, d->seg_dtype);
+  int st = pcl::class_stats(&d->g, d->labels, d->seg, d->predict, d->keys, d->chunk_pref, d->counts, stream, d->seg_dtype);
   if (st != PCL_OK) return st;
   return pcl_plan_anchors(&d->g, d->counts, d->plan, stream);
 }
@@ -75,13 +75,13 @@ static int step_forward(const pcl_step_desc* d, unsigned long long* ctr, void* s
     if (st != PCL_OK) return st;
     st = pcl::select_gather_ex(&d->g, d->embed, d->keys, d->chunk_pref, d->plan, ctr ? nullptr : d->ranks, d->seed,
                                d->normalize, d->anchor_meta, d->anchors_f32, d->anchors_bf16, d->inv_norm, nullptr, d->row_m2,
-                               m2_scale, d->partials, n_slot_rows, stream, ctr);
+                               m2_scale, d->partials, n_slot_rows, stream, ctr, nullptr, nullptr, nullptr, d->embed_dtype);
     if (st != PCL_OK) return st;
     return pcl::tc_fwd_ex(&t, d->row_m2, d->partials, d->rowstats, d->loss, stream, true, ctr);
   }
   int st = pcl::select_gather_ex(&d->g, d->embed, d->keys, d->chunk_pref, d->plan, ctr ? nullptr : d->ranks, d->seed,
                                  d->normalize, d->anchor_meta, d->anchors_f32, d->anchors_bf16, d->inv_norm, d->norm_max,
-                                 nullptr, 0.f, nullptr, 0, stream, ctr);
+                                 nullptr, 0.f, nullptr, 0, stream, ctr, nullptr, nullptr, nullptr, d->embed_dtype);
   if (st != PCL_OK) return st;
   pcl_sweep_desc w;
   fill_sweep(d, &w);
@@ -100,7 +100,7 @@ extern "C" int pcl_step_backward(const pcl_step_desc* d, const float* grad_loss,
       st = pcl::tc_bwd_ex(&t, d->row_m2, d->rowstats, grad_loss, d->dpartials, nullptr, stream, &splits, &a_pad);
       if (st != PCL_OK) return st;
       return pcl::zero_scatter_reduce(&d->g, d->plan, d->anchor_meta, d->dpartials, splits, a_pad, 1.f / d->temperature,
-                                      grad_loss, d->grad_embed, stream);
+                                      grad_loss, d->grad_embed, stream, d->embed_dtype);
     }
     st = pcl_infonce_tc_bwd(&t, d->row_m2, d->rowstats, grad_loss, d->dpartials, d->dA, stream);
   } else {
@@ -109,8 +109,8 @@ extern "C" int pcl_step_backward(const pcl_step_desc* d, const float* grad_loss,
     st = pcl_infonce_bwd(&w, d->rowstats, grad_loss, d->dpartials, d->dA, stream);
   }
   if (st != PCL_OK) return st;
-  return pcl_scatter_grad(&d->g, d->plan, d->anchor_meta, d->dA, d->anchors_f32, d->inv_norm, d->normalize,
-                          d->grad_embed, stream);
+  return pcl::scatter_grad(&d->g, d->plan, d->anchor_meta, d->dA, d->anchors_f32, d->inv_norm, d->normalize,
+                           d->grad_embed, stream, d->embed_dtype);
 }
 
 // Backward for a dense-gradient buffer the caller has ALREADY zero-filled (the 268 MB fill is the HBM floor of the
@@ -128,7 +128,7 @@ extern "C" int pcl_step_backward_prezeroed(const pcl_step_desc* d, const float* 
       st = pcl::tc_bwd_ex(&t, d->row_m2, d->rowstats, grad_loss, d->dpartials, nullptr, stream, &splits, &a_pad);
       if (st != PCL_OK) return st;
       return pcl::scatter_reduce_rows(&d->g, d->plan, d->anchor_meta, d->dpartials, splits, 0, a_pad, 1.f / d->temperature,
-                                      grad_loss, d->grad_embed, nullptr, stream, d->sync);
+                                      grad_loss, d->grad_embed, nullptr, stream, d->sync, nullptr, d->embed_dtype);
     }
     st = pcl_infonce_tc_bwd(&t, d->row_m2, d->rowstats, grad_loss, d->dpartials, d->dA, stream);
   } else {
@@ -138,13 +138,14 @@ extern "C" int pcl_step_backward_prezeroed(const pcl_step_desc* d, const float* 
   }
   if (st != PCL_OK) return st;
   return pcl::scatter_rows(&d->g, d->plan, d->anchor_meta, d->dA, d->anchors_f32, d->inv_norm, d->normalize,
-                           d->grad_embed, stream);
+                           d->grad_embed, stream, d->embed_dtype);
 }
 
 // ---- fused small-anchor step (include/pcl.h: pcl_step_fused_*) ----
 extern "C" int pcl_step_fused_supported(const pcl_step_desc* d) {
   if (!d || d->mode != 0 || d->precision != 1 || d->normalize != 0 || d->sync == nullptr) return 0;
   if (d->g.D != 256 || d->g.max_samples < 1 || d->g.max_samples > 1024) return 0;
+  if (!pcl::dtype_ok(d->embed_dtype) || !pcl::dtype_ok(d->seg_dtype)) return 0;      // fp32, bf16 and fp16 inputs qualify
   return 1;
 }
 
@@ -162,7 +163,7 @@ extern "C" int pcl_step_fused_select(const pcl_step_desc* d, const uint64_t* ste
   return pcl::select_gather_ex(&d->g, d->embed, d->keys, d->chunk_pref, d->plan, step_counter ? nullptr : d->ranks, d->seed,
                                0, d->anchor_meta, d->anchors_f32, d->anchors_bf16, d->inv_norm, nullptr, d->row_m2, m2_scale,
                                nullptr, 0, stream, reinterpret_cast<const unsigned long long*>(step_counter), d->sync,
-                               prev_rows, d->grad_embed);
+                               prev_rows, d->grad_embed, d->embed_dtype);
 }
 
 extern "C" int pcl_step_fused_loss(const pcl_step_desc* d, void* stream) {
@@ -180,13 +181,15 @@ extern "C" int pcl_step_fused_scatter(const pcl_step_desc* d, const float* grad_
   const int a_pad = ((d->g.max_samples + 127) / 128) * 128;
   const int splits = (a_pad + 255) / 256;
   return pcl::scatter_reduce_rows(&d->g, d->plan, d->anchor_meta, d->dpartials, splits, 256, a_pad, 1.f / d->temperature, grad_scale,
-                                  d->grad_embed, reinterpret_cast<unsigned long long*>(step_counter), stream, d->sync, prev_rows);
+                                  d->grad_embed, reinterpret_cast<unsigned long long*>(step_counter), stream, d->sync, prev_rows,
+                                  d->embed_dtype);
 }
 
 // zero-fill of the step's dense gradient on the engine's fill kernel (the caller picks the stream: a parallel branch)
 extern "C" int pcl_step_fused_fill(const pcl_step_desc* d, void* stream) {
-  if (!d || !d->grad_embed) return PCL_ERR_ARG;
-  const uint64_t bytes = (uint64_t)d->g.B * d->g.D * d->g.h * d->g.w * sizeof(float);
+  if (!d || !d->grad_embed || !pcl::dtype_ok(d->embed_dtype)) return PCL_ERR_ARG;
+  // sized by the gradient's element size: a half gradient is half the bytes (still a multiple of 16: D % 32 == 0)
+  const uint64_t bytes = (uint64_t)d->g.B * d->g.D * d->g.h * d->g.w * pcl::dtype_size(d->embed_dtype);
   if ((bytes & 15) != 0 || ((uintptr_t)d->grad_embed & 15) != 0) return PCL_ERR_UNSUPPORTED;
   // The fill forks right before the fused InfoNCE kernel (at most 8 x 4 = 32 CTAs, one per SM).  Its CTAs OWN their SMs
   // and leave 32 free: the InfoNCE kernel starts at once, next to the fill, instead of waiting for fill CTAs to retire

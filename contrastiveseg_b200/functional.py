@@ -57,6 +57,18 @@ class _on_device:
         return False
 
 
+# Element types the engine reads natively (embed, seg, bank keys): converted to fp32 on load inside the kernels, the
+# dense gradient written in embed's dtype (the fp32 gradient rounded once to nearest-even).
+DTYPE_CODES = {torch.float32: _abi.DT_F32, torch.bfloat16: _abi.DT_BF16, torch.float16: _abi.DT_F16}
+
+
+def dtype_code(t: torch.Tensor, name: str) -> int:
+    code = DTYPE_CODES.get(t.dtype)
+    if code is None:
+        raise _abi.PclError(f"{name} must be float32, bfloat16 or float16, got {t.dtype}")
+    return code
+
+
 def _require_cuda(t: torch.Tensor, name: str) -> None:
     if not t.is_cuda:
         raise _abi.PclError(f"{name} must be a CUDA tensor: the engine has no CPU path")
@@ -316,8 +328,9 @@ class _PixelContrastFn(torch.autograd.Function):
         lib = _abi.load()
         _require_cuda(embed, "embed")
         device = embed.device
-        if embed.dtype != torch.float32:
-            raise _abi.PclError("embed must be float32 (the reference trainer runs without AMP)")
+        embed_dt = dtype_code(embed, "embed")
+        if embed_dt != _abi.DT_F32 and opts.topk_negatives:
+            raise _abi.PclError("topk_negatives needs a float32 embed (the top-k sweeps have no half-precision input)")
         embed_c = embed if embed.is_contiguous() else embed.contiguous()
         labels_c = labels
         if labels.device != device or labels.dtype != torch.int64 or not labels.is_contiguous():
@@ -328,8 +341,10 @@ class _PixelContrastFn(torch.autograd.Function):
         seg_c = pred_c = None
         if seg is not None:
             seg_c = seg.detach()
-            if seg_c.dtype != torch.float32 or not seg_c.is_contiguous():
-                seg_c = seg_c.to(torch.float32).contiguous()
+            if seg_c.dtype not in DTYPE_CODES:          # bf16 / fp16 logits are read as they are (autocast)
+                seg_c = seg_c.to(torch.float32)
+            if not seg_c.is_contiguous():
+                seg_c = seg_c.contiguous()
             if seg_c.shape[0] != B or tuple(seg_c.shape[2:]) != (h, w):
                 raise _abi.PclError("seg must be (B, K, h, w) at the embedding resolution")
         elif predict is not None:
@@ -373,6 +388,9 @@ class _PixelContrastFn(torch.autograd.Function):
         d = ws.desc
         d.embed, d.labels = embed_c.data_ptr(), labels_c.data_ptr()
         d.seg = _abi.ptr(seg_c)
+        # every call: the descriptor is cached with the workspace, an fp32 call after a half one must not inherit its types
+        d.embed_dtype = embed_dt
+        d.seg_dtype = DTYPE_CODES[seg_c.dtype] if seg_c is not None else _abi.DT_F32
         d.predict = _abi.ptr(pred_c)
         d.segment_queue, d.pixel_queue = _abi.ptr(segq_c), _abi.ptr(pixq_c)
         d.temperature, d.base_temperature = opts.temperature, opts.base_temperature
@@ -426,7 +444,7 @@ class _PixelContrastFn(torch.autograd.Function):
                 ctx.topk = None
                 _abi.check(lib.pcl_step_forward(C.byref(d), stream), "pcl_step_forward")
         ctx.ws = ws
-        ctx.embed_shape = tuple(embed_c.shape)
+        ctx.embed_shape, ctx.embed_dtype = tuple(embed_c.shape), embed_c.dtype
         ctx.keep = (embed_c, labels_c, seg_c, pred_c, segq_c, pixq_c, shadow_c)   # keep inputs alive until kernels ran
         if ctx.needs_input_grad[0]:          # (grad mode is always off inside forward: ask the ctx, not torch)
             ws.busy = True
@@ -451,12 +469,13 @@ class _PixelContrastFn(torch.autograd.Function):
         if ctx.keep is None or ws.token != getattr(ctx, "token", None):
             raise _abi.PclError("pixel_contrast_loss: backward ran twice on the same graph (retain_graph=True is not "
                                 "supported: the engine keeps no copy of the forward's scratch); call the loss again")
-        grad = torch.empty(ctx.embed_shape, dtype=torch.float32, device=device)
+        grad = torch.empty(ctx.embed_shape, dtype=ctx.embed_dtype, device=device)     # written in embed's dtype
         go = grad_out
         if go.device != device or go.dtype != torch.float32 or not go.is_contiguous():
             go = go.detach().to(device=device, dtype=torch.float32).contiguous()
         d = ws.desc
         d.grad_embed = grad.data_ptr()
+        d.embed_dtype = DTYPE_CODES[ctx.embed_dtype]
         with _on_device(device):
             if ctx.topk is not None:
                 _topk_step_backward(lib, ws, d, ctx.topk, go, _stream_ptr(device))
@@ -473,8 +492,10 @@ def pixel_contrast_loss(embed: torch.Tensor, labels: torch.Tensor, *, seg: Optio
                         options: Optional[ContrastOptions] = None):
     """Pixel-contrast loss (lib/loss/loss_contrast.py:130-147 / loss_contrast_mem.py:154-171) on the GPU engine.
 
-    embed (B,D,h,w) fp32 CUDA; labels (B,Himg,Wimg) int64; either seg (B,K,h,w) logits (argmax fused) or
-    predict (B,h,w) int64; optional bank queues (K,M,D).  Returns a 0-dim tensor with autograd to embed."""
+    embed (B,D,h,w) fp32, bf16 or fp16 CUDA; labels (B,Himg,Wimg) int64; either seg (B,K,h,w) logits (fp32, bf16 or
+    fp16; argmax fused) or predict (B,h,w) int64; optional bank queues (K,M,D) fp32.  Returns a 0-dim fp32 tensor with
+    autograd to embed; the gradient has embed's dtype.  Half inputs are read in place and converted on load, so loss
+    and gradient equal those of the fp32 copies (the gradient rounded once)."""
     return _PixelContrastFn.apply(embed, labels, seg, predict, segment_queue, pixel_queue, bank_shadow,
                                   options or ContrastOptions())
 

@@ -49,6 +49,16 @@ def _canonical(t: Optional[torch.Tensor], dtype: torch.dtype, name: str, device:
     return t
 
 
+def _canonical_float(t: Optional[torch.Tensor], name: str, device: torch.device) -> Optional[torch.Tensor]:
+    """embed / seg / bank keys: fp32, bf16 or fp16, read in place in their own dtype."""
+    if t is None:
+        return None
+    if t.device != device or t.dtype not in _fn.DTYPE_CODES or not t.is_contiguous():
+        raise _abi.PclError(f"{name} must be a contiguous float32, bfloat16 or float16 tensor on {device}: a captured "
+                            "graph reads it in place on every replay, so no converted copy can be made")
+    return t
+
+
 class GraphedContrastStep:
     """loss, d loss/d embed of ``pixel_contrast_loss`` for fixed tensors, as one CUDA-graph replay.
 
@@ -62,7 +72,8 @@ class GraphedContrastStep:
                  options: Optional[ContrastOptions] = None, grad_scale: float = 1.0, capture: bool = True,
                  warmup: int = 2, overlap_zero_fill: bool = True, enqueue: Optional[dict] = None,
                  fused: Optional[bool] = None, sparse_reset: bool = False):
-        """enqueue (bank steps): dict(bank=MemoryBank, keys=(B,D,h,w) fp32 [default: embed], labels=(B,Himg,Wimg) int64
+        """embed and seg may be fp32, bf16 or fp16 (each independently); ``grad`` has embed's dtype.
+        enqueue (bank steps): dict(bank=MemoryBank, keys=(B,D,h,w) fp32/bf16/fp16 [default: embed], labels=(B,Himg,Wimg) int64
         [default: labels], network_stride=int, pixel_update_freq=int, seed=int, group=process group or None)."""
         self.lib = _abi.load()
         opts = options or ContrastOptions()
@@ -71,9 +82,11 @@ class GraphedContrastStep:
         if opts.rng != "device" or opts.perm_fn is not None:
             raise _abi.PclError("a captured step draws its anchors on the device: rng must be 'device'")
         self.opts = opts
-        self.embed = _canonical(embed.detach(), torch.float32, "embed", device)
+        self.embed = _canonical_float(embed.detach(), "embed", device)
+        if self.embed.dtype != torch.float32 and opts.topk_negatives:
+            raise _abi.PclError("topk_negatives needs a float32 embed (the top-k sweeps have no half-precision input)")
         self.labels = _canonical(labels, torch.int64, "labels", device)
-        self.seg = _canonical(None if seg is None else seg.detach(), torch.float32, "seg", device)
+        self.seg = _canonical_float(None if seg is None else seg.detach(), "seg", device)
         self.predict = _canonical(predict, torch.int64, "predict", device)
         if self.seg is None and self.predict is None:
             raise _abi.PclError("either seg or predict is required")
@@ -102,6 +115,8 @@ class GraphedContrastStep:
         d = self.ws.desc
         d.embed, d.labels = self.embed.data_ptr(), self.labels.data_ptr()
         d.seg, d.predict = _abi.ptr(self.seg), _abi.ptr(self.predict if self.seg is None else None)
+        d.embed_dtype = _fn.DTYPE_CODES[self.embed.dtype]
+        d.seg_dtype = _fn.DTYPE_CODES[self.seg.dtype] if self.seg is not None else _abi.DT_F32
         d.segment_queue, d.pixel_queue = _abi.ptr(self.segq), _abi.ptr(self.pixq)
         d.temperature, d.base_temperature = opts.temperature, opts.base_temperature
         d.nan_safe, d.normalize = int(opts.nan_safe), int(opts.normalize)
@@ -168,7 +183,7 @@ class GraphedContrastStep:
         if self.segq is None or bank.segment_queue.data_ptr() != self.segq.data_ptr():
             raise _abi.PclError("enqueue=: the step must read the bank it writes (pass bank.segment_queue / pixel_queue)")
         dev = self.device
-        keys = _canonical(e.get("keys", self.embed).detach(), torch.float32, "keys", dev)
+        keys = _canonical_float(e.get("keys", self.embed).detach(), "keys", dev)
         labels = _canonical(e.get("labels", self.labels), torch.int64, "lb_key", dev)
         B, D, h, w = keys.shape
         g = _abi.BankGeom(B, D, h, w, labels.shape[1], labels.shape[2], bank.num_classes, bank.memory_size,
@@ -192,7 +207,14 @@ class GraphedContrastStep:
 
     def _enqueue_packet(self, stream: int) -> None:
         q = self.enq
-        _abi.check(self.lib.pcl_bank_packet_dev(C.byref(q["g"]), q["keys"].data_ptr(), q["labels"].data_ptr(), q["seed"],
+        keys = q["keys"]
+        if keys.dtype != torch.float32:        # bf16 / fp16 keys: converted on load, same packet as from fp32 keys
+            _abi.check(self.lib.pcl_bank_packet_dev_dt(C.byref(q["g"]), keys.data_ptr(), _fn.DTYPE_CODES[keys.dtype],
+                                                       q["labels"].data_ptr(), q["seed"], self.enq_counter.data_ptr(),
+                                                       q["scratch"].data_ptr(), q["packet"].data_ptr(), stream),
+                       "pcl_bank_packet_dev_dt")
+            return
+        _abi.check(self.lib.pcl_bank_packet_dev(C.byref(q["g"]), keys.data_ptr(), q["labels"].data_ptr(), q["seed"],
                                                 self.enq_counter.data_ptr(), q["scratch"].data_ptr(), q["packet"].data_ptr(),
                                                 stream), "pcl_bank_packet_dev")
 

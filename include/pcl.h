@@ -45,6 +45,10 @@ typedef enum {
 enum { PCL_PLAN_TC = 0, PCL_PLAN_V = 1, PCL_PLAN_A = 2, PCL_PLAN_FLAGS = 3, PCL_PLAN_NPAIR_MAX = 4 };
 /* PCL_PLAN_FLAGS bits */
 enum { PCL_FLAG_NO_CLASS = 1, PCL_FLAG_ZERO_VIEWS = 2, PCL_FLAG_SPLIT_ERROR = 4 };
+/* Element type of an input that may be half precision (pcl_step_desc.embed_dtype / seg_dtype, pcl_bank_packet_dt).
+ * Half inputs are converted to fp32 on load (exact) and everything downstream computes in fp32 as for fp32 inputs; a
+ * half dense gradient is the fp32 gradient rounded once to nearest-even. */
+enum { PCL_DT_F32 = 0, PCL_DT_BF16 = 1, PCL_DT_F16 = 2 };
 
 int         pcl_version(void);
 const char* pcl_strerror(int status);
@@ -260,6 +264,13 @@ int pcl_bank_packet(const pcl_bank_geom* g, const float* keys, const int64_t* la
 int pcl_bank_packet_dev(const pcl_bank_geom* g, const float* keys, const int64_t* labels, uint64_t seed,
                         const uint64_t* seed_offset, float* scratch, float* packet, void* stream);
 
+/* The two calls above for keys of element type keys_dtype (PCL_DT_*; bf16 / fp16 keys are converted on load, the
+ * packet is fp32 and bit-identical to the one built from the keys converted to fp32). */
+int pcl_bank_packet_dt(const pcl_bank_geom* g, const void* keys, int32_t keys_dtype, const int64_t* labels,
+                       const int32_t* ranks, uint64_t seed, float* scratch, float* packet, void* stream);
+int pcl_bank_packet_dev_dt(const pcl_bank_geom* g, const void* keys, int32_t keys_dtype, const int64_t* labels,
+                           uint64_t seed, const uint64_t* seed_offset, float* scratch, float* packet, void* stream);
+
 /* Apply `world` packets (contiguous, rank-major) to the queues in place, with the result of the reference's sequential
  * per-image loop over the gathered batch (trainer_contrastive.py:96-139): every queue row is written once, by the LAST
  * of the world * B slots that would have written it.  world * B <= 1024 (PCL_ERR_UNSUPPORTED otherwise).
@@ -366,6 +377,10 @@ typedef struct {
                                   * Non-NULL: pcl_step_stats runs as ONE launch (plan folded into the scan's last block).
                                   * Words [0,8): counters; word 7 != 0 turns on the diagnostic timeline in words [16,1024)
                                   * (csrc/pcl_common.cuh: per-kernel min start / max end of %globaltimer) */
+  /* element types (PCL_DT_*; 0 = fp32, so a zero-initialised descriptor reads fp32).  embed_dtype != 0: `embed` and
+   * `grad_embed` point to 2-byte elements; seg_dtype != 0: `seg` does.  The sampled anchors, the loss and every scratch
+   * buffer stay fp32. */
+  int32_t embed_dtype, seg_dtype;
 } pcl_step_desc;
 
 int pcl_step_stats(const pcl_step_desc* d, void* stream);      /* pcl_class_stats + pcl_plan_anchors      */
@@ -412,7 +427,8 @@ int pcl_step_fused_select(const pcl_step_desc* d, const uint64_t* step_counter, 
 int pcl_step_fused_loss(const pcl_step_desc* d, void* stream);
 int pcl_step_fused_scatter(const pcl_step_desc* d, const float* grad_scale, uint64_t* step_counter, int32_t* prev_rows,
                            void* stream);
-int pcl_step_fused_fill(const pcl_step_desc* d, void* stream);   /* zero-fill of d->grad_embed (B*D*h*w floats) */
+int pcl_step_fused_fill(const pcl_step_desc* d, void* stream);   /* zero-fill of d->grad_embed (B*D*h*w elements of
+                                                                    d->embed_dtype) */
 /* Zero-fill `bytes` (multiple of 16, 16-byte aligned) with 16-byte stores on the engine's own fill kernel. */
 int pcl_fill_zero(void* ptr, uint64_t bytes, void* stream);
 
