@@ -105,6 +105,8 @@ SIGNATURES = {
     "pcl_proj_pack": (c_i32, [c_vp, c_i32, c_vp, c_vp]),
     "pcl_proj_fwd": (c_i32, [c_vp, c_vp, c_vp, c_i32, c_i32, c_i64, c_vp, c_vp, c_vp]),
     "pcl_proj_bwd": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "pcl_proj_fwd_dt": (c_i32, [c_vp, c_i32, c_vp, c_vp, c_i32, c_i32, c_i64, c_vp, c_vp, c_vp]),
+    "pcl_proj_bwd_dt": (c_i32, [c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "pcl_seg_ce_scratch_floats": (c_i64, [c_i32, c_i32, c_i32]),
     "pcl_seg_ce_fwd": (c_i32, [c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_vp, c_vp, c_vp]),
     "pcl_seg_ce_bwd": (c_i32, [c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_vp, c_vp, c_vp,

@@ -109,8 +109,13 @@ extern "C" int pcl_l2norm_bwd(const float* x, const float* gy, float* gx, int32_
 //                  the threads into the MN-major layout.  Channel Cin of the converted tile is 1 (valid pixels), so
 //                  column Cin of the product is gb = sum_p gz[:, p].
 //   k_proj_reduce  fixed-order sum of the split partials -> gW, gb (bit-reproducible).
-// Pixel tiles never straddle images, so any H x W works; the fp32 activations are read with scalar loads (per-image
-// rows of HW floats are not 16-byte aligned in general), coalesced along the pixel dimension.
+// Pixel tiles never straddle images, so any H x W works; the activations are read with scalar loads (per-image rows of
+// HW elements are not 16-byte aligned in general), coalesced along the pixel dimension.
+// Activation element type T (x, zn, gzn, gx) is float or __nv_bfloat16.  bf16 x goes into the bf16 operand tile as its
+// raw bits (what the fp32 path's round-to-bf16 gives for the same values), zn and gzn convert to fp32 on load (exact),
+// and every sum runs in fp32 in the same order for both, so a bf16 call computes what the fp32 call computes on the
+// converted inputs; bf16 zn and gx are the fp32 values rounded once to nearest-even.  inv_norm, the bf16 gz workspace,
+// the split-K partials, gW and gb are fp32 / bf16 alike for both types.
 
 namespace pcl {
 namespace proj {
@@ -179,8 +184,15 @@ __device__ __forceinline__ float inv_norm_of(float ss) {
   return r < NORM_EPS_INV ? r : NORM_EPS_INV;
 }
 
-// 8 channels [c, c + 8) of pixel p of one fp32 NCHW image -> v.  Channels >= Cin read as 0, channel `ones` as 1 (the
-// wgrad's bias column); pixels >= HW read as 0.  Nothing beyond the tensor is dereferenced.
+// One channel value of the activation tile between its load and its store into the swizzled bf16 tile: fp32 values are
+// rounded to bf16 at the store; a bf16 activation already is the GEMM operand, so its raw 16 bits are carried through
+// unconverted (bf16 -> fp32 -> bf16 would be the identity).  Keeping the raw bits also keeps every load of a K-block
+// independent of any arithmetic until the tile store, so all of them are in flight together as in the fp32 path.
+template <class T> struct Staged { using type = float; };
+template <> struct Staged<__nv_bfloat16> { using type = uint16_t; };
+
+// 8 channels [c, c + 8) of pixel p of one NCHW image -> v.  Channels >= Cin read as 0, channel `ones` as 1 (the wgrad's
+// bias column); pixels >= HW read as 0.  Nothing beyond the tensor is dereferenced.
 __device__ __forceinline__ void load8(const float* __restrict__ img, int Cin, int64_t HW, int c, int64_t p, int ones,
                                       float (&v)[8]) {
   const bool pv = p < HW;
@@ -190,11 +202,28 @@ __device__ __forceinline__ void load8(const float* __restrict__ img, int Cin, in
     v[i] = (pv && ch < Cin) ? img[(int64_t)ch * HW + p] : ((pv && ch == ones) ? 1.f : 0.f);
   }
 }
+__device__ __forceinline__ void load8(const __nv_bfloat16* __restrict__ img, int Cin, int64_t HW, int c, int64_t p,
+                                      int ones, uint16_t (&v)[8]) {
+  constexpr uint16_t BF16_ONE = 0x3F80;
+  const uint16_t* __restrict__ bits = reinterpret_cast<const uint16_t*>(img);
+  const bool pv = p < HW;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const int ch = c + i;
+    v[i] = (pv && ch < Cin) ? bits[(int64_t)ch * HW + p] : ((pv && ch == ones) ? BF16_ONE : (uint16_t)0);
+  }
+}
 // 8 values -> one 16-byte chunk of a 128B-swizzled row (row `r` of a 1024-aligned tile, chunk index `ch` in [0, 8))
 __device__ __forceinline__ void store8(uint8_t* tile, int r, int ch, const float (&v)[8]) {
   uint4 u;
   u.x = pack_bf16x2(v[0], v[1]); u.y = pack_bf16x2(v[2], v[3]);
   u.z = pack_bf16x2(v[4], v[5]); u.w = pack_bf16x2(v[6], v[7]);
+  *reinterpret_cast<uint4*>(tile + r * 128 + ((ch ^ (r & 7)) << 4)) = u;
+}
+__device__ __forceinline__ void store8(uint8_t* tile, int r, int ch, const uint16_t (&v)[8]) {
+  uint4 u;
+  u.x = v[0] | ((uint32_t)v[1] << 16); u.y = v[2] | ((uint32_t)v[3] << 16);
+  u.z = v[4] | ((uint32_t)v[5] << 16); u.w = v[6] | ((uint32_t)v[7] << 16);
   *reinterpret_cast<uint4*>(tile + r * 128 + ((ch ^ (r & 7)) << 4)) = u;
 }
 
@@ -210,18 +239,20 @@ __global__ void k_proj_pack(const float* __restrict__ w, int Cin, int cin64, int
 }
 
 // ------------------------------------------------------------------------------------------------------------------
+template <class T>
 struct FwdArgs {
-  const float* x; const float* bias; float* zn; float* inv_norm;
+  const T* x; const float* bias; T* zn; float* inv_norm;
   int Cin, nkb; int64_t HW; int tiles_per_img;
 };
 
-__global__ void __launch_bounds__(NT, 1) k_proj_fwd(const __grid_constant__ CUtensorMap tmW, FwdArgs a) {
+template <class T>
+__global__ void __launch_bounds__(NT, 1) k_proj_fwd(const __grid_constant__ CUtensorMap tmW, FwdArgs<T> a) {
   extern __shared__ uint8_t smem_raw[];
   FwdSmem& sm = aligned_smem<FwdSmem>(smem_raw);
   const int t = threadIdx.x, g = t >> 7, lane = t & 31, wt = t & 127;
   const int b = blockIdx.x / a.tiles_per_img;
   const int64_t p0 = (int64_t)(blockIdx.x - b * a.tiles_per_img) * BM;
-  const float* img = a.x + (int64_t)b * a.Cin * a.HW;
+  const T* img = a.x + (int64_t)b * a.Cin * a.HW;
   if (t == 0) {
     ptx::prefetch_tmap(&tmW);
     for (int s = 0; s < FWD_WSTAGES; ++s) ptx::mbar_init(&sm.full[s], 1);
@@ -235,7 +266,7 @@ __global__ void __launch_bounds__(NT, 1) k_proj_fwd(const __grid_constant__ CUte
       ptx::tma_load_2d(sm.w[kb], &tmW, &sm.full[kb], kb * BK, 0);
     }
   // conversion items of this thread: pixel row wt, 16-byte channel chunks g, g + 2, g + 4, g + 6 of each K-block
-  float v[4][8];
+  typename Staged<T>::type v[4][8];
 #pragma unroll
   for (int j = 0; j < 4; ++j) load8(img, a.Cin, a.HW, 8 * (g + 2 * j), p0 + wt, -1, v[j]);
 #pragma unroll
@@ -276,7 +307,14 @@ __global__ void __launch_bounds__(NT, 1) k_proj_fwd(const __grid_constant__ CUte
 
   // epilogue on the fragment: acc[4 i + 2 h + e] = pixel fr + 8 h of the warpgroup, channel 8 i + 2 q + e
   const int fr = 16 * (wt >> 5) + (lane >> 2), q = lane & 3;
-  float* out = a.zn + (int64_t)b * DOUT * a.HW;
+  T* out = a.zn + (int64_t)b * DOUT * a.HW;
+  // 2-byte zn: straight from the fragment a warp store would write 16-byte pieces of 4 channel rows; instead the tile
+  // is staged [channel][pixel] in the retired weight stages and written out along pixels, 64 contiguous bytes per warp
+  // store.  The row pitch of ZS_LD elements (68 words) spreads a fragment store's 4 channel pairs over distinct banks.
+  constexpr int ZS_LD = BM + 8;
+  static_assert(DOUT * ZS_LD * 2 <= sizeof(FwdSmem::w), "zn staging tile fits the weight stages");
+  T* stage = reinterpret_cast<T*>(sm.w[0]);
+  if constexpr (sizeof(T) == 2) __syncthreads();      // both warpgroups' last wgmma has read sm.w
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     float ss = 0.f;
@@ -292,21 +330,42 @@ __global__ void __launch_bounds__(NT, 1) k_proj_fwd(const __grid_constant__ CUte
     const int64_t p = p0 + g * 64 + fr + 8 * h;
     if (p < a.HW) {
       if (q == 0) a.inv_norm[(int64_t)b * a.HW + p] = inv;
+      if constexpr (sizeof(T) == 4) {
+#pragma unroll
+        for (int i = 0; i < 32; ++i)
+#pragma unroll
+          for (int e = 0; e < 2; ++e)
+            out[(int64_t)(8 * i + 2 * q + e) * a.HW + p] = from_f32<T>(acc[4 * i + 2 * h + e] * inv);
+      }
+    }
+    if constexpr (sizeof(T) == 2) {
 #pragma unroll
       for (int i = 0; i < 32; ++i)
 #pragma unroll
-        for (int e = 0; e < 2; ++e) out[(int64_t)(8 * i + 2 * q + e) * a.HW + p] = acc[4 * i + 2 * h + e] * inv;
+        for (int e = 0; e < 2; ++e)
+          stage[(8 * i + 2 * q + e) * ZS_LD + g * 64 + fr + 8 * h] = from_f32<T>(acc[4 * i + 2 * h + e] * inv);
     }
+  }
+  if constexpr (sizeof(T) == 2) {
+    __syncthreads();
+    for (int c = t >> 5; c < DOUT; c += NT / 32)
+#pragma unroll
+      for (int j = 0; j < BM / 32; ++j) {
+        const int px = 32 * j + lane;
+        if (p0 + px < a.HW) out[(int64_t)c * a.HW + p0 + px] = stage[c * ZS_LD + px];
+      }
   }
 }
 
 // ------------------------------------------------------------------------------------------------------------------
+template <class T>
 struct DgradArgs {
-  const float* zn; const float* gzn; const float* inv_norm; float* gx; __nv_bfloat16* gz;
+  const T* zn; const T* gzn; const float* inv_norm; T* gx; __nv_bfloat16* gz;
   int Cin, npass; int64_t HW, HWp; int tiles_per_img;
 };
 
-__global__ void __launch_bounds__(NT, 1) k_proj_dgrad(const __grid_constant__ CUtensorMap tmWt, DgradArgs a) {
+template <class T>
+__global__ void __launch_bounds__(NT, 1) k_proj_dgrad(const __grid_constant__ CUtensorMap tmWt, DgradArgs<T> a) {
   extern __shared__ uint8_t smem_raw[];
   DgradSmem& sm = aligned_smem<DgradSmem>(smem_raw);
   const int t = threadIdx.x, g = t >> 7, lane = t & 31, wt = t & 127;
@@ -335,8 +394,8 @@ __global__ void __launch_bounds__(NT, 1) k_proj_dgrad(const __grid_constant__ CU
 #pragma unroll
       for (int i = 0; i < 32; ++i) {
         const int64_t o = img + (int64_t)(32 * grp + i) * a.HW + p;
-        z[i] = pv ? a.zn[o] : 0.f;
-        gy[i] = pv ? a.gzn[o] : 0.f;
+        z[i] = pv ? to_f32(a.zn[o]) : 0.f;
+        gy[i] = pv ? to_f32(a.gzn[o]) : 0.f;
       }
 #pragma unroll
       for (int i = 0; i < 32; ++i) dot = fmaf(z[i], gy[i], dot);
@@ -368,7 +427,7 @@ __global__ void __launch_bounds__(NT, 1) k_proj_dgrad(const __grid_constant__ CU
 
   const int fr = 16 * (wt >> 5) + (lane >> 2), q = lane & 3;
   const uint32_t a_base = ptx::smem_u32(sm.a[0]) + g * WG_ROWS_BYTES, w_base = ptx::smem_u32(sm.wt[0]);
-  float* gx = a.gx + (int64_t)b * a.Cin * a.HW;
+  T* gx = a.gx + (int64_t)b * a.Cin * a.HW;
   float acc[128];
   for (int np = 0; np < a.npass; ++np) {
     wait_full(&sm.full, (uint32_t)np & 1u);
@@ -394,7 +453,7 @@ __global__ void __launch_bounds__(NT, 1) k_proj_dgrad(const __grid_constant__ CU
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
             const int c = np * DOUT + 8 * i + 2 * q + e;
-            if (c < a.Cin) gx[(int64_t)c * a.HW + p] = acc[4 * i + 2 * h + e];
+            if (c < a.Cin) gx[(int64_t)c * a.HW + p] = from_f32<T>(acc[4 * i + 2 * h + e]);
           }
       }
     }
@@ -402,12 +461,14 @@ __global__ void __launch_bounds__(NT, 1) k_proj_dgrad(const __grid_constant__ CU
 }
 
 // ------------------------------------------------------------------------------------------------------------------
+template <class T>
 struct WgradArgs {
-  const float* x; float* partials;
+  const T* x; float* partials;
   int Cin, ldp; int64_t HW; int blk_per_img; int64_t units; int splits;
 };
 
-__global__ void __launch_bounds__(NT, 1) k_proj_wgrad(const __grid_constant__ CUtensorMap tmG, WgradArgs a) {
+template <class T>
+__global__ void __launch_bounds__(NT, 1) k_proj_wgrad(const __grid_constant__ CUtensorMap tmG, WgradArgs<T> a) {
   extern __shared__ uint8_t smem_raw[];
   WgradSmem& sm = aligned_smem<WgradSmem>(smem_raw);
   const int t = threadIdx.x, g = t >> 7, lane = t & 31, wt = t & 127;
@@ -426,10 +487,10 @@ __global__ void __launch_bounds__(NT, 1) k_proj_wgrad(const __grid_constant__ CU
   };
   // conversion items: pixel row (t & 63) of the block, 16-byte channel chunks (t >> 6) + 4 j, j < 8 (32 chunks = 256 ch)
   const int pr = t & 63, cg = t >> 6;
-  float v[8][8];
+  typename Staged<T>::type v[8][8];
   auto load_b = [&](int64_t u) {
     const int bb = (int)(u / a.blk_per_img), pb = (int)(u - (int64_t)bb * a.blk_per_img);
-    const float* img = a.x + (int64_t)bb * a.Cin * a.HW;
+    const T* img = a.x + (int64_t)bb * a.Cin * a.HW;
 #pragma unroll
     for (int j = 0; j < 8; ++j) load8(img, a.Cin, a.HW, c0 + 8 * (cg + 4 * j), (int64_t)pb * WB + pr, a.Cin, v[j]);
   };
@@ -553,27 +614,42 @@ extern "C" int pcl_proj_pack(const float* weight, int32_t Cin, void* wpack, void
   return PCL_OK;
 }
 
-extern "C" int pcl_proj_fwd(const float* x, const void* wpack, const float* bias, int32_t B, int32_t Cin, int64_t HW,
-                            float* zn, float* inv_norm, void* stream) {
+template <class T>
+static int proj_fwd(const T* x, const void* wpack, const float* bias, int32_t B, int32_t Cin, int64_t HW, T* zn,
+                    float* inv_norm, void* stream) {
   PCL_REQUIRE(x && wpack && zn && inv_norm && proj::shape_ok(B, Cin, HW));
   const proj::Layout L = proj::layout(B, Cin, HW);
   CUtensorMap tmW;
   int st = tc_make_tmap_cols(&tmW, wpack, (uint64_t)L.cin64, proj::DOUT, proj::DOUT);
   if (st != PCL_OK) return st;
-  proj::FwdArgs a;
+  proj::FwdArgs<T> a;
   a.x = x; a.bias = bias; a.zn = zn; a.inv_norm = inv_norm;
   a.Cin = Cin; a.nkb = L.cin64 / proj::BK; a.HW = HW;
   a.tiles_per_img = (int)ceil_div64(HW, proj::BM);
   const size_t smem = sizeof(proj::FwdSmem) + 1024;
-  PCL_SMEM_OPT_IN(proj::k_proj_fwd, smem);
-  proj::k_proj_fwd<<<(unsigned)(B * a.tiles_per_img), proj::NT, smem, (cudaStream_t)stream>>>(tmW, a);
+  PCL_SMEM_OPT_IN(proj::k_proj_fwd<T>, smem);
+  proj::k_proj_fwd<T><<<(unsigned)(B * a.tiles_per_img), proj::NT, smem, (cudaStream_t)stream>>>(tmW, a);
   PCL_LAUNCH_CHECK();
   return PCL_OK;
 }
 
-extern "C" int pcl_proj_bwd(const float* x, const float* zn, const float* inv_norm, const float* gzn, const void* wpack,
-                            int32_t B, int32_t Cin, int64_t HW, void* scratch, float* gx, float* gw, float* gb,
-                            void* stream) {
+extern "C" int pcl_proj_fwd(const float* x, const void* wpack, const float* bias, int32_t B, int32_t Cin, int64_t HW,
+                            float* zn, float* inv_norm, void* stream) {
+  return pcl_proj_fwd_dt(x, PCL_DT_F32, wpack, bias, B, Cin, HW, zn, inv_norm, stream);
+}
+
+extern "C" int pcl_proj_fwd_dt(const void* x, int32_t dtype, const void* wpack, const float* bias, int32_t B,
+                               int32_t Cin, int64_t HW, void* zn, float* inv_norm, void* stream) {
+  if (dtype == PCL_DT_F32)
+    return proj_fwd((const float*)x, wpack, bias, B, Cin, HW, (float*)zn, inv_norm, stream);
+  if (dtype == PCL_DT_BF16)
+    return proj_fwd((const __nv_bfloat16*)x, wpack, bias, B, Cin, HW, (__nv_bfloat16*)zn, inv_norm, stream);
+  return PCL_ERR_ARG;                    // fp16 would be rounded to the bf16 GEMM operands: not offered
+}
+
+template <class T>
+static int proj_bwd(const T* x, const T* zn, const float* inv_norm, const T* gzn, const void* wpack, int32_t B,
+                    int32_t Cin, int64_t HW, void* scratch, T* gx, float* gw, float* gb, void* stream) {
   PCL_REQUIRE(x && zn && inv_norm && gzn && wpack && scratch && gx && gw && proj::shape_ok(B, Cin, HW));
   const proj::Layout L = proj::layout(B, Cin, HW);
   cudaStream_t s = (cudaStream_t)stream;
@@ -586,25 +662,43 @@ extern "C" int pcl_proj_bwd(const float* x, const float* zn, const float* inv_no
   st = tc_make_tmap_cols(&tmG, gz, (uint64_t)L.HWp, (uint64_t)B * proj::DOUT, 128);
   if (st != PCL_OK) return st;
 
-  proj::DgradArgs d;
+  proj::DgradArgs<T> d;
   d.zn = zn; d.gzn = gzn; d.inv_norm = inv_norm; d.gx = gx; d.gz = gz;
   d.Cin = Cin; d.npass = L.cin256 / proj::DOUT; d.HW = HW; d.HWp = L.HWp;
   d.tiles_per_img = (int)ceil_div64(HW, proj::BM);
   const size_t smem_d = sizeof(proj::DgradSmem) + 1024;
-  PCL_SMEM_OPT_IN(proj::k_proj_dgrad, smem_d);
-  proj::k_proj_dgrad<<<(unsigned)(B * d.tiles_per_img), proj::NT, smem_d, s>>>(tmWt, d);
+  PCL_SMEM_OPT_IN(proj::k_proj_dgrad<T>, smem_d);
+  proj::k_proj_dgrad<T><<<(unsigned)(B * d.tiles_per_img), proj::NT, smem_d, s>>>(tmWt, d);
   PCL_LAUNCH_CHECK();
 
-  proj::WgradArgs w;
+  proj::WgradArgs<T> w;
   w.x = x; w.partials = part; w.Cin = Cin; w.ldp = L.ldp; w.HW = HW; w.blk_per_img = L.blk_per_img;
   w.units = L.units; w.splits = L.splits;
   const size_t smem_w = sizeof(proj::WgradSmem) + 1024;
-  PCL_SMEM_OPT_IN(proj::k_proj_wgrad, smem_w);
-  proj::k_proj_wgrad<<<dim3(proj::DOUT / 128, L.ctiles, L.splits), proj::NT, smem_w, s>>>(tmG, w);
+  PCL_SMEM_OPT_IN(proj::k_proj_wgrad<T>, smem_w);
+  proj::k_proj_wgrad<T><<<dim3(proj::DOUT / 128, L.ctiles, L.splits), proj::NT, smem_w, s>>>(tmG, w);
   PCL_LAUNCH_CHECK();
 
   const int64_t n = (int64_t)proj::DOUT * (Cin + 1);
   proj::k_proj_reduce<<<(unsigned)ceil_div64(n, 256), 256, 0, s>>>(part, L.splits, Cin, L.ldp, gw, gb);
   PCL_LAUNCH_CHECK();
   return PCL_OK;
+}
+
+extern "C" int pcl_proj_bwd(const float* x, const float* zn, const float* inv_norm, const float* gzn, const void* wpack,
+                            int32_t B, int32_t Cin, int64_t HW, void* scratch, float* gx, float* gw, float* gb,
+                            void* stream) {
+  return pcl_proj_bwd_dt(x, PCL_DT_F32, zn, inv_norm, gzn, wpack, B, Cin, HW, scratch, gx, gw, gb, stream);
+}
+
+extern "C" int pcl_proj_bwd_dt(const void* x, int32_t dtype, const void* zn, const float* inv_norm, const void* gzn,
+                               const void* wpack, int32_t B, int32_t Cin, int64_t HW, void* scratch, void* gx, float* gw,
+                               float* gb, void* stream) {
+  if (dtype == PCL_DT_F32)
+    return proj_bwd((const float*)x, (const float*)zn, inv_norm, (const float*)gzn, wpack, B, Cin, HW, scratch,
+                    (float*)gx, gw, gb, stream);
+  if (dtype == PCL_DT_BF16)
+    return proj_bwd((const __nv_bfloat16*)x, (const __nv_bfloat16*)zn, inv_norm, (const __nv_bfloat16*)gzn, wpack, B,
+                    Cin, HW, scratch, (__nv_bfloat16*)gx, gw, gb, stream);
+  return PCL_ERR_ARG;
 }

@@ -647,28 +647,43 @@ def _proj_dims(x: torch.Tensor, weight: torch.Tensor):
     return B, Cin, H * W
 
 
+# activation dtypes of the fused head -> PCL_DT_* code (fp16 is refused: its values would be rounded to the bf16 operands)
+_PROJ_DTYPES = {torch.float32: _abi.DT_F32, torch.bfloat16: _abi.DT_BF16}
+
+
+def proj_dtype_code(dtype: torch.dtype, what: str = "project_normalize") -> int:
+    """PCL_DT_* code of a fused-head activation dtype; PclError for anything but float32 / bfloat16."""
+    code = _PROJ_DTYPES.get(dtype)
+    if code is None:
+        raise _abi.PclError(f"{what}: x must be float32 or bfloat16, got {dtype}")
+    return code
+
+
 class _ProjNormFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, weight, bias):
         lib = _abi.load()
         _require_cuda(x, "x")
-        if x.dtype != torch.float32:
-            raise _abi.PclError(f"project_normalize: x must be float32, got {x.dtype}")
+        dt = proj_dtype_code(x.dtype)
         B, Cin, HW = _proj_dims(x, weight)
         dev = x.device
         xc = x.contiguous()
         w = weight.detach().to(device=dev, dtype=torch.float32).reshape(PROJ_DIM, Cin).contiguous()
         bc = None if bias is None else bias.detach().to(device=dev, dtype=torch.float32).contiguous()
         wpack = torch.empty(lib.pcl_proj_workspace_bytes(B, Cin, HW, 0), dtype=torch.uint8, device=dev)
-        zn = torch.empty((B, PROJ_DIM) + tuple(x.shape[2:]), dtype=torch.float32, device=dev)
+        zn = torch.empty((B, PROJ_DIM) + tuple(x.shape[2:]), dtype=x.dtype, device=dev)
         inv = torch.empty(B * HW, dtype=torch.float32, device=dev)
         with _on_device(dev):
             s = _stream_ptr(dev)
             _abi.check(lib.pcl_proj_pack(w.data_ptr(), Cin, wpack.data_ptr(), s), "pcl_proj_pack")
-            _abi.check(lib.pcl_proj_fwd(xc.data_ptr(), wpack.data_ptr(), _abi.ptr(bc), B, Cin, HW, zn.data_ptr(),
-                                        inv.data_ptr(), s), "pcl_proj_fwd")
+            if dt == _abi.DT_F32:
+                _abi.check(lib.pcl_proj_fwd(xc.data_ptr(), wpack.data_ptr(), _abi.ptr(bc), B, Cin, HW, zn.data_ptr(),
+                                            inv.data_ptr(), s), "pcl_proj_fwd")
+            else:
+                _abi.check(lib.pcl_proj_fwd_dt(xc.data_ptr(), dt, wpack.data_ptr(), _abi.ptr(bc), B, Cin, HW,
+                                               zn.data_ptr(), inv.data_ptr(), s), "pcl_proj_fwd_dt")
         ctx.save_for_backward(xc, zn, inv, wpack)
-        ctx.dims = (B, Cin, HW, tuple(weight.shape), bias is not None)
+        ctx.dims = (B, Cin, HW, tuple(weight.shape), bias is not None, dt)
         return zn
 
     @staticmethod
@@ -676,24 +691,31 @@ class _ProjNormFn(torch.autograd.Function):
     def backward(ctx, gzn):
         lib = _abi.load()
         xc, zn, inv, wpack = ctx.saved_tensors
-        B, Cin, HW, wshape, has_bias = ctx.dims
+        B, Cin, HW, wshape, has_bias, dt = ctx.dims
         dev = xc.device
-        g = gzn.to(device=dev, dtype=torch.float32).contiguous()
+        g = gzn.to(device=dev, dtype=zn.dtype).contiguous()
         scratch = torch.empty(lib.pcl_proj_workspace_bytes(B, Cin, HW, 1), dtype=torch.uint8, device=dev)
         gx = torch.empty_like(xc)
         gw = torch.empty((PROJ_DIM, Cin), dtype=torch.float32, device=dev)
         gb = torch.empty(PROJ_DIM, dtype=torch.float32, device=dev) if has_bias else None
         with _on_device(dev):
-            _abi.check(lib.pcl_proj_bwd(xc.data_ptr(), zn.data_ptr(), inv.data_ptr(), g.data_ptr(), wpack.data_ptr(), B,
-                                        Cin, HW, scratch.data_ptr(), gx.data_ptr(), gw.data_ptr(), _abi.ptr(gb),
-                                        _stream_ptr(dev)), "pcl_proj_bwd")
+            if dt == _abi.DT_F32:
+                _abi.check(lib.pcl_proj_bwd(xc.data_ptr(), zn.data_ptr(), inv.data_ptr(), g.data_ptr(), wpack.data_ptr(),
+                                            B, Cin, HW, scratch.data_ptr(), gx.data_ptr(), gw.data_ptr(), _abi.ptr(gb),
+                                            _stream_ptr(dev)), "pcl_proj_bwd")
+            else:
+                _abi.check(lib.pcl_proj_bwd_dt(xc.data_ptr(), dt, zn.data_ptr(), inv.data_ptr(), g.data_ptr(),
+                                               wpack.data_ptr(), B, Cin, HW, scratch.data_ptr(), gx.data_ptr(),
+                                               gw.data_ptr(), _abi.ptr(gb), _stream_ptr(dev)), "pcl_proj_bwd_dt")
         return gx, gw.view(wshape), gb
 
 
 def project_normalize(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor] = None) -> torch.Tensor:
     """F.normalize(F.conv2d(x, weight, bias), p=2, dim=1) for a 1x1 convolution to 256 channels, as one bf16 wgmma GEMM
     with the normalise in its epilogue (fp32 accumulate; backward: gz in bf16, split-K weight gradient reduced in a
-    fixed order).  x (B, Cin, H, W) fp32 CUDA, weight (256, Cin, 1, 1), bias (256) or None."""
+    fixed order).  x (B, Cin, H, W) fp32 or bf16 CUDA, weight (256, Cin, 1, 1), bias (256) or None.  zn and x's
+    gradient have x's dtype; a bf16 x computes exactly what x.float() computes, with zn and the gradient rounded once to
+    bf16.  The autocast state is not consulted: the dtype of x decides."""
     return _ProjNormFn.apply(x, weight, bias)
 
 

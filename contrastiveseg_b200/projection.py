@@ -3,12 +3,13 @@
 By default the 1x1 convolutions / BatchNorm stay cuDNN / PyTorch and only the final F.normalize(p=2, dim=1) runs on
 the engine kernel.  ``fused=True`` runs the last Conv2d (Cin -> 256) and the normalise as one wgmma GEMM with the
 normalise in its epilogue (functional.project_normalize, bf16 operands, fp32 accumulate); the 720 -> 720 conv, BN and
-ReLU of ``convmlp`` still run in torch.  The module tree and state_dict keys are the same either way.
+ReLU of ``convmlp`` still run in torch.  The fused head takes a float32 or bfloat16 input; the dtype of the tensor
+reaching the last conv decides the output's (under ``torch.autocast(dtype=torch.bfloat16)`` the ``convmlp`` prefix
+hands it bf16, so zn is bf16).  The module tree and state_dict keys are the same either way.
 ``normalize=False`` returns the raw projection for the fused loss path (PixelContrastLoss(..., normalize=True) then
 normalises only the sampled columns)."""
 from __future__ import annotations
 
-import torch
 import torch.nn as nn
 
 from . import functional as _fn
@@ -37,12 +38,13 @@ class ProjectionHead(nn.Module):
     def forward(self, x):
         if self.fused:
             _fn._require_cuda(x, "x")
-            if x.dtype != torch.float32:
-                raise PclError(f"ProjectionHead(fused=True) needs a float32 input, got {x.dtype}")
+            _fn.proj_dtype_code(x.dtype, "ProjectionHead(fused=True)")
             if isinstance(self.proj, nn.Conv2d):
                 last, y = self.proj, x
             else:
                 last, y = self.proj[-1], self.proj[:-1](x)
+            # the tensor reaching the fused conv decides zn's dtype: bf16 under autocast for convmlp
+            _fn.proj_dtype_code(y.dtype, "ProjectionHead(fused=True)")
             return project_normalize(y, last.weight, last.bias)
         y = self.proj(x)
         return l2_normalize(y) if self.normalize else y

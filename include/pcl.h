@@ -220,6 +220,18 @@ int pcl_proj_fwd(const float* x, const void* wpack, const float* bias, int32_t B
 int pcl_proj_bwd(const float* x, const float* zn, const float* inv_norm, const float* gzn, const void* wpack, int32_t B,
                  int32_t Cin, int64_t HW, void* scratch, float* gx, float* gw, float* gb, void* stream);
 
+/* The two calls above with the activations x, zn, gzn and gx of element type `dtype`: PCL_DT_F32 (exactly the calls
+ * above) or PCL_DT_BF16; any other code, PCL_DT_F16 included, returns PCL_ERR_ARG (an fp16 activation would be rounded
+ * to the bf16 GEMM operand).  bf16 activations are converted to fp32 on load (exact) and everything is computed as for
+ * fp32 activations, so against the fp32 call on the converted inputs: zn and gx are its zn and gx rounded to
+ * nearest-even, inv_norm, gw and gb are bit-identical.  inv_norm, weight, bias, gw and gb stay fp32; wpack and scratch
+ * are sized and packed as above. */
+int pcl_proj_fwd_dt(const void* x, int32_t dtype, const void* wpack, const float* bias, int32_t B, int32_t Cin,
+                    int64_t HW, void* zn, float* inv_norm, void* stream);
+int pcl_proj_bwd_dt(const void* x, int32_t dtype, const void* zn, const float* inv_norm, const void* gzn,
+                    const void* wpack, int32_t B, int32_t Cin, int64_t HW, void* scratch, void* gx, float* gw,
+                    float* gb, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * §8f row 1 (next row): the segmentation CE of ContrastCELoss.forward, fused.  Replaces
  * lib/loss/loss_contrast.py:180-181 (F.interpolate(seg, (Himg,Wimg), bilinear, align_corners=True)) +
