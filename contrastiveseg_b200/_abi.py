@@ -74,7 +74,8 @@ class StepDesc(C.Structure):
                 ("precision", c_i32), ("shadow_bf16", c_vp), ("shadow_rows", c_i64), ("contrast_norm_bound", c_f32),
                 ("row_m2", c_vp),
                 ("loss", c_vp), ("grad_embed", c_vp), ("sync", c_vp),
-                ("embed_dtype", c_i32), ("seg_dtype", c_i32)]
+                ("embed_dtype", c_i32), ("seg_dtype", c_i32),
+                ("topk_negatives", c_i32), ("topk_scratch", c_vp)]
 
 
 ABI_STRUCTS = (Geom, SelectSizes, SweepDesc, SweepSizes, BankGeom, TcDesc, StepDesc)   # pcl_abi_sizeof ids 0..6

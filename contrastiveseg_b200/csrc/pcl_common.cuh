@@ -66,8 +66,10 @@ int select_gather_ex(const pcl_geom* g, const void* embed, const uint16_t* keys,
                      const int32_t* prev_rows = nullptr, void* grad_clear = nullptr, int embed_dtype = PCL_DT_F32);
 int tc_fwd_ex(const pcl_tc_desc* d, float* row_m2, float* partials, float* rowstats, float* loss, void* stream,
               bool skip_prep, unsigned long long* step_counter = nullptr);
-int simt_fwd_ex(const pcl_sweep_desc* d, float* partials, float* rowstats, float* loss, void* stream,
-                unsigned long long* step_counter);
+int simt_fwd_ex(const pcl_sweep_desc* d, int k, uint32_t* scratch, float* partials, float* rowstats, float* loss,
+                void* stream, unsigned long long* step_counter);
+int simt_bwd_ex(const pcl_sweep_desc* d, int k, uint32_t* scratch, const float* rowstats, const float* grad_loss,
+                float* dpartials, float* dA, void* stream);
 int tc_fwd_topk_ex(const pcl_tc_desc* d, int k, uint32_t* scratch, float* row_m2, float* partials, float* rowstats,
                    float* loss, void* stream, bool skip_prep, unsigned long long* step_counter);
 int tc_query(const pcl_tc_desc* d, int64_t* n_slot_rows, float* m2_scale);

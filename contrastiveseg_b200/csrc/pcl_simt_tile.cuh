@@ -1,4 +1,5 @@
-// Tile machinery of the exact fp32 (SIMT) InfoNCE sweeps, shared by pcl_infonce_simt.cu and pcl_topk.cu.
+// Tile machinery of the exact fp32 (SIMT) InfoNCE sweep (pcl_infonce_simt.cu: the stock and the top-k modes; pcl_topk.cu
+// sizes the top-k scratch by its row tile).
 #pragma once
 #include "pcl_common.cuh"
 #include "pcl_sweep.cuh"
@@ -39,10 +40,9 @@ __device__ __forceinline__ void load_tile_T(float* __restrict__ dst, const float
   }
 }
 
-// host side (pcl_infonce_simt.cu): descriptor validation + split geometry, shared-memory size of one sweep CTA,
-// and a launcher of the stock POS sweep for callers in other translation units
+// host side (pcl_infonce_simt.cu): descriptor validation + split geometry, shared-memory size of one sweep CTA
+// (topk: the four per-row / per-column selection arrays of the top-k modes, 1 KB more)
 int simt_make_args(const pcl_sweep_desc* d, SweepArgs* a);
-size_t simt_sweep_smem(int D, bool bwd);
-int simt_launch_pos(const SweepArgs& a, float* partials, const float* rowstats, cudaStream_t s);
+size_t simt_sweep_smem(int D, bool bwd, bool topk);
 
 }  // namespace pcl

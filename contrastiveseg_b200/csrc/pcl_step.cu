@@ -50,6 +50,11 @@ extern "C" int pcl_step_stats(const pcl_step_desc* d, void* stream) {
   return pcl_plan_anchors(&d->g, d->counts, d->plan, stream);
 }
 
+// a10: topk_negatives 0 = all negatives, k >= 1 needs the selection scratch, < 0 is refused
+static bool topk_ok(const pcl_step_desc* d) {
+  return d->topk_negatives == 0 || (d->topk_negatives > 0 && d->topk_scratch != nullptr);
+}
+
 static int step_forward(const pcl_step_desc* d, unsigned long long* ctr, void* stream);
 
 extern "C" int pcl_step_forward(const pcl_step_desc* d, void* stream) { return step_forward(d, nullptr, stream); }
@@ -63,8 +68,9 @@ extern "C" int pcl_step_forward_ctr(const pcl_step_desc* d, uint64_t* step_count
 }
 
 static int step_forward(const pcl_step_desc* d, unsigned long long* ctr, void* stream) {
-  if (!d) return PCL_ERR_ARG;
-  if (d->precision == 1) {
+  if (!d || !topk_ok(d)) return PCL_ERR_ARG;
+  const int k = d->topk_negatives;
+  if (d->precision == 1 && k == 0) {
     // tensor path: the selection kernel also writes the row stabilisers and initialises the partial slots
     if (!d->anchors_bf16 || !d->row_m2 || (d->mode == 1 && !d->shadow_bf16)) return PCL_ERR_ARG;
     pcl_tc_desc t;
@@ -83,18 +89,27 @@ static int step_forward(const pcl_step_desc* d, unsigned long long* ctr, void* s
                                  d->normalize, d->anchor_meta, d->anchors_f32, d->anchors_bf16, d->inv_norm, d->norm_max,
                                  nullptr, 0.f, nullptr, 0, stream, ctr, nullptr, nullptr, nullptr, d->embed_dtype);
   if (st != PCL_OK) return st;
+  if (d->precision == 1) {
+    // top-k on the tensor path: the selection above leaves the stabilisers and the partial slots to the top-k forward's
+    // own prep (k_select would round the stabiliser differently: sqrt * (cbound * k1 * 1.0001) against
+    // ((sqrt * cbound) * k1) * 1.0001 in k_tc_prep)
+    pcl_tc_desc t;
+    fill_tc(d, &t);
+    return pcl::tc_fwd_topk_ex(&t, k, d->topk_scratch, d->row_m2, d->partials, d->rowstats, d->loss, stream, false, ctr);
+  }
   pcl_sweep_desc w;
   fill_sweep(d, &w);
-  return pcl::simt_fwd_ex(&w, d->partials, d->rowstats, d->loss, stream, ctr);
+  return pcl::simt_fwd_ex(&w, k, d->topk_scratch, d->partials, d->rowstats, d->loss, stream, ctr);
 }
 
 extern "C" int pcl_step_backward(const pcl_step_desc* d, const float* grad_loss, void* stream) {
-  if (!d) return PCL_ERR_ARG;
+  if (!d || !topk_ok(d)) return PCL_ERR_ARG;
+  const int k = d->topk_negatives;
   int st;
   if (d->precision == 1) {
     pcl_tc_desc t;
     fill_tc(d, &t);
-    if (!d->normalize) {
+    if (!d->normalize && k == 0) {
       // fused tail: the dense-gradient writer sums the per-split partials itself (no (A, D) gradient round trip)
       int splits = 0, a_pad = 0;
       st = pcl::tc_bwd_ex(&t, d->row_m2, d->rowstats, grad_loss, d->dpartials, nullptr, stream, &splits, &a_pad);
@@ -102,11 +117,12 @@ extern "C" int pcl_step_backward(const pcl_step_desc* d, const float* grad_loss,
       return pcl::zero_scatter_reduce(&d->g, d->plan, d->anchor_meta, d->dpartials, splits, a_pad, 1.f / d->temperature,
                                       grad_loss, d->grad_embed, stream, d->embed_dtype);
     }
-    st = pcl_infonce_tc_bwd(&t, d->row_m2, d->rowstats, grad_loss, d->dpartials, d->dA, stream);
+    st = pcl::tc_bwd_ex(&t, d->row_m2, d->rowstats, grad_loss, d->dpartials, d->dA, stream, nullptr, nullptr,
+                        k > 0 ? d->topk_scratch : nullptr);
   } else {
     pcl_sweep_desc w;
     fill_sweep(d, &w);
-    st = pcl_infonce_bwd(&w, d->rowstats, grad_loss, d->dpartials, d->dA, stream);
+    st = pcl::simt_bwd_ex(&w, k, d->topk_scratch, d->rowstats, grad_loss, d->dpartials, d->dA, stream);
   }
   if (st != PCL_OK) return st;
   return pcl::scatter_grad(&d->g, d->plan, d->anchor_meta, d->dA, d->anchors_f32, d->inv_norm, d->normalize,
@@ -118,6 +134,7 @@ extern "C" int pcl_step_backward(const pcl_step_desc* d, const float* grad_loss,
 // selection and sweep kernels): backward sweep -> (A, D) gradient rows -> scatter of those rows only.
 extern "C" int pcl_step_backward_prezeroed(const pcl_step_desc* d, const float* grad_loss, void* stream) {
   if (!d) return PCL_ERR_ARG;
+  if (d->topk_negatives != 0) return PCL_ERR_UNSUPPORTED;
   int st;
   if (d->precision == 1) {
     pcl_tc_desc t;
@@ -143,7 +160,7 @@ extern "C" int pcl_step_backward_prezeroed(const pcl_step_desc* d, const float* 
 
 // ---- fused small-anchor step (include/pcl.h: pcl_step_fused_*) ----
 extern "C" int pcl_step_fused_supported(const pcl_step_desc* d) {
-  if (!d || d->mode != 0 || d->precision != 1 || d->normalize != 0 || d->sync == nullptr) return 0;
+  if (!d || d->mode != 0 || d->precision != 1 || d->normalize != 0 || d->sync == nullptr || d->topk_negatives != 0) return 0;
   if (d->g.D != 256 || d->g.max_samples < 1 || d->g.max_samples > 1024) return 0;
   if (!pcl::dtype_ok(d->embed_dtype) || !pcl::dtype_ok(d->seg_dtype)) return 0;      // fp32, bf16 and fp16 inputs qualify
   return 1;
@@ -188,6 +205,7 @@ extern "C" int pcl_step_fused_scatter(const pcl_step_desc* d, const float* grad_
 // zero-fill of the step's dense gradient on the engine's fill kernel (the caller picks the stream: a parallel branch)
 extern "C" int pcl_step_fused_fill(const pcl_step_desc* d, void* stream) {
   if (!d || !d->grad_embed || !pcl::dtype_ok(d->embed_dtype)) return PCL_ERR_ARG;
+  if (d->topk_negatives != 0) return PCL_ERR_UNSUPPORTED;
   // sized by the gradient's element size: a half gradient is half the bytes (still a multiple of 16: D % 32 == 0)
   const uint64_t bytes = (uint64_t)d->g.B * d->g.D * d->g.h * d->g.w * pcl::dtype_size(d->embed_dtype);
   if ((bytes & 15) != 0 || ((uintptr_t)d->grad_embed & 15) != 0) return PCL_ERR_UNSUPPORTED;

@@ -27,25 +27,6 @@ __device__ __forceinline__ int live_rows(const SweepArgs& a) {
 }
 
 
-// Combine the NEG partials of all splits (fixed order) and add the analytic zero tail (Q3).
-static __global__ void k_combine_neg(SweepArgs a, const float* __restrict__ partials, float* __restrict__ rowstats) {
-  const int r = blockIdx.x * blockDim.x + threadIdx.x;
-  const int A = live_rows(a);
-  if (r >= a.a_rows) return;
-  if (r >= A) { rowstats[r] = 0.f; rowstats[a.a_rows + r] = 0.f; return; }
-  float m = -CUDART_INF_F;
-  for (int p = 0; p < a.splits; ++p) m = fmaxf(m, partials[((int64_t)0 * a.splits + p) * a.a_pad + r]);
-  if (a.tail_count > 0) m = fmaxf(m, 0.f);
-  float n = 0.f;
-  for (int p = 0; p < a.splits; ++p) {
-    float pm = partials[((int64_t)0 * a.splits + p) * a.a_pad + r];
-    if (pm != -CUDART_INF_F) n += partials[((int64_t)1 * a.splits + p) * a.a_pad + r] * expf(pm - m);
-  }
-  if (a.tail_count > 0 && a.acls[r] != 0) n += (float)a.tail_count * expf(-m);
-  rowstats[r] = m;
-  rowstats[a.a_rows + r] = n;
-}
-
 // Combine the POS partials, add the zero-tail positives of class-0 anchors, row losses and the mean.
 static __global__ void __launch_bounds__(1024)
 k_finalize(SweepArgs a, const float* __restrict__ partials, float* __restrict__ rowstats, float* __restrict__ loss,

@@ -1,317 +1,14 @@
-// a10 (SURVEY §8): per-anchor top-k hard-negative selection for the exact fp32 InfoNCE sweep.
+// a10 (SURVEY §8): C entry points of the per-anchor top-k hard-negative selection on the exact fp32 sweep.
 //
-// Not in the reference code (lib/loss/loss_contrast.py:116-117 sums ALL negatives); this is the extension the
-// north star names, default OFF.  Semantics (oracle/ref_port.py: infonce_topk):
-//   Neg_i = sum over the k negatives of anchor i with the largest logits of exp(l_ij - m_i);
-//   tau_i = k-th largest negative logit, G_i = #{l > tau_i}, E_i = #{l == tau_i}: every negative with l > tau_i has
-//   weight 1, the E_i ties at tau_i share the remaining k - G_i slots equally (weight (k-G_i)/E_i) — order
-//   independent, and the forward value equals "any k largest" because tied logits have equal exp;
-//   rows with <= k negatives keep all of them (== reference);  backward: G_in = c_i * w_in * e_in * S_i.
-//   The analytic zero tail of the bank (Q3: R rows, logit +0, label 0) takes part in the selection.
-//
-// Streaming realisation (the A x N logits are never stored): an exact 3-level radix select (11 + 11 + 10 bits) on
-// the order-preserving integer image of the fp32 logit — three histogram sweeps with per-row bins in global memory,
-// each followed by a warp-per-row scan — then the weighted NEG sweep, the stock POS sweep and finalize.  The logit of
-// an (anchor, column) pair is the same float in every sweep (same FMA order, explicit round of the 1/T product).
+// Not in the reference code (lib/loss/loss_contrast.py:116-117 sums ALL negatives); default off.  The kernels are modes
+// of the shared SIMT sweep (k_sweep<H1..H3, NEGW, BWDW> in pcl_infonce_simt.cu) and the radix-level scan of
+// pcl_topk.cuh; the loss step reaches them through pcl_step_desc.topk_negatives.  These are the calls on explicit
+// operands, thin wrappers of the sweep's forward / backward with k >= 1.
 #include "pcl_common.cuh"
-#include "pcl_sweep.cuh"
 #include "pcl_simt_tile.cuh"
 #include "pcl_topk.cuh"
 
-namespace pcl {
-
-enum { TK_H1 = 0, TK_H2 = 1, TK_H3 = 2, TK_NEG = 3, TK_BWD = 4 };
-
-template <int PASS>
-__global__ void __launch_bounds__(SWEEP_THREADS, 1)
-k_topk_sweep(SweepArgs a, TopkArgs tk, float* __restrict__ partials, const float* __restrict__ rowstats,
-             float* __restrict__ dpartials) {
-  extern __shared__ __align__(16) float smem[];
-  const int D = a.D;
-  float* As_t = smem;                         // [D][LDT]
-  float* Ct = As_t + D * LDT;                 // [D][LDT]
-  float* Gs = Ct + D * LDT;                   // [TM][LDT]   (BWD only)
-  float* s_extra = Gs + (PASS == TK_BWD ? TM * LDT : 0);
-  const float** s_ptr = reinterpret_cast<const float**>(s_extra);                  // [64]
-  int* s_rcls = reinterpret_cast<int*>(s_ptr + 64);                                // [64]
-  int* s_rdiag = s_rcls + 64;                                                      // [64]
-  int* s_clab = s_rdiag + 64;                                                      // [64] (-2 = invalid column)
-  float* s_rm = reinterpret_cast<float*>(s_clab + 64);                             // [64]
-  float* s_rneg = s_rm + 64;
-  float* s_rs = s_rneg + 64;
-  float* s_rc = s_rs + 64;
-  float* s_cm = s_rc + 64;                                                         // column stats (self BWD)
-  float* s_cneg = s_cm + 64;
-  float* s_cs = s_cneg + 64;
-  float* s_cc = s_cs + 64;
-  uint32_t* s_rtau = reinterpret_cast<uint32_t*>(s_cc + 64);                       // row: key prefix / tau key
-  float* s_rw = reinterpret_cast<float*>(s_rtau + 64);                             // row: weight of the ties
-  uint32_t* s_ctau = reinterpret_cast<uint32_t*>(s_rw + 64);                       // column as anchor (self BWD)
-  float* s_cw = reinterpret_cast<float*>(s_ctau + 64);
-
-  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-  const int rt = blockIdx.x, split = blockIdx.y;
-  const int A = live_rows(a);
-  const int row0 = rt * TM;
-  if (row0 >= A) return;
-  const int64_t ncols = a.mode == 0 ? (int64_t)A : a.n_cols;
-  const float rs_scale = a.T_over_bT / (float)A;
-
-  if (tid < 64) {
-    int r = row0 + tid;
-    bool ok = r < A;
-    s_ptr[tid] = ok ? a.anchors + (int64_t)r * D : nullptr;
-    s_rcls[tid] = ok ? a.acls[r] : -1;
-    s_rdiag[tid] = ok ? (a.mode == 0 ? r : (a.diag ? a.diag[r] : -1)) : -1;
-    s_rtau[tid] = (ok && PASS != TK_H1) ? tk.sel[r] : TK_ALL;
-    s_rw[tid] = (ok && (PASS == TK_NEG || PASS == TK_BWD)) ? __uint_as_float(tk.sel[a.a_rows + r]) : 0.f;
-    if (PASS == TK_BWD) {
-      const float* st = rowstats;
-      s_rm[tid] = ok ? st[r] : 0.f;
-      s_rneg[tid] = ok ? st[a.a_rows + r] : 1.f;
-      s_rs[tid] = ok ? st[3 * a.a_rows + r] : 0.f;
-      float np = ok ? st[4 * a.a_rows + r] : 1.f;
-      float c = rs_scale / np;
-      if (a.nan_safe && !(np > 0.f)) c = 0.f;
-      s_rc[tid] = ok ? c : 0.f;
-    }
-  }
-  __syncthreads();
-  load_tile_T(As_t, s_ptr, D);
-
-  const int t_hi = (int)((ncols + TN - 1) / TN);
-  const int per = (t_hi + a.splits - 1) / a.splits;
-  const int my_lo = split * per;
-  const int my_hi = min(t_hi, my_lo + per);
-
-  float run_m[4], run_a[4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) { run_m[i] = -CUDART_INF_F; run_a[i] = 0.f; }
-  float dacc[4][QMAX];
-  if (PASS == TK_BWD) {
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-      for (int q = 0; q < QMAX; ++q) dacc[i][q] = 0.f;
-  }
-  const int nq = D / 16;
-
-  for (int ct = my_lo; ct < my_hi; ++ct) {
-    __syncthreads();                          // previous tile fully consumed (Ct, Gs, column arrays)
-    if (tid < 64) {
-      int64_t n = (int64_t)ct * TN + tid;
-      int lab = -2;
-      const float* p = nullptr;
-      if (n < ncols) p = col_row(a, n, lab);
-      s_ptr[tid] = p;
-      s_clab[tid] = lab;
-      if (PASS == TK_BWD && a.mode == 0) {
-        bool ok = n < ncols;
-        s_cm[tid] = ok ? rowstats[n] : 0.f;
-        s_cneg[tid] = ok ? rowstats[a.a_rows + n] : 1.f;
-        s_cs[tid] = ok ? rowstats[3 * a.a_rows + n] : 0.f;
-        float np = ok ? rowstats[4 * a.a_rows + n] : 1.f;
-        float c = rs_scale / np;
-        if (a.nan_safe && !(np > 0.f)) c = 0.f;
-        s_cc[tid] = ok ? c : 0.f;
-        s_ctau[tid] = ok ? tk.sel[n] : TK_ALL;
-        s_cw[tid] = ok ? __uint_as_float(tk.sel[a.a_rows + n]) : 0.f;
-      }
-    }
-    __syncthreads();
-    load_tile_T(Ct, s_ptr, D);
-    __syncthreads();
-
-    float acc[4][4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-      for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
-#pragma unroll 8
-    for (int k = 0; k < D; ++k) {
-      float4 av = *reinterpret_cast<const float4*>(As_t + k * LDT + ty * 4);
-      float4 bv = *reinterpret_cast<const float4*>(Ct + k * LDT + tx * 4);
-      const float ar[4] = {av.x, av.y, av.z, av.w};
-      const float br[4] = {bv.x, bv.y, bv.z, bv.w};
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(ar[i], br[j], acc[i][j]);
-    }
-
-    const int64_t col_base = (int64_t)ct * TN + tx * 4;
-    if (PASS == TK_H1 || PASS == TK_H2 || PASS == TK_H3) {
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int r = ty * 4 + i;
-        const int rcls = s_rcls[r];
-        const uint32_t prefix = s_rtau[r];
-        uint32_t* hrow = tk.hist + (int64_t)(row0 + r) * TK_BINS;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int lab = s_clab[tx * 4 + j];
-          if (lab != -2 && rcls >= 0 && lab != rcls) {
-            const uint32_t key = sortable_key(__fmul_rn(acc[i][j], a.inv_T));
-            if (PASS == TK_H1) {
-              atomicAdd(hrow + (key >> 21), 1u);
-            } else if (PASS == TK_H2) {
-              if ((key >> 21) == prefix) atomicAdd(hrow + ((key >> 10) & 0x7FFu), 1u);
-            } else {
-              if ((key >> 10) == prefix) atomicAdd(hrow + (key & 0x3FFu), 1u);
-            }
-          }
-        }
-      }
-    } else if (PASS == TK_NEG) {
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int r = ty * 4 + i;
-        const int rcls = s_rcls[r];
-        const uint32_t tau = s_rtau[r];
-        const float tw = s_rw[r];
-        float lv[4];
-        float tmax = -CUDART_INF_F;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          lv[j] = __fmul_rn(acc[i][j], a.inv_T);
-          if (s_clab[tx * 4 + j] != -2) tmax = fmaxf(tmax, lv[j]);
-        }
-        if (tmax > run_m[i]) {
-          run_a[i] = (run_m[i] == -CUDART_INF_F) ? 0.f : run_a[i] * expf(run_m[i] - tmax);
-          run_m[i] = tmax;
-        }
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int lab = s_clab[tx * 4 + j];
-          if (lab != -2 && lab != rcls) {
-            const float w = topk_weight(sortable_key(lv[j]), tau, tw);
-            if (w > 0.f) run_a[i] += w * expf(lv[j] - run_m[i]);
-          }
-        }
-      }
-    } else {
-      // gradient tile G: closed form of SURVEY appendix A with the selection weight on the negatives
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int r = ty * 4 + i;
-        const int rcls = s_rcls[r], rdiag = s_rdiag[r];
-        const float m = s_rm[r], neg = s_rneg[r], S = s_rs[r], c = s_rc[r];
-        const uint32_t tau = s_rtau[r];
-        const float tw = s_rw[r];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int cj = tx * 4 + j;
-          const int lab = s_clab[cj];
-          float gval = 0.f;
-          if (lab != -2 && rcls >= 0) {
-            const float l = __fmul_rn(acc[i][j], a.inv_T);
-            const uint32_t key = sortable_key(l);
-            const float e = expf(l - m);
-            if (lab == rcls) {
-              if ((col_base + j) != (int64_t)rdiag) gval = -c * (1.f - e / (e + neg));
-            } else {
-              gval = c * e * S * topk_weight(key, tau, tw);
-            }
-            if (a.mode == 0) {               // + G_ji: the column is an anchor too (self-contrast); l_ji == l_ij bitwise
-              const float e2 = expf(l - s_cm[cj]);
-              if (lab == rcls) {
-                if ((col_base + j) != (int64_t)rdiag) gval += -s_cc[cj] * (1.f - e2 / (e2 + s_cneg[cj]));
-              } else {
-                gval += s_cc[cj] * e2 * s_cs[cj] * topk_weight(key, s_ctau[cj], s_cw[cj]);
-              }
-            }
-          }
-          Gs[r * LDT + cj] = gval;
-        }
-      }
-      __syncthreads();
-      // dA[r][d] += sum_j G[r][j] * C[j][d],  C[j][d] = Ct[d*LDT + j]
-#pragma unroll 4
-      for (int j4 = 0; j4 < TN; j4 += 4) {
-        float4 gv[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) gv[i] = *reinterpret_cast<const float4*>(Gs + (ty * 4 + i) * LDT + j4);
-#pragma unroll
-        for (int q = 0; q < QMAX; ++q) {
-          if (q < nq) {
-            float4 cv = *reinterpret_cast<const float4*>(Ct + (tx + 16 * q) * LDT + j4);
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-              dacc[i][q] += gv[i].x * cv.x + gv[i].y * cv.y + gv[i].z * cv.z + gv[i].w * cv.w;
-          }
-        }
-      }
-    }
-  }
-
-  if (PASS == TK_NEG) {
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      float m = run_m[i], n = run_a[i];
-#pragma unroll
-      for (int o = 1; o < 16; o <<= 1) {
-        float om = __shfl_xor_sync(0xffffffffu, m, o), on = __shfl_xor_sync(0xffffffffu, n, o);
-        float nm = fmaxf(m, om);
-        float s0 = (m == -CUDART_INF_F) ? 0.f : n * expf(m - nm);
-        float s1 = (om == -CUDART_INF_F) ? 0.f : on * expf(om - nm);
-        n = s0 + s1; m = nm;
-      }
-      if (tx == 0) {
-        int r = row0 + ty * 4 + i;
-        partials[((int64_t)0 * a.splits + split) * a.a_pad + r] = m;
-        partials[((int64_t)1 * a.splits + split) * a.a_pad + r] = n;
-      }
-    }
-  } else if (PASS == TK_BWD) {
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      int r = row0 + ty * 4 + i;
-      float* dst = dpartials + ((int64_t)split * a.a_pad + r) * D;
-#pragma unroll
-      for (int q = 0; q < QMAX; ++q)
-        if (q < nq) dst[tx + 16 * q] = dacc[i][q];
-    }
-  }
-}
-
-// k_combine_neg with the selection weight on the analytic zero tail.
-static __global__ void k_combine_neg_topk(SweepArgs a, TopkArgs tk, const float* __restrict__ partials,
-                                          float* __restrict__ rowstats) {
-  const int r = blockIdx.x * blockDim.x + threadIdx.x;
-  const int A = live_rows(a);
-  if (r >= a.a_rows) return;
-  if (r >= A) { rowstats[r] = 0.f; rowstats[a.a_rows + r] = 0.f; return; }
-  float m = -CUDART_INF_F;
-  for (int p = 0; p < a.splits; ++p) m = fmaxf(m, partials[((int64_t)0 * a.splits + p) * a.a_pad + r]);
-  if (a.tail_count > 0) m = fmaxf(m, 0.f);
-  float n = 0.f;
-  for (int p = 0; p < a.splits; ++p) {
-    float pm = partials[((int64_t)0 * a.splits + p) * a.a_pad + r];
-    if (pm != -CUDART_INF_F) n += partials[((int64_t)1 * a.splits + p) * a.a_pad + r] * expf(pm - m);
-  }
-  if (a.tail_count > 0 && a.acls[r] != 0) {
-    const float w = topk_weight(KEY_ZERO, tk.sel[r], __uint_as_float(tk.sel[a.a_rows + r]));
-    n += w * (float)a.tail_count * expf(-m);
-  }
-  rowstats[r] = m;
-  rowstats[a.a_rows + r] = n;
-}
-
-}  // namespace pcl
-
 using namespace pcl;
-
-static size_t topk_smem(int D, bool bwd) { return simt_sweep_smem(D, bwd) + 4 * 64 * sizeof(float); }
-
-static int topk_args(const pcl_sweep_desc* d, int32_t k, uint32_t* scratch, SweepArgs* a, TopkArgs* tk) {
-  int st = simt_make_args(d, a);
-  if (st != PCL_OK) return st;
-  if (k < 1 || !scratch) return PCL_ERR_ARG;
-  tk->k = k;
-  tk->hist = scratch;
-  tk->sel = scratch + (int64_t)a->a_pad * TK_BINS;
-  return PCL_OK;
-}
 
 extern "C" int64_t pcl_topk_scratch_u32(const pcl_sweep_desc* d) {
   if (!d) return PCL_ERR_ARG;
@@ -322,60 +19,13 @@ extern "C" int64_t pcl_topk_scratch_u32(const pcl_sweep_desc* d) {
   return a_pad * TK_BINS + 4 * (int64_t)d->a_rows;
 }
 
+// k < 1 maps to -1: an error here, not "all negatives" (k = 0 of the sweep)
 extern "C" int pcl_infonce_topk_fwd(const pcl_sweep_desc* d, int32_t k, uint32_t* scratch, float* partials,
                                     float* rowstats, float* loss, void* stream) {
-  SweepArgs a;
-  TopkArgs tk;
-  int st = topk_args(d, k, scratch, &a, &tk);
-  if (st != PCL_OK) return st;
-  PCL_REQUIRE(partials && rowstats && loss);
-  cudaStream_t s = (cudaStream_t)stream;
-  const size_t smem = topk_smem(a.D, false);
-  PCL_SMEM_OPT_IN(k_topk_sweep<TK_H1>, topk_smem(256, false));
-  PCL_SMEM_OPT_IN(k_topk_sweep<TK_H2>, topk_smem(256, false));
-  PCL_SMEM_OPT_IN(k_topk_sweep<TK_H3>, topk_smem(256, false));
-  PCL_SMEM_OPT_IN(k_topk_sweep<TK_NEG>, topk_smem(256, false));
-  PCL_CUDA(cudaMemsetAsync(tk.hist, 0, (size_t)a.a_pad * TK_BINS * sizeof(uint32_t), s));
-  const dim3 grid(a.row_tiles, a.splits);
-  const int scan_blocks = ceil_div(a.a_rows, 8);          // 8 warps (rows) per 256-thread block
-  k_topk_sweep<TK_H1><<<grid, SWEEP_THREADS, smem, s>>>(a, tk, nullptr, nullptr, nullptr);
-  PCL_LAUNCH_CHECK();
-  k_topk_scan<1><<<scan_blocks, 256, 0, s>>>(a, tk);
-  PCL_LAUNCH_CHECK();
-  k_topk_sweep<TK_H2><<<grid, SWEEP_THREADS, smem, s>>>(a, tk, nullptr, nullptr, nullptr);
-  PCL_LAUNCH_CHECK();
-  k_topk_scan<2><<<scan_blocks, 256, 0, s>>>(a, tk);
-  PCL_LAUNCH_CHECK();
-  k_topk_sweep<TK_H3><<<grid, SWEEP_THREADS, smem, s>>>(a, tk, nullptr, nullptr, nullptr);
-  PCL_LAUNCH_CHECK();
-  k_topk_scan<3><<<scan_blocks, 256, 0, s>>>(a, tk);
-  PCL_LAUNCH_CHECK();
-  k_topk_sweep<TK_NEG><<<grid, SWEEP_THREADS, smem, s>>>(a, tk, partials, nullptr, nullptr);
-  PCL_LAUNCH_CHECK();
-  k_combine_neg_topk<<<ceil_div(a.a_rows, 256), 256, 0, s>>>(a, tk, partials, rowstats);
-  PCL_LAUNCH_CHECK();
-  st = simt_launch_pos(a, partials, rowstats, s);          // positives are untouched by the selection
-  if (st != PCL_OK) return st;
-  k_finalize<<<1, 1024, 0, s>>>(a, partials, rowstats, loss, nullptr);
-  PCL_LAUNCH_CHECK();
-  return PCL_OK;
+  return pcl::simt_fwd_ex(d, k < 1 ? -1 : k, scratch, partials, rowstats, loss, stream, nullptr);
 }
 
 extern "C" int pcl_infonce_topk_bwd(const pcl_sweep_desc* d, int32_t k, uint32_t* scratch, const float* rowstats,
                                     const float* grad_loss, float* dpartials, float* dA, void* stream) {
-  SweepArgs a;
-  TopkArgs tk;
-  int st = topk_args(d, k, scratch, &a, &tk);
-  if (st != PCL_OK) return st;
-  PCL_REQUIRE(rowstats && dpartials && dA);
-  cudaStream_t s = (cudaStream_t)stream;
-  const size_t smem = topk_smem(a.D, true);
-  PCL_SMEM_OPT_IN(k_topk_sweep<TK_BWD>, topk_smem(256, true));
-  const dim3 grid(a.row_tiles, a.splits);
-  k_topk_sweep<TK_BWD><<<grid, SWEEP_THREADS, smem, s>>>(a, tk, nullptr, rowstats, dpartials);
-  PCL_LAUNCH_CHECK();
-  const int64_t total = (int64_t)a.a_rows * a.D;
-  k_reduce_dA<<<(unsigned)ceil_div64(total, 256), 256, 0, s>>>(a, dpartials, grad_loss, dA);
-  PCL_LAUNCH_CHECK();
-  return PCL_OK;
+  return pcl::simt_bwd_ex(d, k < 1 ? -1 : k, scratch, rowstats, grad_loss, dpartials, dA, stream);
 }

@@ -1,5 +1,6 @@
-// a10 (SURVEY §8): pieces of the per-anchor top-k hard-negative selection shared by the exact fp32 sweep (pcl_topk.cu)
-// and the tensor-core sweep (pcl_infonce_tc.cu): the order-preserving key, the selection state, the radix-level scan.
+// a10 (SURVEY §8): pieces of the per-anchor top-k hard-negative selection shared by the exact fp32 sweep
+// (pcl_infonce_simt.cu) and the tensor-core sweep (pcl_infonce_tc.cu): the order-preserving key, the selection state,
+// the radix-level scan.
 #pragma once
 #include "pcl_common.cuh"
 #include "pcl_sweep.cuh"

@@ -93,6 +93,9 @@ class ContrastWorkspace:
         _abi.check(lib.pcl_sweep_sizes(C.byref(sw), C.byref(ss)), "pcl_sweep_sizes")
         self.sweep_sizes = ss
         n_partial, n_dpartial = ss.partial_f32, ss.dpartial_f32
+        n_topk = lib.pcl_topk_scratch_u32(C.byref(sw))              # a10 selection scratch (negative: pcl_status)
+        if n_topk < 0:
+            _abi.check(int(n_topk), "pcl_topk_scratch_u32")
         self.tc_ok = D == 256
         if self.tc_ok:                       # the tensor sweep uses its own split count: size for the larger of the two
             td = _abi.TcDesc()
@@ -106,6 +109,10 @@ class ContrastWorkspace:
             ts = _abi.SweepSizes()
             _abi.check(lib.pcl_tc_sizes(C.byref(td), C.byref(ts)), "pcl_tc_sizes")
             n_partial, n_dpartial = max(n_partial, ts.partial_f32), max(n_dpartial, ts.dpartial_f32)
+            n_tc_topk = lib.pcl_tc_topk_scratch_u32(C.byref(td))
+            if n_tc_topk < 0:
+                _abi.check(int(n_tc_topk), "pcl_tc_topk_scratch_u32")
+            n_topk = max(n_topk, n_tc_topk)
             if mode == 0 and ms <= 1024:     # the fused self-contrast kernel: one slot per 256-column tile
                 a_pad = -(-ms // 128) * 128
                 s_max = -(-a_pad // 256)
@@ -121,7 +128,6 @@ class ContrastWorkspace:
         self.anchors_f32 = torch.empty((ms, D), **f32)
         self.anchors_bf16 = torch.empty((-(-ms // 128) * 128, D), dtype=torch.bfloat16, device=device)
         self.inv_norm = torch.empty(ms, **f32)
-        self.norm_max = torch.zeros(1, **f32)
         self.partials = torch.empty(5 * n_partial, **f32)
         self.rowstats = torch.empty(6 * ss.rowstat_f32, **f32)
         self.dpartials = torch.empty(n_dpartial, **f32)
@@ -131,6 +137,8 @@ class ContrastWorkspace:
         self.ranks = torch.zeros(ms, **i32)
         self.ranks_host = torch.zeros(ms, dtype=torch.int32).pin_memory() if torch.cuda.is_available() else None
         self.sync = torch.zeros(1024, **i32)      # inter-CTA counters of the fused kernels (re-armed by the kernels themselves)
+        self.topk_scratch_u32 = int(n_topk)
+        self.topk_scratch = None     # a10 selection state (radix bins + per-row result), allocated by the first top-k step
         self.busy = False
         self.token = 0               # generation counter: a stale autograd node must not release a re-used workspace
         self.bank_key = None         # (device index, segment_queue address) while a backward that re-reads that bank is pending
@@ -142,6 +150,15 @@ class ContrastWorkspace:
                      "partials", "rowstats", "dpartials", "dA", "loss", "row_m2", "sync"):   # norm_max: optional, unused
             setattr(d, name, getattr(self, name).data_ptr())
         self.desc = d
+
+    def set_topk(self, k: int) -> None:
+        """a10 fields of the step descriptor: keep the k hardest negatives of every anchor (0 = all, the reference)."""
+        if k < 0:
+            raise _abi.PclError("topk_negatives must be >= 1 (None disables the selection)")
+        if k and self.topk_scratch is None:
+            self.topk_scratch = torch.empty(self.topk_scratch_u32, dtype=torch.int32, device=self.device)
+        self.desc.topk_negatives = k
+        self.desc.topk_scratch = _abi.ptr(self.topk_scratch)
 
     # views used by tests / diagnostics
     def plan_header(self):
@@ -236,92 +253,6 @@ def _release_workspace(ws, token) -> None:
         ws.busy = False
 
 
-def _step_sweep_desc(ws, d) -> "_abi.SweepDesc":
-    """pcl_sweep_desc of the step's exact sweep (what pcl_step.cu:fill_sweep builds on the C side)."""
-    ms = ws.geom.max_samples
-    sw = _abi.SweepDesc()
-    sw.anchors = ws.anchors_f32.data_ptr()
-    sw.anchor_cls = ws.anchor_meta.data_ptr() + 4 * 2 * ms
-    sw.diag_col = ws.anchor_meta.data_ptr() + 4 * 3 * ms
-    sw.plan = ws.plan.data_ptr()
-    sw.a_rows, sw.D, sw.mode = ms, ws.geom.D, d.mode
-    sw.segment_queue, sw.pixel_queue = d.segment_queue, d.pixel_queue
-    sw.bank_K, sw.bank_M0, sw.bank_M1 = d.bank_K, d.bank_M0, d.bank_M1
-    sw.temperature, sw.base_temperature, sw.nan_safe = d.temperature, d.base_temperature, d.nan_safe
-    return sw
-
-
-def _step_tc_desc(ws, d) -> "_abi.TcDesc":
-    """pcl_tc_desc of the step's tensor sweep (what pcl_step.cu:fill_tc builds on the C side)."""
-    ms = ws.geom.max_samples
-    t = _abi.TcDesc()
-    t.anchors_bf16 = ws.anchors_bf16.data_ptr()
-    t.anchor_cls = ws.anchor_meta.data_ptr() + 4 * 2 * ms
-    t.diag_col = ws.anchor_meta.data_ptr() + 4 * 3 * ms
-    t.plan = ws.plan.data_ptr()
-    t.a_rows, t.D, t.mode = ms, ws.geom.D, d.mode
-    t.contrast_bf16, t.contrast_rows_alloc = d.shadow_bf16, d.shadow_rows
-    t.bank_K, t.bank_R, t.sorted = d.bank_K, d.bank_M0 + d.bank_M1, 1
-    t.contrast_norm_bound = d.contrast_norm_bound
-    t.temperature, t.base_temperature, t.nan_safe = d.temperature, d.base_temperature, d.nan_safe
-    return t
-
-
-def _topk_step_forward(lib, ws, d, opts, stream):
-    """a10: selection + gather as usual, then the top-k InfoNCE sweep (exact fp32 path, or the tensor path: the radix
-    select then runs in the wgmma sweep's epilogue on the fp32-accumulated logits of the bf16 operands)."""
-    k = int(opts.topk_negatives)
-    if k < 1:
-        raise _abi.PclError("topk_negatives must be >= 1 (None disables the selection)")
-    g = ws.geom
-    if opts.precision == "bf16":
-        _abi.check(lib.pcl_select_gather(C.byref(g), d.embed, ws.keys.data_ptr(), ws.chunk_pref.data_ptr(),
-                                         ws.plan.data_ptr(), d.ranks, d.seed, d.normalize, ws.anchor_meta.data_ptr(),
-                                         ws.anchors_f32.data_ptr(), ws.anchors_bf16.data_ptr(), ws.inv_norm.data_ptr(),
-                                         ws.norm_max.data_ptr(), stream), "pcl_select_gather")
-        t = _step_tc_desc(ws, d)
-        n = lib.pcl_tc_topk_scratch_u32(C.byref(t))
-        if n < 0:
-            _abi.check(int(n), "pcl_tc_topk_scratch_u32")
-        scratch = getattr(ws, "topk_scratch", None)
-        if scratch is None or scratch.numel() < n:
-            scratch = ws.topk_scratch = torch.empty(n, dtype=torch.int32, device=ws.device)
-        _abi.check(lib.pcl_infonce_tc_topk_fwd(C.byref(t), k, scratch.data_ptr(), ws.row_m2.data_ptr(), ws.partials.data_ptr(),
-                                               ws.rowstats.data_ptr(), d.loss, stream), "pcl_infonce_tc_topk_fwd")
-        return t, k, scratch
-    _abi.check(lib.pcl_select_gather(C.byref(g), d.embed, ws.keys.data_ptr(), ws.chunk_pref.data_ptr(),
-                                     ws.plan.data_ptr(), d.ranks, d.seed, d.normalize, ws.anchor_meta.data_ptr(),
-                                     ws.anchors_f32.data_ptr(), ws.anchors_bf16.data_ptr(), ws.inv_norm.data_ptr(),
-                                     ws.norm_max.data_ptr(), stream), "pcl_select_gather")
-    sw = _step_sweep_desc(ws, d)
-    n = lib.pcl_topk_scratch_u32(C.byref(sw))
-    if n < 0:
-        _abi.check(int(n), "pcl_topk_scratch_u32")
-    scratch = getattr(ws, "topk_scratch", None)
-    if scratch is None or scratch.numel() < n:
-        scratch = ws.topk_scratch = torch.empty(n, dtype=torch.int32, device=ws.device)
-    _abi.check(lib.pcl_infonce_topk_fwd(C.byref(sw), k, scratch.data_ptr(), ws.partials.data_ptr(),
-                                        ws.rowstats.data_ptr(), d.loss, stream), "pcl_infonce_topk_fwd")
-    return sw, k, scratch
-
-
-def _topk_step_backward(lib, ws, d, topk, go, stream):
-    sw, k, scratch = topk
-    if isinstance(sw, _abi.TcDesc):
-        _abi.check(lib.pcl_infonce_tc_topk_bwd(C.byref(sw), k, scratch.data_ptr(), ws.row_m2.data_ptr(), ws.rowstats.data_ptr(),
-                                               go.data_ptr(), ws.dpartials.data_ptr(), ws.dA.data_ptr(), stream),
-                   "pcl_infonce_tc_topk_bwd")
-        _abi.check(lib.pcl_scatter_grad(C.byref(ws.geom), ws.plan.data_ptr(), ws.anchor_meta.data_ptr(), ws.dA.data_ptr(),
-                                        ws.anchors_f32.data_ptr(), ws.inv_norm.data_ptr(), d.normalize, d.grad_embed,
-                                        stream), "pcl_scatter_grad")
-        return
-    _abi.check(lib.pcl_infonce_topk_bwd(C.byref(sw), k, scratch.data_ptr(), ws.rowstats.data_ptr(), go.data_ptr(),
-                                        ws.dpartials.data_ptr(), ws.dA.data_ptr(), stream), "pcl_infonce_topk_bwd")
-    _abi.check(lib.pcl_scatter_grad(C.byref(ws.geom), ws.plan.data_ptr(), ws.anchor_meta.data_ptr(), ws.dA.data_ptr(),
-                                    ws.anchors_f32.data_ptr(), ws.inv_norm.data_ptr(), d.normalize, d.grad_embed,
-                                    stream), "pcl_scatter_grad")
-
-
 class _PixelContrastFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, embed, labels, seg, predict, segq, pixq, shadow, opts: ContrastOptions):
@@ -396,6 +327,7 @@ class _PixelContrastFn(torch.autograd.Function):
         d.temperature, d.base_temperature = opts.temperature, opts.base_temperature
         d.nan_safe = int(opts.nan_safe)
         d.normalize = int(opts.normalize)
+        ws.set_topk(int(opts.topk_negatives or 0))
         d.precision = 0
         shadow_c = None
         if opts.precision == "bf16":
@@ -438,11 +370,7 @@ class _PixelContrastFn(torch.autograd.Function):
                 d.ranks = None
             else:
                 raise _abi.PclError(f"unknown rng mode {opts.rng!r}")
-            if opts.topk_negatives:
-                ctx.topk = _topk_step_forward(lib, ws, d, opts, stream)
-            else:
-                ctx.topk = None
-                _abi.check(lib.pcl_step_forward(C.byref(d), stream), "pcl_step_forward")
+            _abi.check(lib.pcl_step_forward(C.byref(d), stream), "pcl_step_forward")
         ctx.ws = ws
         ctx.embed_shape, ctx.embed_dtype = tuple(embed_c.shape), embed_c.dtype
         ctx.keep = (embed_c, labels_c, seg_c, pred_c, segq_c, pixq_c, shadow_c)   # keep inputs alive until kernels ran
@@ -477,10 +405,7 @@ class _PixelContrastFn(torch.autograd.Function):
         d.grad_embed = grad.data_ptr()
         d.embed_dtype = DTYPE_CODES[ctx.embed_dtype]
         with _on_device(device):
-            if ctx.topk is not None:
-                _topk_step_backward(lib, ws, d, ctx.topk, go, _stream_ptr(device))
-            else:
-                _abi.check(lib.pcl_step_backward(C.byref(d), go.data_ptr(), _stream_ptr(device)), "pcl_step_backward")
+            _abi.check(lib.pcl_step_backward(C.byref(d), go.data_ptr(), _stream_ptr(device)), "pcl_step_backward")
         _release_workspace(ws, getattr(ctx, "token", ws.token))     # also applies bank writes held back for this backward
         ctx.keep = None
         return grad, None, None, None, None, None, None, None

@@ -4,7 +4,7 @@ The eager step costs ~0.14 ms of host time (Python + autograd + 8 kernel launche
 time at the Cityscapes shape, so it is host-launch-bound as soon as the host slows down (8 ranks on one box).  The C
 ABI neither allocates nor synchronises and all scratch is caller-owned, so the whole sequence
 
-    pcl_step_stats -> pcl_step_ranks -> pcl_step_forward -> pcl_step_backward[_prezeroed]
+    pcl_step_stats -> pcl_step_forward_ctr -> pcl_step_backward[_prezeroed]
 
 is capturable: a replay is ONE graph launch.  The zero-fill of the dense gradient (the HBM floor of the step) runs as
 a parallel branch of the graph from the start of the step (``overlap_zero_fill``), hidden behind the latency-bound
@@ -12,15 +12,15 @@ selection and sweep kernels; the backward then scatters only the sampled columns
 
 * static shapes and static addresses: the tensors given to the constructor are read in place on every replay —
   refill them (``embed.copy_(...)`` or let the producer write into them), do not replace them;
-* sampling stays fresh: kernel arguments are frozen in a graph, so the anchor ranks are drawn on the device from a
-  counter in device memory (``pcl_step_ranks``) instead of the by-value seed of the eager path;
+* sampling stays fresh: kernel arguments are frozen in a graph, so the selection kernel draws the anchor ranks from a
+  counter in device memory (``pcl_step_forward_ctr``) instead of the by-value seed of the eager path;
 * the upstream gradient is a device scalar (``grad_scale``, default 1) folded into the dense gradient by the
   backward kernels, not an autograd input: use it for the loss weight (``contrast.loss_weight``).
 
 The reference RNG stream (``rng='torch_cpu'`` / injected permutations) needs a host round trip and is not capturable.
 
 Memory-bank steps (``enqueue=``): the trainer's order loss -> enqueue -> backward (trainer_contrastive.py:241-255) is part
-of the captured sequence: stats -> ranks -> forward -> enqueue packet | all_gather | backward -> bank write.  One rank: a
+of the captured sequence: stats -> forward -> enqueue packet | all_gather | backward -> bank write.  One rank: a
 single graph.  Several ranks: three graphs and ONE NCCL all_gather of the packet — forward + packet, then the backward
 sweep with the all_gather next to it on its own stream, then the bank write (four host calls per step, nothing
 allocated, no host synchronisation; ``PCL_GATHER_OVERLAP=0``: two graphs with the all_gather between them); the bank
@@ -120,6 +120,7 @@ class GraphedContrastStep:
         d.segment_queue, d.pixel_queue = _abi.ptr(self.segq), _abi.ptr(self.pixq)
         d.temperature, d.base_temperature = opts.temperature, opts.base_temperature
         d.nan_safe, d.normalize = int(opts.nan_safe), int(opts.normalize)
+        self.ws.set_topk(int(opts.topk_negatives or 0))
         d.precision = 0
         self.shadow = None
         if opts.precision == "bf16":
@@ -138,17 +139,11 @@ class GraphedContrastStep:
         elif opts.precision != "fp32":
             raise _abi.PclError(f"unknown precision {opts.precision!r}")
         d.seed = int(opts.seed) & 0xFFFFFFFFFFFFFFFF          # base seed; the per-replay part is the device counter
-        d.ranks = self.ws.ranks.data_ptr()
         d.loss, d.grad_embed = self.loss.data_ptr(), self.grad.data_ptr()
         # Small-anchor shape (no bank, tensor path, D = 256, max_samples <= 1024: BASELINE configs[1]): four launches
         # instead of eleven — scan+plan, selection, ONE kernel for the InfoNCE forward and backward (logits stay in tensor
         # memory), scatter — with the engine's own zero-fill of the dense gradient on a parallel branch.
-        ok = bool(self.lib.pcl_step_fused_supported(C.byref(d))) and enqueue is None and not opts.topk_negatives
-        self.topk = None
-        if opts.topk_negatives:
-            # a10 (per-anchor top-k hard negatives): the radix-select sweeps + weighted NEG sweep are part of the captured
-            # sequence; their backward writes the dense gradient itself (zero-fill + scatter), so no parallel fill branch
-            overlap_zero_fill = False
+        ok = bool(self.lib.pcl_step_fused_supported(C.byref(d))) and enqueue is None
         if fused and not ok:
             raise _abi.PclError("fused=True: the step does not qualify (needs no bank, precision='bf16', D=256, "
                                 "max_samples<=1024, normalize=False)")
@@ -171,7 +166,8 @@ class GraphedContrastStep:
             self._init_enqueue(enqueue)
         # The zero-fill of the dense gradient (B*D*h*w*4 bytes, the HBM floor of the step) does not depend on anything
         # the step computes: run it on a second stream from the start of the step, behind the latency-bound selection
-        # and sweep kernels, and let the backward scatter only the sampled columns (pcl_step_backward_prezeroed).
+        # and sweep kernels, and let the backward scatter only the sampled columns (pcl_step_backward_prezeroed).  Not for
+        # top-k steps: their backward writes the dense gradient itself (zero-fill + scatter).
         self.overlap_zero_fill = bool(overlap_zero_fill) and not opts.topk_negatives
         self.side = None
         if capture:
@@ -259,7 +255,7 @@ class GraphedContrastStep:
 
     # the launch sequence (also usable eagerly: capture=False)
     def _enqueue_a(self, stream: int) -> None:
-        """First half: (zero-fill branch ||) stats -> ranks -> forward -> this rank's enqueue packet."""
+        """First half: (zero-fill branch ||) stats -> forward -> this rank's enqueue packet."""
         lib, d = self.lib, self.ws.desc
         if self.fused:
             early = bool(os.environ.get("PCL_FILL_FORK_EARLY")) and not self.sparse_reset      # tuning runs
@@ -281,11 +277,8 @@ class GraphedContrastStep:
         if side:
             self._fork_zero_fill()
         _abi.check(lib.pcl_step_stats(C.byref(d), stream), "pcl_step_stats")
-        if self.opts.topk_negatives:
-            _abi.check(lib.pcl_step_ranks(C.byref(d), self.counter.data_ptr(), self.ws.ranks.data_ptr(), stream), "pcl_step_ranks")
-            self.topk = _fn._topk_step_forward(lib, self.ws, d, self.opts, stream)
-        else:     # the selection kernel draws the anchors from the device counter itself (no separate rank-draw launch)
-            _abi.check(lib.pcl_step_forward_ctr(C.byref(d), self.counter.data_ptr(), stream), "pcl_step_forward_ctr")
+        # the selection kernel draws the anchors from the device counter itself (no separate rank-draw launch)
+        _abi.check(lib.pcl_step_forward_ctr(C.byref(d), self.counter.data_ptr(), stream), "pcl_step_forward_ctr")
         if side:
             self._join_zero_fill()
 
@@ -296,9 +289,7 @@ class GraphedContrastStep:
             _abi.check(lib.pcl_step_fused_scatter(C.byref(d), self.scale.data_ptr(), self.counter.data_ptr(),
                                                   _abi.ptr(self.prev_rows), stream), "pcl_step_fused_scatter")
             return
-        if self.opts.topk_negatives:
-            _fn._topk_step_backward(lib, self.ws, d, self.topk, self.scale, stream)
-        elif self.overlap_zero_fill:
+        if self.overlap_zero_fill:
             _abi.check(lib.pcl_step_backward_prezeroed(C.byref(d), self.scale.data_ptr(), stream),
                        "pcl_step_backward_prezeroed")
         else:

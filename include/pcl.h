@@ -393,14 +393,24 @@ typedef struct {
    * `grad_embed` point to 2-byte elements; seg_dtype != 0: `seg` does.  The sampled anchors, the loss and every scratch
    * buffer stay fp32. */
   int32_t embed_dtype, seg_dtype;
+  /* a10: k >= 1 keeps the k hardest negatives of every anchor (pcl_infonce_topk_fwd / pcl_infonce_tc_topk_fwd on the
+   * step's sweep), 0 = all negatives (the reference), < 0 is PCL_ERR_ARG.  Needs an fp32 embed.  topk_scratch: the
+   * sweep's pcl_topk_scratch_u32 / pcl_tc_topk_scratch_u32 uint32 words (radix bins + the selection state, which the
+   * backward reads: one step owns it from its forward to its backward). */
+  int32_t topk_negatives;
+  uint32_t* topk_scratch;
 } pcl_step_desc;
 
+/* pcl_step_forward: pcl_select_gather + pcl_infonce_fwd (pcl_infonce_tc_fwd with precision 1); with topk_negatives the
+ * selection + gather, then the top-k forward of the step's sweep.  pcl_step_backward: the backward sweep (the top-k one
+ * with topk_negatives) + pcl_scatter_grad. */
 int pcl_step_stats(const pcl_step_desc* d, void* stream);      /* pcl_class_stats + pcl_plan_anchors      */
-int pcl_step_forward(const pcl_step_desc* d, void* stream);    /* pcl_select_gather + pcl_infonce_fwd     */
-int pcl_step_backward(const pcl_step_desc* d, const float* grad_loss, void* stream); /* bwd + scatter     */
+int pcl_step_forward(const pcl_step_desc* d, void* stream);
+int pcl_step_backward(const pcl_step_desc* d, const float* grad_loss, void* stream);
 /* Same backward for a grad_embed buffer the caller has already zero-filled (e.g. on a second stream, overlapped with
  * the forward: the 268 MB fill is the HBM floor of the step, the selection and sweep kernels are latency-bound): runs
- * the backward sweep and scatters only the sampled columns.  Nothing else of grad_embed is written. */
+ * the backward sweep and scatters only the sampled columns.  Nothing else of grad_embed is written.  Not for top-k
+ * steps (PCL_ERR_UNSUPPORTED): their backward writes the dense gradient itself. */
 int pcl_step_backward_prezeroed(const pcl_step_desc* d, const float* grad_loss, void* stream);
 
 /* CUDA-graph capture of a step (SURVEY §8f row 4).  The three calls above neither allocate nor synchronise, so a
@@ -433,7 +443,8 @@ int pcl_step_forward_ctr(const pcl_step_desc* d, uint64_t* step_counter, void* s
  *   sparse reset  prev_rows != NULL (1 + 2 * max_samples int32, zero before the first call, owned by the step): the buffer
  *                 persists between steps, zero-filled ONCE by the caller; the selection kernel clears exactly the entries
  *                 the previous step scattered and the scatter records its own.  The caller must not write the buffer.
- * d->sync is required.  pcl_step_fused_supported: 1 if the descriptor qualifies, else 0. */
+ * d->sync is required.  pcl_step_fused_supported: 1 if the descriptor qualifies, else 0.  A top-k step
+ * (topk_negatives != 0) never qualifies, and every pcl_step_fused_* call returns PCL_ERR_UNSUPPORTED for it. */
 int pcl_step_fused_supported(const pcl_step_desc* d);
 int pcl_step_fused_select(const pcl_step_desc* d, const uint64_t* step_counter, const int32_t* prev_rows, void* stream);
 int pcl_step_fused_loss(const pcl_step_desc* d, void* stream);

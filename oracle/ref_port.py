@@ -190,7 +190,7 @@ def infonce_closed_form(anchors: torch.Tensor, ya: torch.Tensor, contrast: torch
 
 def topk_negative_weights(l: torch.Tensor, neg_mask: torch.Tensor, k: Optional[int]):
     """a10 selection weights (EXTENSION — the reference has no top-k code; semantics defined by SURVEY §8 a10 and
-    contrastiveseg_b200/csrc/pcl_topk.cu).  l (A,N) logits, neg_mask (A,N) bool.  Per row: tau = k-th largest
+    contrastiveseg_b200/csrc/pcl_topk.cuh).  l (A,N) logits, neg_mask (A,N) bool.  Per row: tau = k-th largest
     negative logit, weight 1 above tau, (k - G)/E on the E ties at tau, 0 below; rows with <= k negatives keep all.
     Returns (w, tau, G, E) with tau = -inf / E = 0 for rows that keep everything."""
     A, N = l.shape

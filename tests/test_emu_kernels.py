@@ -91,7 +91,7 @@ TOPK += (
 
 @pytest.mark.parametrize("fn,kw", TOPK)
 def test_topk_kernels_on_emulation(emu, fn, kw):
-    """a10: the radix-select / weighted-sweep kernels of csrc/pcl_topk.cu against the sort-based oracle."""
+    """a10: the radix-select / weighted-sweep kernels (csrc/pcl_topk.cuh, the top-k modes of csrc/pcl_infonce_simt.cu) against the sort-based oracle."""
     fn(**kw)
 
 

@@ -1,4 +1,4 @@
-"""GPU parity tests of the a10 extension (per-anchor top-k hard negatives, csrc/pcl_topk.cu) against the oracle's
+"""GPU parity tests of the a10 extension (per-anchor top-k hard negatives, csrc/pcl_topk.cuh) against the oracle's
 sort-based definition.  a10 is not in the reference code, default off and excluded from the reference parity bar
 (SURVEY §8 a10); these tests pin the kernels to the oracle semantics.
 

@@ -143,55 +143,65 @@ def test_bank_step_passes_queues_and_seed_changes(rec):
     assert not Fn.last_workspace(embed.device).busy       # no grad requested: workspace never locked
 
 
-def test_topk_step_call_sequence(rec):
+def test_topk_step_runs_through_the_step_descriptor(rec):
+    """topk_negatives rides on the step descriptor: the C step runs selection + gather and the top-k sweeps, and its
+    backward the top-k backward + scatter, with the SAME selection scratch."""
     embed, labels, seg = _inputs()
     opts = cs.ContrastOptions(max_samples=64, max_views=4, topk_negatives=7, normalize=True)
     loss = cs.pixel_contrast_loss(embed, labels, seg=seg, options=opts)
-    names = [c[0] for c in rec.calls]
-    assert names == ["pcl_step_stats", "pcl_select_gather", "pcl_infonce_topk_fwd"]
+    assert [c[0] for c in rec.calls] == ["pcl_step_stats", "pcl_step_forward"]
     ws = Fn.last_workspace(embed.device)
     ms = 64
-    sg = rec.calls[1][1]
-    assert sg[1] == embed.data_ptr() and sg[2] == ws.keys.data_ptr() and sg[3] == ws.chunk_pref.data_ptr()
-    assert sg[4] == ws.plan.data_ptr() and sg[5] is None and sg[7] == 1            # ranks NULL (device rng), normalize
-    assert sg[8] == ws.anchor_meta.data_ptr() and sg[9] == ws.anchors_f32.data_ptr() and sg[-1] == 0x5EED
-    sw, k, scratch = rec.calls[2][1][0], rec.calls[2][1][1], rec.calls[2][1][2]
-    assert k == 7 and scratch == ws.topk_scratch.data_ptr()
-    assert sw.anchors == ws.anchors_f32.data_ptr() and sw.plan == ws.plan.data_ptr()
-    assert sw.anchor_cls == ws.anchor_meta.data_ptr() + 4 * 2 * ms          # class column of anchor_meta (int32)
-    assert sw.diag_col == ws.anchor_meta.data_ptr() + 4 * 3 * ms            # reference row index (Q1)
-    assert (sw.a_rows, sw.D, sw.mode) == (ms, 32, 0)
-    assert ws.topk_scratch.numel() == 64 * 2048 + 4 * ms
-    assert rec.calls[2][1][3] == ws.partials.data_ptr() and rec.calls[2][1][4] == ws.rowstats.data_ptr()
-    assert rec.calls[2][1][5] == loss.data_ptr()
+    d = rec.calls[1][1][0]
+    assert d.topk_negatives == 7 and d.topk_scratch == ws.topk_scratch.data_ptr()
+    assert ws.topk_scratch.numel() == 64 * 2048 + 4 * ms                   # pcl_topk_scratch_u32: a_pad * bins + sel[4]
+    assert d.embed == embed.data_ptr() and d.keys == ws.keys.data_ptr() and d.chunk_pref == ws.chunk_pref.data_ptr()
+    assert d.plan == ws.plan.data_ptr() and d.ranks is None and d.normalize == 1      # ranks NULL (device rng)
+    assert d.anchor_meta == ws.anchor_meta.data_ptr() and d.anchors_f32 == ws.anchors_f32.data_ptr()
+    assert (d.g.max_samples, d.g.D, d.mode, d.precision) == (ms, 32, 0, 0)
+    assert d.partials == ws.partials.data_ptr() and d.rowstats == ws.rowstats.data_ptr() and d.loss == loss.data_ptr()
+    assert rec.calls[1][1][1] == 0x5EED
     loss.backward()
-    names = [c[0] for c in rec.calls]
-    assert names[3:] == ["pcl_infonce_topk_bwd", "pcl_scatter_grad"]
-    bw = rec.calls[3][1]
-    assert bw[1] == 7 and bw[2] == ws.topk_scratch.data_ptr() and bw[3] == ws.rowstats.data_ptr()
-    assert bw[5] == ws.dpartials.data_ptr() and bw[6] == ws.dA.data_ptr()
-    sc = rec.calls[4][1]
-    assert sc[1] == ws.plan.data_ptr() and sc[3] == ws.dA.data_ptr() and sc[6] == 1 and sc[7] == embed.grad.data_ptr()
+    assert [c[0] for c in rec.calls][2:] == ["pcl_step_backward"]
+    db, go = rec.calls[2][1][0], rec.calls[2][1][1]
+    assert db.topk_negatives == 7 and db.topk_scratch == ws.topk_scratch.data_ptr() and go is not None
+    assert db.rowstats == ws.rowstats.data_ptr() and db.dpartials == ws.dpartials.data_ptr() and db.dA == ws.dA.data_ptr()
+    assert db.plan == ws.plan.data_ptr() and db.normalize == 1 and db.grad_embed == embed.grad.data_ptr()
 
 
-def test_topk_on_the_tensor_path_call_sequence_and_bad_k(rec):
-    """precision='bf16' + topk_negatives: selection, then the tensor-path top-k forward (radix select in the wgmma sweep's
-    epilogue) and its backward with the SAME scratch (selection state)."""
+def test_topk_on_the_tensor_path_runs_through_the_step_descriptor_and_bad_k(rec):
+    """precision='bf16' + topk_negatives: the same two step calls (the C step picks the tensor-path top-k sweeps), one
+    selection scratch sized for either sweep; a negative k is refused."""
     embed, labels, seg = _inputs(D=256)
     loss = cs.pixel_contrast_loss(embed, labels, seg=seg,
                                   options=cs.ContrastOptions(max_samples=64, max_views=4, topk_negatives=3, precision="bf16"))
     ws = Fn.last_workspace(embed.device)
-    assert [c[0] for c in rec.calls] == ["pcl_step_stats", "pcl_select_gather", "pcl_infonce_tc_topk_fwd"]
-    fw = rec.calls[2][1]
-    assert fw[1] == 3 and fw[2] == ws.topk_scratch.data_ptr() and fw[3] == ws.row_m2.data_ptr()
-    assert fw[0].anchors_bf16 == ws.anchors_bf16.data_ptr() and fw[0].mode == 0 and fw[0].a_rows == 64
+    assert [c[0] for c in rec.calls] == ["pcl_step_stats", "pcl_step_forward"]
+    d = rec.calls[1][1][0]
+    assert d.precision == 1 and d.topk_negatives == 3 and d.topk_scratch == ws.topk_scratch.data_ptr()
+    assert ws.topk_scratch.numel() == 128 * 2048 + 4 * 64                  # pcl_tc_topk_scratch_u32 (128-row tiles)
+    assert d.row_m2 == ws.row_m2.data_ptr() and d.anchors_bf16 == ws.anchors_bf16.data_ptr()
+    assert d.mode == 0 and d.g.max_samples == 64 and d.loss == loss.data_ptr()
     loss.backward()
-    assert [c[0] for c in rec.calls][3:] == ["pcl_infonce_tc_topk_bwd", "pcl_scatter_grad"]
-    assert rec.calls[3][1][1] == 3 and rec.calls[3][1][2] == ws.topk_scratch.data_ptr()
+    assert [c[0] for c in rec.calls][2:] == ["pcl_step_backward"]
+    db = rec.calls[2][1][0]
+    assert db.topk_negatives == 3 and db.topk_scratch == ws.topk_scratch.data_ptr() and db.dA == ws.dA.data_ptr()
+    assert db.grad_embed == embed.grad.data_ptr()
     rec.calls.clear()
     with pytest.raises(_abi.PclError):
         cs.pixel_contrast_loss(embed, labels, seg=seg,
                                options=cs.ContrastOptions(max_samples=64, max_views=4, topk_negatives=-2))
+    # the C step itself (host-side checks, before any launch): a negative k or a missing scratch is PCL_ERR_ARG; a top-k
+    # step has no prezeroed backward and no fused path
+    real = rec._real
+    for k, scratch in ((-2, None), (3, None)):
+        bad = _abi.StepDesc()
+        bad.topk_negatives, bad.topk_scratch = k, scratch
+        assert real.pcl_step_forward(C.byref(bad), None) == -1 and real.pcl_step_backward(C.byref(bad), None, None) == -1
+    ws.desc.sync = ws.sync.data_ptr()
+    assert real.pcl_step_fused_supported(C.byref(ws.desc)) == 0
+    assert real.pcl_step_backward_prezeroed(C.byref(ws.desc), None, None) == -3
+    assert real.pcl_step_fused_loss(C.byref(ws.desc), None) == -3
 
 
 def test_loss_module_reads_topk_key():

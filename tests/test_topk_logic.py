@@ -1,6 +1,7 @@
 """a10 top-k hard negatives (extension, SURVEY §8 a10): CPU checks of the oracle semantics and of the streamed
-radix-select algorithm the kernels implement (contrastiveseg_b200/csrc/pcl_topk.cu), emulated step by step in numpy:
-order-preserving key, 11+11+10-bit levels, warp-lane bin partition, analytic zero tail, tie weights."""
+radix-select algorithm the kernels implement (contrastiveseg_b200/csrc/pcl_topk.cuh and the top-k modes of
+pcl_infonce_simt.cu), emulated step by step in numpy: order-preserving key, 11+11+10-bit levels, warp-lane bin partition,
+analytic zero tail, tie weights."""
 import numpy as np
 import pytest
 import torch

@@ -1,5 +1,6 @@
-"""a10 (per-anchor top-k hard negatives, csrc/pcl_topk.cu) at the bank shape of BASELINE configs[2] for ncu: three
+"""a10 (per-anchor top-k hard negatives, csrc/pcl_topk.cuh) at the bank shape of BASELINE configs[2] for ncu: three
 histogram sweeps + scans + weighted NEG sweep + POS + finalize (forward) and the top-k backward, exact fp32 path."""
+import hashlib
 import json
 import os
 import sys
@@ -38,4 +39,4 @@ for it in range(3):
     e2.record()
     torch.cuda.synchronize()
 print(json.dumps({"path": path, "A": A, "N": (K - 1) * 2 * M, "k": k, "fwd_ms": e0.elapsed_time(e1), "bwd_ms": e1.elapsed_time(e2),
-                  "loss": float(loss.item())}))
+                  "loss": float(loss.item()), "dA_sha256": hashlib.sha256(dA.cpu().numpy().tobytes()).hexdigest()}))
