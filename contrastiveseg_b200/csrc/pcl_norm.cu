@@ -4,6 +4,8 @@
 // HBM-bound: forward reads x once and writes y once (2 * B*D*HW*4 bytes); backward reads x and gy once and
 // writes gx once.  One CTA covers 32 consecutive pixels x all D channels: lanes run along the pixel
 // dimension (coalesced 128 B rows), the 8 warps split the channels and keep their values in registers.
+#include <type_traits>
+
 #include "pcl_common.cuh"
 #include "ptx_sm90.cuh"
 
@@ -151,6 +153,14 @@ struct WgradSmem {
 static_assert(sizeof(FwdSmem) + 1024 <= 227 * 1024, "shared memory of one H100 block");
 static_assert(sizeof(DgradSmem) + 1024 <= 227 * 1024, "shared memory of one H100 block");
 static_assert(sizeof(WgradSmem) + 1024 <= 227 * 1024, "shared memory of one H100 block");
+struct WgradBnSmem : WgradSmem {
+  alignas(16) float ss[2][DOUT];                 // scale, shift of the CTA's 256 channels (16-byte vector loads)
+};
+static_assert(sizeof(WgradBnSmem) + 1024 <= 227 * 1024, "shared memory of one H100 block");
+struct DgradBnSmem : DgradSmem {
+  float bnred[2][NT / 32][DOUT];                 // per-warp channel sums of g_u and g_u x_hat, one 256-channel pass
+};
+static_assert(sizeof(DgradBnSmem) + 1024 <= 227 * 1024, "shared memory of one H100 block");
 
 template <class T>
 __device__ __forceinline__ T& aligned_smem(uint8_t* raw) {
@@ -227,6 +237,49 @@ __device__ __forceinline__ void store8(uint8_t* tile, int r, int ch, const uint1
   *reinterpret_cast<uint4*>(tile + r * 128 + ((ch ^ (r & 7)) << 4)) = u;
 }
 
+// BatchNorm + ReLU in front of the GEMM (the BN = true instantiations).  `ss` is the per-channel state written by
+// k_bn_finalize: scale at [0, ldp), shift at [ldp, 2 ldp), batch (or running) mean at [2 ldp, 3 ldp), invstd at
+// [3 ldp, 4 ldp), 1 / count at 4 ldp.  ldp = the wgrad's column count (Cin + 1 rounded up to 256), so every channel any
+// kernel converts has an entry: scale = shift = 0 beyond Cin, except scale = 1 at channel Cin, so the wgrad's constant-1
+// bias channel passes through the affine unchanged (max(0, 1 * 1 + 0) = 1) and zero channels stay exactly 0.
+struct BnPro {
+  const float* ss; const void* y; float* part;   // y: the BN input (dgrad epilogue); part: per-tile sums (dgrad)
+  int ldp;
+};
+template <class A> struct WithBn : A { BnPro bn; };
+template <class A, bool BN> using ArgsBn = typename std::conditional<BN, WithBn<A>, A>::type;
+template <class A> __device__ __forceinline__ BnPro bn_of(const A&) { return BnPro{nullptr, nullptr, nullptr, 0}; }
+template <class A> __device__ __forceinline__ BnPro bn_of(const WithBn<A>& a) { return a.bn; }
+
+__device__ __forceinline__ float raw_f32(float v) { return v; }
+__device__ __forceinline__ float raw_f32(uint16_t v) { return __uint_as_float((uint32_t)v << 16); }
+
+// u = max(0, y scale_c + shift_c) for channels [c, c + 8) in fp32; exactly 0 at pixels >= HW (pv false).  Runs at the
+// tile store, after every raw load of the K-block has been issued.
+template <class S>
+__device__ __forceinline__ void bn_relu8(const S (&v)[8], const float* scale, const float* shift, bool pv,
+                                         float (&u)[8]) {
+  const float4* sc = reinterpret_cast<const float4*>(scale);
+  const float4* sh = reinterpret_cast<const float4*>(shift);
+  const float4 s0 = sc[0], s1 = sc[1], h0 = sh[0], h1 = sh[1];
+  const float s[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
+  const float h[8] = {h0.x, h0.y, h0.z, h0.w, h1.x, h1.y, h1.z, h1.w};
+#pragma unroll
+  for (int i = 0; i < 8; ++i) u[i] = pv ? fmaxf(fmaf(raw_f32(v[i]), s[i], h[i]), 0.f) : 0.f;
+}
+// store8 of the staged activations, through the BatchNorm + ReLU when BN (scale at ss[c], shift at ss[ld + c])
+template <bool BN, class S>
+__device__ __forceinline__ void put8(uint8_t* tile, int r, int ch, const S (&v)[8], const float* ss, int ld, int c,
+                                     bool pv) {
+  if constexpr (BN) {
+    float u[8];
+    bn_relu8(v, ss + c, ss + ld + c, pv, u);
+    store8(tile, r, ch, u);
+  } else {
+    store8(tile, r, ch, v);
+  }
+}
+
 // ------------------------------------------------------------------------------------------------------------------
 __global__ void k_proj_pack(const float* __restrict__ w, int Cin, int cin64, int cin256, __nv_bfloat16* __restrict__ wk,
                             __nv_bfloat16* __restrict__ wt) {
@@ -245,14 +298,15 @@ struct FwdArgs {
   int Cin, nkb; int64_t HW; int tiles_per_img;
 };
 
-template <class T>
-__global__ void __launch_bounds__(NT, 1) k_proj_fwd(const __grid_constant__ CUtensorMap tmW, FwdArgs<T> a) {
+template <class T, bool BN = false>
+__global__ void __launch_bounds__(NT, 1) k_proj_fwd(const __grid_constant__ CUtensorMap tmW, ArgsBn<FwdArgs<T>, BN> a) {
   extern __shared__ uint8_t smem_raw[];
   FwdSmem& sm = aligned_smem<FwdSmem>(smem_raw);
   const int t = threadIdx.x, g = t >> 7, lane = t & 31, wt = t & 127;
   const int b = blockIdx.x / a.tiles_per_img;
   const int64_t p0 = (int64_t)(blockIdx.x - b * a.tiles_per_img) * BM;
   const T* img = a.x + (int64_t)b * a.Cin * a.HW;
+  const BnPro bn = bn_of(a);
   if (t == 0) {
     ptx::prefetch_tmap(&tmW);
     for (int s = 0; s < FWD_WSTAGES; ++s) ptx::mbar_init(&sm.full[s], 1);
@@ -270,7 +324,7 @@ __global__ void __launch_bounds__(NT, 1) k_proj_fwd(const __grid_constant__ CUte
 #pragma unroll
   for (int j = 0; j < 4; ++j) load8(img, a.Cin, a.HW, 8 * (g + 2 * j), p0 + wt, -1, v[j]);
 #pragma unroll
-  for (int j = 0; j < 4; ++j) store8(sm.a[0], wt, g + 2 * j, v[j]);
+  for (int j = 0; j < 4; ++j) put8<BN>(sm.a[0], wt, g + 2 * j, v[j], bn.ss, bn.ldp, 8 * (g + 2 * j), p0 + wt < a.HW);
   ptx::fence_proxy_async();
 
   float acc[128];
@@ -298,7 +352,9 @@ __global__ void __launch_bounds__(NT, 1) k_proj_fwd(const __grid_constant__ CUte
     ptx::wgmma_commit();
     if (more) {
 #pragma unroll
-      for (int j = 0; j < 4; ++j) store8(sm.a[sa ^ 1], wt, g + 2 * j, v[j]);
+      for (int j = 0; j < 4; ++j)
+        put8<BN>(sm.a[sa ^ 1], wt, g + 2 * j, v[j], bn.ss, bn.ldp, (kb + 1) * BK + 8 * (g + 2 * j),
+                 p0 + wt < a.HW);
       ptx::fence_proxy_async();
     }
     ptx::wgmma_wait<0>();
@@ -364,10 +420,12 @@ struct DgradArgs {
   int Cin, npass; int64_t HW, HWp; int tiles_per_img;
 };
 
-template <class T>
-__global__ void __launch_bounds__(NT, 1) k_proj_dgrad(const __grid_constant__ CUtensorMap tmWt, DgradArgs<T> a) {
+template <class T, bool BN = false>
+__global__ void __launch_bounds__(NT, 1) k_proj_dgrad(const __grid_constant__ CUtensorMap tmWt,
+                                                      ArgsBn<DgradArgs<T>, BN> a) {
   extern __shared__ uint8_t smem_raw[];
-  DgradSmem& sm = aligned_smem<DgradSmem>(smem_raw);
+  using Smem = typename std::conditional<BN, DgradBnSmem, DgradSmem>::type;
+  Smem& sm = aligned_smem<Smem>(smem_raw);
   const int t = threadIdx.x, g = t >> 7, lane = t & 31, wt = t & 127;
   const int b = blockIdx.x / a.tiles_per_img;
   const int64_t p0 = (int64_t)(blockIdx.x - b * a.tiles_per_img) * BM;
@@ -444,6 +502,53 @@ __global__ void __launch_bounds__(NT, 1) k_proj_dgrad(const __grid_constant__ CU
       ptx::mbar_arrive_expect_tx(&sm.full, DOUT / BK * W_KB);
       for (int kb = 0; kb < DOUT / BK; ++kb) ptx::tma_load_2d(sm.wt[kb], &tmWt, &sm.full, kb * BK, (np + 1) * DOUT);
     }
+    if constexpr (BN) {
+      // acc is g_a, the gradient of the ReLU output.  g_u = g_a [y scale + shift > 0] (the forward's test) goes to gx;
+      // this tile's per-channel sums of g_u and g_u x_hat, x_hat = (y - mean) invstd, go to the partials, reduced in a
+      // fixed order: over the warp's 16 pixels by shuffles, over the 8 warps through shared memory.
+      const BnPro bn = a.bn;
+      const T* y = static_cast<const T*>(bn.y) + (int64_t)b * a.Cin * a.HW;
+#pragma unroll
+      for (int i = 0; i < 32; ++i)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int cl = 8 * i + 2 * q + e, c = np * DOUT + cl;
+          const float sc = bn.ss[c], sh = bn.ss[bn.ldp + c], mu = bn.ss[2 * bn.ldp + c], is = bn.ss[3 * bn.ldp + c];
+          float yv[2];
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int64_t p = p0 + g * 64 + fr + 8 * h;
+            yv[h] = (p < a.HW && c < a.Cin) ? to_f32(y[(int64_t)c * a.HW + p]) : 0.f;
+          }
+          float s1 = 0.f, s2 = 0.f;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int64_t p = p0 + g * 64 + fr + 8 * h;
+            if (p < a.HW && c < a.Cin) {
+              const float gu = fmaf(yv[h], sc, sh) > 0.f ? acc[4 * i + 2 * h + e] : 0.f;
+              gx[(int64_t)c * a.HW + p] = from_f32<T>(gu);
+              s1 += gu;
+              s2 = fmaf(gu, (yv[h] - mu) * is, s2);
+            }
+          }
+#pragma unroll
+          for (int m = 4; m < 32; m <<= 1) {
+            s1 += __shfl_xor_sync(0xffffffffu, s1, m);
+            s2 += __shfl_xor_sync(0xffffffffu, s2, m);
+          }
+          if (lane < 4) {
+            sm.bnred[0][t >> 5][cl] = s1;
+            sm.bnred[1][t >> 5][cl] = s2;
+          }
+        }
+      __syncthreads();                   // bnred is rewritten by the next pass only after its post-wgmma barrier
+      float r1 = 0.f, r2 = 0.f;
+#pragma unroll
+      for (int w = 0; w < NT / 32; ++w) { r1 += sm.bnred[0][w][t]; r2 += sm.bnred[1][w][t]; }     // fixed order
+      float* part = bn.part + (int64_t)blockIdx.x * 2 * bn.ldp + np * DOUT + t;
+      part[0] = r1;
+      part[bn.ldp] = r2;
+    } else {
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int64_t p = p0 + g * 64 + fr + 8 * h;
@@ -457,6 +562,7 @@ __global__ void __launch_bounds__(NT, 1) k_proj_dgrad(const __grid_constant__ CU
           }
       }
     }
+    }
   }
 }
 
@@ -467,10 +573,11 @@ struct WgradArgs {
   int Cin, ldp; int64_t HW; int blk_per_img; int64_t units; int splits;
 };
 
-template <class T>
-__global__ void __launch_bounds__(NT, 1) k_proj_wgrad(const __grid_constant__ CUtensorMap tmG, WgradArgs<T> a) {
+template <class T, bool BN = false>
+__global__ void __launch_bounds__(NT, 1) k_proj_wgrad(const __grid_constant__ CUtensorMap tmG, ArgsBn<WgradArgs<T>, BN> a) {
   extern __shared__ uint8_t smem_raw[];
-  WgradSmem& sm = aligned_smem<WgradSmem>(smem_raw);
+  using Smem = typename std::conditional<BN, WgradBnSmem, WgradSmem>::type;
+  Smem& sm = aligned_smem<Smem>(smem_raw);
   const int t = threadIdx.x, g = t >> 7, lane = t & 31, wt = t & 127;
   const int n0 = blockIdx.x * 128, c0 = blockIdx.y * DOUT, s = blockIdx.z;
   const int64_t u0 = a.units * s / a.splits, u1 = a.units * (s + 1) / a.splits;
@@ -478,6 +585,13 @@ __global__ void __launch_bounds__(NT, 1) k_proj_wgrad(const __grid_constant__ CU
     ptx::prefetch_tmap(&tmG);
     for (int i = 0; i < 3; ++i) ptx::mbar_init(&sm.full[i], 1);
     ptx::fence_barrier_init();
+  }
+  const float* sss = nullptr;                           // BN: scale / shift of this CTA's 256 channels
+  if constexpr (BN) {
+    const BnPro bn = a.bn;
+    sm.ss[0][t] = bn.ss[c0 + t];
+    sm.ss[1][t] = bn.ss[bn.ldp + c0 + t];
+    sss = sm.ss[0];
   }
   __syncthreads();
   auto issue_a = [&](int64_t u, int stage) {
@@ -488,9 +602,11 @@ __global__ void __launch_bounds__(NT, 1) k_proj_wgrad(const __grid_constant__ CU
   // conversion items: pixel row (t & 63) of the block, 16-byte channel chunks (t >> 6) + 4 j, j < 8 (32 chunks = 256 ch)
   const int pr = t & 63, cg = t >> 6;
   typename Staged<T>::type v[8][8];
+  bool pvb = false;                                     // BN: the staged pixel is < HW
   auto load_b = [&](int64_t u) {
     const int bb = (int)(u / a.blk_per_img), pb = (int)(u - (int64_t)bb * a.blk_per_img);
     const T* img = a.x + (int64_t)bb * a.Cin * a.HW;
+    if constexpr (BN) pvb = (int64_t)pb * WB + pr < a.HW;
 #pragma unroll
     for (int j = 0; j < 8; ++j) load8(img, a.Cin, a.HW, c0 + 8 * (cg + 4 * j), (int64_t)pb * WB + pr, a.Cin, v[j]);
   };
@@ -498,7 +614,7 @@ __global__ void __launch_bounds__(NT, 1) k_proj_wgrad(const __grid_constant__ CU
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       const int chunk = cg + 4 * j;                     // 64-channel block chunk >> 3, 16-byte chunk chunk & 7
-      store8(sm.b[stage] + (chunk >> 3) * (WB * 128), pr, chunk & 7, v[j]);
+      put8<BN>(sm.b[stage] + (chunk >> 3) * (WB * 128), pr, chunk & 7, v[j], sss, DOUT, 8 * chunk, pvb);
     }
   };
   if (t == 0)
@@ -556,11 +672,149 @@ __global__ void k_proj_reduce(const float* __restrict__ partials, int splits, in
 }
 
 // ------------------------------------------------------------------------------------------------------------------
+// BatchNorm statistics of y (B, C, HW), one CTA per channel: sum y and sum y^2 in fp64 (y^2 of an fp32 value is exact in
+// fp64, so var = E[y^2] - E[y]^2 keeps ~1e-16 relative accuracy where fp32 would cancel), in a fixed order (per-thread
+// strided sums, then a fixed shuffle tree and a fixed-order sum over the warps): bit-reproducible.  fp64 sums add up
+// across ranks, so SyncBatchNorm all-reduces them as they are.  sums[C + c] = sum y^2, sums[2 C] = B * HW.
+constexpr int ST_NT = 256, ST_UNROLL = 8;
+template <class T>
+__global__ void __launch_bounds__(ST_NT) k_bn_stats(const T* __restrict__ y, int B, int C, int64_t HW,
+                                                     double* __restrict__ sums) {
+  __shared__ double red[2][ST_NT / 32];
+  const int c = blockIdx.x, t = threadIdx.x;
+  double s = 0., s2 = 0.;
+  for (int b = 0; b < B; ++b) {
+    const T* row = y + ((int64_t)b * C + c) * HW;
+    for (int64_t p0 = 0; p0 < HW; p0 += (int64_t)ST_NT * ST_UNROLL) {
+      float v[ST_UNROLL];
+#pragma unroll
+      for (int k = 0; k < ST_UNROLL; ++k) {             // every load of the batch before any arithmetic
+        const int64_t p = p0 + k * ST_NT + t;
+        v[k] = p < HW ? to_f32(row[p]) : 0.f;
+      }
+#pragma unroll
+      for (int k = 0; k < ST_UNROLL; ++k) {
+        const double d = v[k];
+        s += d;
+        s2 = fma(d, d, s2);
+      }
+    }
+  }
+#pragma unroll
+  for (int m = 16; m > 0; m >>= 1) {
+    s += __shfl_xor_sync(0xffffffffu, s, m);
+    s2 += __shfl_xor_sync(0xffffffffu, s2, m);
+  }
+  if ((t & 31) == 0) { red[0][t >> 5] = s; red[1][t >> 5] = s2; }
+  __syncthreads();
+  if (t == 0) {
+    double r = 0., r2 = 0.;
+    for (int w = 0; w < ST_NT / 32; ++w) { r += red[0][w]; r2 += red[1][w]; }
+    sums[c] = r;
+    sums[C + c] = r2;
+    if (c == 0) sums[2 * C] = (double)B * (double)HW;
+  }
+}
+
+// sums (or the running buffers) -> the per-channel state of BnPro; training: running buffers updated in place as
+// nn.BatchNorm2d does (momentum, unbiased variance over the global count)
+__global__ void k_bn_finalize(const double* __restrict__ sums, const float* __restrict__ gamma,
+                              const float* __restrict__ beta, float* __restrict__ rmean, float* __restrict__ rvar, int C,
+                              int ldp, float eps, float momentum, int training, float* __restrict__ st) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= ldp) return;
+  float scale = c == C ? 1.f : 0.f, shift = 0.f, mean = 0.f, invstd = 0.f;
+  if (c < C) {
+    double m, var;
+    if (training) {
+      const double n = sums[2 * C];
+      m = sums[c] / n;
+      var = fmax(sums[C + c] / n - m * m, 0.);
+      rmean[c] = (float)((1. - momentum) * rmean[c] + momentum * m);
+      rvar[c] = (float)((1. - momentum) * rvar[c] + momentum * var * n / (n - 1.));
+    } else {
+      m = rmean[c];
+      var = rvar[c];
+    }
+    invstd = (float)(1. / sqrt(var + (double)eps));
+    mean = (float)m;
+    scale = gamma[c] * invstd;
+    shift = beta[c] - mean * scale;
+  }
+  st[c] = scale;
+  st[ldp + c] = shift;
+  st[2 * ldp + c] = mean;
+  st[3 * ldp + c] = invstd;
+  if (c == 0) st[4 * ldp] = training ? (float)(1. / sums[2 * C]) : 0.f;
+}
+
+// per-tile sums of g_u and g_u x_hat (the dgrad epilogue's partials, [tile][2][ldp]) -> per channel, in a fixed order;
+// gsum = (sum g_u, sum g_u x_hat) for the input gradient, gbeta / ggamma the same local sums
+constexpr int GR_NT = 1024;
+__global__ void __launch_bounds__(GR_NT) k_bn_grad_reduce(const float* __restrict__ part, int ntiles, int C, int ldp,
+                                                          float* __restrict__ gsum, float* __restrict__ ggamma,
+                                                          float* __restrict__ gbeta) {
+  __shared__ float red[2][GR_NT / 32][33];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, c = blockIdx.x * 32 + lane;
+  float s1 = 0.f, s2 = 0.f;
+  if (c < C)
+    for (int tile = w; tile < ntiles; tile += GR_NT / 32) {
+      s1 += part[(int64_t)tile * 2 * ldp + c];
+      s2 += part[(int64_t)tile * 2 * ldp + ldp + c];
+    }
+  red[0][w][lane] = s1;
+  red[1][w][lane] = s2;
+  __syncthreads();
+  if (w == 0 && c < C) {
+    float r1 = 0.f, r2 = 0.f;
+    for (int k = 0; k < GR_NT / 32; ++k) { r1 += red[0][k][lane]; r2 += red[1][k][lane]; }
+    gsum[c] = r1;
+    gsum[C + c] = r2;
+    if (gbeta) gbeta[c] = r1;
+    if (ggamma) ggamma[c] = r2;
+  }
+}
+
+// BatchNorm input gradient, in place over g (= g_u in, g_y out): training g_y = scale (g_u - mean(g_u) - x_hat
+// mean(g_u x_hat)) with the means over the (global) count; eval g_y = scale g_u.  scale = gamma invstd.
+constexpr int IG_NT = 256, IG_UNROLL = 8;
+template <class T>
+__global__ void __launch_bounds__(IG_NT) k_bn_input_grad(const T* __restrict__ y, T* __restrict__ g,
+                                                          const float* __restrict__ st, const float* __restrict__ gsum,
+                                                          int C, int ldp, int64_t HW, int training) {
+  const int64_t row = blockIdx.x;                       // b * C + c
+  const int c = (int)(row % C);
+  const float a = st[c], mu = st[2 * ldp + c], is = st[3 * ldp + c];
+  float k1 = 0.f, k2 = 0.f;
+  if (training) {
+    const float invn = st[4 * ldp];
+    k1 = gsum[c] * invn;
+    k2 = gsum[C + c] * invn * is;
+  }
+  const int64_t p0 = (int64_t)blockIdx.y * IG_NT * IG_UNROLL + threadIdx.x;
+  const T* yr = y + row * HW;
+  T* gr = g + row * HW;
+  float yv[IG_UNROLL], gv[IG_UNROLL];
+#pragma unroll
+  for (int k = 0; k < IG_UNROLL; ++k) {
+    const int64_t p = p0 + k * IG_NT;
+    yv[k] = p < HW ? to_f32(yr[p]) : 0.f;
+    gv[k] = p < HW ? to_f32(gr[p]) : 0.f;
+  }
+#pragma unroll
+  for (int k = 0; k < IG_UNROLL; ++k) {
+    const int64_t p = p0 + k * IG_NT;
+    if (p < HW) gr[p] = from_f32<T>(a * (gv[k] - k1 - (yv[k] - mu) * k2));
+  }
+}
+
+// ------------------------------------------------------------------------------------------------------------------
 struct Layout {
   int cin64, cin256, ctiles, ldp;                // wgrad columns: Cin + 1 (the bias column) rounded up to 256
   int64_t HWp, wk_bytes, wt_off, pack_bytes;
   int64_t gz_bytes, part_off, scratch_bytes;
   int64_t units; int splits, blk_per_img;
+  int64_t ntiles, bn_part_off, bn_scratch_bytes, bn_state_bytes;   // BatchNorm + ReLU variant
 };
 static inline int64_t align1k(int64_t v) { return (v + 1023) & ~(int64_t)1023; }
 static Layout layout(int B, int Cin, int64_t HW) {
@@ -583,6 +837,10 @@ static Layout layout(int B, int Cin, int64_t HW) {
   L.gz_bytes = align1k((int64_t)B * DOUT * L.HWp * 2);
   L.part_off = L.gz_bytes;
   L.scratch_bytes = L.part_off + align1k((int64_t)L.splits * DOUT * L.ldp * 4);
+  L.ntiles = (int64_t)B * ceil_div64(HW, BM);
+  L.bn_part_off = L.scratch_bytes;
+  L.bn_scratch_bytes = L.bn_part_off + align1k(L.ntiles * 2 * L.ldp * 4);
+  L.bn_state_bytes = align1k(((int64_t)4 * L.ldp + 4) * 4);
   return L;
 }
 static inline bool shape_ok(int B, int Cin, int64_t HW) {
@@ -614,21 +872,22 @@ extern "C" int pcl_proj_pack(const float* weight, int32_t Cin, void* wpack, void
   return PCL_OK;
 }
 
-template <class T>
+template <class T, bool BN = false>
 static int proj_fwd(const T* x, const void* wpack, const float* bias, int32_t B, int32_t Cin, int64_t HW, T* zn,
-                    float* inv_norm, void* stream) {
+                    float* inv_norm, void* stream, proj::BnPro bn = {}) {
   PCL_REQUIRE(x && wpack && zn && inv_norm && proj::shape_ok(B, Cin, HW));
   const proj::Layout L = proj::layout(B, Cin, HW);
   CUtensorMap tmW;
   int st = tc_make_tmap_cols(&tmW, wpack, (uint64_t)L.cin64, proj::DOUT, proj::DOUT);
   if (st != PCL_OK) return st;
-  proj::FwdArgs<T> a;
+  proj::ArgsBn<proj::FwdArgs<T>, BN> a;
   a.x = x; a.bias = bias; a.zn = zn; a.inv_norm = inv_norm;
   a.Cin = Cin; a.nkb = L.cin64 / proj::BK; a.HW = HW;
   a.tiles_per_img = (int)ceil_div64(HW, proj::BM);
+  if constexpr (BN) a.bn = bn;
   const size_t smem = sizeof(proj::FwdSmem) + 1024;
-  PCL_SMEM_OPT_IN(proj::k_proj_fwd<T>, smem);
-  proj::k_proj_fwd<T><<<(unsigned)(B * a.tiles_per_img), proj::NT, smem, (cudaStream_t)stream>>>(tmW, a);
+  PCL_SMEM_OPT_IN((proj::k_proj_fwd<T, BN>), smem);
+  proj::k_proj_fwd<T, BN><<<(unsigned)(B * a.tiles_per_img), proj::NT, smem, (cudaStream_t)stream>>>(tmW, a);
   PCL_LAUNCH_CHECK();
   return PCL_OK;
 }
@@ -647,9 +906,10 @@ extern "C" int pcl_proj_fwd_dt(const void* x, int32_t dtype, const void* wpack, 
   return PCL_ERR_ARG;                    // fp16 would be rounded to the bf16 GEMM operands: not offered
 }
 
-template <class T>
+template <class T, bool BN = false>
 static int proj_bwd(const T* x, const T* zn, const float* inv_norm, const T* gzn, const void* wpack, int32_t B,
-                    int32_t Cin, int64_t HW, void* scratch, T* gx, float* gw, float* gb, void* stream) {
+                    int32_t Cin, int64_t HW, void* scratch, T* gx, float* gw, float* gb, void* stream,
+                    proj::BnPro bn = {}) {
   PCL_REQUIRE(x && zn && inv_norm && gzn && wpack && scratch && gx && gw && proj::shape_ok(B, Cin, HW));
   const proj::Layout L = proj::layout(B, Cin, HW);
   cudaStream_t s = (cudaStream_t)stream;
@@ -662,21 +922,23 @@ static int proj_bwd(const T* x, const T* zn, const float* inv_norm, const T* gzn
   st = tc_make_tmap_cols(&tmG, gz, (uint64_t)L.HWp, (uint64_t)B * proj::DOUT, 128);
   if (st != PCL_OK) return st;
 
-  proj::DgradArgs<T> d;
+  proj::ArgsBn<proj::DgradArgs<T>, BN> d;
   d.zn = zn; d.gzn = gzn; d.inv_norm = inv_norm; d.gx = gx; d.gz = gz;
   d.Cin = Cin; d.npass = L.cin256 / proj::DOUT; d.HW = HW; d.HWp = L.HWp;
   d.tiles_per_img = (int)ceil_div64(HW, proj::BM);
-  const size_t smem_d = sizeof(proj::DgradSmem) + 1024;
-  PCL_SMEM_OPT_IN(proj::k_proj_dgrad<T>, smem_d);
-  proj::k_proj_dgrad<T><<<(unsigned)(B * d.tiles_per_img), proj::NT, smem_d, s>>>(tmWt, d);
+  if constexpr (BN) d.bn = bn;
+  const size_t smem_d = (BN ? sizeof(proj::DgradBnSmem) : sizeof(proj::DgradSmem)) + 1024;
+  PCL_SMEM_OPT_IN((proj::k_proj_dgrad<T, BN>), smem_d);
+  proj::k_proj_dgrad<T, BN><<<(unsigned)(B * d.tiles_per_img), proj::NT, smem_d, s>>>(tmWt, d);
   PCL_LAUNCH_CHECK();
 
-  proj::WgradArgs<T> w;
+  proj::ArgsBn<proj::WgradArgs<T>, BN> w;
   w.x = x; w.partials = part; w.Cin = Cin; w.ldp = L.ldp; w.HW = HW; w.blk_per_img = L.blk_per_img;
   w.units = L.units; w.splits = L.splits;
-  const size_t smem_w = sizeof(proj::WgradSmem) + 1024;
-  PCL_SMEM_OPT_IN(proj::k_proj_wgrad<T>, smem_w);
-  proj::k_proj_wgrad<T><<<dim3(proj::DOUT / 128, L.ctiles, L.splits), proj::NT, smem_w, s>>>(tmG, w);
+  if constexpr (BN) w.bn = bn;
+  const size_t smem_w = (BN ? sizeof(proj::WgradBnSmem) : sizeof(proj::WgradSmem)) + 1024;
+  PCL_SMEM_OPT_IN((proj::k_proj_wgrad<T, BN>), smem_w);
+  proj::k_proj_wgrad<T, BN><<<dim3(proj::DOUT / 128, L.ctiles, L.splits), proj::NT, smem_w, s>>>(tmG, w);
   PCL_LAUNCH_CHECK();
 
   const int64_t n = (int64_t)proj::DOUT * (Cin + 1);
@@ -701,4 +963,102 @@ extern "C" int pcl_proj_bwd_dt(const void* x, int32_t dtype, const void* zn, con
     return proj_bwd((const __nv_bfloat16*)x, (const __nv_bfloat16*)zn, inv_norm, (const __nv_bfloat16*)gzn, wpack, B,
                     Cin, HW, scratch, (__nv_bfloat16*)gx, gw, gb, stream);
   return PCL_ERR_ARG;
+}
+
+// (3) BatchNorm2d / SyncBatchNorm + ReLU in front of the fused last conv (ProjectionHead(fused=True, fuse_bn_relu=True)).
+// Replaces lib/models/modules/projection.py:17-24's BN and ReLU: the statistics pass reads y once, the GEMMs apply
+// max(0, y scale + shift) where they convert the activation tile, the dgrad epilogue masks g_a by the ReLU and sums the
+// BN backward's per-channel terms, and one elementwise pass forms the input gradient.
+//   k_bn_stats        fp64 sum y, sum y^2 per channel (one CTA per channel, fixed order)
+//   k_bn_finalize     -> scale, shift, mean, invstd (+ running buffers in training)
+//   k_proj_fwd<T, true>, k_proj_dgrad<T, true>, k_proj_wgrad<T, true>   the GEMMs with the BN + ReLU prologue / epilogue
+//   k_bn_grad_reduce  per-tile sums of the dgrad epilogue -> sum g_u, sum g_u x_hat (fixed order)
+//   k_bn_input_grad   g_u -> g_y in place
+extern "C" int64_t pcl_proj_bn_workspace_bytes(int32_t B, int32_t Cin, int64_t HW, int32_t which) {
+  if (!proj::shape_ok(B, Cin, HW) || (which != 0 && which != 1)) return PCL_ERR_ARG;
+  const proj::Layout L = proj::layout(B, Cin, HW);
+  return which == 0 ? L.bn_state_bytes : L.bn_scratch_bytes;
+}
+
+static inline bool bn_dtype_ok(int32_t dtype) { return dtype == PCL_DT_F32 || dtype == PCL_DT_BF16; }
+static inline bool bn_shape_ok(int32_t B, int32_t Cin, int64_t HW) {
+  return proj::shape_ok(B, Cin, HW) && (int64_t)B * Cin < (1ll << 31) &&
+         ceil_div64(HW, (int64_t)proj::IG_NT * proj::IG_UNROLL) <= 65535;
+}
+
+extern "C" int pcl_proj_bn_stats_dt(const void* y, int32_t dtype, int32_t B, int32_t Cin, int64_t HW, double* sums,
+                                    void* stream) {
+  PCL_REQUIRE(y && sums && bn_dtype_ok(dtype) && bn_shape_ok(B, Cin, HW));
+  cudaStream_t s = (cudaStream_t)stream;
+  if (dtype == PCL_DT_F32)
+    proj::k_bn_stats<float><<<(unsigned)Cin, proj::ST_NT, 0, s>>>((const float*)y, B, Cin, HW, sums);
+  else
+    proj::k_bn_stats<__nv_bfloat16><<<(unsigned)Cin, proj::ST_NT, 0, s>>>((const __nv_bfloat16*)y, B, Cin, HW, sums);
+  PCL_LAUNCH_CHECK();
+  return PCL_OK;
+}
+
+extern "C" int pcl_proj_bn_finalize(const double* sums, const float* gamma, const float* beta, float* running_mean,
+                                    float* running_var, int32_t Cin, float eps, float momentum, int32_t training,
+                                    void* bn_state, void* stream) {
+  PCL_REQUIRE(gamma && beta && running_mean && running_var && bn_state && Cin > 0 && Cin <= (1 << 20) && eps >= 0.f);
+  PCL_REQUIRE(training == 0 || (training == 1 && sums));
+  const proj::Layout L = proj::layout(1, Cin, 1);
+  proj::k_bn_finalize<<<(unsigned)ceil_div(L.ldp, 256), 256, 0, (cudaStream_t)stream>>>(
+      sums, gamma, beta, running_mean, running_var, Cin, L.ldp, eps, momentum, training, (float*)bn_state);
+  PCL_LAUNCH_CHECK();
+  return PCL_OK;
+}
+
+extern "C" int pcl_proj_bn_fwd_dt(const void* y, int32_t dtype, const void* bn_state, const void* wpack,
+                                  const float* bias, int32_t B, int32_t Cin, int64_t HW, void* zn, float* inv_norm,
+                                  void* stream) {
+  PCL_REQUIRE(bn_state && ((uintptr_t)bn_state & 15) == 0 && bn_dtype_ok(dtype) && bn_shape_ok(B, Cin, HW));
+  const proj::Layout L = proj::layout(B, Cin, HW);
+  const proj::BnPro bn{(const float*)bn_state, y, nullptr, L.ldp};
+  if (dtype == PCL_DT_F32)
+    return proj_fwd<float, true>((const float*)y, wpack, bias, B, Cin, HW, (float*)zn, inv_norm, stream, bn);
+  return proj_fwd<__nv_bfloat16, true>((const __nv_bfloat16*)y, wpack, bias, B, Cin, HW, (__nv_bfloat16*)zn, inv_norm,
+                                       stream, bn);
+}
+
+extern "C" int pcl_proj_bn_bwd_dt(const void* y, int32_t dtype, const void* bn_state, const void* zn,
+                                  const float* inv_norm, const void* gzn, const void* wpack, int32_t B, int32_t Cin,
+                                  int64_t HW, void* scratch, void* gu, float* gw, float* gb, float* gsum, float* ggamma,
+                                  float* gbeta, void* stream) {
+  PCL_REQUIRE(bn_state && ((uintptr_t)bn_state & 15) == 0 && gsum && scratch && bn_dtype_ok(dtype) &&
+              bn_shape_ok(B, Cin, HW));
+  const proj::Layout L = proj::layout(B, Cin, HW);
+  float* part = (float*)((uint8_t*)scratch + L.bn_part_off);
+  const proj::BnPro bn{(const float*)bn_state, y, part, L.ldp};
+  int st;
+  if (dtype == PCL_DT_F32)
+    st = proj_bwd<float, true>((const float*)y, (const float*)zn, inv_norm, (const float*)gzn, wpack, B, Cin, HW,
+                               scratch, (float*)gu, gw, gb, stream, bn);
+  else
+    st = proj_bwd<__nv_bfloat16, true>((const __nv_bfloat16*)y, (const __nv_bfloat16*)zn, inv_norm,
+                                       (const __nv_bfloat16*)gzn, wpack, B, Cin, HW, scratch, (__nv_bfloat16*)gu, gw,
+                                       gb, stream, bn);
+  if (st != PCL_OK) return st;
+  proj::k_bn_grad_reduce<<<(unsigned)ceil_div(Cin, 32), proj::GR_NT, 0, (cudaStream_t)stream>>>(
+      part, (int)L.ntiles, Cin, L.ldp, gsum, ggamma, gbeta);
+  PCL_LAUNCH_CHECK();
+  return PCL_OK;
+}
+
+extern "C" int pcl_proj_bn_input_grad_dt(const void* y, int32_t dtype, const void* bn_state, const float* gsum,
+                                         int32_t B, int32_t Cin, int64_t HW, int32_t training, void* g, void* stream) {
+  PCL_REQUIRE(y && g && bn_state && bn_dtype_ok(dtype) && bn_shape_ok(B, Cin, HW));
+  PCL_REQUIRE(training == 0 || (training == 1 && gsum));
+  const proj::Layout L = proj::layout(B, Cin, HW);
+  const dim3 grid((unsigned)((int64_t)B * Cin), (unsigned)ceil_div64(HW, (int64_t)proj::IG_NT * proj::IG_UNROLL));
+  cudaStream_t s = (cudaStream_t)stream;
+  if (dtype == PCL_DT_F32)
+    proj::k_bn_input_grad<float><<<grid, proj::IG_NT, 0, s>>>((const float*)y, (float*)g, (const float*)bn_state, gsum,
+                                                              Cin, L.ldp, HW, training);
+  else
+    proj::k_bn_input_grad<__nv_bfloat16><<<grid, proj::IG_NT, 0, s>>>(
+        (const __nv_bfloat16*)y, (__nv_bfloat16*)g, (const float*)bn_state, gsum, Cin, L.ldp, HW, training);
+  PCL_LAUNCH_CHECK();
+  return PCL_OK;
 }

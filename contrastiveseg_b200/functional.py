@@ -644,6 +644,113 @@ def project_normalize(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torc
     return _ProjNormFn.apply(x, weight, bias)
 
 
+def _bn_sync_group(bn):
+    """The process group a SyncBatchNorm in training mode reduces over (as torch's SyncBatchNorm.forward decides), or
+    None: BatchNorm2d, eval mode, no initialised process group, or a group of one rank."""
+    if not isinstance(bn, torch.nn.SyncBatchNorm) or not bn.training:
+        return None
+    import torch.distributed as dist
+    if not (dist.is_available() and dist.is_initialized()):
+        return None
+    group = bn.process_group or dist.group.WORLD
+    return group if dist.get_world_size(group) > 1 else None
+
+
+def _check_bn(bn) -> None:
+    if not isinstance(bn, (torch.nn.BatchNorm2d, torch.nn.SyncBatchNorm)):
+        raise _abi.PclError(f"bn_relu_project_normalize: bn must be BatchNorm2d or SyncBatchNorm, got {type(bn).__name__}")
+    if not bn.affine or not bn.track_running_stats:
+        raise _abi.PclError("bn_relu_project_normalize: bn needs affine=True and track_running_stats=True")
+    if bn.momentum is None:
+        raise _abi.PclError("bn_relu_project_normalize: momentum=None (cumulative moving average) is not supported")
+    for name in ("weight", "bias", "running_mean", "running_var"):
+        if getattr(bn, name).dtype != torch.float32:
+            raise _abi.PclError(f"bn_relu_project_normalize: bn.{name} must be float32")
+
+
+class _BnProjNormFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, y, gamma, beta, weight, bias, bn):
+        lib = _abi.load()
+        _require_cuda(y, "y")
+        dt = proj_dtype_code(y.dtype, "bn_relu_project_normalize")
+        B, Cin, HW = _proj_dims(y, weight)
+        if gamma.numel() != Cin:
+            raise _abi.PclError(f"bn_relu_project_normalize: bn has {gamma.numel()} channels, y has {Cin}")
+        training = bn.training
+        if training and B * HW == 1:
+            raise ValueError(f"Expected more than 1 value per channel when training, got input size {tuple(y.shape)}")
+        group = _bn_sync_group(bn)
+        dev = y.device
+        yc = y.contiguous()
+        w = weight.detach().to(device=dev, dtype=torch.float32).reshape(PROJ_DIM, Cin).contiguous()
+        bc = None if bias is None else bias.detach().to(device=dev, dtype=torch.float32).contiguous()
+        g32, b32 = gamma.detach().contiguous(), beta.detach().contiguous()
+        state = torch.empty(lib.pcl_proj_bn_workspace_bytes(B, Cin, HW, 0), dtype=torch.uint8, device=dev)
+        wpack = torch.empty(lib.pcl_proj_workspace_bytes(B, Cin, HW, 0), dtype=torch.uint8, device=dev)
+        zn = torch.empty((B, PROJ_DIM) + tuple(y.shape[2:]), dtype=y.dtype, device=dev)
+        inv = torch.empty(B * HW, dtype=torch.float32, device=dev)
+        with _on_device(dev):
+            s = _stream_ptr(dev)
+            sums = None
+            if training:
+                sums = torch.empty(2 * Cin + 1, dtype=torch.float64, device=dev)
+                _abi.check(lib.pcl_proj_bn_stats_dt(yc.data_ptr(), dt, B, Cin, HW, sums.data_ptr(), s),
+                           "pcl_proj_bn_stats_dt")
+                if group is not None:                    # fp64 sums and counts add up over the ranks
+                    torch.distributed.all_reduce(sums, group=group)
+                bn.num_batches_tracked.add_(1)
+            _abi.check(lib.pcl_proj_bn_finalize(_abi.ptr(sums), g32.data_ptr(), b32.data_ptr(),
+                                                bn.running_mean.data_ptr(), bn.running_var.data_ptr(), Cin, bn.eps,
+                                                bn.momentum, int(training), state.data_ptr(), s), "pcl_proj_bn_finalize")
+            _abi.check(lib.pcl_proj_pack(w.data_ptr(), Cin, wpack.data_ptr(), s), "pcl_proj_pack")
+            _abi.check(lib.pcl_proj_bn_fwd_dt(yc.data_ptr(), dt, state.data_ptr(), wpack.data_ptr(), _abi.ptr(bc), B,
+                                              Cin, HW, zn.data_ptr(), inv.data_ptr(), s), "pcl_proj_bn_fwd_dt")
+        ctx.save_for_backward(yc, zn, inv, wpack, state)
+        ctx.meta = (B, Cin, HW, tuple(weight.shape), bias is not None, dt, training, group, gamma.dtype)
+        return zn
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, gzn):
+        lib = _abi.load()
+        yc, zn, inv, wpack, state = ctx.saved_tensors
+        B, Cin, HW, wshape, has_bias, dt, training, group, gdtype = ctx.meta
+        dev = yc.device
+        g = gzn.to(device=dev, dtype=zn.dtype).contiguous()
+        scratch = torch.empty(lib.pcl_proj_bn_workspace_bytes(B, Cin, HW, 1), dtype=torch.uint8, device=dev)
+        gy = torch.empty_like(yc)
+        gw = torch.empty((PROJ_DIM, Cin), dtype=torch.float32, device=dev)
+        gb = torch.empty(PROJ_DIM, dtype=torch.float32, device=dev) if has_bias else None
+        gsum = torch.empty(2 * Cin, dtype=torch.float32, device=dev)
+        ggamma = torch.empty(Cin, dtype=torch.float32, device=dev)
+        gbeta = torch.empty(Cin, dtype=torch.float32, device=dev)
+        with _on_device(dev):
+            s = _stream_ptr(dev)
+            _abi.check(lib.pcl_proj_bn_bwd_dt(yc.data_ptr(), dt, state.data_ptr(), zn.data_ptr(), inv.data_ptr(),
+                                              g.data_ptr(), wpack.data_ptr(), B, Cin, HW, scratch.data_ptr(),
+                                              gy.data_ptr(), gw.data_ptr(), _abi.ptr(gb), gsum.data_ptr(),
+                                              ggamma.data_ptr(), gbeta.data_ptr(), s), "pcl_proj_bn_bwd_dt")
+            if training and group is not None:           # gamma / beta gradients stay rank-local, as in torch
+                torch.distributed.all_reduce(gsum, group=group)
+            _abi.check(lib.pcl_proj_bn_input_grad_dt(yc.data_ptr(), dt, state.data_ptr(), gsum.data_ptr(), B, Cin, HW,
+                                                     int(training), gy.data_ptr(), s), "pcl_proj_bn_input_grad_dt")
+        return gy, ggamma.to(gdtype), gbeta.to(gdtype), gw.view(wshape), gb, None
+
+
+def bn_relu_project_normalize(y: torch.Tensor, bn: torch.nn.Module, weight: torch.Tensor,
+                              bias: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """F.normalize(F.conv2d(relu(bn(y)), weight, bias), p=2, dim=1): the projection head from the output y of its
+    first conv to zn, with bn a BatchNorm2d or SyncBatchNorm (affine, tracking running stats, numeric momentum).  In
+    training mode the batch statistics (fp64 sums; over all ranks of a SyncBatchNorm's process group, one all_reduce
+    each way) normalise y, and running_mean / running_var / num_batches_tracked are updated as nn.BatchNorm2d does; in
+    eval mode the running statistics are used.  The BN output and the ReLU output are never written: the GEMMs apply
+    max(0, y scale + shift) where they convert their activation tile.  y (B, Cin, H, W) fp32 or bf16 CUDA, as for
+    project_normalize; autograd reaches y, bn.weight, bn.bias, weight and bias (bn's gradients rank-local)."""
+    _check_bn(bn)
+    return _BnProjNormFn.apply(y, bn.weight, bn.bias, weight, bias, bn)
+
+
 # ------------------------------------------------------------------------------------------------
 # tensor-core (wgmma) InfoNCE on explicit operands — D must be 256
 # ------------------------------------------------------------------------------------------------

@@ -6,6 +6,9 @@ normalise in its epilogue (functional.project_normalize, bf16 operands, fp32 acc
 ReLU of ``convmlp`` still run in torch.  The fused head takes a float32 or bfloat16 input; the dtype of the tensor
 reaching the last conv decides the output's (under ``torch.autocast(dtype=torch.bfloat16)`` the ``convmlp`` prefix
 hands it bf16, so zn is bf16).  The module tree and state_dict keys are the same either way.
+``fuse_bn_relu=True`` (with ``fused=True``, ``convmlp`` only) runs everything after the 720 -> 720 conv on the engine:
+its output y goes through functional.bn_relu_project_normalize, which applies the BatchNorm (batch statistics in
+training, running ones in eval; SyncBatchNorm reduces over its process group) and the ReLU inside the fused GEMM.
 ``normalize=False`` returns the raw projection for the fused loss path (PixelContrastLoss(..., normalize=True) then
 normalises only the sampled columns)."""
 from __future__ import annotations
@@ -14,12 +17,17 @@ import torch.nn as nn
 
 from . import functional as _fn
 from ._abi import PclError
-from .functional import l2_normalize, project_normalize
+from .functional import bn_relu_project_normalize, l2_normalize, project_normalize
 
 
 class ProjectionHead(nn.Module):
-    def __init__(self, dim_in, proj_dim=256, proj="convmlp", bn_type="torchsyncbn", normalize=True, fused=False):
+    def __init__(self, dim_in, proj_dim=256, proj="convmlp", bn_type="torchsyncbn", normalize=True, fused=False,
+                 fuse_bn_relu=False):
         super().__init__()
+        if fuse_bn_relu and not fused:
+            raise PclError("ProjectionHead(fuse_bn_relu=True) needs fused=True")
+        if fuse_bn_relu and proj != "convmlp":
+            raise PclError(f"ProjectionHead(fuse_bn_relu=True) needs proj='convmlp', got {proj!r}")
         if fused and proj_dim != _fn.PROJ_DIM:
             raise PclError(f"ProjectionHead(fused=True) needs proj_dim == {_fn.PROJ_DIM}, got {proj_dim}")
         if fused and not normalize:
@@ -34,11 +42,15 @@ class ProjectionHead(nn.Module):
             raise ValueError(f"unknown projection type {proj!r}")
         self.normalize = normalize
         self.fused = fused
+        self.fuse_bn_relu = fuse_bn_relu
 
     def forward(self, x):
         if self.fused:
             _fn._require_cuda(x, "x")
             _fn.proj_dtype_code(x.dtype, "ProjectionHead(fused=True)")
+            if self.fuse_bn_relu:
+                return bn_relu_project_normalize(self.proj[0](x), self.proj[1][0], self.proj[2].weight,
+                                                 self.proj[2].bias)
             if isinstance(self.proj, nn.Conv2d):
                 last, y = self.proj, x
             else:

@@ -232,6 +232,34 @@ int pcl_proj_bwd_dt(const void* x, int32_t dtype, const void* zn, const float* i
                     const void* wpack, int32_t B, int32_t Cin, int64_t HW, void* scratch, void* gx, float* gw,
                     float* gb, void* stream);
 
+/* The head's BatchNorm2d / SyncBatchNorm and ReLU fused into the calls above: zn = normalize(conv(relu(bn(y)))) with
+ * y (B,Cin,HW) of element type `dtype` (PCL_DT_F32 or PCL_DT_BF16; anything else returns PCL_ERR_ARG).  Training:
+ *   pcl_proj_bn_stats_dt     sums (2*Cin + 1 doubles): sum y, sum y^2 per channel, then the count B*HW.  fp64 and
+ *                            bit-reproducible; sums of several ranks add up (SyncBatchNorm all-reduces them).
+ *   pcl_proj_bn_finalize     training 1: batch mean / biased variance from sums; running_mean / running_var updated
+ *                            in place (momentum, unbiased variance over the count); training 0: the running buffers,
+ *                            nothing updated, sums may be NULL.  Writes bn_state (pcl_proj_bn_workspace_bytes(.., 0) bytes,
+ *                            16-byte aligned).
+ *   pcl_proj_bn_fwd_dt       pcl_proj_fwd_dt on max(0, (y - mean) invstd gamma + beta), never materialised.
+ *   pcl_proj_bn_bwd_dt       pcl_proj_bwd_dt through the ReLU: gu = the gradient of the BN output (B,Cin,HW, dtype),
+ *                            gw, gb as above; gsum (2*Cin floats) = sum gu, sum gu x_hat per channel; gbeta, ggamma
+ *                            (may be NULL) the same local sums.  scratch: pcl_proj_bn_workspace_bytes(.., 1) bytes.
+ *   pcl_proj_bn_input_grad_dt  gu -> the gradient of y, in place in g.  training 1 uses gsum (summed over ranks for
+ *                            SyncBatchNorm) and the count of the statistics; training 0: gamma invstd gu.
+ * No call synchronises with the host. */
+int64_t pcl_proj_bn_workspace_bytes(int32_t B, int32_t Cin, int64_t HW, int32_t which);
+int pcl_proj_bn_stats_dt(const void* y, int32_t dtype, int32_t B, int32_t Cin, int64_t HW, double* sums, void* stream);
+int pcl_proj_bn_finalize(const double* sums, const float* gamma, const float* beta, float* running_mean,
+                         float* running_var, int32_t Cin, float eps, float momentum, int32_t training, void* bn_state,
+                         void* stream);
+int pcl_proj_bn_fwd_dt(const void* y, int32_t dtype, const void* bn_state, const void* wpack, const float* bias,
+                       int32_t B, int32_t Cin, int64_t HW, void* zn, float* inv_norm, void* stream);
+int pcl_proj_bn_bwd_dt(const void* y, int32_t dtype, const void* bn_state, const void* zn, const float* inv_norm,
+                       const void* gzn, const void* wpack, int32_t B, int32_t Cin, int64_t HW, void* scratch, void* gu,
+                       float* gw, float* gb, float* gsum, float* ggamma, float* gbeta, void* stream);
+int pcl_proj_bn_input_grad_dt(const void* y, int32_t dtype, const void* bn_state, const float* gsum, int32_t B,
+                              int32_t Cin, int64_t HW, int32_t training, void* g, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * §8f row 1 (next row): the segmentation CE of ContrastCELoss.forward, fused.  Replaces
  * lib/loss/loss_contrast.py:180-181 (F.interpolate(seg, (Himg,Wimg), bilinear, align_corners=True)) +

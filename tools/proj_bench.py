@@ -1,8 +1,10 @@
 """Projection head's last 1x1 conv + L2 normalise: cuDNN Conv2d + cs.l2_normalize vs the fused wgmma GEMM
 (cs.project_normalize), forward alone and forward + backward, at S1 (8, 720, 128, 256) and DeepLab C4 (2, 2048, 66, 66),
 with fp32 activations and with bf16 activations (the fused GEMM on bf16 x against the autocast baseline: cuDNN bf16
-conv + cs.l2_normalize); then one stand-in training iteration (the structure of bench.py's train_iter) with
-ProjectionHead(fused=False / True), in fp32 and under torch.autocast(bfloat16).
+conv + cs.l2_normalize); then the convmlp head from conv1's output on: conv1 + torch BatchNorm2d + ReLU + the fused GEMM
+(ProjectionHead(fused=True)) against conv1 + cs.bn_relu_project_normalize (fuse_bn_relu=True), training mode, fp32 and
+under autocast; then one stand-in training iteration (the structure of bench.py's train_iter) with
+ProjectionHead(fused=False / True / True + fuse_bn_relu), in fp32 and under torch.autocast(bfloat16).
 
     python tools/proj_bench.py [--iters 20] [--rounds 3]
 
@@ -146,6 +148,53 @@ def head_pair(shape, iters, rounds):
               f"{fl[k] / HBM * 1e3:6.3f} ms")
 
 
+def floors_bn(B, Cin, HW, esize):
+    """bytes from conv1's output y to zn (conv1 itself excluded): (torch BN + ReLU + fused GEMM fwd, fwd+bwd, fused BN
+    path fwd, fwd+bwd); Y, Z = y and zn sizes.  torch: BN reads y twice (stats, normalise) and writes its output, ReLU
+    reads and writes, the GEMM reads; backward 10Y + 3Z.  Fused: stats and GEMM read y; backward dgrad reads zn, gzn, y
+    and writes g_u, wgrad reads y, the input gradient reads y, g_u and writes g_y (bf16 gz workspace counted in Z)."""
+    Y, Z = esize * B * Cin * HW, esize * B * 256 * HW
+    tf, tb = 6 * Y + Z, 10 * Y + 3 * Z
+    ff, fb = 2 * Y + Z, 6 * Y + 3 * Z
+    return tf, tf + tb, ff, ff + fb
+
+
+def bn_head_pair(shape, iters, rounds):
+    """conv1 -> (torch BN + ReLU + fused GEMM) against conv1 -> bn_relu_project_normalize, training mode."""
+    B, Cin, H, W = shape
+    dev = torch.device("cuda:0")
+    torch.manual_seed(0)
+    heads = {f: cs.ProjectionHead(Cin, 256, "convmlp", bn_type="torchbn", fused=True, fuse_bn_relu=f).to(dev)
+             for f in (False, True)}
+    heads[True].load_state_dict(heads[False].state_dict())
+    g = torch.Generator(device=dev).manual_seed(0)
+    x = torch.randn(shape, device=dev, generator=g).requires_grad_(True)
+    gzn = torch.randn((B, 256, H, W), device=dev, generator=g)
+    res = {}
+    for _ in range(rounds):
+        for amp in (False, True):
+            for f, head in heads.items():
+                def fwd(head=head, amp=amp):
+                    with torch.autocast("cuda", dtype=torch.bfloat16, enabled=amp):
+                        return head(x)
+
+                def fb(fwd=fwd, head=head):
+                    x.grad = None
+                    head.zero_grad(set_to_none=True)
+                    y = fwd()
+                    y.backward(gzn.to(y.dtype))
+                with torch.no_grad():
+                    res.setdefault((amp, f, "fwd"), []).append(timeit(fwd, iters))
+                res.setdefault((amp, f, "fwd+bwd"), []).append(timeit(fb, iters))
+    HW = H * W
+    for (amp, f, ph), v in res.items():
+        fl = floors_bn(B, Cin, HW, 2 if amp else 4)
+        floor = fl[(2 if f else 0) + (ph == "fwd+bwd")]
+        name = f"{'bf16' if amp else 'fp32'} {'bn_relu fused' if f else 'torch bn_relu'} {ph}"
+        print(f"  {name:28s} {min(v):8.3f} - {max(v):8.3f} ms   y->zn byte floor {floor / 1e9:6.3f} GB = "
+              f"{floor / HBM * 1e3:6.3f} ms (conv1 not counted)")
+
+
 def train_iter_pair(iters, rounds):
     """Stand-in iteration: conv body (720-channel stride-4 features) -> 19-class head + convmlp projection head ->
     ContrastCELoss (fused seg CE + pixel contrast) -> backward -> SGD step, as in bench.py's train_iter."""
@@ -156,12 +205,13 @@ def train_iter_pair(iters, rounds):
     target = data["target"].to(dev)
 
     class StandIn(nn.Module):
-        def __init__(self, fused):
+        def __init__(self, fused, fuse_bn_relu):
             super().__init__()
             self.body = nn.Sequential(nn.Conv2d(3, 64, 3, 2, 1), nn.BatchNorm2d(64), nn.ReLU(inplace=True),
                                       nn.Conv2d(64, C, 3, 2, 1), nn.BatchNorm2d(C), nn.ReLU(inplace=True))
             self.cls = nn.Conv2d(C, K, 1)
-            self.proj = cs.ProjectionHead(C, D, proj="convmlp", bn_type="torchbn", fused=fused)
+            self.proj = cs.ProjectionHead(C, D, proj="convmlp", bn_type="torchbn", fused=fused,
+                                          fuse_bn_relu=fuse_bn_relu)
 
         def forward(self, x):
             f = self.body(x)
@@ -170,9 +220,9 @@ def train_iter_pair(iters, rounds):
     x = torch.randn(B, 3, Hi, Wi, device=dev)
     runs = {}
     for amp in (False, True):
-        for fused in (False, True):
+        for fused, fuse_bn in ((False, False), (True, False), (True, True)):
             torch.manual_seed(304)
-            net = StandIn(fused).to(dev)
+            net = StandIn(fused, fuse_bn).to(dev)
             opt = torch.optim.SGD(net.parameters(), lr=0.01, momentum=0.9, weight_decay=5e-4)
             crit = cs.ContrastCELoss(cs.Configer(cs.cityscapes_contrast_config())).to(dev)
 
@@ -182,14 +232,15 @@ def train_iter_pair(iters, rounds):
                 opt.zero_grad(set_to_none=True)
                 loss.backward()
                 opt.step()
-            runs[(amp, fused)] = it
+            runs[(amp, fused, fuse_bn)] = it
     res = {k: [] for k in runs}
     for _ in range(rounds):
         for k in runs:
             res[k].append(timeit(runs[k], iters))
-    for (amp, fused), v in res.items():
+    for (amp, fused, fuse_bn), v in res.items():
         mode = "autocast(bf16)" if amp else "fp32          "
-        print(f"  train iter {mode}, ProjectionHead(fused={fused!s:5s}) {min(v):8.3f} - {max(v):8.3f} ms")
+        print(f"  train iter {mode}, ProjectionHead(fused={fused!s:5s}, fuse_bn_relu={fuse_bn!s:5s}) "
+              f"{min(v):8.3f} - {max(v):8.3f} ms")
 
 
 def main():
@@ -202,6 +253,9 @@ def main():
     print(f"card: {card()}   torch.backends.cudnn.allow_tf32 = {torch.backends.cudnn.allow_tf32}")
     for shape in ((8, 720, 128, 256), (2, 2048, 66, 66)):
         head_pair(shape, args.iters, args.rounds)
+    for shape in ((8, 720, 128, 256), (2, 2048, 66, 66)):
+        print(f"convmlp head from conv1 on, training mode, shape {shape}:")
+        bn_head_pair(shape, args.iters, args.rounds)
     train_iter_pair(max(3, args.iters // 4), args.rounds)
 
 
