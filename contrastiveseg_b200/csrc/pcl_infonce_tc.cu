@@ -232,8 +232,13 @@ k_tc_fwd(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtens
   if (w0.persistent) {
     const int R_live = (A + BM - 1) / BM;
     w0.P = (long long)R_live * T_all;
-    w0.p = ((long long)blockIdx.x * w0.P) / gridDim.x;
-    w0.p_end = ((long long)(blockIdx.x + 1) * w0.P) / gridDim.x;
+    // The grid is sized on the host for a_rows; with a device-side plan fewer pairs may be live.  Spreading them over
+    // more CTAs than pairs would leave idle CTAs between the working ones, and a CTA's ordinal among those touching a
+    // row tile (its partial slot) could then pass the slots the workspace has: the CTAs past P stay idle instead.
+    if (w0.G > w0.P) w0.G = (int)w0.P;
+    if (blockIdx.x >= w0.G) return;
+    w0.p = ((long long)blockIdx.x * w0.P) / w0.G;
+    w0.p_end = ((long long)(blockIdx.x + 1) * w0.P) / w0.G;
     if (w0.p >= w0.p_end) return;
   } else {
     const int row0 = blockIdx.x * BM;

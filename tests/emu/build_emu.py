@@ -4,6 +4,7 @@ threads (fibers) with g++, so CPU-only test runs execute the real kernel code.  
 Source rewriting (text level, the .cu files themselves are untouched):
   kernel<<<grid, block, smem, stream>>>(args)   ->  emu::cfg(grid, block, smem, stream).bind(kernel)(args)
   extern __shared__ [__align__(n)] T name[];     ->  T* name = reinterpret_cast<T*>(emu::dyn_smem());
+  __shared__ T a[N], b[M];                       ->  __shared__ emu::SharedArray<T, (N)> a; ... (index checked)
   asm volatile("bar.sync id, %0;" :: "n"(N) ...) ->  emu::named_barrier(id, N);
 The tensor path (pcl_infonce_tc.cu, pcl_infonce_fused.cu) compiles against shim/ptx_sm90.cuh, a functional model of the
 mbarrier / TMA / wgmma primitives with the product header's names (found first on the include path).
@@ -26,10 +27,18 @@ SOURCES = ["pcl_api.cu", "pcl_select.cu", "pcl_infonce_simt.cu", "pcl_topk.cu", 
 LAUNCH = re.compile(r"([A-Za-z_][\w:]*(?:<[^<>;()]*>)?)\s*<<<(.*?)>>>", re.S)
 NAMED_BARRIER = re.compile(r'asm volatile\("bar\.sync (\d+), %0;" ::"n"\((\w+)\) : "memory"\);')
 EXTERN_SHARED = re.compile(r"extern\s+__shared__\s+(?:__align__\(\d+\)\s+)?([A-Za-z_][\w ]*?)\s+(\w+)\s*\[\s*\]\s*;")
+# fixed-size 1-D __shared__ arrays, one or several declarators: `__shared__ float a[N], b[M];`
+FIXED_SHARED = re.compile(r"__shared__\s+([A-Za-z_][\w ]*?)\s+((?:\w+\s*\[[^\[\];]+\]\s*,\s*)*\w+\s*\[[^\[\];]+\])\s*;")
+DECLARATOR = re.compile(r"(\w+)\s*\[([^\[\];]+)\]")
+
+
+def _checked_shared(m: re.Match) -> str:
+    return " ".join(f"__shared__ emu::SharedArray<{m.group(1)}, ({n})> {name};" for name, n in DECLARATOR.findall(m.group(2)))
 
 
 def rewrite(text: str) -> str:
     text = EXTERN_SHARED.sub(lambda m: f"{m.group(1)}* {m.group(2)} = reinterpret_cast<{m.group(1)}*>(emu::dyn_smem());", text)
+    text = FIXED_SHARED.sub(_checked_shared, text)
     text = NAMED_BARRIER.sub(lambda m: f"emu::named_barrier({m.group(1)}, {m.group(2)});", text)
     return LAUNCH.sub(lambda m: f"emu::cfg({m.group(2)}).bind({m.group(1)})", text)
 

@@ -277,6 +277,22 @@ template <class G, class Bk>
 inline CfgBinder cfg(G g, Bk b, size_t smem = 0, cudaStream_t s = nullptr) { return CfgBinder{cfg_make(dim3(g), dim3(b), smem, s)}; }
 
 inline void* dyn_smem() { return g_blk->dyn; }
+// Fixed-size 1-D __shared__ arrays (build_emu.py rewrites `__shared__ T a[N];` to `__shared__ SharedArray<T, N> a;`):
+// an index outside [0, N) aborts, as the access would fault or corrupt a neighbouring array on the GPU.  On the host
+// the array is a process static, and a write past it lands in neighbouring storage that nothing reads back wrong, so
+// the overflow would go unseen.  Decays to T* like the array it stands for; pointer arithmetic is not checked.
+template <class T, long long N>
+struct SharedArray {
+  T v[N];
+  template <class I> T& operator[](I i) {
+    if ((long long)i < 0 || (long long)i >= N) {
+      fprintf(stderr, "emu: __shared__ array index %lld outside [0, %lld)\n", (long long)i, N);
+      abort();
+    }
+    return v[i];
+  }
+  operator T*() { return v; }
+};
 inline void named_barrier(int id, int nthreads) {
   Fiber* f = g_blk->cur;
   f->named_id = id; f->named_n = nthreads;
