@@ -115,6 +115,10 @@ SIGNATURES = {
     "pcl_proj_bn_bwd_dt": (c_i32, [c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_i64, c_vp, c_vp, c_vp,
                                    c_vp, c_vp, c_vp, c_vp, c_vp]),
     "pcl_proj_bn_input_grad_dt": (c_i32, [c_vp, c_i32, c_vp, c_vp, c_i32, c_i32, c_i64, c_i32, c_vp, c_vp]),
+    "pcl_proj_conv1_workspace_bytes": (c_i64, [c_i32, c_i32, c_i64, c_i32]),
+    "pcl_proj_conv1_pack": (c_i32, [c_vp, c_i32, c_vp, c_vp]),
+    "pcl_proj_conv1_fwd_dt": (c_i32, [c_vp, c_i32, c_vp, c_vp, c_i32, c_i32, c_i64, c_vp, c_vp, c_vp, c_vp]),
+    "pcl_proj_conv1_bwd_dt": (c_i32, [c_vp, c_i32, c_vp, c_vp, c_i32, c_i32, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "pcl_seg_ce_scratch_floats":(c_i64, [c_i32, c_i32, c_i32]),
     "pcl_seg_ce_fwd": (c_i32, [c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_vp, c_vp, c_vp]),
     "pcl_seg_ce_bwd": (c_i32, [c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_vp, c_vp, c_vp,

@@ -848,6 +848,228 @@ static inline bool shape_ok(int B, int Cin, int64_t HW) {
          ceil_div64(HW, BM) * B < (1ll << 31) && Cin <= (1 << 20);
 }
 
+// ------------------------------------------------------------------------------------------------------------------
+// (4) The head's first 1x1 convolution, C -> C, in front of (3) (ProjectionHead(..., fuse_conv1=True)).
+// Replaces lib/models/modules/projection.py:17-19's Conv2d(dim_in, dim_in, 1), its autograd backward and (3)'s
+// statistics pass over y.  bf16 operands, fp32 accumulate, as (2).
+//   k_conv1_pack     W1 (C, C) fp32 -> W1 and W1^T bf16, each (C up to 256 rows, C up to 64 columns), zero-padded
+//   k_conv1_gemm     out = W . a per pixel: CTA = 128 pixels of one image x one 256-channel band of the output; A = the
+//                    activation tile converted by the threads as in k_proj_fwd, B = the band's 256 rows of W by TMA.
+//                    The bands of one pixel tile are consecutive CTAs, so the tile is read from HBM about once and
+//                    from L2 by its other bands.  The epilogue stages the tile [channel][pixel] in the retired weight
+//                    stages (two halves of 128 channels) and writes it along pixels.
+//                    Forward (W1, x -> y): + b1, and per tile and channel the fp64 sums of the stored y and y^2 (the
+//                    values as rounded to y's type), over 32 lanes by a fixed shuffle tree.
+//                    Data gradient (W1^T, g_y -> gx).
+//   k_conv1_stats    per-tile sums -> sums[2 C + 1] in pcl_proj_bn_stats_dt's layout (fp64, fixed order)
+//   k_conv1_gy_pack  g_y -> bf16 in 256-row bands [band][b][256][HW up to 64], zero-padded: the TMA operand of
+//   k_proj_wgrad, k_proj_reduce  run once per band of gW1's rows; the band's gb1 comes from the constant-1 channel.
+struct Conv1Layout {
+  int kp, np, nbands, tiles_per_img;             // K padded to 64, rows padded to 256 = nbands x 256
+  int64_t ptiles, wt_off, pack_bytes, fwd_bytes;
+  int64_t gy_bytes, part_off, gpad_off, bwd_bytes;
+  Layout w;                                      // the weight gradient's pixel blocks and split-K partials
+};
+static Conv1Layout conv1_layout(int B, int C, int64_t HW) {
+  Conv1Layout L;
+  L.kp = ceil_div(C, BK) * BK;
+  L.nbands = ceil_div(C, DOUT);
+  L.np = L.nbands * DOUT;
+  L.tiles_per_img = (int)ceil_div64(HW, BM);
+  L.ptiles = (int64_t)B * L.tiles_per_img;
+  L.wt_off = align1k((int64_t)L.np * L.kp * 2);
+  L.pack_bytes = 2 * L.wt_off;
+  L.fwd_bytes = align1k(L.ptiles * 2 * L.np * 8);
+  L.w = layout(B, C, HW);
+  L.gy_bytes = align1k((int64_t)L.np * B * L.w.HWp * 2);
+  L.part_off = L.gy_bytes;
+  L.gpad_off = L.part_off + align1k((int64_t)L.w.splits * DOUT * L.w.ldp * 4);
+  L.bwd_bytes = L.gpad_off + align1k((int64_t)DOUT * (C + 1) * 4);
+  return L;
+}
+constexpr int GP_NT = 256, GP_UNROLL = 8;
+static inline bool conv1_shape_ok(int B, int C, int64_t HW) {
+  if (!shape_ok(B, C, HW)) return false;
+  const int64_t nb = ceil_div(C, DOUT), HWp = ceil_div64(HW, WB) * WB;
+  return ceil_div64(HW, BM) * B * nb < (1ll << 31) && (int64_t)B * nb * DOUT < (1ll << 31) &&
+         ceil_div64(HWp, (int64_t)GP_NT * GP_UNROLL) <= 65535;
+}
+
+__global__ void k_conv1_pack(const float* __restrict__ w, int C, int kp, int64_t n, __nv_bfloat16* __restrict__ wk,
+                             __nv_bfloat16* __restrict__ wt) {
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= n) return;
+  const int r = (int)(idx / kp), k = (int)(idx % kp);
+  const bool in = r < C && k < C;
+  wk[idx] = __float2bfloat16(in ? w[(int64_t)r * C + k] : 0.f);
+  wt[idx] = __float2bfloat16(in ? w[(int64_t)k * C + r] : 0.f);
+}
+
+template <class T>
+struct Conv1Args {
+  const T* a; const float* bias; T* out; double* part;   // bias, part (per-tile sums) may be null
+  int C, nkb, nbands, np; int64_t HW; int tiles_per_img;
+};
+
+template <class T>
+__global__ void __launch_bounds__(NT, 1) k_conv1_gemm(const __grid_constant__ CUtensorMap tmW, Conv1Args<T> a) {
+  extern __shared__ uint8_t smem_raw[];
+  FwdSmem& sm = aligned_smem<FwdSmem>(smem_raw);
+  const int t = threadIdx.x, g = t >> 7, lane = t & 31, wt = t & 127;
+  const int band = blockIdx.x % a.nbands, tile = blockIdx.x / a.nbands;
+  const int b = tile / a.tiles_per_img, n0 = band * DOUT;
+  const int64_t p0 = (int64_t)(tile - b * a.tiles_per_img) * BM;
+  const T* img = a.a + (int64_t)b * a.C * a.HW;
+  if (t == 0) {
+    ptx::prefetch_tmap(&tmW);
+    for (int s = 0; s < FWD_WSTAGES; ++s) ptx::mbar_init(&sm.full[s], 1);
+    ptx::fence_barrier_init();
+  }
+  sm.bias[t] = (a.bias && n0 + t < a.C) ? a.bias[n0 + t] : 0.f;
+  __syncthreads();
+  if (t == 0)
+    for (int kb = 0; kb < 2 && kb < a.nkb; ++kb) {
+      ptx::mbar_arrive_expect_tx(&sm.full[kb], W_KB);
+      ptx::tma_load_2d(sm.w[kb], &tmW, &sm.full[kb], kb * BK, n0);
+    }
+  // conversion items of this thread: pixel row wt, 16-byte channel chunks g, g + 2, g + 4, g + 6 of each K-block
+  typename Staged<T>::type v[4][8];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) load8(img, a.C, a.HW, 8 * (g + 2 * j), p0 + wt, -1, v[j]);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) store8(sm.a[0], wt, g + 2 * j, v[j]);
+  ptx::fence_proxy_async();
+
+  float acc[128];
+  const uint32_t a_off = g * WG_ROWS_BYTES;
+  for (int kb = 0; kb < a.nkb; ++kb) {
+    const int sa = kb & 1, sw = kb % FWD_WSTAGES;
+    __syncthreads();                     // A[sa] complete; every wgmma of K-block kb - 1 retired (stage reuse below)
+    if (t == 0 && kb + 2 < a.nkb) {
+      const int s2 = (kb + 2) % FWD_WSTAGES;
+      ptx::mbar_arrive_expect_tx(&sm.full[s2], W_KB);
+      ptx::tma_load_2d(sm.w[s2], &tmW, &sm.full[s2], (kb + 2) * BK, n0);
+    }
+    const bool more = kb + 1 < a.nkb;
+    if (more) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) load8(img, a.C, a.HW, (kb + 1) * BK + 8 * (g + 2 * j), p0 + wt, -1, v[j]);
+    }
+    wait_full(&sm.full[sw], (uint32_t)(kb / FWD_WSTAGES) & 1u);
+    const uint32_t abase = ptx::smem_u32(sm.a[sa]) + a_off, wbase = ptx::smem_u32(sm.w[sw]);
+    ptx::wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < BK / 16; ++k)
+      ptx::wgmma_m64n256k16<0>(acc, ptx::make_desc_kmajor_sw128(abase + k * 32), ptx::make_desc_kmajor_sw128(wbase + k * 32),
+                               (kb | k) != 0 ? 1u : 0u);
+    ptx::wgmma_commit();
+    if (more) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) store8(sm.a[sa ^ 1], wt, g + 2 * j, v[j]);
+      ptx::fence_proxy_async();
+    }
+    ptx::wgmma_wait<0>();
+    ptx::fence_operands(acc);
+  }
+
+  // epilogue: acc[4 i + 2 h + e] = pixel g 64 + fr + 8 h of the tile, channel n0 + 8 i + 2 q + e.  Staging pitch LD (in
+  // elements): a fragment store's 8 pixel rows x 4 channel pairs fall on distinct banks (132 words; 68 words for 2-byte T).
+  const int fr = 16 * (wt >> 5) + (lane >> 2), q = lane & 3;
+  constexpr int HALF = DOUT / 2, LD = sizeof(T) == 4 ? BM + 4 : BM + 8;
+  static_assert(HALF * LD * sizeof(T) <= sizeof(FwdSmem::w), "half a staged tile fits the weight stages");
+  T* stage = reinterpret_cast<T*>(sm.w[0]);
+  T* out = a.out + (int64_t)b * a.C * a.HW;
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    __syncthreads();                     // hh 0: every wgmma has read sm.w; hh 1: the first half is written out
+#pragma unroll
+    for (int i = 0; i < HALF / 8; ++i)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int cl = 8 * i + 2 * q + e;
+          stage[cl * LD + g * 64 + fr + 8 * h] = from_f32<T>(acc[4 * (HALF / 8 * hh + i) + 2 * h + e] +
+                                                             sm.bias[HALF * hh + cl]);
+        }
+    __syncthreads();
+    for (int cl = t >> 5; cl < HALF; cl += NT / 32) {          // warp = channel row, lane = pixel
+      const int c = n0 + HALF * hh + cl;
+      if (c >= a.C) break;
+      double s = 0., s2 = 0.;
+#pragma unroll
+      for (int j = 0; j < BM / 32; ++j) {
+        const int px = 32 * j + lane;
+        if (p0 + px < a.HW) {
+          const T v = stage[cl * LD + px];
+          out[(int64_t)c * a.HW + p0 + px] = v;
+          const double d = to_f32(v);
+          s += d;
+          s2 = fma(d, d, s2);
+        }
+      }
+      if (a.part) {
+#pragma unroll
+        for (int m = 16; m > 0; m >>= 1) {
+          s += __shfl_xor_sync(0xffffffffu, s, m);
+          s2 += __shfl_xor_sync(0xffffffffu, s2, m);
+        }
+        if (lane == 0) {
+          a.part[(int64_t)tile * 2 * a.np + c] = s;
+          a.part[((int64_t)tile * 2 + 1) * a.np + c] = s2;
+        }
+      }
+    }
+  }
+}
+
+// per-tile sums [tile][2][np] -> sums: 32 channels per block, the 32 warps stride the tiles, then a fixed-order sum
+constexpr int CS_NT = 1024;
+__global__ void __launch_bounds__(CS_NT) k_conv1_stats(const double* __restrict__ part, int64_t ntiles, int C, int np,
+                                                       double count, double* __restrict__ sums) {
+  __shared__ double red[2][CS_NT / 32][33];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, c = blockIdx.x * 32 + lane;
+  double s1 = 0., s2 = 0.;
+  if (c < C)
+    for (int64_t tile = w; tile < ntiles; tile += CS_NT / 32) {
+      s1 += part[tile * 2 * np + c];
+      s2 += part[(tile * 2 + 1) * np + c];
+    }
+  red[0][w][lane] = s1;
+  red[1][w][lane] = s2;
+  __syncthreads();
+  if (w == 0 && c < C) {
+    double r1 = 0., r2 = 0.;
+    for (int k = 0; k < CS_NT / 32; ++k) { r1 += red[0][k][lane]; r2 += red[1][k][lane]; }
+    sums[c] = r1;
+    sums[C + c] = r2;
+    if (c == 0) sums[2 * C] = count;
+  }
+}
+
+// g_y (B, C, HW) -> bf16 [band][b][256][HWp]: block row = (band B + b) 256 + r, zeros beyond C and HW
+template <class T>
+__global__ void __launch_bounds__(GP_NT) k_conv1_gy_pack(const T* __restrict__ gy, int B, int C, int64_t HW,
+                                                         int64_t HWp, __nv_bfloat16* __restrict__ out) {
+  const int64_t row = blockIdx.x;
+  const int r = (int)(row % DOUT), bb = (int)(row / DOUT);
+  const int b = bb % B, c = (bb / B) * DOUT + r;
+  const T* src = gy + ((int64_t)b * C + c) * HW;
+  __nv_bfloat16* dst = out + row * HWp;
+  const int64_t p0 = (int64_t)blockIdx.y * GP_NT * GP_UNROLL + threadIdx.x;
+  float v[GP_UNROLL];
+#pragma unroll
+  for (int k = 0; k < GP_UNROLL; ++k) {
+    const int64_t p = p0 + k * GP_NT;
+    v[k] = (c < C && p < HW) ? to_f32(src[p]) : 0.f;
+  }
+#pragma unroll
+  for (int k = 0; k < GP_UNROLL; ++k) {
+    const int64_t p = p0 + k * GP_NT;
+    if (p < HWp) dst[p] = __float2bfloat16(v[k]);
+  }
+}
+
 }  // namespace proj
 }  // namespace pcl
 
@@ -1061,4 +1283,114 @@ extern "C" int pcl_proj_bn_input_grad_dt(const void* y, int32_t dtype, const voi
         (const __nv_bfloat16*)y, (__nv_bfloat16*)g, (const float*)bn_state, gsum, Cin, L.ldp, HW, training);
   PCL_LAUNCH_CHECK();
   return PCL_OK;
+}
+
+// (4) the head's first 1x1 convolution (see the kernels above)
+extern "C" int64_t pcl_proj_conv1_workspace_bytes(int32_t B, int32_t C, int64_t HW, int32_t which) {
+  if (!proj::conv1_shape_ok(B, C, HW) || which < 0 || which > 2) return PCL_ERR_ARG;
+  const proj::Conv1Layout L = proj::conv1_layout(B, C, HW);
+  return which == 0 ? L.pack_bytes : which == 1 ? L.fwd_bytes : L.bwd_bytes;
+}
+
+extern "C" int pcl_proj_conv1_pack(const float* w1, int32_t C, void* pack, void* stream) {
+  PCL_REQUIRE(w1 && pack && C > 0 && C <= (1 << 20));
+  const proj::Conv1Layout L = proj::conv1_layout(1, C, 1);
+  uint8_t* base = (uint8_t*)pack;
+  const int64_t n = (int64_t)L.np * L.kp;
+  proj::k_conv1_pack<<<(unsigned)ceil_div64(n, 256), 256, 0, (cudaStream_t)stream>>>(
+      w1, C, L.kp, n, (__nv_bfloat16*)base, (__nv_bfloat16*)(base + L.wt_off));
+  PCL_LAUNCH_CHECK();
+  return PCL_OK;
+}
+
+// out (B, C, HW) = W a per pixel, W = one of the packed (np, kp) bf16 matrices
+template <class T>
+static int conv1_gemm(const T* a, const void* wmat, const float* bias, int32_t B, int32_t C, int64_t HW, T* out,
+                      double* part, cudaStream_t s) {
+  const proj::Conv1Layout L = proj::conv1_layout(B, C, HW);
+  CUtensorMap tmW;
+  int st = tc_make_tmap_cols(&tmW, wmat, (uint64_t)L.kp, (uint64_t)L.np, proj::DOUT);
+  if (st != PCL_OK) return st;
+  proj::Conv1Args<T> g{a, bias, out, part, C, L.kp / proj::BK, L.nbands, L.np, HW, L.tiles_per_img};
+  const size_t smem = sizeof(proj::FwdSmem) + 1024;
+  PCL_SMEM_OPT_IN((proj::k_conv1_gemm<T>), smem);
+  proj::k_conv1_gemm<T><<<(unsigned)(L.ptiles * L.nbands), proj::NT, smem, s>>>(tmW, g);
+  PCL_LAUNCH_CHECK();
+  return PCL_OK;
+}
+
+template <class T>
+static int conv1_fwd(const T* x, const void* pack, const float* b1, int32_t B, int32_t C, int64_t HW, T* y,
+                     double* sums, void* scratch, cudaStream_t s) {
+  const proj::Conv1Layout L = proj::conv1_layout(B, C, HW);
+  double* part = sums ? (double*)scratch : nullptr;
+  const int st = conv1_gemm(x, pack, b1, B, C, HW, y, part, s);
+  if (st != PCL_OK || !sums) return st;
+  proj::k_conv1_stats<<<(unsigned)ceil_div(C, 32), proj::CS_NT, 0, s>>>(part, L.ptiles, C, L.np,
+                                                                        (double)B * (double)HW, sums);
+  PCL_LAUNCH_CHECK();
+  return PCL_OK;
+}
+
+extern "C" int pcl_proj_conv1_fwd_dt(const void* x, int32_t dtype, const void* pack, const float* b1, int32_t B,
+                                     int32_t C, int64_t HW, void* y, double* sums, void* scratch, void* stream) {
+  PCL_REQUIRE(x && pack && y && (!sums || scratch) && bn_dtype_ok(dtype) && proj::conv1_shape_ok(B, C, HW));
+  cudaStream_t s = (cudaStream_t)stream;
+  if (dtype == PCL_DT_F32) return conv1_fwd((const float*)x, pack, b1, B, C, HW, (float*)y, sums, scratch, s);
+  return conv1_fwd((const __nv_bfloat16*)x, pack, b1, B, C, HW, (__nv_bfloat16*)y, sums, scratch, s);
+}
+
+template <class T>
+static int conv1_bwd(const T* x, const T* gy, const void* pack, int32_t B, int32_t C, int64_t HW, void* scratch,
+                     T* gx, float* gw1, float* gb1, cudaStream_t s) {
+  const proj::Conv1Layout L = proj::conv1_layout(B, C, HW);
+  const proj::Layout& W = L.w;
+  uint8_t* sc = (uint8_t*)scratch;
+  __nv_bfloat16* gyb = (__nv_bfloat16*)sc;
+  float* part = (float*)(sc + L.part_off);
+  float* gpad = (float*)(sc + L.gpad_off);                    // a last band of fewer than 256 rows: gW1 rows, gb1
+  if (gx) {
+    const int st = conv1_gemm(gy, (const uint8_t*)pack + L.wt_off, nullptr, B, C, HW, gx, nullptr, s);
+    if (st != PCL_OK) return st;
+  }
+  const dim3 grid((unsigned)((int64_t)B * L.np), (unsigned)ceil_div64(W.HWp, (int64_t)proj::GP_NT * proj::GP_UNROLL));
+  proj::k_conv1_gy_pack<T><<<grid, proj::GP_NT, 0, s>>>(gy, B, C, HW, W.HWp, gyb);
+  PCL_LAUNCH_CHECK();
+  const size_t smem_w = sizeof(proj::WgradSmem) + 1024;
+  PCL_SMEM_OPT_IN((proj::k_proj_wgrad<T, false>), smem_w);
+  const int64_t nred = (int64_t)proj::DOUT * (C + 1);
+  for (int j = 0; j < L.nbands; ++j) {
+    CUtensorMap tmG;
+    const int st = tc_make_tmap_cols(&tmG, gyb + (int64_t)j * B * proj::DOUT * W.HWp, (uint64_t)W.HWp,
+                                     (uint64_t)B * proj::DOUT, 128);
+    if (st != PCL_OK) return st;
+    proj::WgradArgs<T> w;
+    w.x = x; w.partials = part; w.Cin = C; w.ldp = W.ldp; w.HW = HW; w.blk_per_img = W.blk_per_img;
+    w.units = W.units; w.splits = W.splits;
+    proj::k_proj_wgrad<T, false><<<dim3(proj::DOUT / 128, W.ctiles, W.splits), proj::NT, smem_w, s>>>(tmG, w);
+    PCL_LAUNCH_CHECK();
+    const int rows = C - j * proj::DOUT < proj::DOUT ? C - j * proj::DOUT : proj::DOUT;
+    const bool full = rows == proj::DOUT;
+    float* gwj = full ? gw1 + (int64_t)j * proj::DOUT * C : gpad;
+    float* gbj = gb1 ? (full ? gb1 + j * proj::DOUT : gpad + (int64_t)proj::DOUT * C) : nullptr;
+    proj::k_proj_reduce<<<(unsigned)ceil_div64(nred, 256), 256, 0, s>>>(part, W.splits, C, W.ldp, gwj, gbj);
+    PCL_LAUNCH_CHECK();
+    if (!full) {
+      PCL_CUDA(cudaMemcpyAsync(gw1 + (int64_t)j * proj::DOUT * C, gpad, (size_t)rows * C * 4, cudaMemcpyDeviceToDevice,
+                               s));
+      if (gb1) PCL_CUDA(cudaMemcpyAsync(gb1 + j * proj::DOUT, gbj, (size_t)rows * 4, cudaMemcpyDeviceToDevice, s));
+    }
+  }
+  return PCL_OK;
+}
+
+extern "C" int pcl_proj_conv1_bwd_dt(const void* x, int32_t dtype, const void* gy, const void* pack, int32_t B,
+                                     int32_t C, int64_t HW, void* scratch, void* gx, float* gw1, float* gb1,
+                                     void* stream) {
+  PCL_REQUIRE(x && gy && pack && scratch && gw1 && bn_dtype_ok(dtype) && proj::conv1_shape_ok(B, C, HW));
+  cudaStream_t s = (cudaStream_t)stream;
+  if (dtype == PCL_DT_F32)
+    return conv1_bwd((const float*)x, (const float*)gy, pack, B, C, HW, scratch, (float*)gx, gw1, gb1, s);
+  return conv1_bwd((const __nv_bfloat16*)x, (const __nv_bfloat16*)gy, pack, B, C, HW, scratch, (__nv_bfloat16*)gx,
+                   gw1, gb1, s);
 }

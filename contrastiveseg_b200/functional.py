@@ -668,6 +668,57 @@ def _check_bn(bn) -> None:
             raise _abi.PclError(f"bn_relu_project_normalize: bn.{name} must be float32")
 
 
+def _bn_head_forward(lib, yc, dt, bn, gamma, beta, weight, bias, sums, group, s):
+    """From conv1's output y on: (training) the all-reduce of the statistics ``sums`` for a multi-rank SyncBatchNorm and
+    the counter, the BN state (batch or running statistics, running buffers updated), the last conv's packed weight
+    and the fused GEMM.  Returns zn, inv_norm, wpack, bn_state."""
+    B, Cin, HW = yc.shape[0], yc.shape[1], yc[0, 0].numel()
+    dev = yc.device
+    w = weight.detach().to(device=dev, dtype=torch.float32).reshape(PROJ_DIM, Cin).contiguous()
+    bc = None if bias is None else bias.detach().to(device=dev, dtype=torch.float32).contiguous()
+    g32, b32 = gamma.detach().contiguous(), beta.detach().contiguous()
+    state = torch.empty(lib.pcl_proj_bn_workspace_bytes(B, Cin, HW, 0), dtype=torch.uint8, device=dev)
+    wpack = torch.empty(lib.pcl_proj_workspace_bytes(B, Cin, HW, 0), dtype=torch.uint8, device=dev)
+    zn = torch.empty((B, PROJ_DIM) + tuple(yc.shape[2:]), dtype=yc.dtype, device=dev)
+    inv = torch.empty(B * HW, dtype=torch.float32, device=dev)
+    training = sums is not None
+    if training:
+        if group is not None:                            # fp64 sums and counts add up over the ranks
+            torch.distributed.all_reduce(sums, group=group)
+        bn.num_batches_tracked.add_(1)
+    _abi.check(lib.pcl_proj_bn_finalize(_abi.ptr(sums), g32.data_ptr(), b32.data_ptr(), bn.running_mean.data_ptr(),
+                                        bn.running_var.data_ptr(), Cin, bn.eps, bn.momentum, int(training),
+                                        state.data_ptr(), s), "pcl_proj_bn_finalize")
+    _abi.check(lib.pcl_proj_pack(w.data_ptr(), Cin, wpack.data_ptr(), s), "pcl_proj_pack")
+    _abi.check(lib.pcl_proj_bn_fwd_dt(yc.data_ptr(), dt, state.data_ptr(), wpack.data_ptr(), _abi.ptr(bc), B, Cin, HW,
+                                      zn.data_ptr(), inv.data_ptr(), s), "pcl_proj_bn_fwd_dt")
+    return zn, inv, wpack, state
+
+
+def _bn_head_backward(lib, yc, dt, zn, inv, wpack, state, gzn, has_bias, training, group, s):
+    """The backward of _bn_head_forward: returns the gradients of y, gamma, beta (rank-local), weight (256, Cin) and
+    bias (or None)."""
+    B, Cin, HW = yc.shape[0], yc.shape[1], yc[0, 0].numel()
+    dev = yc.device
+    g = gzn.to(device=dev, dtype=zn.dtype).contiguous()
+    scratch = torch.empty(lib.pcl_proj_bn_workspace_bytes(B, Cin, HW, 1), dtype=torch.uint8, device=dev)
+    gy = torch.empty_like(yc)
+    gw = torch.empty((PROJ_DIM, Cin), dtype=torch.float32, device=dev)
+    gb = torch.empty(PROJ_DIM, dtype=torch.float32, device=dev) if has_bias else None
+    gsum = torch.empty(2 * Cin, dtype=torch.float32, device=dev)
+    ggamma = torch.empty(Cin, dtype=torch.float32, device=dev)
+    gbeta = torch.empty(Cin, dtype=torch.float32, device=dev)
+    _abi.check(lib.pcl_proj_bn_bwd_dt(yc.data_ptr(), dt, state.data_ptr(), zn.data_ptr(), inv.data_ptr(), g.data_ptr(),
+                                      wpack.data_ptr(), B, Cin, HW, scratch.data_ptr(), gy.data_ptr(), gw.data_ptr(),
+                                      _abi.ptr(gb), gsum.data_ptr(), ggamma.data_ptr(), gbeta.data_ptr(), s),
+               "pcl_proj_bn_bwd_dt")
+    if training and group is not None:                   # gamma / beta gradients stay rank-local, as in torch
+        torch.distributed.all_reduce(gsum, group=group)
+    _abi.check(lib.pcl_proj_bn_input_grad_dt(yc.data_ptr(), dt, state.data_ptr(), gsum.data_ptr(), B, Cin, HW,
+                                             int(training), gy.data_ptr(), s), "pcl_proj_bn_input_grad_dt")
+    return gy, ggamma, gbeta, gw, gb
+
+
 class _BnProjNormFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, y, gamma, beta, weight, bias, bn):
@@ -683,13 +734,6 @@ class _BnProjNormFn(torch.autograd.Function):
         group = _bn_sync_group(bn)
         dev = y.device
         yc = y.contiguous()
-        w = weight.detach().to(device=dev, dtype=torch.float32).reshape(PROJ_DIM, Cin).contiguous()
-        bc = None if bias is None else bias.detach().to(device=dev, dtype=torch.float32).contiguous()
-        g32, b32 = gamma.detach().contiguous(), beta.detach().contiguous()
-        state = torch.empty(lib.pcl_proj_bn_workspace_bytes(B, Cin, HW, 0), dtype=torch.uint8, device=dev)
-        wpack = torch.empty(lib.pcl_proj_workspace_bytes(B, Cin, HW, 0), dtype=torch.uint8, device=dev)
-        zn = torch.empty((B, PROJ_DIM) + tuple(y.shape[2:]), dtype=y.dtype, device=dev)
-        inv = torch.empty(B * HW, dtype=torch.float32, device=dev)
         with _on_device(dev):
             s = _stream_ptr(dev)
             sums = None
@@ -697,17 +741,9 @@ class _BnProjNormFn(torch.autograd.Function):
                 sums = torch.empty(2 * Cin + 1, dtype=torch.float64, device=dev)
                 _abi.check(lib.pcl_proj_bn_stats_dt(yc.data_ptr(), dt, B, Cin, HW, sums.data_ptr(), s),
                            "pcl_proj_bn_stats_dt")
-                if group is not None:                    # fp64 sums and counts add up over the ranks
-                    torch.distributed.all_reduce(sums, group=group)
-                bn.num_batches_tracked.add_(1)
-            _abi.check(lib.pcl_proj_bn_finalize(_abi.ptr(sums), g32.data_ptr(), b32.data_ptr(),
-                                                bn.running_mean.data_ptr(), bn.running_var.data_ptr(), Cin, bn.eps,
-                                                bn.momentum, int(training), state.data_ptr(), s), "pcl_proj_bn_finalize")
-            _abi.check(lib.pcl_proj_pack(w.data_ptr(), Cin, wpack.data_ptr(), s), "pcl_proj_pack")
-            _abi.check(lib.pcl_proj_bn_fwd_dt(yc.data_ptr(), dt, state.data_ptr(), wpack.data_ptr(), _abi.ptr(bc), B,
-                                              Cin, HW, zn.data_ptr(), inv.data_ptr(), s), "pcl_proj_bn_fwd_dt")
+            zn, inv, wpack, state = _bn_head_forward(lib, yc, dt, bn, gamma, beta, weight, bias, sums, group, s)
         ctx.save_for_backward(yc, zn, inv, wpack, state)
-        ctx.meta = (B, Cin, HW, tuple(weight.shape), bias is not None, dt, training, group, gamma.dtype)
+        ctx.meta = (tuple(weight.shape), bias is not None, dt, training, group, gamma.dtype)
         return zn
 
     @staticmethod
@@ -715,26 +751,11 @@ class _BnProjNormFn(torch.autograd.Function):
     def backward(ctx, gzn):
         lib = _abi.load()
         yc, zn, inv, wpack, state = ctx.saved_tensors
-        B, Cin, HW, wshape, has_bias, dt, training, group, gdtype = ctx.meta
+        wshape, has_bias, dt, training, group, gdtype = ctx.meta
         dev = yc.device
-        g = gzn.to(device=dev, dtype=zn.dtype).contiguous()
-        scratch = torch.empty(lib.pcl_proj_bn_workspace_bytes(B, Cin, HW, 1), dtype=torch.uint8, device=dev)
-        gy = torch.empty_like(yc)
-        gw = torch.empty((PROJ_DIM, Cin), dtype=torch.float32, device=dev)
-        gb = torch.empty(PROJ_DIM, dtype=torch.float32, device=dev) if has_bias else None
-        gsum = torch.empty(2 * Cin, dtype=torch.float32, device=dev)
-        ggamma = torch.empty(Cin, dtype=torch.float32, device=dev)
-        gbeta = torch.empty(Cin, dtype=torch.float32, device=dev)
         with _on_device(dev):
-            s = _stream_ptr(dev)
-            _abi.check(lib.pcl_proj_bn_bwd_dt(yc.data_ptr(), dt, state.data_ptr(), zn.data_ptr(), inv.data_ptr(),
-                                              g.data_ptr(), wpack.data_ptr(), B, Cin, HW, scratch.data_ptr(),
-                                              gy.data_ptr(), gw.data_ptr(), _abi.ptr(gb), gsum.data_ptr(),
-                                              ggamma.data_ptr(), gbeta.data_ptr(), s), "pcl_proj_bn_bwd_dt")
-            if training and group is not None:           # gamma / beta gradients stay rank-local, as in torch
-                torch.distributed.all_reduce(gsum, group=group)
-            _abi.check(lib.pcl_proj_bn_input_grad_dt(yc.data_ptr(), dt, state.data_ptr(), gsum.data_ptr(), B, Cin, HW,
-                                                     int(training), gy.data_ptr(), s), "pcl_proj_bn_input_grad_dt")
+            gy, ggamma, gbeta, gw, gb = _bn_head_backward(lib, yc, dt, zn, inv, wpack, state, gzn, has_bias, training,
+                                                          group, _stream_ptr(dev))
         return gy, ggamma.to(gdtype), gbeta.to(gdtype), gw.view(wshape), gb, None
 
 
@@ -749,6 +770,80 @@ def bn_relu_project_normalize(y: torch.Tensor, bn: torch.nn.Module, weight: torc
     project_normalize; autograd reaches y, bn.weight, bn.bias, weight and bias (bn's gradients rank-local)."""
     _check_bn(bn)
     return _BnProjNormFn.apply(y, bn.weight, bn.bias, weight, bias, bn)
+
+
+class _ConvBnProjNormFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, w1, b1, gamma, beta, w2, b2, bn):
+        lib = _abi.load()
+        _require_cuda(x, "x")
+        dt = proj_dtype_code(x.dtype, "conv_bn_relu_project_normalize")
+        B, C, HW = _proj_dims(x, w2)
+        if w1.shape[0] != C or w1.numel() != C * C:
+            raise _abi.PclError(f"conv_bn_relu_project_normalize: w1 must be ({C}, {C}, 1, 1), got {tuple(w1.shape)}")
+        if b1 is not None and b1.numel() != C:
+            raise _abi.PclError(f"conv_bn_relu_project_normalize: b1 must have {C} elements, got {b1.numel()}")
+        if gamma.numel() != C:
+            raise _abi.PclError(f"conv_bn_relu_project_normalize: bn has {gamma.numel()} channels, x has {C}")
+        training = bn.training
+        if training and B * HW == 1:
+            raise ValueError(f"Expected more than 1 value per channel when training, got input size {tuple(x.shape)}")
+        group = _bn_sync_group(bn)
+        dev = x.device
+        xc = x.contiguous()
+        w = w1.detach().to(device=dev, dtype=torch.float32).reshape(C, C).contiguous()
+        bc = None if b1 is None else b1.detach().to(device=dev, dtype=torch.float32).contiguous()
+        pack = torch.empty(lib.pcl_proj_conv1_workspace_bytes(B, C, HW, 0), dtype=torch.uint8, device=dev)
+        y = torch.empty_like(xc)
+        with _on_device(dev):
+            s = _stream_ptr(dev)
+            sums = scratch = None
+            if training:                                 # the statistics of y come out of conv1's epilogue
+                sums = torch.empty(2 * C + 1, dtype=torch.float64, device=dev)
+                scratch = torch.empty(lib.pcl_proj_conv1_workspace_bytes(B, C, HW, 1), dtype=torch.uint8, device=dev)
+            _abi.check(lib.pcl_proj_conv1_pack(w.data_ptr(), C, pack.data_ptr(), s), "pcl_proj_conv1_pack")
+            _abi.check(lib.pcl_proj_conv1_fwd_dt(xc.data_ptr(), dt, pack.data_ptr(), _abi.ptr(bc), B, C, HW,
+                                                 y.data_ptr(), _abi.ptr(sums), _abi.ptr(scratch), s),
+                       "pcl_proj_conv1_fwd_dt")
+            zn, inv, wpack, state = _bn_head_forward(lib, y, dt, bn, gamma, beta, w2, b2, sums, group, s)
+        ctx.save_for_backward(xc, y, zn, inv, pack, wpack, state)
+        ctx.meta = (tuple(w1.shape), b1 is not None, tuple(w2.shape), b2 is not None, dt, training, group, gamma.dtype)
+        return zn
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, gzn):
+        lib = _abi.load()
+        xc, y, zn, inv, pack, wpack, state = ctx.saved_tensors
+        w1shape, has_b1, w2shape, has_b2, dt, training, group, gdtype = ctx.meta
+        B, C, HW = xc.shape[0], xc.shape[1], xc[0, 0].numel()
+        dev = xc.device
+        gx = torch.empty_like(xc) if ctx.needs_input_grad[0] else None
+        gw1 = torch.empty((C, C), dtype=torch.float32, device=dev)
+        gb1 = torch.empty(C, dtype=torch.float32, device=dev) if has_b1 else None
+        with _on_device(dev):
+            s = _stream_ptr(dev)
+            gy, ggamma, gbeta, gw2, gb2 = _bn_head_backward(lib, y, dt, zn, inv, wpack, state, gzn, has_b2, training,
+                                                            group, s)
+            scratch = torch.empty(lib.pcl_proj_conv1_workspace_bytes(B, C, HW, 2), dtype=torch.uint8, device=dev)
+            _abi.check(lib.pcl_proj_conv1_bwd_dt(xc.data_ptr(), dt, gy.data_ptr(), pack.data_ptr(), B, C, HW,
+                                                 scratch.data_ptr(), _abi.ptr(gx), gw1.data_ptr(), _abi.ptr(gb1), s),
+                       "pcl_proj_conv1_bwd_dt")
+        return (gx, gw1.view(w1shape), gb1, ggamma.to(gdtype), gbeta.to(gdtype), gw2.view(w2shape), gb2, None)
+
+
+def conv_bn_relu_project_normalize(x: torch.Tensor, w1: torch.Tensor, b1: Optional[torch.Tensor], bn: torch.nn.Module,
+                                   w2: torch.Tensor, b2: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """F.normalize(F.conv2d(relu(bn(F.conv2d(x, w1, b1))), w2, b2), p=2, dim=1): the whole ``convmlp`` projection head
+    on the engine.  The first 1x1 convolution (w1 (C, C, 1, 1), b1 (C) or None) is a bf16 wgmma GEMM whose epilogue
+    also sums the BatchNorm statistics of its output y; y then goes through bn_relu_project_normalize's kernels (same
+    rules for bn: batch statistics in training with the running buffers and num_batches_tracked updated, SyncBatchNorm
+    reduced over its process group, running statistics in eval).  x (B, C, H, W) fp32 or bf16 CUDA decides y's and
+    zn's dtype (fp32 x is rounded to the bf16 GEMM operand).  autograd reaches x, w1, b1, bn.weight, bn.bias, w2 and b2
+    (bn's gradients rank-local); x's gradient is skipped when x needs none.  No cuDNN call: forward and backward are
+    capturable and bit-reproducible run to run."""
+    _check_bn(bn)
+    return _ConvBnProjNormFn.apply(x, w1, b1, bn.weight, bn.bias, w2, b2, bn)
 
 
 # ------------------------------------------------------------------------------------------------

@@ -260,6 +260,28 @@ int pcl_proj_bn_bwd_dt(const void* y, int32_t dtype, const void* bn_state, const
 int pcl_proj_bn_input_grad_dt(const void* y, int32_t dtype, const void* bn_state, const float* gsum, int32_t B,
                               int32_t Cin, int64_t HW, int32_t training, void* g, void* stream);
 
+/* The head's first 1x1 convolution (Conv2d(C, C, 1), lib/models/modules/projection.py:17-19) in front of the calls
+ * above, as bf16 wgmma GEMMs (fp32 accumulate), forward and backward, with the BatchNorm statistics of its output in the
+ * forward's epilogue.  x, y, gy and gx (B,C,HW) have element type `dtype` (PCL_DT_F32 or PCL_DT_BF16; anything else
+ * returns PCL_ERR_ARG); an fp32 x is rounded to bf16 to nearest-even, a bf16 x is the operand as it is.  w1 (C,C),
+ * b1 (C), gw1 (C,C) and gb1 (C) are fp32.  Any C >= 1 and any HW.
+ *   pack     pcl_proj_conv1_workspace_bytes(B, C, HW, 0) bytes: the bf16 copies of w1 written by pcl_proj_conv1_pack;
+ *            pack again whenever w1 changes.  Used by the forward and the backward.
+ *   pcl_proj_conv1_fwd_dt  y = w1 x + b1 per pixel (b1 may be NULL), stored in `dtype`.  sums (may be NULL: no
+ *            statistics) gets exactly what pcl_proj_bn_stats_dt(y, ...) writes: the fp64 sums of the stored y and y^2
+ *            per channel, then the count B*HW, in a fixed order (bit-reproducible).  scratch (may be NULL when sums
+ *            is): pcl_proj_conv1_workspace_bytes(.., 1) bytes.
+ *   pcl_proj_conv1_bwd_dt  gx = w1^T gy per pixel (gx may be NULL: not computed), gw1 = sum over pixels of gy x^T and
+ *            gb1 (may be NULL) = sum over pixels of gy, gy rounded to bf16 for the GEMMs; gw1 and gb1 are reduced in a
+ *            fixed order (bit-reproducible).  scratch: pcl_proj_conv1_workspace_bytes(.., 2) bytes.
+ * The size query returns a negative pcl_status for an unsupported shape.  No call synchronises with the host. */
+int64_t pcl_proj_conv1_workspace_bytes(int32_t B, int32_t C, int64_t HW, int32_t which);
+int pcl_proj_conv1_pack(const float* w1, int32_t C, void* pack, void* stream);
+int pcl_proj_conv1_fwd_dt(const void* x, int32_t dtype, const void* pack, const float* b1, int32_t B, int32_t C,
+                          int64_t HW, void* y, double* sums, void* scratch, void* stream);
+int pcl_proj_conv1_bwd_dt(const void* x, int32_t dtype, const void* gy, const void* pack, int32_t B, int32_t C,
+                          int64_t HW, void* scratch, void* gx, float* gw1, float* gb1, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * §8f row 1 (next row): the segmentation CE of ContrastCELoss.forward, fused.  Replaces
  * lib/loss/loss_contrast.py:180-181 (F.interpolate(seg, (Himg,Wimg), bilinear, align_corners=True)) +

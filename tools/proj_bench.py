@@ -3,8 +3,10 @@
 with fp32 activations and with bf16 activations (the fused GEMM on bf16 x against the autocast baseline: cuDNN bf16
 conv + cs.l2_normalize); then the convmlp head from conv1's output on: conv1 + torch BatchNorm2d + ReLU + the fused GEMM
 (ProjectionHead(fused=True)) against conv1 + cs.bn_relu_project_normalize (fuse_bn_relu=True), training mode, fp32 and
-under autocast; then one stand-in training iteration (the structure of bench.py's train_iter) with
-ProjectionHead(fused=False / True / True + fuse_bn_relu), in fp32 and under torch.autocast(bfloat16).
+under autocast, and the whole head on the engine (fuse_conv1=True); conv1 alone (cuDNN Conv2d(C, C, 1) against the
+engine's pcl_proj_conv1_* GEMMs) with its byte and operation floors; then one stand-in training iteration (the
+structure of bench.py's train_iter) with ProjectionHead(fused=False / True / True + fuse_bn_relu / True + fuse_bn_relu +
+fuse_conv1), in fp32 and under torch.autocast(bfloat16).
 
     python tools/proj_bench.py [--iters 20] [--rounds 3]
 
@@ -24,6 +26,7 @@ import torch.nn.functional as F  # noqa: E402
 import contrastiveseg_b200 as cs  # noqa: E402
 
 HBM = 3.35e12
+BF16_DENSE = 989e12
 
 
 def card():
@@ -160,13 +163,15 @@ def floors_bn(B, Cin, HW, esize):
 
 
 def bn_head_pair(shape, iters, rounds):
-    """conv1 -> (torch BN + ReLU + fused GEMM) against conv1 -> bn_relu_project_normalize, training mode."""
+    """conv1 -> (torch BN + ReLU + fused GEMM) against conv1 -> bn_relu_project_normalize and against the whole head on
+    the engine (conv_bn_relu_project_normalize), training mode."""
     B, Cin, H, W = shape
     dev = torch.device("cuda:0")
     torch.manual_seed(0)
-    heads = {f: cs.ProjectionHead(Cin, 256, "convmlp", bn_type="torchbn", fused=True, fuse_bn_relu=f).to(dev)
-             for f in (False, True)}
-    heads[True].load_state_dict(heads[False].state_dict())
+    heads = {f: cs.ProjectionHead(Cin, 256, "convmlp", bn_type="torchbn", fused=True, fuse_bn_relu=f != "off",
+                                  fuse_conv1=f == "conv1").to(dev) for f in ("off", "bn_relu", "conv1")}
+    for f in ("bn_relu", "conv1"):
+        heads[f].load_state_dict(heads["off"].state_dict())
     g = torch.Generator(device=dev).manual_seed(0)
     x = torch.randn(shape, device=dev, generator=g).requires_grad_(True)
     gzn = torch.randn((B, 256, H, W), device=dev, generator=g)
@@ -188,11 +193,88 @@ def bn_head_pair(shape, iters, rounds):
                 res.setdefault((amp, f, "fwd+bwd"), []).append(timeit(fb, iters))
     HW = H * W
     for (amp, f, ph), v in res.items():
+        name = f"{'bf16' if amp else 'fp32'} {HEAD_NAMES[f]} {ph}"
+        if f == "conv1":
+            print(f"  {name:28s} {min(v):8.3f} - {max(v):8.3f} ms   (whole head, conv1 included)")
+            continue
         fl = floors_bn(B, Cin, HW, 2 if amp else 4)
-        floor = fl[(2 if f else 0) + (ph == "fwd+bwd")]
-        name = f"{'bf16' if amp else 'fp32'} {'bn_relu fused' if f else 'torch bn_relu'} {ph}"
+        floor = fl[(2 if f == "bn_relu" else 0) + (ph == "fwd+bwd")]
         print(f"  {name:28s} {min(v):8.3f} - {max(v):8.3f} ms   y->zn byte floor {floor / 1e9:6.3f} GB = "
               f"{floor / HBM * 1e3:6.3f} ms (conv1 not counted)")
+
+
+HEAD_NAMES = {"off": "torch bn_relu", "bn_relu": "bn_relu fused", "conv1": "conv1+bn_relu fused"}
+
+
+def conv1_pair(shape, iters, rounds):
+    """conv1 alone: cuDNN Conv2d(C, C, 1) (fp32 with TF32 allowed; bf16 under autocast) against the engine's
+    pcl_proj_conv1_* calls (pack + GEMM with the BN sums; backward: data gradient, g_y packing, weight gradient), forward
+    and forward + backward.  Floors: bytes = x read and y written (forward), g_y read and gx written (data gradient),
+    x and g_y read (weight gradient); operations = 2 B HW C^2 per GEMM at the dense bf16 rate."""
+    from contrastiveseg_b200 import _abi
+    from contrastiveseg_b200 import functional as Fn
+    B, C, H, W = shape
+    HW = H * W
+    dev = torch.device("cuda:0")
+    lib = _abi.load()
+    torch.manual_seed(0)
+    conv = nn.Conv2d(C, C, 1).to(dev)
+    g = torch.Generator(device=dev).manual_seed(0)
+    x32 = torch.randn(shape, device=dev, generator=g).requires_grad_(True)
+    gy32 = torch.randn(shape, device=dev, generator=g)
+    x16 = x32.detach().to(torch.bfloat16).requires_grad_(True)
+    gy16 = gy32.to(torch.bfloat16)
+    pack = torch.empty(lib.pcl_proj_conv1_workspace_bytes(B, C, HW, 0), dtype=torch.uint8, device=dev)
+    fscr = torch.empty(lib.pcl_proj_conv1_workspace_bytes(B, C, HW, 1), dtype=torch.uint8, device=dev)
+    bscr = torch.empty(lib.pcl_proj_conv1_workspace_bytes(B, C, HW, 2), dtype=torch.uint8, device=dev)
+    sums = torch.empty(2 * C + 1, dtype=torch.float64, device=dev)
+    w = conv.weight.detach().reshape(C, C).contiguous()
+    gw1 = torch.empty((C, C), device=dev)
+    gb1 = torch.empty(C, device=dev)
+    bufs = {torch.float32: (torch.empty_like(x32), torch.empty_like(x32)),
+            torch.bfloat16: (torch.empty_like(x16), torch.empty_like(x16))}
+
+    def engine(x, gy, bwd):
+        dt = Fn.proj_dtype_code(x.dtype)
+        y, gx = bufs[x.dtype]
+
+        def run():
+            s = torch.cuda.current_stream().cuda_stream
+            _abi.check(lib.pcl_proj_conv1_pack(w.data_ptr(), C, pack.data_ptr(), s))
+            _abi.check(lib.pcl_proj_conv1_fwd_dt(x.data_ptr(), dt, pack.data_ptr(), conv.bias.data_ptr(), B, C, HW,
+                                                 y.data_ptr(), sums.data_ptr(), fscr.data_ptr(), s))
+            if bwd:
+                _abi.check(lib.pcl_proj_conv1_bwd_dt(x.data_ptr(), dt, gy.data_ptr(), pack.data_ptr(), B, C, HW,
+                                                     bscr.data_ptr(), gx.data_ptr(), gw1.data_ptr(), gb1.data_ptr(),
+                                                     s))
+        return run
+
+    def cudnn(x, gy, bwd, amp):
+        def run():
+            with torch.autocast("cuda", dtype=torch.bfloat16, enabled=amp):
+                y = conv(x)
+            if bwd:
+                x.grad = None
+                conv.weight.grad = conv.bias.grad = None
+                y.backward(gy.to(y.dtype))
+        return run
+
+    arms = {}
+    for act, x, gy, amp in (("fp32", x32, gy32, False), ("bf16", x16, gy16, True)):
+        for ph, bwd in (("fwd", False), ("fwd+bwd", True)):
+            arms[(act, "cudnn", ph)] = cudnn(x32 if amp else x, gy, bwd, amp)
+            arms[(act, "engine", ph)] = engine(x, gy, bwd)
+    res = {k: [] for k in arms}
+    for _ in range(rounds):
+        for k, fn in arms.items():                           # every arm once per round, fp32 and bf16 alternating
+            res[k].append(timeit(fn, iters))
+    print(f"conv1 alone, shape {shape} (cudnn fp32: TF32 allowed = {torch.backends.cudnn.allow_tf32}; "
+          f"bf16: cudnn under autocast from an fp32 x, the engine on a bf16 x):")
+    for (act, name, ph), v in res.items():
+        X = (4 if act == "fp32" else 2) * B * C * HW
+        nbytes, flop = (2 * X, 2 * B * HW * C * C) if ph == "fwd" else (6 * X, 6 * B * HW * C * C)
+        print(f"  {act} {name:7s} {ph:8s} {min(v):8.3f} - {max(v):8.3f} ms   byte floor {nbytes / 1e9:6.3f} GB = "
+              f"{nbytes / HBM * 1e3:6.3f} ms   op floor {flop / 1e9:7.1f} GFLOP = {flop / BF16_DENSE * 1e3:6.3f} ms")
 
 
 def train_iter_pair(iters, rounds):
@@ -205,13 +287,13 @@ def train_iter_pair(iters, rounds):
     target = data["target"].to(dev)
 
     class StandIn(nn.Module):
-        def __init__(self, fused, fuse_bn_relu):
+        def __init__(self, fused, fuse_bn_relu, fuse_conv1):
             super().__init__()
             self.body = nn.Sequential(nn.Conv2d(3, 64, 3, 2, 1), nn.BatchNorm2d(64), nn.ReLU(inplace=True),
                                       nn.Conv2d(64, C, 3, 2, 1), nn.BatchNorm2d(C), nn.ReLU(inplace=True))
             self.cls = nn.Conv2d(C, K, 1)
             self.proj = cs.ProjectionHead(C, D, proj="convmlp", bn_type="torchbn", fused=fused,
-                                          fuse_bn_relu=fuse_bn_relu)
+                                          fuse_bn_relu=fuse_bn_relu, fuse_conv1=fuse_conv1)
 
         def forward(self, x):
             f = self.body(x)
@@ -220,9 +302,10 @@ def train_iter_pair(iters, rounds):
     x = torch.randn(B, 3, Hi, Wi, device=dev)
     runs = {}
     for amp in (False, True):
-        for fused, fuse_bn in ((False, False), (True, False), (True, True)):
+        for fused, fuse_bn, fuse_c1 in ((False, False, False), (True, False, False), (True, True, False),
+                                        (True, True, True)):
             torch.manual_seed(304)
-            net = StandIn(fused, fuse_bn).to(dev)
+            net = StandIn(fused, fuse_bn, fuse_c1).to(dev)
             opt = torch.optim.SGD(net.parameters(), lr=0.01, momentum=0.9, weight_decay=5e-4)
             crit = cs.ContrastCELoss(cs.Configer(cs.cityscapes_contrast_config())).to(dev)
 
@@ -232,15 +315,15 @@ def train_iter_pair(iters, rounds):
                 opt.zero_grad(set_to_none=True)
                 loss.backward()
                 opt.step()
-            runs[(amp, fused, fuse_bn)] = it
+            runs[(amp, fused, fuse_bn, fuse_c1)] = it
     res = {k: [] for k in runs}
     for _ in range(rounds):
         for k in runs:
             res[k].append(timeit(runs[k], iters))
-    for (amp, fused, fuse_bn), v in res.items():
+    for (amp, fused, fuse_bn, fuse_c1), v in res.items():
         mode = "autocast(bf16)" if amp else "fp32          "
-        print(f"  train iter {mode}, ProjectionHead(fused={fused!s:5s}, fuse_bn_relu={fuse_bn!s:5s}) "
-              f"{min(v):8.3f} - {max(v):8.3f} ms")
+        print(f"  train iter {mode}, ProjectionHead(fused={fused!s:5s}, fuse_bn_relu={fuse_bn!s:5s}, "
+              f"fuse_conv1={fuse_c1!s:5s}) {min(v):8.3f} - {max(v):8.3f} ms")
 
 
 def main():
@@ -253,6 +336,8 @@ def main():
     print(f"card: {card()}   torch.backends.cudnn.allow_tf32 = {torch.backends.cudnn.allow_tf32}")
     for shape in ((8, 720, 128, 256), (2, 2048, 66, 66)):
         head_pair(shape, args.iters, args.rounds)
+    for shape in ((8, 720, 128, 256), (2, 2048, 66, 66)):
+        conv1_pair(shape, args.iters, args.rounds)
     for shape in ((8, 720, 128, 256), (2, 2048, 66, 66)):
         print(f"convmlp head from conv1 on, training mode, shape {shape}:")
         bn_head_pair(shape, args.iters, args.rounds)
