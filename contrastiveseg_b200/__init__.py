@@ -8,6 +8,7 @@ hand-written sm_90a kernels (csrc/) behind the C ABI of include/pcl.h; there is 
 from .configer import Configer, cityscapes_contrast_config            # noqa: F401
 from .functional import ContrastOptions, l2_normalize, pixel_contrast_loss, project_normalize, upsample_cross_entropy  # noqa: F401,E501
 from .functional import bn_relu_project_normalize                     # noqa: F401
+from .functional import upsample_rmi_loss                             # noqa: F401
 from .functional import conv_bn_relu_project_normalize                # noqa: F401
 from .loss import (ContrastAuxCELoss, ContrastCELoss, MemContrastCELoss, PixelContrastLoss, SEG_LOSS_DICT,  # noqa: F401
                    get_seg_loss)

@@ -1,3 +1,7 @@
+// Fused segmentation losses of the contrast wrappers: the plain CE (first part of this file) and the RMI loss of
+// contrast.use_rmi (second part).  Both up-sample the logits bilinearly inside the kernels and share the tile geometry
+// and transposed bilinear map of pcl_upsample.cuh.
+//
 // Fused segmentation cross-entropy of ContrastCELoss.forward (SURVEY §8f row 1, the next row after the contrast path):
 // replaces  F.interpolate(seg, (Himg,Wimg), bilinear, align_corners=True)  +  nn.CrossEntropyLoss(weight, ignore_index,
 // reduction='mean')  (lib/loss/loss_contrast.py:180-181, lib/loss/loss_helper.py:169-212) without materialising the
@@ -12,7 +16,7 @@
 //                the last ulp or two (summation order of <= 4 addends), which the parity tolerance (1e-5 max|g|) covers
 // HBM: reads seg (B*K*h*w*4) + labels (B*Himg*Wimg*8), writes lse (B*Himg*Wimg*4); backward re-reads them and writes
 // dseg.  Everything else stays in L1/L2 (a 4x4 block of label pixels shares its 4 source logits).
-#include "pcl_common.cuh"
+#include "pcl_upsample.cuh"
 #include <math_constants.h>
 
 namespace pcl {
@@ -23,24 +27,8 @@ struct SegCeArgs {
   float ry, rx;                 // (h-1)/(H-1), (w-1)/(W-1)   (align_corners=True)
 };
 
-__device__ __forceinline__ void src_coord(int o, float r, int in_size, int& i0, int& i1, float& l1) {
-  const float s = r * (float)o;                       // ATen area_pixel_compute_source_index, align_corners=True
-  i0 = (int)s;
-  if (i0 > in_size - 1) i0 = in_size - 1;
-  i1 = i0 + (i0 < in_size - 1 ? 1 : 0);
-  l1 = s - (float)i0;
-}
-
 constexpr int CE_THREADS = 256;
-constexpr int BT = 32;                 // tile width  (label pixels)
-constexpr int BTY = 8;                 // tile height: 32 x 8 = 256 threads per CTA -> several CTAs per SM hide the
-                                       // load latency of the bulk-synchronous phases (a 32 x 32 tile ran 1 CTA/SM)
 constexpr int KC_FWD_MAX = 32;         // classes staged per pass in the forward (one pass for K <= 32: one exposed load latency)
-
-// Source patch geometry of a tile (identical for every thread of the CTA).
-struct TileGeo {
-  int ys_base, xs_base, ys_n, xs_n, ny, nx;
-};
 
 // Forward, tile formulation: the <= (32*ry+2) x (32*rx+2) source logits of the tile are staged in shared memory per class
 // chunk; every thread (one label pixel) runs an online log-sum-exp over the classes from shared memory.
@@ -56,19 +44,8 @@ k_segce_fwd(SegCeArgs a, float* __restrict__ lse_out, float* __restrict__ part_n
   const int X0 = blockIdx.x * BT, Y0 = blockIdx.y * BTY;
   const int x = X0 + tx, y = Y0 + ty;
   const int64_t hw = (int64_t)a.h * a.w, HWo = (int64_t)a.H * a.W;
-  if (threadIdx.x < BT) {
-    int i0, i1; float l;
-    if (threadIdx.x < BTY) {
-      src_coord(min(Y0 + (int)threadIdx.x, a.H - 1), a.ry, a.h, i0, i1, l);
-      s_y0[threadIdx.x] = i0; s_y1[threadIdx.x] = i1; s_ly[threadIdx.x] = l;
-    }
-    src_coord(min(X0 + (int)threadIdx.x, a.W - 1), a.rx, a.w, i0, i1, l);
-    s_x0[threadIdx.x] = i0; s_x1[threadIdx.x] = i1; s_lx[threadIdx.x] = l;
-  }
-  __syncthreads();
-  const int ys_base = s_y0[0], xs_base = s_x0[0];
-  const int ny = min(Y0 + BTY, a.H) - Y0, nx = min(X0 + BT, a.W) - X0;
-  const int ys_n = s_y1[ny - 1] - ys_base + 1, xs_n = s_x1[nx - 1] - xs_base + 1;
+  const UpTile g = up_tile_coords(X0, Y0, a.H, a.W, a.h, a.w, a.ry, a.rx, s_y0, s_y1, s_ly, s_x0, s_x1, s_lx);
+  const int ys_base = g.ys_base, xs_base = g.xs_base, ys_n = g.ys_n, xs_n = g.xs_n;
   const bool inside = x < a.W && y < a.H;
   const int ly0 = s_y0[ty] - ys_base, ly1 = s_y1[ty] - ys_base, lx0 = s_x0[tx] - xs_base, lx1 = s_x1[tx] - xs_base;
   const float ly = s_ly[ty], lx = s_lx[tx];
@@ -134,16 +111,12 @@ k_segce_finalize(const float* __restrict__ part_nll, const float* __restrict__ p
   }
 }
 
-// Backward, tile formulation: one CTA = a 32 x 32 tile of label pixels of one image, classes in chunks of kc.
-//   A  thread per label pixel: G[c] = coef * w_t * (softmax_c - [c == t]) from the staged source patch -> shared memory
-//   B  separable transpose of the bilinear map, x direction:  Hx[c][row][xs] = sum_x wx(x, xs) * G[c][row][x]
-//   C  y direction + flush: dseg[c][ys][xs] += sum_row wy(row, ys) * Hx[c][row][xs]   (global atomics only on the
-//      source cells of the tile; a cell is shared by at most 4 tiles)
+// Backward, tile formulation: one CTA = a 32 x 8 tile of label pixels of one image, classes in chunks of kc.
+//   A  a thread per label pixel: G[c] = coef * w_t * (softmax_c - [c == t]) from the staged source patch -> shared memory
+//   B, C  the transposed bilinear map into dseg (up_tile_flush, pcl_upsample.cuh)
 // Each (pixel, class) softmax is evaluated once (the per-logit gather below needs 16x as many); B and C only visit the
 // label columns / rows inside the footprint of their source cell.
-constexpr int SRC_MAX = 34;            // source cells per tile edge (scale >= 1: up to 32 + 2)
-
-__global__ void __launch_bounds__(BT * BTY)
+__global__ void __launch_bounds__(BT * BTY, 5)     // 5 CTAs per SM: holds the kernel at 48 registers
 k_segce_bwd_tile(SegCeArgs a, const float* __restrict__ lse, const float* __restrict__ fin,
                  const float* __restrict__ grad_out, float* __restrict__ dseg, int kc, int pitch) {
   extern __shared__ float sm[];
@@ -152,25 +125,16 @@ k_segce_bwd_tile(SegCeArgs a, const float* __restrict__ lse, const float* __rest
   float* S = Hx + (size_t)kc * BTY * SRC_MAX;      // [kc][pitch] source patch
   __shared__ int s_y0[BTY], s_y1[BTY], s_x0[BT], s_x1[BT];
   __shared__ float s_ly[BTY], s_lx[BT];
+  __shared__ float s_wx[SRC_MAX * (BT + 1)], s_wy[SRC_MAX * (BTY + 1)];
+  __shared__ short s_xlo[SRC_MAX], s_xhi[SRC_MAX], s_ylo[SRC_MAX], s_yhi[SRC_MAX];
   const int tx = threadIdx.x & (BT - 1), ty = threadIdx.x >> 5;
   const int b = blockIdx.z;
   const int X0 = blockIdx.x * BT, Y0 = blockIdx.y * BTY;
   const int x = X0 + tx, y = Y0 + ty;
   const int64_t hw = (int64_t)a.h * a.w, HWo = (int64_t)a.H * a.W;
-  if (threadIdx.x < BT) {
-    int i0, i1; float l;
-    if (threadIdx.x < BTY) {
-      src_coord(min(Y0 + (int)threadIdx.x, a.H - 1), a.ry, a.h, i0, i1, l);
-      s_y0[threadIdx.x] = i0; s_y1[threadIdx.x] = i1; s_ly[threadIdx.x] = l;
-    }
-    src_coord(min(X0 + (int)threadIdx.x, a.W - 1), a.rx, a.w, i0, i1, l);
-    s_x0[threadIdx.x] = i0; s_x1[threadIdx.x] = i1; s_lx[threadIdx.x] = l;
-  }
-  __syncthreads();
-  const int ys_base = s_y0[0], xs_base = s_x0[0];
-  const int ny = min(Y0 + BTY, a.H) - Y0, nx = min(X0 + BT, a.W) - X0;         // valid rows / cols of the tile
-  const int ys_n = s_y1[ny - 1] - ys_base + 1, xs_n = s_x1[nx - 1] - xs_base + 1;
-  const int patch = ys_n * xs_n;
+  const UpTile g = up_tile_coords(X0, Y0, a.H, a.W, a.h, a.w, a.ry, a.rx, s_y0, s_y1, s_ly, s_x0, s_x1, s_lx);
+  const int ys_base = g.ys_base, xs_base = g.xs_base, xs_n = g.xs_n;
+  const int patch = g.ys_n * xs_n;
   const bool inside = x < a.W && y < a.H;
   const float scale = (grad_out ? grad_out[0] : 1.f) / fin[1];
   int64_t t = -1;
@@ -188,49 +152,7 @@ k_segce_bwd_tile(SegCeArgs a, const float* __restrict__ lse, const float* __rest
   const float ly = s_ly[ty], lx = s_lx[tx];
   const float w00 = (1.f - ly) * (1.f - lx), w01 = (1.f - ly) * lx, w10 = ly * (1.f - lx), w11 = ly * lx;
   const int i00 = ly0 * xs_n + lx0, i01 = ly0 * xs_n + lx1, i10 = ly1 * xs_n + lx0, i11 = ly1 * xs_n + lx1;
-  const float inv_rx = a.rx > 0.f ? 1.f / a.rx : 0.f, inv_ry = a.ry > 0.f ? 1.f / a.ry : 0.f;
-  // The transposed bilinear map of the tile, once per CTA (it is the same for every class and row): weight of label
-  // column k in source column xs (s_wx), of label row k in source row ys (s_wy), and the label range [klo, khi] inside
-  // a source cell's footprint.  Phases B and C below were evaluating these (two compares, floorf / ceilf) per class, per
-  // row and per k: 152 times each.  Row stride 33 / 9: different source cells of one k fall into different banks.
-  __shared__ float s_wx[SRC_MAX * (BT + 1)], s_wy[SRC_MAX * (BTY + 1)];
-  __shared__ short s_xlo[SRC_MAX], s_xhi[SRC_MAX], s_ylo[SRC_MAX], s_yhi[SRC_MAX];
-  for (int i = threadIdx.x; i < xs_n * BT; i += BT * BTY) {
-    const int xs = i / BT, k = i - xs * BT, xg = xs_base + xs;
-    float wgt = 0.f;
-    if (k < nx) {
-      if (s_x0[k] == xg) wgt += 1.f - s_lx[k];
-      if (s_x1[k] == xg) wgt += s_lx[k];
-    }
-    s_wx[xs * (BT + 1) + k] = wgt;
-  }
-  for (int i = threadIdx.x; i < ys_n * BTY; i += BT * BTY) {
-    const int ysl = i / BTY, k = i - ysl * BTY, yg = ys_base + ysl;
-    float wgt = 0.f;
-    if (k < ny) {
-      if (s_y0[k] == yg) wgt += 1.f - s_ly[k];
-      if (s_y1[k] == yg) wgt += s_ly[k];
-    }
-    s_wy[ysl * (BTY + 1) + k] = wgt;
-  }
-  if (threadIdx.x < xs_n) {
-    const int xg = xs_base + threadIdx.x;
-    int klo = 0, khi = nx - 1;
-    if (a.rx > 0.f) {
-      klo = max(0, (int)floorf(((float)xg - 1.f) * inv_rx) - 1 - X0);
-      khi = min(nx - 1, (int)ceilf(((float)xg + 1.f) * inv_rx) + 1 - X0);
-    }
-    s_xlo[threadIdx.x] = (short)klo; s_xhi[threadIdx.x] = (short)khi;
-  }
-  if (threadIdx.x >= 64 && threadIdx.x < 64 + ys_n) {
-    const int ysl = threadIdx.x - 64, yg = ys_base + ysl;
-    int klo = 0, khi = ny - 1;
-    if (a.ry > 0.f) {
-      klo = max(0, (int)floorf(((float)yg - 1.f) * inv_ry) - 1 - Y0);
-      khi = min(ny - 1, (int)ceilf(((float)yg + 1.f) * inv_ry) + 1 - Y0);
-    }
-    s_ylo[ysl] = (short)klo; s_yhi[ysl] = (short)khi;
-  }
+  up_tile_tables(g, a.ry, a.rx, s_y0, s_y1, s_ly, s_x0, s_x1, s_lx, s_wx, s_wy, s_xlo, s_xhi, s_ylo, s_yhi);
   __syncthreads();
   for (int c0 = 0; c0 < a.K; c0 += kc) {
     const int cn = min(kc, a.K - c0);
@@ -242,36 +164,17 @@ k_segce_bwd_tile(SegCeArgs a, const float* __restrict__ lse, const float* __rest
     __syncthreads();
     // ---- A: gradient w.r.t. the (virtual) up-sampled logits ----
     for (int cc = 0; cc < cn; ++cc) {
-      float g = 0.f;
+      float gv = 0.f;
       if (t >= 0) {
         const float* p = S + cc * pitch;
         const float v = w00 * p[i00] + w01 * p[i01] + w10 * p[i10] + w11 * p[i11];
-        g = coef * (__expf(v - lse_p) - ((c0 + cc) == (int)t ? 1.f : 0.f));
+        gv = coef * (__expf(v - lse_p) - ((c0 + cc) == (int)t ? 1.f : 0.f));
       }
-      G[((size_t)cc * BTY + ty) * BT + tx] = g;
+      G[((size_t)cc * BTY + ty) * BT + tx] = gv;
     }
     __syncthreads();
-    // ---- B: x direction (only the label columns whose footprint touches source column xg) ----
-    for (int i = threadIdx.x; i < cn * BTY * xs_n; i += BT * BTY) {
-      const int xs = i % xs_n, row = (i / xs_n) % BTY, cc = i / (xs_n * BTY);
-      const int klo = s_xlo[xs], khi = s_xhi[xs];
-      const float* gr = G + ((size_t)cc * BTY + row) * BT;
-      const float* wr = s_wx + xs * (BT + 1);
-      float acc = 0.f;
-      for (int k = klo; k <= khi; ++k) acc += wr[k] * gr[k];
-      Hx[((size_t)cc * BTY + row) * SRC_MAX + xs] = acc;
-    }
-    __syncthreads();
-    // ---- C: y direction, flush ----
-    for (int i = threadIdx.x; i < cn * ys_n * xs_n; i += BT * BTY) {
-      const int xs = i % xs_n, ysl = (i / xs_n) % ys_n, cc = i / (xs_n * ys_n);
-      const int yg = ys_base + ysl;
-      const int klo = s_ylo[ysl], khi = s_yhi[ysl];
-      const float* wr = s_wy + ysl * (BTY + 1);
-      float acc = 0.f;
-      for (int k = klo; k <= khi; ++k) acc += wr[k] * Hx[((size_t)cc * BTY + k) * SRC_MAX + xs];
-      if (acc != 0.f) atomicAdd(&dseg[((int64_t)b * a.K + c0 + cc) * hw + (int64_t)yg * a.w + xs_base + xs], acc);
-    }
+    // ---- B, C: transposed bilinear map, flush ----
+    up_tile_flush(g, cn, G, Hx, s_wx, s_wy, s_xlo, s_xhi, s_ylo, s_yhi, dseg + ((int64_t)b * a.K + c0) * hw, hw, a.w);
     __syncthreads();
   }
 }
@@ -344,11 +247,7 @@ static int make_ce(const float* seg, const int64_t* target, const float* weight,
   return PCL_OK;
 }
 
-static int patch_pitch(const SegCeArgs& a) {
-  // upper bound of the source cells a 32 x BTY label tile touches (ys_n * xs_n), + 1 to de-phase the class planes
-  const int py = (int)((float)(BTY - 1) * a.ry) + 3, px = (int)(31.f * a.rx) + 3;
-  return (py < a.h + 1 ? py : a.h + 1) * (px < a.w + 1 ? px : a.w + 1) + 1;
-}
+static int patch_pitch(const SegCeArgs& a) { return up_patch_pitch(a.h, a.w, a.ry, a.rx); }
 
 extern "C" int64_t pcl_seg_ce_scratch_floats(int32_t B, int32_t H, int32_t W) {
   const int64_t blocks = (int64_t)ceil_div(H, BTY) * ceil_div(W, BT) * B;
@@ -411,6 +310,639 @@ extern "C" int pcl_seg_ce_bwd(const float* seg, const int64_t* target, const flo
   PCL_SMEM_OPT_IN(k_segce_bwd_tile, 200 * 1024);
   k_segce_bwd_tile<<<dim3((unsigned)ceil_div(W, BT), (unsigned)ceil_div(H, BTY), B), BT * BTY, smem, s>>>(a, lse, fin, grad_loss,
                                                                                                      dseg, kc, pitch);
+  PCL_LAUNCH_CHECK();
+  return PCL_OK;
+}
+
+// ==================================================================================================================
+// Fused RMI (Region Mutual Information) segmentation loss, sigmoid path: replaces
+//   F.interpolate(seg, (Himg,Wimg), bilinear, align_corners=True)  +  RMILoss.forward -> forward_sigmoid ->
+//   rmi_lower_bound  (lib/loss/rmi_loss.py:200-402, used by FSRMILoss / FSAuxRMILoss, lib/loss/loss_helper.py:316-369)
+// and its autograd backward, without materialising the (B,K,Himg,Wimg) up-sampled logits, one-hot labels and sigmoid
+// probabilities, or the float64 (B,K,r*r,n) neighbour vectors (629 MB each at B=8, K=19, 512x1024, r=3, stride 3).
+//   k_rmi_pool      one thread per pooled pixel: bilinear logits of its s x s window (source patch staged per class
+//                   chunk), sigmoid, max / avg pooling of the probabilities and the label presence, argmax slot; the
+//                   BCE of every label pixel (pixels below / right of the last window included); per-CTA partials
+//   k_rmi_moments   per (b, c, band of 16 point rows): float64 sums of x, y, x x^T, y y^T, x y^T over the band's
+//                   r x r neighbour vectors (fixed order, no atomics: the forward is bit-reproducible)
+//   k_rmi_solve     per (b, c): band sums -> centred moments, Cholesky of P and M in float64, log-det; the backward
+//                   coefficients 2 dP = A^T M^-1 A and dQ^T = -A^T M^-1 (A = Q P^-1) scaled by the loss weights
+//   k_rmi_finalize  BCE and per-class sums -> the scalar loss (fixed order)
+//   k_rmi_dpool     dL / d(pooled p) from the r*r neighbour vectors that contain each pooled pixel
+//   k_rmi_bwd_tile  per label tile: un-pool (argmax slot or 1/s^2) x sigmoid' + the BCE gradient, then the transposed
+//                   bilinear map into dseg (up_tile_flush, shared with the seg CE; fp32 atomics on the <= 4 tiles that
+//                   share a source cell, so dseg is reproducible to the last ulp or two, the loss bit for bit)
+
+namespace pcl {
+
+constexpr int RMI_R_MAX = 4;
+constexpr int RMI_S_MAX = 4;
+constexpr int PT_X = 32, PT_Y = 8;                       // pooled pixels per k_rmi_pool CTA
+constexpr int REG_ROWS = PT_Y * RMI_S_MAX + 2 * RMI_S_MAX, REG_COLS = PT_X * RMI_S_MAX + 2 * RMI_S_MAX;
+constexpr int MB_Y = 16, MB_X = 64;                      // points per k_rmi_moments band row / column tile
+constexpr int MB_PITCH = MB_X + RMI_R_MAX - 1;
+constexpr double RMI_ALPHA = 1e-3;                       // _POS_ALPHA
+constexpr float RMI_CLIP_MIN = 1e-6f;                    // _CLIP_MIN
+
+struct RmiArgs {
+  const float* seg; const int64_t* target;
+  int B, K, h, w, H, W;
+  float ry, rx;                 // (h-1)/(H-1), (w-1)/(W-1)   (align_corners=True)
+  int r, way, s, pad;           // radius, pool way (0 max, 1 avg), pool size == stride, padding s/2
+  int Hp, Wp, nY, nX;           // pooled map, neighbour-vector points (Hp-r+1) x (Wp-r+1)
+  float lw, wb, wr;             // loss_weight, BCE weight, RMI weight (lambda_way: lambda, 1-lambda; else 1, lambda)
+};
+
+__host__ __device__ constexpr int rmi_entries(int R) { return 2 * R * R + R * R * R * R + R * R * (R * R + 1); }
+
+// label value of a pooled pixel: presence flag (max pool) or count / s^2 in fp32 (avg pool, as F.avg_pool2d)
+__device__ __forceinline__ float rmi_label_value(uint8_t cnt, int way, int s) {
+  return way == 0 ? (cnt ? 1.f : 0.f) : (float)cnt / (float)(s * s);
+}
+
+// ---- forward: pooling + BCE -----------------------------------------------------------------------
+__global__ void __launch_bounds__(PT_X * PT_Y)
+k_rmi_pool(RmiArgs a, float* __restrict__ P, uint8_t* __restrict__ L, uint8_t* __restrict__ A, float* __restrict__ part_bce,
+           int* __restrict__ part_cnt, int pitch, int kc) {
+  extern __shared__ float sm[];
+  short* lab = reinterpret_cast<short*>(sm);                        // [REG_ROWS][REG_COLS] class id or -1
+  float* S = sm + REG_ROWS * REG_COLS / 2;                          // [kc][pitch] source patch
+  __shared__ int s_y0[REG_ROWS], s_y1[REG_ROWS], s_x0[REG_COLS], s_x1[REG_COLS];
+  __shared__ float s_ly[REG_ROWS], s_lx[REG_COLS];
+  __shared__ float s_b[PT_X * PT_Y / 32];
+  __shared__ int s_c[PT_X * PT_Y / 32];
+  const int tx = threadIdx.x & (PT_X - 1), ty = threadIdx.x >> 5;
+  const int b = blockIdx.z;
+  const int ox0 = blockIdx.x * PT_X, oy0 = blockIdx.y * PT_Y;
+  const int ox = ox0 + tx, oy = oy0 + ty;
+  const int s = a.s, pad = a.pad;
+  // label rows [lo(o), hi(o)) of pooled row o: its window, and for the last one every row below it (BCE only)
+  const int oyl = min(oy0 + PT_Y, a.Hp) - 1, oxl = min(ox0 + PT_X, a.Wp) - 1;
+  const int R0 = max(0, oy0 * s - pad), C0 = max(0, ox0 * s - pad);
+  const int R1 = oyl == a.Hp - 1 ? a.H : min(a.H, (oyl + 1) * s - pad);
+  const int C1 = oxl == a.Wp - 1 ? a.W : min(a.W, (oxl + 1) * s - pad);
+  const int nr = R1 - R0, nc = C1 - C0;
+  for (int i = threadIdx.x; i < nr; i += PT_X * PT_Y) {
+    int i0, i1; float l;
+    src_coord(R0 + i, a.ry, a.h, i0, i1, l);
+    s_y0[i] = i0; s_y1[i] = i1; s_ly[i] = l;
+  }
+  for (int i = threadIdx.x; i < nc; i += PT_X * PT_Y) {
+    int i0, i1; float l;
+    src_coord(C0 + i, a.rx, a.w, i0, i1, l);
+    s_x0[i] = i0; s_x1[i] = i1; s_lx[i] = l;
+  }
+  const int64_t HWo = (int64_t)a.H * a.W, hw = (int64_t)a.h * a.w;
+  for (int i = threadIdx.x; i < nr * nc; i += PT_X * PT_Y) {
+    const int lr = i / nc, lc = i - lr * nc;
+    int64_t t = a.target[(int64_t)b * HWo + (int64_t)(R0 + lr) * a.W + C0 + lc];
+    if (t < 0) t = 255;                                              // label[label < 0] = 255
+    lab[lr * REG_COLS + lc] = (short)(t < a.K ? t : -1);             // valid: label < num_classes
+  }
+  __syncthreads();
+  const int ys_base = s_y0[0], xs_base = s_x0[0];
+  const int xs_n = s_x1[nc - 1] - xs_base + 1, patch = (s_y1[nr - 1] - ys_base + 1) * xs_n;
+  const bool active = oy < a.Hp && ox < a.Wp;
+  const int wy0 = oy * s - pad, wx0 = ox * s - pad;                  // window origin (may lie in the padding)
+  int ylo = 0, yhi = 0, xlo = 0, xhi = 0;
+  if (active) {
+    ylo = max(0, wy0) - R0; yhi = (oy == a.Hp - 1 ? a.H : min(a.H, wy0 + s)) - R0;
+    xlo = max(0, wx0) - C0; xhi = (ox == a.Wp - 1 ? a.W : min(a.W, wx0 + s)) - C0;
+  }
+  const int wy1 = wy0 + s - R0, wx1 = wx0 + s - C0;                  // window end, region coordinates
+  int nvalid = 0;
+  for (int lr = ylo; lr < yhi; ++lr)
+    for (int lc = xlo; lc < xhi; ++lc) nvalid += lab[lr * REG_COLS + lc] >= 0;
+  float bce = 0.f;
+  const int64_t HWp = (int64_t)a.Hp * a.Wp;
+  for (int c0 = 0; c0 < a.K; c0 += kc) {
+    const int cn = min(kc, a.K - c0);
+    for (int i = threadIdx.x; i < cn * patch; i += PT_X * PT_Y) {
+      const int cc = i / patch, r = i - cc * patch;
+      const int yy = r / xs_n, xx = r - yy * xs_n;
+      S[cc * pitch + r] = a.seg[((int64_t)b * a.K + c0 + cc) * hw + (int64_t)(ys_base + yy) * a.w + xs_base + xx];
+    }
+    __syncthreads();
+    if (active) {
+      for (int cc = 0; cc < cn; ++cc) {
+        const int c = c0 + cc;
+        const float* p = S + cc * pitch;
+        float pmax = -CUDART_INF_F, psum = 0.f;
+        int slot = 0, cnt = 0;
+        for (int lr = ylo; lr < yhi; ++lr) {
+          const int y0 = s_y0[lr] - ys_base, y1 = s_y1[lr] - ys_base;
+          const float ly = s_ly[lr];
+          for (int lc = xlo; lc < xhi; ++lc) {
+            const int x0 = s_x0[lc] - xs_base, x1 = s_x1[lc] - xs_base;
+            const float lx = s_lx[lc];
+            const float z = (1.f - ly) * ((1.f - lx) * p[y0 * xs_n + x0] + lx * p[y0 * xs_n + x1]) +
+                            ly * ((1.f - lx) * p[y1 * xs_n + x0] + lx * p[y1 * xs_n + x1]);
+            const int tv = lab[lr * REG_COLS + lc];
+            const float yv = tv == c ? 1.f : 0.f;
+            if (tv >= 0) bce += (1.f - yv) * z + fmaxf(-z, 0.f) + log1pf(expf(-fabsf(z)));
+            if (lr < wy1 && lc < wx1) {
+              const float pr = (tv >= 0 ? 1.f / (1.f + expf(-z)) : 0.f) + RMI_CLIP_MIN;
+              if (pr > pmax) { pmax = pr; slot = (lr + R0 - wy0) * s + (lc + C0 - wx0); }   // first maximum wins
+              psum += pr;
+              cnt += tv == c;
+            }
+          }
+        }
+        const int64_t o = ((int64_t)b * a.K + c) * HWp + (int64_t)oy * a.Wp + ox;
+        P[o] = a.way == 0 ? pmax : psum / (float)(s * s);
+        L[o] = (uint8_t)cnt;
+        A[o] = (uint8_t)slot;
+      }
+    }
+    __syncthreads();
+  }
+  bce = warp_sum(bce);
+  nvalid = warp_sum_i(nvalid);
+  if ((threadIdx.x & 31) == 0) { s_b[threadIdx.x >> 5] = bce; s_c[threadIdx.x >> 5] = nvalid; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float ab = 0.f; int ac = 0;
+    for (int i = 0; i < PT_X * PT_Y / 32; ++i) { ab += s_b[i]; ac += s_c[i]; }      // fixed order
+    const int64_t blk = ((int64_t)blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
+    part_bce[blk] = ab;
+    part_cnt[blk] = ac;
+  }
+}
+
+// ---- forward: moments ------------------------------------------------------------------------------
+// Entry e of the per-(b,c) sum vector: [0, D) sum x_k, [D, 2D) sum y_k, then D*D sum x_k y_l, then the upper triangles
+// (k <= l, row-major) of sum x_k x_l and of sum y_k y_l.  Each operand is (plane, offset k) with plane 0 = x, 1 = y, 2 = 1.
+template <int R>
+__device__ __forceinline__ void rmi_entry(int e, int& pa, int& ka, int& pb, int& kb) {
+  constexpr int D = R * R;
+  if (e < D) { pa = 0; ka = e; pb = 2; kb = 0; return; }
+  if (e < 2 * D) { pa = 1; ka = e - D; pb = 2; kb = 0; return; }
+  e -= 2 * D;
+  if (e < D * D) { pa = 0; ka = e / D; pb = 1; kb = e % D; return; }
+  e -= D * D;
+  const int plane = e < D * (D + 1) / 2 ? 0 : 1;
+  if (plane) e -= D * (D + 1) / 2;
+  int k = 0;
+  while (e >= D - k) { e -= D - k; ++k; }
+  pa = pb = plane; ka = k; kb = k + e;
+}
+
+template <int R>
+__global__ void __launch_bounds__(256)
+k_rmi_moments(RmiArgs a, const float* __restrict__ P, const uint8_t* __restrict__ L, double* __restrict__ part) {
+  constexpr int NE = rmi_entries(R), EPT = (NE + 255) / 256;
+  constexpr int ROWS = MB_Y + R - 1;
+  __shared__ double pl[3 * (MB_Y + RMI_R_MAX - 1) * MB_PITCH];       // x | y | ones
+  const int band = blockIdx.x, bc = blockIdx.y;
+  const int py0 = band * MB_Y, npy = min(MB_Y, a.nY - py0);
+  const int64_t HWp = (int64_t)a.Hp * a.Wp;
+  const float* Pb = P + (int64_t)bc * HWp;
+  const uint8_t* Lb = L + (int64_t)bc * HWp;
+  constexpr int PLANE = (MB_Y + RMI_R_MAX - 1) * MB_PITCH;
+  const double* pa_ptr[EPT];
+  const double* pb_ptr[EPT];
+  double acc[EPT];
+#pragma unroll
+  for (int i = 0; i < EPT; ++i) {
+    acc[i] = 0.0;
+    const int e = threadIdx.x + i * 256;
+    int pa = 2, ka = 0, pb = 2, kb = 0;
+    if (e < NE) rmi_entry<R>(e, pa, ka, pb, kb);
+    pa_ptr[i] = pl + pa * PLANE + (ka / R) * MB_PITCH + ka % R;
+    pb_ptr[i] = pl + pb * PLANE + (kb / R) * MB_PITCH + kb % R;
+  }
+  for (int i = threadIdx.x; i < PLANE; i += 256) pl[2 * PLANE + i] = 1.0;
+  for (int px0 = 0; px0 < a.nX; px0 += MB_X) {
+    const int npx = min(MB_X, a.nX - px0), cols = npx + R - 1;
+    __syncthreads();
+    for (int i = threadIdx.x; i < ROWS * cols; i += 256) {
+      const int rr = i / cols, cc = i - rr * cols;
+      double xv = 0.0, yv = 0.0;
+      if (rr < npy + R - 1) {
+        const int64_t o = (int64_t)(py0 + rr) * a.Wp + px0 + cc;
+        xv = (double)rmi_label_value(Lb[o], a.way, a.s);
+        yv = (double)Pb[o];
+      }
+      pl[rr * MB_PITCH + cc] = xv;
+      pl[PLANE + rr * MB_PITCH + cc] = yv;
+    }
+    __syncthreads();
+    for (int py = 0; py < npy; ++py)
+      for (int px = 0; px < npx; ++px) {
+        const int o = py * MB_PITCH + px;
+#pragma unroll
+        for (int i = 0; i < EPT; ++i) acc[i] = fma(pa_ptr[i][o], pb_ptr[i][o], acc[i]);
+      }
+  }
+#pragma unroll
+  for (int i = 0; i < EPT; ++i) {
+    const int e = threadIdx.x + i * 256;
+    if (e < NE) part[((int64_t)bc * gridDim.x + band) * NE + e] = acc[i];
+  }
+}
+
+// ---- forward: per-(b,c) solve ---------------------------------------------------------------------------
+// In-place Cholesky of the D x D SPD matrix M (lower factor), then the inverse M^-1 = L^-T L^-1 into Minv.  One warp;
+// Wk is D*D scratch.  Returns sum log(diag(L) + 1e-8) on every lane.
+__device__ double rmi_chol_inv(double* M, double* Minv, double* Wk, int D, int lane) {
+  if (lane == 0) {
+    for (int j = 0; j < D; ++j) {
+      double d = M[j * D + j];
+      for (int k = 0; k < j; ++k) d -= M[j * D + k] * M[j * D + k];
+      d = sqrt(d);
+      M[j * D + j] = d;
+      for (int i = j + 1; i < D; ++i) {
+        double v = M[i * D + j];
+        for (int k = 0; k < j; ++k) v -= M[i * D + k] * M[j * D + k];
+        M[i * D + j] = v / d;
+      }
+    }
+  }
+  __syncwarp();
+  if (lane < D) {                                            // column `lane` of L^-1 by forward substitution
+    const int c = lane;
+    for (int i = 0; i < D; ++i) {
+      double v = i == c ? 1.0 : 0.0;
+      for (int k = c; k < i; ++k) v -= M[i * D + k] * Wk[k * D + c];
+      Wk[i * D + c] = i < c ? 0.0 : v / M[i * D + i];
+    }
+  }
+  __syncwarp();
+  for (int e = lane; e < D * D; e += 32) {
+    const int i = e / D, j = e % D;
+    double v = 0.0;
+    for (int k = (i > j ? i : j); k < D; ++k) v += Wk[k * D + i] * Wk[k * D + j];
+    Minv[e] = v;
+  }
+  double ld = 0.0;
+  for (int j = 0; j < D; ++j) ld += log(M[j * D + j] + 1e-8);
+  __syncwarp();
+  return ld;
+}
+
+template <int R>
+__global__ void __launch_bounds__(32)
+k_rmi_solve(RmiArgs a, const double* __restrict__ part, int nbands, double* __restrict__ rmi_bc, double* __restrict__ g1,
+            double* __restrict__ g2, double* __restrict__ mxy) {
+  constexpr int D = R * R, NE = rmi_entries(R);
+  __shared__ double Sm[NE];
+  __shared__ double X[D * D], Pm[D * D], Q[D * D], Am[D * D], Wk[D * D], Inv[D * D];
+  const int bc = blockIdx.x, lane = threadIdx.x;
+  for (int e = lane; e < NE; e += 32) {
+    double v = 0.0;
+    for (int k = 0; k < nbands; ++k) v += part[((int64_t)bc * nbands + k) * NE + e];   // fixed order
+    Sm[e] = v;
+  }
+  __syncwarp();
+  const double n = (double)a.nY * (double)a.nX;
+  const double* Sx = Sm; const double* Sy = Sm + D; const double* Sxy = Sm + 2 * D;
+  const double* Sxx = Sxy + D * D; const double* Syy = Sxx + D * (D + 1) / 2;
+  for (int e = lane; e < D * D; e += 32) {
+    const int k = e / D, l = e % D, lo = k < l ? k : l, hi = k < l ? l : k;
+    const int t = lo * D - lo * (lo - 1) / 2 + (hi - lo);
+    X[e] = Sxx[t] - Sx[k] * Sx[l] / n;
+    Pm[e] = Syy[t] - Sy[k] * Sy[l] / n + (k == l ? RMI_ALPHA : 0.0);
+    Q[e] = Sxy[e] - Sx[k] * Sy[l] / n;
+  }
+  __syncwarp();
+  rmi_chol_inv(Pm, Inv, Wk, D, lane);                         // Inv = P^-1
+  for (int e = lane; e < D * D; e += 32) {                    // A = Q P^-1
+    const int i = e / D, j = e % D;
+    double v = 0.0;
+    for (int k = 0; k < D; ++k) v += Q[i * D + k] * Inv[k * D + j];
+    Am[e] = v;
+  }
+  __syncwarp();
+  for (int e = lane; e < D * D; e += 32) {                    // M = X - A Q^T + alpha I   (into X)
+    const int i = e / D, j = e % D;
+    double v = 0.0;
+    for (int k = 0; k < D; ++k) v += Am[i * D + k] * Q[j * D + k];
+    X[e] = X[e] - v + (i == j ? RMI_ALPHA : 0.0);
+  }
+  __syncwarp();
+  const double ld = rmi_chol_inv(X, Inv, Wk, D, lane);        // Inv = M^-1, ld = 0.5 * log det M (chol diagonal)
+  const double coef = (double)a.lw * (double)a.wr / ((double)a.B * (double)D);
+  for (int e = lane; e < D * D; e += 32) {                    // T = A^T M^-1 (into Pm)
+    const int i = e / D, j = e % D;
+    double v = 0.0;
+    for (int k = 0; k < D; ++k) v += Am[k * D + i] * Inv[k * D + j];
+    Pm[e] = v;
+  }
+  __syncwarp();
+  for (int e = lane; e < D * D; e += 32) {                    // 2 dP = T A,  dQ^T = -T
+    const int i = e / D, j = e % D;
+    double v = 0.0;
+    for (int k = 0; k < D; ++k) v += Pm[i * D + k] * Am[k * D + j];
+    g1[(int64_t)bc * D * D + e] = coef * v;
+    g2[(int64_t)bc * D * D + e] = -coef * Pm[e];
+  }
+  if (lane < D) {
+    mxy[(int64_t)bc * 2 * D + lane] = Sx[lane] / n;
+    mxy[(int64_t)bc * 2 * D + D + lane] = Sy[lane] / n;
+  }
+  if (lane == 0) rmi_bc[bc] = ld;
+}
+
+__global__ void __launch_bounds__(1024)
+k_rmi_finalize(RmiArgs a, const float* __restrict__ part_bce, const int* __restrict__ part_cnt, int64_t n,
+               const double* __restrict__ rmi_bc, double* __restrict__ fin, float* __restrict__ out) {
+  __shared__ double s_b[1024];
+  __shared__ long long s_c[1024];
+  double ab = 0.0; long long ac = 0;
+  for (int64_t i = threadIdx.x; i < n; i += 1024) { ab += part_bce[i]; ac += part_cnt[i]; }
+  s_b[threadIdx.x] = ab; s_c[threadIdx.x] = ac;
+  __syncthreads();
+  for (int o = 512; o > 0; o >>= 1) {
+    if (threadIdx.x < o) { s_b[threadIdx.x] += s_b[threadIdx.x + o]; s_c[threadIdx.x] += s_c[threadIdx.x + o]; }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    const double inv_n = 1.0 / ((double)s_c[0] + 1.0);
+    double rmi = 0.0;
+    for (int c = 0; c < a.K; ++c) {                           // sum_c mean_b(rmi_bc) / half_d
+      double m = 0.0;
+      for (int b = 0; b < a.B; ++b) m += rmi_bc[b * a.K + c];
+      rmi += m / (double)a.B;
+    }
+    rmi /= (double)(a.r * a.r);
+    const double loss = (double)a.lw * ((double)a.wb * s_b[0] * inv_n + (double)a.wr * rmi);
+    fin[0] = loss;
+    fin[1] = (double)a.lw * (double)a.wb * inv_n;             // d loss / d (sum of the BCE terms)
+    fin[2] = rmi;
+    fin[3] = (double)s_c[0];
+    out[0] = (float)loss;
+  }
+}
+
+// ---- backward ----------------------------------------------------------------------------------------
+template <int R>
+__global__ void __launch_bounds__(256)
+k_rmi_dpool(RmiArgs a, const float* __restrict__ P, const uint8_t* __restrict__ L, const double* __restrict__ g1,
+            const double* __restrict__ g2, const double* __restrict__ mxy, const float* __restrict__ grad_out,
+            float* __restrict__ dP) {
+  constexpr int D = R * R;
+  __shared__ double G1[D * D], G2[D * D], mx[D], my[D];
+  const int bc = blockIdx.y;
+  for (int e = threadIdx.x; e < D * D; e += 256) { G1[e] = g1[(int64_t)bc * D * D + e]; G2[e] = g2[(int64_t)bc * D * D + e]; }
+  if (threadIdx.x < D) { mx[threadIdx.x] = mxy[(int64_t)bc * 2 * D + threadIdx.x]; my[threadIdx.x] = mxy[(int64_t)bc * 2 * D + D + threadIdx.x]; }
+  __syncthreads();
+  const int64_t HWp = (int64_t)a.Hp * a.Wp;
+  const int64_t u = (int64_t)blockIdx.x * 256 + threadIdx.x;
+  if (u >= HWp) return;
+  const int uy = (int)(u / a.Wp), ux = (int)(u - (int64_t)uy * a.Wp);
+  const float* Pb = P + (int64_t)bc * HWp;
+  const uint8_t* Lb = L + (int64_t)bc * HWp;
+  double acc = 0.0;
+#pragma unroll
+  for (int k = 0; k < D; ++k) {
+    const int jy = uy - k / R, jx = ux - k % R;               // point whose neighbour k is this pooled pixel
+    if (jy < 0 || jx < 0 || jy >= a.nY || jx >= a.nX) continue;
+    double v = 0.0;
+#pragma unroll
+    for (int l = 0; l < D; ++l) {
+      const int64_t o = (int64_t)(jy + l / R) * a.Wp + jx + l % R;
+      v += G1[k * D + l] * ((double)Pb[o] - my[l]) + G2[k * D + l] * ((double)rmi_label_value(Lb[o], a.way, a.s) - mx[l]);
+    }
+    acc += v;
+  }
+  dP[(int64_t)bc * HWp + u] = (float)(acc * (grad_out ? (double)grad_out[0] : 1.0));
+}
+
+__global__ void __launch_bounds__(BT * BTY)
+k_rmi_bwd_tile(RmiArgs a, const float* __restrict__ dP, const uint8_t* __restrict__ Am, const double* __restrict__ fin,
+               const float* __restrict__ grad_out, float* __restrict__ dseg, int kc, int pitch) {
+  extern __shared__ float sm[];
+  float* G = sm;                                   // [kc][BTY][BT]
+  float* Hx = G + (size_t)kc * BTY * BT;           // [kc][BTY][SRC_MAX]
+  float* S = Hx + (size_t)kc * BTY * SRC_MAX;      // [kc][pitch] source patch
+  __shared__ int s_y0[BTY], s_y1[BTY], s_x0[BT], s_x1[BT];
+  __shared__ float s_ly[BTY], s_lx[BT];
+  __shared__ float s_wx[SRC_MAX * (BT + 1)], s_wy[SRC_MAX * (BTY + 1)];
+  __shared__ short s_xlo[SRC_MAX], s_xhi[SRC_MAX], s_ylo[SRC_MAX], s_yhi[SRC_MAX];
+  const int tx = threadIdx.x & (BT - 1), ty = threadIdx.x >> 5;
+  const int b = blockIdx.z;
+  const int X0 = blockIdx.x * BT, Y0 = blockIdx.y * BTY;
+  const int x = X0 + tx, y = Y0 + ty;
+  const int64_t hw = (int64_t)a.h * a.w, HWo = (int64_t)a.H * a.W, HWp = (int64_t)a.Hp * a.Wp;
+  const UpTile g = up_tile_coords(X0, Y0, a.H, a.W, a.h, a.w, a.ry, a.rx, s_y0, s_y1, s_ly, s_x0, s_x1, s_lx);
+  const int ys_base = g.ys_base, xs_base = g.xs_base, xs_n = g.xs_n;
+  const int patch = g.ys_n * xs_n;
+  const float cb = (float)fin[1] * (grad_out ? grad_out[0] : 1.f);
+  int tv = -1;
+  int64_t u = -1;                                  // pooled pixel whose window holds this label pixel
+  int slot = 0;
+  if (x < a.W && y < a.H) {
+    int64_t t = a.target[(int64_t)b * HWo + (int64_t)y * a.W + x];
+    if (t < 0) t = 255;
+    tv = t < a.K ? (int)t : -1;
+    const int uy = (y + a.pad) / a.s, ux = (x + a.pad) / a.s;
+    if (uy < a.Hp && ux < a.Wp) {
+      u = (int64_t)uy * a.Wp + ux;
+      slot = (y + a.pad - uy * a.s) * a.s + (x + a.pad - ux * a.s);
+    }
+  }
+  const float inv_s2 = 1.f / (float)(a.s * a.s);
+  const int ly0 = s_y0[ty] - ys_base, ly1 = s_y1[ty] - ys_base, lx0 = s_x0[tx] - xs_base, lx1 = s_x1[tx] - xs_base;
+  const float ly = s_ly[ty], lx = s_lx[tx];
+  const int i00 = ly0 * xs_n + lx0, i01 = ly0 * xs_n + lx1, i10 = ly1 * xs_n + lx0, i11 = ly1 * xs_n + lx1;
+  up_tile_tables(g, a.ry, a.rx, s_y0, s_y1, s_ly, s_x0, s_x1, s_lx, s_wx, s_wy, s_xlo, s_xhi, s_ylo, s_yhi);
+  __syncthreads();
+  for (int c0 = 0; c0 < a.K; c0 += kc) {
+    const int cn = min(kc, a.K - c0);
+    for (int i = threadIdx.x; i < cn * patch; i += BT * BTY) {
+      const int cc = i / patch, r = i - cc * patch;
+      const int yy = r / xs_n, xx = r - yy * xs_n;
+      S[cc * pitch + r] = a.seg[((int64_t)b * a.K + c0 + cc) * hw + (int64_t)(ys_base + yy) * a.w + xs_base + xx];
+    }
+    __syncthreads();
+    for (int cc = 0; cc < cn; ++cc) {
+      float gv = 0.f;
+      if (tv >= 0) {
+        const int c = c0 + cc;
+        const float* p = S + cc * pitch;
+        const float z = (1.f - ly) * ((1.f - lx) * p[i00] + lx * p[i01]) + ly * ((1.f - lx) * p[i10] + lx * p[i11]);
+        const float sg = 1.f / (1.f + expf(-z));
+        gv = cb * (sg - (tv == c ? 1.f : 0.f));                                  // BCE with logits
+        if (u >= 0) {
+          const int64_t o = ((int64_t)b * a.K + c) * HWp + u;
+          const float dp = a.way == 0 ? (Am[o] == slot ? dP[o] : 0.f) : dP[o] * inv_s2;
+          gv += dp * sg * (1.f - sg);
+        }
+      }
+      G[((size_t)cc * BTY + ty) * BT + tx] = gv;
+    }
+    __syncthreads();
+    up_tile_flush(g, cn, G, Hx, s_wx, s_wy, s_xlo, s_xhi, s_ylo, s_yhi, dseg + ((int64_t)b * a.K + c0) * hw, hw, a.w);
+    __syncthreads();
+  }
+}
+
+}  // namespace pcl
+
+using namespace pcl;
+
+namespace {
+
+struct RmiLayout {
+  size_t P, L, A, dP, bce, cnt, part, rmi, g1, g2, mxy, fin, total;
+  int64_t pool_blocks;
+  int nbands;
+};
+
+size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+
+// Validates the geometry and parameters; fills the pooled-map sizes.  Refuses (PCL_ERR_UNSUPPORTED) what the reference
+// accepts but the engine does not implement: radius 5-10, pool way 2, stride > 4, down-sampling, a pooled map smaller
+// than the radius, more than 256 classes.
+int rmi_geometry(int B, int K, int h, int w, int H, int W, int radius, int way, int stride, RmiArgs* a) {
+  if (B <= 0 || K <= 0 || h <= 0 || w <= 0 || H <= 0 || W <= 0) return PCL_ERR_ARG;
+  if (radius < 1 || radius > 10 || way < 0 || way > 3 || stride < 1) return PCL_ERR_ARG;
+  if (radius > RMI_R_MAX || way > 1 || stride > RMI_S_MAX || K > 256 || H < h || W < w) return PCL_ERR_UNSUPPORTED;
+  a->B = B; a->K = K; a->h = h; a->w = w; a->H = H; a->W = W;
+  a->ry = H > 1 ? (float)(h - 1) / (float)(H - 1) : 0.f;
+  a->rx = W > 1 ? (float)(w - 1) / (float)(W - 1) : 0.f;
+  a->r = radius; a->way = way; a->s = stride; a->pad = stride / 2;
+  a->Hp = (H + 2 * a->pad - stride) / stride + 1;
+  a->Wp = (W + 2 * a->pad - stride) / stride + 1;
+  if (a->Hp < radius || a->Wp < radius) return PCL_ERR_UNSUPPORTED;
+  a->nY = a->Hp - radius + 1; a->nX = a->Wp - radius + 1;
+  return PCL_OK;
+}
+
+RmiLayout rmi_layout(const RmiArgs& a) {
+  RmiLayout l;
+  const int64_t n = (int64_t)a.B * a.K * a.Hp * a.Wp, BK = (int64_t)a.B * a.K;
+  const int D = a.r * a.r;
+  l.pool_blocks = (int64_t)ceil_div(a.Wp, PT_X) * ceil_div(a.Hp, PT_Y) * a.B;
+  l.nbands = ceil_div(a.nY, MB_Y);
+  size_t o = 0;
+  l.P = o;    o = align256(o + n * sizeof(float));
+  l.dP = o;   o = align256(o + n * sizeof(float));
+  l.L = o;    o = align256(o + n);
+  l.A = o;    o = align256(o + n);
+  l.bce = o;  o = align256(o + l.pool_blocks * sizeof(float));
+  l.cnt = o;  o = align256(o + l.pool_blocks * sizeof(int));
+  l.part = o; o = align256(o + (size_t)BK * l.nbands * rmi_entries(a.r) * sizeof(double));
+  l.rmi = o;  o = align256(o + BK * sizeof(double));
+  l.g1 = o;   o = align256(o + BK * D * D * sizeof(double));
+  l.g2 = o;   o = align256(o + BK * D * D * sizeof(double));
+  l.mxy = o;  o = align256(o + BK * 2 * D * sizeof(double));
+  l.fin = o;  o = align256(o + 4 * sizeof(double));
+  l.total = o;
+  return l;
+}
+
+int rmi_make(const float* seg, const int64_t* target, int B, int K, int h, int w, int H, int W, int radius, int way,
+             int stride, float weight_lambda, int lambda_way, float loss_weight, RmiArgs* a) {
+  if (!seg || !target) return PCL_ERR_ARG;
+  const int st = rmi_geometry(B, K, h, w, H, W, radius, way, stride, a);
+  if (st != PCL_OK) return st;
+  a->seg = seg; a->target = target;
+  a->lw = loss_weight;
+  a->wb = lambda_way ? weight_lambda : 1.f;
+  a->wr = lambda_way ? 1.f - weight_lambda : weight_lambda;
+  return PCL_OK;
+}
+
+template <int R>
+int rmi_moments_solve(const RmiArgs& a, const RmiLayout& l, char* sc, cudaStream_t s) {
+  k_rmi_moments<R><<<dim3((unsigned)l.nbands, (unsigned)(a.B * a.K)), 256, 0, s>>>(
+      a, (const float*)(sc + l.P), (const uint8_t*)(sc + l.L), (double*)(sc + l.part));
+  PCL_LAUNCH_CHECK();
+  k_rmi_solve<R><<<a.B * a.K, 32, 0, s>>>(a, (const double*)(sc + l.part), l.nbands, (double*)(sc + l.rmi),
+                                          (double*)(sc + l.g1), (double*)(sc + l.g2), (double*)(sc + l.mxy));
+  PCL_LAUNCH_CHECK();
+  return PCL_OK;
+}
+
+template <int R>
+int rmi_dpool(const RmiArgs& a, const RmiLayout& l, const char* sc, const float* grad_loss, cudaStream_t s) {
+  const int64_t HWp = (int64_t)a.Hp * a.Wp;
+  k_rmi_dpool<R><<<dim3((unsigned)ceil_div64(HWp, 256), (unsigned)(a.B * a.K)), 256, 0, s>>>(
+      a, (const float*)(sc + l.P), (const uint8_t*)(sc + l.L), (const double*)(sc + l.g1), (const double*)(sc + l.g2),
+      (const double*)(sc + l.mxy), grad_loss, (float*)(sc + l.dP));
+  PCL_LAUNCH_CHECK();
+  return PCL_OK;
+}
+
+}  // namespace
+
+extern "C" int64_t pcl_rmi_scratch_bytes(int32_t B, int32_t K, int32_t h, int32_t w, int32_t Himg, int32_t Wimg,
+                                         int32_t radius, int32_t pool_way, int32_t pool_stride) {
+  RmiArgs a;
+  const int st = rmi_geometry(B, K, h, w, Himg, Wimg, radius, pool_way, pool_stride, &a);
+  if (st != PCL_OK) return st;
+  return (int64_t)rmi_layout(a).total;
+}
+
+extern "C" int pcl_rmi_fwd(const float* seg, const int64_t* target, int32_t B, int32_t K, int32_t h, int32_t w,
+                           int32_t Himg, int32_t Wimg, int32_t radius, int32_t pool_way, int32_t pool_stride,
+                           float weight_lambda, int32_t lambda_way, float loss_weight, void* scratch, float* loss,
+                           void* stream) {
+  RmiArgs a;
+  const int st = rmi_make(seg, target, B, K, h, w, Himg, Wimg, radius, pool_way, pool_stride, weight_lambda, lambda_way,
+                          loss_weight, &a);
+  if (st != PCL_OK) return st;
+  PCL_REQUIRE(scratch && loss);
+  cudaStream_t s = (cudaStream_t)stream;
+  const RmiLayout l = rmi_layout(a);
+  char* sc = (char*)scratch;
+  // source patch of a pool tile: label rows / columns of REG_ROWS x REG_COLS at most
+  const int py = (int)((float)(REG_ROWS - 1) * a.ry) + 3, px = (int)((float)(REG_COLS - 1) * a.rx) + 3;
+  const int pitch = (py < h + 1 ? py : h + 1) * (px < w + 1 ? px : w + 1) + 1;
+  const size_t lab_bytes = (size_t)REG_ROWS * REG_COLS * sizeof(short);
+  int kc = K < 32 ? K : 32;
+  while (kc > 1 && lab_bytes + (size_t)kc * pitch * sizeof(float) > 96 * 1024) --kc;
+  const size_t smem = lab_bytes + (size_t)kc * pitch * sizeof(float);
+  if (smem > 200 * 1024) return PCL_ERR_UNSUPPORTED;
+  PCL_SMEM_OPT_IN(k_rmi_pool, 200 * 1024);
+  k_rmi_pool<<<dim3((unsigned)ceil_div(a.Wp, PT_X), (unsigned)ceil_div(a.Hp, PT_Y), B), PT_X * PT_Y, smem, s>>>(
+      a, (float*)(sc + l.P), (uint8_t*)(sc + l.L), (uint8_t*)(sc + l.A), (float*)(sc + l.bce), (int*)(sc + l.cnt),
+      pitch, kc);
+  PCL_LAUNCH_CHECK();
+  int rc = PCL_OK;
+  switch (radius) {
+    case 1: rc = rmi_moments_solve<1>(a, l, sc, s); break;
+    case 2: rc = rmi_moments_solve<2>(a, l, sc, s); break;
+    case 3: rc = rmi_moments_solve<3>(a, l, sc, s); break;
+    default: rc = rmi_moments_solve<4>(a, l, sc, s); break;
+  }
+  if (rc != PCL_OK) return rc;
+  k_rmi_finalize<<<1, 1024, 0, s>>>(a, (const float*)(sc + l.bce), (const int*)(sc + l.cnt), l.pool_blocks,
+                                    (const double*)(sc + l.rmi), (double*)(sc + l.fin), loss);
+  PCL_LAUNCH_CHECK();
+  return PCL_OK;
+}
+
+extern "C" int pcl_rmi_bwd(const float* seg, const int64_t* target, int32_t B, int32_t K, int32_t h, int32_t w,
+                           int32_t Himg, int32_t Wimg, int32_t radius, int32_t pool_way, int32_t pool_stride,
+                           float weight_lambda, int32_t lambda_way, float loss_weight, void* scratch,
+                           const float* grad_loss, float* dseg, void* stream) {
+  RmiArgs a;
+  const int st = rmi_make(seg, target, B, K, h, w, Himg, Wimg, radius, pool_way, pool_stride, weight_lambda, lambda_way,
+                          loss_weight, &a);
+  if (st != PCL_OK) return st;
+  PCL_REQUIRE(scratch && dseg);
+  cudaStream_t s = (cudaStream_t)stream;
+  const RmiLayout l = rmi_layout(a);
+  char* sc = (char*)scratch;
+  int rc = PCL_OK;
+  switch (radius) {
+    case 1: rc = rmi_dpool<1>(a, l, sc, grad_loss, s); break;
+    case 2: rc = rmi_dpool<2>(a, l, sc, grad_loss, s); break;
+    case 3: rc = rmi_dpool<3>(a, l, sc, grad_loss, s); break;
+    default: rc = rmi_dpool<4>(a, l, sc, grad_loss, s); break;
+  }
+  if (rc != PCL_OK) return rc;
+  PCL_CUDA(cudaMemsetAsync(dseg, 0, (size_t)B * K * h * w * sizeof(float), s));
+  const int pitch = up_patch_pitch(h, w, a.ry, a.rx);
+  int kc = K < 24 ? K : 24;
+  while (kc > 1 && (size_t)kc * (BTY * BT + BTY * SRC_MAX + pitch) * sizeof(float) > 200 * 1024) --kc;
+  const size_t smem = (size_t)kc * (BTY * BT + BTY * SRC_MAX + pitch) * sizeof(float);
+  if (smem > 200 * 1024) return PCL_ERR_UNSUPPORTED;
+  PCL_SMEM_OPT_IN(k_rmi_bwd_tile, 200 * 1024);
+  k_rmi_bwd_tile<<<dim3((unsigned)ceil_div(Wimg, BT), (unsigned)ceil_div(Himg, BTY), B), BT * BTY, smem, s>>>(
+      a, (const float*)(sc + l.dP), (const uint8_t*)(sc + l.A), (const double*)(sc + l.fin), grad_loss, dseg, kc, pitch);
   PCL_LAUNCH_CHECK();
   return PCL_OK;
 }

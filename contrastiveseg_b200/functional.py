@@ -1021,3 +1021,68 @@ def upsample_cross_entropy(seg: torch.Tensor, target: torch.Tensor, weight: Opti
     == F.cross_entropy(F.interpolate(seg, target.shape[1:], mode='bilinear', align_corners=True), target,
                        weight, ignore_index=ignore_index)  without the (B,K,Himg,Wimg) intermediate."""
     return _SegCeFn.apply(seg, target, weight, ignore_index)
+
+
+# ------------------------------------------------------------------------------------------------
+# §8f row f5: fused bilinear up-sampling (align_corners=True) + RMI loss, sigmoid path
+# (lib/loss/rmi_loss.py:200-402 via lib/loss/loss_helper.py:316-369)
+# ------------------------------------------------------------------------------------------------
+class _RmiFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, seg, target, params):
+        lib = _abi.load()
+        _require_cuda(seg, "seg")
+        dev = seg.device
+        seg_c = seg if (seg.dtype == torch.float32 and seg.is_contiguous()) else seg.to(torch.float32).contiguous()
+        tgt = target
+        if tgt.device != dev or tgt.dtype != torch.int64 or not tgt.is_contiguous():
+            tgt = tgt.to(device=dev, dtype=torch.int64).contiguous()
+        B, K, h, w = seg_c.shape
+        H, W = tgt.shape[1], tgt.shape[2]
+        n = lib.pcl_rmi_scratch_bytes(B, K, h, w, H, W, params[0], params[1], params[2])
+        if n < 0:
+            _abi.check(n, "pcl_rmi_scratch_bytes")
+        scratch = torch.empty(n, dtype=torch.uint8, device=dev)
+        out = torch.empty((), dtype=torch.float32, device=dev)
+        with _on_device(dev):
+            _abi.check(lib.pcl_rmi_fwd(seg_c.data_ptr(), tgt.data_ptr(), B, K, h, w, H, W, *params, scratch.data_ptr(),
+                                       out.data_ptr(), _stream_ptr(dev)), "pcl_rmi_fwd")
+        ctx.keep = (seg_c, tgt, scratch)
+        ctx.dims = (B, K, h, w, H, W)
+        ctx.params = params
+        ctx.seg_dtype = seg.dtype
+        return out
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out):
+        lib = _abi.load()
+        seg_c, tgt, scratch = ctx.keep
+        dev = seg_c.device
+        go = grad_out
+        if go.device != dev or go.dtype != torch.float32 or not go.is_contiguous():
+            go = go.detach().to(device=dev, dtype=torch.float32).contiguous()
+        dseg = torch.empty_like(seg_c)
+        with _on_device(dev):
+            _abi.check(lib.pcl_rmi_bwd(seg_c.data_ptr(), tgt.data_ptr(), *ctx.dims, *ctx.params, scratch.data_ptr(),
+                                       go.data_ptr(), dseg.data_ptr(), _stream_ptr(dev)), "pcl_rmi_bwd")
+        ctx.keep = None
+        return dseg.to(ctx.seg_dtype), None, None
+
+
+def upsample_rmi_loss(seg: torch.Tensor, target: torch.Tensor, *, num_classes: int, radius: int = 3, pool_way: int = 0,
+                      pool_stride: int = 3, weight_lambda: float = 0.5, lambda_way: int = 1,
+                      loss_weight: float = 1.0) -> torch.Tensor:
+    """RMI loss (sigmoid path) of bilinearly (align_corners=True) up-sampled logits against a full-resolution label map,
+    fused: == RMILoss(...)(F.interpolate(seg, target.shape[1:], mode='bilinear', align_corners=True), target) without
+    the (B,K,Himg,Wimg) intermediates.  Labels < 0 count as 255; a pixel is valid when its label < num_classes.
+    ``target`` is not modified (the reference rewrites it in place).  seg fp32, bf16 or fp16 (read as fp32); the
+    gradient comes back in seg's dtype.  radius 1-4, pool_way 0 (max) or 1 (avg), pool_stride 1-4 are implemented;
+    anything else, a label grid smaller than seg, or a pooled map smaller than the radius raises PclError."""
+    if seg.dim() != 4 or target.dim() != 3 or seg.shape[0] != target.shape[0]:
+        raise ValueError(f"seg (B,K,h,w) and target (B,H,W) expected, got {tuple(seg.shape)} and {tuple(target.shape)}")
+    if seg.shape[1] != num_classes:
+        raise ValueError(f"seg has {seg.shape[1]} channels, num_classes is {num_classes}")
+    params = (int(radius), int(pool_way), int(pool_stride), float(weight_lambda), 1 if lambda_way else 0,
+              float(loss_weight))
+    return _RmiFn.apply(seg, target, params)

@@ -2,7 +2,8 @@
 as the reference (lib/loss/loss_contrast.py, lib/loss/loss_contrast_mem.py, lib/loss/loss_manager.py:36-41).
 
 The contrast term runs on the H100 engine (functional.pixel_contrast_loss); the plain segmentation CE runs on
-the fused up-sample + CE kernels (``contrast.fused_seg_ce``, default on).  Engine-only knobs are read from
+the fused up-sample + CE kernels (``contrast.fused_seg_ce``, default on), and with ``contrast.use_rmi`` the RMI seg
+loss runs on the fused up-sample + RMI kernels (same switch: off, F.interpolate runs first).  Engine-only knobs are read from
 optional config keys under ``contrast``: ``rng`` ("device" | "torch_cpu"), ``nan_safe``, ``precision``
 ("fp32" | "bf16"), ``skip_warmup_contrast``, ``topk_negatives`` (a10 extension, default off).
 """
@@ -15,7 +16,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from .functional import ContrastOptions, pixel_contrast_loss, upsample_cross_entropy
-from .loss_helper import FSAuxCELoss, FSCELoss
+from .loss_helper import FSAuxCELoss, FSAuxRMILoss, FSCELoss, FSRMILoss
 
 
 def _opt(configer, key, default):
@@ -102,10 +103,13 @@ class ContrastCELoss(nn.Module):
         self.use_rmi = _opt(configer, "use_rmi", False)
         self.use_lovasz = _opt(configer, "use_lovasz", False)
         if seg_criterion is None:
-            if self.use_rmi or self.use_lovasz:
-                raise NotImplementedError("RMI / Lovasz seg losses are outside the hot path; pass the reference "
-                                          "module via seg_criterion=")
-            seg_criterion = self._default_seg_criterion(configer)
+            if self.use_rmi:
+                seg_criterion = self._rmi_seg_criterion(configer)
+            elif self.use_lovasz:
+                raise NotImplementedError("the Lovasz seg loss (contrast.use_lovasz) is not implemented; pass the "
+                                          "reference module via seg_criterion=")
+            else:
+                seg_criterion = self._default_seg_criterion(configer)
         self.seg_criterion = seg_criterion
         self.contrast_criterion = PixelContrastLoss(configer)
         self.skip_warmup_contrast = bool(_opt(configer, "skip_warmup_contrast", False))
@@ -125,7 +129,23 @@ class ContrastCELoss(nn.Module):
     def _default_seg_criterion(configer):
         return FSCELoss(configer)
 
+    @staticmethod
+    def _rmi_seg_criterion(configer):
+        raise NotImplementedError(
+            "contrast_ce_loss with contrast.use_rmi: the reference hands FSAuxRMILoss one up-sampled tensor, which it "
+            "unpacks along the batch as (aux, seg), so it only runs at batch size 2 and then mixes the two images; use "
+            "contrast_auxce_loss or mem_contrast_ce_loss, or pass a module via seg_criterion=")
+
+    def _rmi_input(self, seg, target):
+        """seg as the RMI module takes it: the low-res logits (up-sampling fused), or up-sampled first when
+        contrast.fused_seg_ce is off."""
+        if self.fused_seg_ce:
+            return seg
+        return F.interpolate(input=seg, size=(target.size(1), target.size(2)), mode="bilinear", align_corners=True)
+
     def _seg_loss(self, preds, target):
+        if isinstance(self.seg_criterion, FSRMILoss):
+            return self.seg_criterion(self._rmi_input(preds["seg"], target), target)
         if self._can_fuse(self.seg_criterion, preds["seg"]):
             return self._fused_ce(preds["seg"], target, self.seg_criterion)
         h, w = target.size(1), target.size(2)
@@ -159,9 +179,21 @@ class ContrastAuxCELoss(ContrastCELoss):
     def _default_seg_criterion(configer):
         return FSAuxCELoss(configer)
 
+    @staticmethod
+    def _rmi_seg_criterion(configer):
+        return FSAuxRMILoss(configer)
+
     def _seg_loss(self, preds, target):
         assert "seg_aux" in preds
         crit = self.seg_criterion
+        if isinstance(crit, FSAuxRMILoss):
+            lw = crit.configer.get("network", "loss_weights")
+            if self._can_fuse(crit.ce_loss, preds["seg_aux"]):
+                aux = self._fused_ce(preds["seg_aux"], target, crit.ce_loss)
+            else:
+                aux = crit.ce_loss(F.interpolate(input=preds["seg_aux"], size=(target.size(1), target.size(2)),
+                                                 mode="bilinear", align_corners=True), target)
+            return lw["seg_loss"] * crit.rmi_loss(self._rmi_input(preds["seg"], target), target) + lw["aux_loss"] * aux
         if isinstance(crit, FSAuxCELoss) and self._can_fuse(crit.ce_loss, preds["seg"]):
             lw = crit.configer.get("network", "loss_weights")
             return (lw["seg_loss"] * self._fused_ce(preds["seg"], target, crit.ce_loss) +
@@ -174,9 +206,14 @@ class ContrastAuxCELoss(ContrastCELoss):
 
 class MemContrastCELoss(ContrastCELoss):
     """lib/loss/loss_contrast_mem.py:174-231 ('mem_contrast_ce_loss'): the contrast set is the memory bank.
-    The two queues are read in place (no 194.6 MB torch.cat per step)."""
+    The two queues are read in place (no 194.6 MB torch.cat per step).  contrast.use_rmi selects FSRMILoss (and takes
+    precedence over use_lovasz, as in the reference)."""
 
     with_memory = True
+
+    @staticmethod
+    def _rmi_seg_criterion(configer):
+        return FSRMILoss(configer)
 
     def _queues(self, preds):
         sq, pq = preds.get("segment_queue"), preds.get("pixel_queue")

@@ -1,14 +1,17 @@
-"""Segmentation cross-entropy used inside ContrastCELoss (lib/loss/loss_helper.py:169-212, :215-280).
+"""Segmentation losses used inside the contrast wrappers (lib/loss/loss_helper.py:169-212, :215-280, :316-369).
 
-OUT OF THE HOT PATH (SURVEY §2 row 6, §8f row 1): kept as plain PyTorch ops so the wrappers are drop-in.
-RMI / Lovasz variants (contrast.use_rmi / use_lovasz) are not re-implemented: pass the reference's own
-module through ``seg_criterion=`` if needed.
+The CE modules are plain PyTorch ops so the wrappers are drop-in (the wrappers run the fused up-sample + CE kernels
+instead when they can, SURVEY §8f row 1).  The RMI modules (contrast.use_rmi) run the fused RMI kernels
+(functional.upsample_rmi_loss, §8f row f5).  The Lovasz variant (contrast.use_lovasz) is not re-implemented: pass the
+reference's own module through ``seg_criterion=`` if needed.
 """
 from __future__ import annotations
 
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
+
+from .functional import upsample_rmi_loss
 
 
 def _ce_params(configer):
@@ -58,3 +61,60 @@ class FSAuxCELoss(nn.Module):
         aux_out, seg_out = inputs
         w = self.configer.get("network", "loss_weights")
         return w["seg_loss"] * self.ce_loss(seg_out, targets) + w["aux_loss"] * self.ce_loss(aux_out, targets)
+
+
+class RMILoss(nn.Module):
+    """lib/loss/rmi_loss.py:200-402 (sigmoid path, ``forward``) on the engine.  Reads the reference's ``loss.params``
+    keys: num_classes, rmi_radius, rmi_pool_way, rmi_pool_size (== rmi_pool_stride), rmi_pool_stride,
+    loss_weight_lambda, loss_weight, lambda_way; use_sigmoid is read and ignored, as the reference's forward always
+    takes the sigmoid path.  ``cls_score`` may be the logits at label resolution (the reference's call) or below it:
+    the bilinear up-sampling (align_corners=True) is fused.  Unlike the reference, ``label`` is left unchanged."""
+
+    def __init__(self, configer=None):
+        super().__init__()
+        p = configer.get("loss", "params")
+        self.use_sigmoid = p["use_sigmoid"]
+        self.num_classes = p["num_classes"]
+        self.rmi_radius = p["rmi_radius"]
+        assert self.rmi_radius in range(1, 11)
+        self.rmi_pool_way = p["rmi_pool_way"]
+        assert self.rmi_pool_way in (0, 1, 2, 3)
+        self.rmi_pool_size = p["rmi_pool_size"]
+        self.rmi_pool_stride = p["rmi_pool_stride"]
+        assert self.rmi_pool_size == self.rmi_pool_stride
+        self.weight_lambda = p["loss_weight_lambda"]
+        self.loss_weight = p["loss_weight"]
+        self.lambda_way = p["lambda_way"]
+
+    def forward(self, cls_score, label, weight=None, **kwargs):
+        return upsample_rmi_loss(cls_score, label, num_classes=self.num_classes, radius=self.rmi_radius,
+                                 pool_way=self.rmi_pool_way, pool_stride=self.rmi_pool_stride,
+                                 weight_lambda=self.weight_lambda, lambda_way=self.lambda_way,
+                                 loss_weight=self.loss_weight)
+
+
+class FSRMILoss(nn.Module):
+    """RMI(seg)  (lib/loss/loss_helper.py:359-369)."""
+
+    def __init__(self, configer=None):
+        super().__init__()
+        self.configer = configer
+        self.rmi_loss = RMILoss(configer)
+
+    def forward(self, inputs, targets, **kwargs):
+        return self.rmi_loss(inputs, targets)
+
+
+class FSAuxRMILoss(nn.Module):
+    """seg_loss_weight * RMI(seg) + aux_loss_weight * CE(aux)  (lib/loss/loss_helper.py:316-330)."""
+
+    def __init__(self, configer=None):
+        super().__init__()
+        self.configer = configer
+        self.ce_loss = FSCELoss(configer)
+        self.rmi_loss = RMILoss(configer)
+
+    def forward(self, inputs, targets, **kwargs):
+        aux_out, seg_out = inputs
+        w = self.configer.get("network", "loss_weights")
+        return w["seg_loss"] * self.rmi_loss(seg_out, targets) + w["aux_loss"] * self.ce_loss(aux_out, targets)

@@ -297,6 +297,28 @@ int pcl_seg_ce_bwd(const float* seg, const int64_t* target, const float* class_w
                    const float* grad_loss, float* dseg, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * §8f row f5: the RMI segmentation loss of the contrast wrappers with contrast.use_rmi, fused.  Replaces
+ * F.interpolate(seg, (Himg,Wimg), bilinear, align_corners=True) + RMILoss.forward (sigmoid path:
+ * lib/loss/rmi_loss.py:200-402, via FSRMILoss / FSAuxRMILoss, lib/loss/loss_helper.py:316-369) and its autograd
+ * backward; neither the (B,K,Himg,Wimg) logits / one-hot / probabilities nor the float64 neighbour vectors are
+ * materialised.  num_classes = K; a label < 0 counts as 255, a pixel is valid when its label < K (target is read only).
+ *   seg (B,K,h,w) fp32 with Himg >= h, Wimg >= w; target (B,Himg,Wimg) int64; radius 1-4; pool_way 0 (max) or 1 (avg);
+ *   pool_stride (== pool size) 1-4; lambda_way != 0: loss_weight * (lambda * bce + (1 - lambda) * rmi), else
+ *   loss_weight * (bce + lambda * rmi).  Radius 5-10, pool way 2, down-sampling, more than 256 classes or a pooled map
+ *   smaller than the radius return PCL_ERR_UNSUPPORTED.
+ *   scratch: pcl_rmi_scratch_bytes (host only; a negative PCL_ERR_* for a refused request).  pcl_rmi_bwd reads the
+ *   scratch its pcl_rmi_fwd wrote.  The loss is bit-reproducible; dseg to the last ulp or two (fp32 atomics).
+ * ----------------------------------------------------------------------------------------------*/
+int64_t pcl_rmi_scratch_bytes(int32_t B, int32_t K, int32_t h, int32_t w, int32_t Himg, int32_t Wimg, int32_t radius,
+                              int32_t pool_way, int32_t pool_stride);
+int pcl_rmi_fwd(const float* seg, const int64_t* target, int32_t B, int32_t K, int32_t h, int32_t w, int32_t Himg,
+                int32_t Wimg, int32_t radius, int32_t pool_way, int32_t pool_stride, float weight_lambda,
+                int32_t lambda_way, float loss_weight, void* scratch, float* loss, void* stream);
+int pcl_rmi_bwd(const float* seg, const int64_t* target, int32_t B, int32_t K, int32_t h, int32_t w, int32_t Himg,
+                int32_t Wimg, int32_t radius, int32_t pool_way, int32_t pool_stride, float weight_lambda,
+                int32_t lambda_way, float loss_weight, void* scratch, const float* grad_loss, float* dseg, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * a7 + a8: memory bank.  Replaces segmentor/trainer_contrastive.py:102-138 (_dequeue_and_enqueue).
  * Step 1 (parallel): build this rank's enqueue packet.  Step 2 (ordered): apply the packets of all
  * ranks in rank order — world 1 reproduces the reference exactly, world > 1 is the allgather merge

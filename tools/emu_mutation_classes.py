@@ -25,7 +25,7 @@ MUTANTS = [   # (name, source file, exact text, replacement, which occurrence)
     ("segce bwd tile: one-hot without the chunk offset", "pcl_segce.cu",
      "((c0 + cc) == (int)t ? 1.f : 0.f)", "(cc == (int)t ? 1.f : 0.f)", 0),
     ("segce bwd tile: dseg flush without the chunk offset", "pcl_segce.cu",
-     "atomicAdd(&dseg[((int64_t)b * a.K + c0 + cc) * hw", "atomicAdd(&dseg[((int64_t)b * a.K + cc) * hw", 0),
+     "dseg + ((int64_t)b * a.K + c0) * hw", "dseg + ((int64_t)b * a.K) * hw", 0),
     ("segce fwd: staged load without the chunk offset", "pcl_segce.cu",
      "sm[cc * pitch + r] = a.seg[((int64_t)b * a.K + c0 + cc) * hw", "sm[cc * pitch + r] = a.seg[((int64_t)b * a.K + cc) * hw",
      0),
