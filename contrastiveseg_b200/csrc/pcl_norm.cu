@@ -100,7 +100,7 @@ extern "C" int pcl_l2norm_bwd(const float* x, const float* gy, float* gx, int32_
 // Replaces lib/models/modules/projection.py:17-24  F.normalize(Conv2d(Cin -> 256, k=1)(x), p=2, dim=1)  and its
 // autograd backward.  bf16 operands, fp32 accumulate (the precision="bf16" contract of the tensor sweep).
 //
-//   k_proj_pack    W (256, Cin) fp32 -> Wk (256, Cin up to 64) bf16 and Wt (Cin up to 256, 256) bf16, zero-padded
+//   k_pack_bf16    W (256, Cin) fp32 -> Wk (256, Cin up to 64) bf16 and Wt (Cin up to 256, 256) bf16, zero-padded
 //   k_proj_fwd     CTA = 128 pixels of one image x 256 channels; A = x tile converted fp32 NCHW -> bf16 by the threads
 //                  into the K-major 128B-swizzled layout (register-staged one K-block ahead), B = Wk by TMA (3 stages).
 //                  Epilogue on the fragment: + bias, row norm = thread-local sum + two quad shuffles, zn and inv_norm.
@@ -281,14 +281,17 @@ __device__ __forceinline__ void put8(uint8_t* tile, int r, int ch, const S (&v)[
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-__global__ void k_proj_pack(const float* __restrict__ w, int Cin, int cin64, int cin256, __nv_bfloat16* __restrict__ wk,
-                            __nv_bfloat16* __restrict__ wt) {
+// W (R, C) fp32 -> wk (ra, ca) = W and wt (rb, cb) = W^T in bf16, zero-padded (ra, cb >= R; ca, rb >= C).  Thread idx
+// writes element idx of each (coalesced stores), so the grid covers the larger of the two.
+__global__ void k_pack_bf16(const float* __restrict__ w, int R, int C, int ra, int ca, int rb, int cb,
+                            __nv_bfloat16* __restrict__ wk, __nv_bfloat16* __restrict__ wt) {
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= (int64_t)DOUT * cin256) return;
-  const int n = (int)(idx / cin256), c = (int)(idx % cin256);
-  const __nv_bfloat16 v = __float2bfloat16(c < Cin ? w[(int64_t)n * Cin + c] : 0.f);
-  if (c < cin64) wk[(int64_t)n * cin64 + c] = v;
-  wt[(int64_t)c * DOUT + n] = v;
+  int r = (int)(idx / ca), c = (int)(idx % ca);
+  if (idx < (int64_t)ra * ca) wk[idx] = __float2bfloat16(r < R && c < C ? w[(int64_t)r * C + c] : 0.f);
+  if (idx < (int64_t)rb * cb) {
+    if (cb != ca) { r = (int)(idx / cb); c = (int)(idx % cb); }   // equal widths (conv1): wk's 64-bit division
+    wt[idx] = __float2bfloat16(r < C && c < R ? w[(int64_t)c * C + r] : 0.f);
+  }
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -298,49 +301,49 @@ struct FwdArgs {
   int Cin, nkb; int64_t HW; int tiles_per_img;
 };
 
-template <class T, bool BN = false>
-__global__ void __launch_bounds__(NT, 1) k_proj_fwd(const __grid_constant__ CUtensorMap tmW, ArgsBn<FwdArgs<T>, BN> a) {
-  extern __shared__ uint8_t smem_raw[];
-  FwdSmem& sm = aligned_smem<FwdSmem>(smem_raw);
-  const int t = threadIdx.x, g = t >> 7, lane = t & 31, wt = t & 127;
-  const int b = blockIdx.x / a.tiles_per_img;
-  const int64_t p0 = (int64_t)(blockIdx.x - b * a.tiles_per_img) * BM;
-  const T* img = a.x + (int64_t)b * a.Cin * a.HW;
-  const BnPro bn = bn_of(a);
+// The K-loop of the forward-shaped GEMMs (k_proj_fwd, k_conv1_gemm): acc = the product of the activation tile (pixels
+// p0 .. p0 + 127 of the NCHW image img, Cin channels) and rows n0 .. n0 + 255 of the K-major bf16 weight behind tmW,
+// nkb K-blocks.  The threads convert the tile into the swizzled bf16 operand through put8<BN>, register-staged one
+// K-block ahead; the weight comes by TMA in FWD_WSTAGES stages.  sm.bias[t] = bias_of(t), the bias of output channel
+// n0 + t.
+template <bool BN, class T, class BiasOf>
+__device__ __forceinline__ void fwd_mainloop(FwdSmem& sm, const CUtensorMap& tmW, const T* img, int Cin, int64_t HW,
+                                             int64_t p0, int n0, int nkb, BiasOf bias_of, const BnPro& bn,
+                                             float (&acc)[128]) {
+  const int t = threadIdx.x, g = t >> 7, wt = t & 127;
   if (t == 0) {
     ptx::prefetch_tmap(&tmW);
     for (int s = 0; s < FWD_WSTAGES; ++s) ptx::mbar_init(&sm.full[s], 1);
     ptx::fence_barrier_init();
   }
-  sm.bias[t] = a.bias ? a.bias[t] : 0.f;
+  sm.bias[t] = bias_of(t);
   __syncthreads();
   if (t == 0)
-    for (int kb = 0; kb < 2 && kb < a.nkb; ++kb) {
+    for (int kb = 0; kb < 2 && kb < nkb; ++kb) {
       ptx::mbar_arrive_expect_tx(&sm.full[kb], W_KB);
-      ptx::tma_load_2d(sm.w[kb], &tmW, &sm.full[kb], kb * BK, 0);
+      ptx::tma_load_2d(sm.w[kb], &tmW, &sm.full[kb], kb * BK, n0);
     }
   // conversion items of this thread: pixel row wt, 16-byte channel chunks g, g + 2, g + 4, g + 6 of each K-block
   typename Staged<T>::type v[4][8];
 #pragma unroll
-  for (int j = 0; j < 4; ++j) load8(img, a.Cin, a.HW, 8 * (g + 2 * j), p0 + wt, -1, v[j]);
+  for (int j = 0; j < 4; ++j) load8(img, Cin, HW, 8 * (g + 2 * j), p0 + wt, -1, v[j]);
 #pragma unroll
-  for (int j = 0; j < 4; ++j) put8<BN>(sm.a[0], wt, g + 2 * j, v[j], bn.ss, bn.ldp, 8 * (g + 2 * j), p0 + wt < a.HW);
+  for (int j = 0; j < 4; ++j) put8<BN>(sm.a[0], wt, g + 2 * j, v[j], bn.ss, bn.ldp, 8 * (g + 2 * j), p0 + wt < HW);
   ptx::fence_proxy_async();
 
-  float acc[128];
   const uint32_t a_off = g * WG_ROWS_BYTES;
-  for (int kb = 0; kb < a.nkb; ++kb) {
+  for (int kb = 0; kb < nkb; ++kb) {
     const int sa = kb & 1, sw = kb % FWD_WSTAGES;
     __syncthreads();                     // A[sa] complete; every wgmma of K-block kb - 1 retired (stage reuse below)
-    if (t == 0 && kb + 2 < a.nkb) {
+    if (t == 0 && kb + 2 < nkb) {
       const int s2 = (kb + 2) % FWD_WSTAGES;
       ptx::mbar_arrive_expect_tx(&sm.full[s2], W_KB);
-      ptx::tma_load_2d(sm.w[s2], &tmW, &sm.full[s2], (kb + 2) * BK, 0);
+      ptx::tma_load_2d(sm.w[s2], &tmW, &sm.full[s2], (kb + 2) * BK, n0);
     }
-    const bool more = kb + 1 < a.nkb;
+    const bool more = kb + 1 < nkb;
     if (more) {
 #pragma unroll
-      for (int j = 0; j < 4; ++j) load8(img, a.Cin, a.HW, (kb + 1) * BK + 8 * (g + 2 * j), p0 + wt, -1, v[j]);
+      for (int j = 0; j < 4; ++j) load8(img, Cin, HW, (kb + 1) * BK + 8 * (g + 2 * j), p0 + wt, -1, v[j]);
     }
     wait_full(&sm.full[sw], (uint32_t)(kb / FWD_WSTAGES) & 1u);
     const uint32_t abase = ptx::smem_u32(sm.a[sa]) + a_off, wbase = ptx::smem_u32(sm.w[sw]);
@@ -353,13 +356,24 @@ __global__ void __launch_bounds__(NT, 1) k_proj_fwd(const __grid_constant__ CUte
     if (more) {
 #pragma unroll
       for (int j = 0; j < 4; ++j)
-        put8<BN>(sm.a[sa ^ 1], wt, g + 2 * j, v[j], bn.ss, bn.ldp, (kb + 1) * BK + 8 * (g + 2 * j),
-                 p0 + wt < a.HW);
+        put8<BN>(sm.a[sa ^ 1], wt, g + 2 * j, v[j], bn.ss, bn.ldp, (kb + 1) * BK + 8 * (g + 2 * j), p0 + wt < HW);
       ptx::fence_proxy_async();
     }
     ptx::wgmma_wait<0>();
     ptx::fence_operands(acc);
   }
+}
+
+template <class T, bool BN = false>
+__global__ void __launch_bounds__(NT, 1) k_proj_fwd(const __grid_constant__ CUtensorMap tmW, ArgsBn<FwdArgs<T>, BN> a) {
+  extern __shared__ uint8_t smem_raw[];
+  FwdSmem& sm = aligned_smem<FwdSmem>(smem_raw);
+  const int t = threadIdx.x, g = t >> 7, lane = t & 31, wt = t & 127;
+  const int b = blockIdx.x / a.tiles_per_img;
+  const int64_t p0 = (int64_t)(blockIdx.x - b * a.tiles_per_img) * BM;
+  float acc[128];
+  fwd_mainloop<BN>(sm, tmW, a.x + (int64_t)b * a.Cin * a.HW, a.Cin, a.HW, p0, 0, a.nkb,
+                   [&](int c) { return a.bias ? a.bias[c] : 0.f; }, bn_of(a), acc);
 
   // epilogue on the fragment: acc[4 i + 2 h + e] = pixel fr + 8 h of the warpgroup, channel 8 i + 2 q + e
   const int fr = 16 * (wt >> 5) + (lane >> 2), q = lane & 3;
@@ -660,10 +674,11 @@ __global__ void __launch_bounds__(NT, 1) k_proj_wgrad(const __grid_constant__ CU
   }
 }
 
-__global__ void k_proj_reduce(const float* __restrict__ partials, int splits, int Cin, int ldp, float* __restrict__ gw,
-                              float* __restrict__ gb) {
+// rows n < `rows` of the partials -> gw (rows, Cin) and gb (rows)
+__global__ void k_proj_reduce(const float* __restrict__ partials, int splits, int rows, int Cin, int ldp,
+                              float* __restrict__ gw, float* __restrict__ gb) {
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= (int64_t)DOUT * (Cin + 1)) return;
+  if (idx >= (int64_t)rows * (Cin + 1)) return;
   const int n = (int)(idx / (Cin + 1)), c = (int)(idx % (Cin + 1));
   float v = 0.f;
   for (int s = 0; s < splits; ++s) v += partials[((int64_t)s * DOUT + n) * ldp + c];     // fixed order
@@ -748,30 +763,34 @@ __global__ void k_bn_finalize(const double* __restrict__ sums, const float* __re
   if (c == 0) st[4 * ldp] = training ? (float)(1. / sums[2 * C]) : 0.f;
 }
 
-// per-tile sums of g_u and g_u x_hat (the dgrad epilogue's partials, [tile][2][ldp]) -> per channel, in a fixed order;
-// gsum = (sum g_u, sum g_u x_hat) for the input gradient, gbeta / ggamma the same local sums
-constexpr int GR_NT = 1024;
-__global__ void __launch_bounds__(GR_NT) k_bn_grad_reduce(const float* __restrict__ part, int ntiles, int C, int ldp,
-                                                          float* __restrict__ gsum, float* __restrict__ ggamma,
-                                                          float* __restrict__ gbeta) {
-  __shared__ float red[2][GR_NT / 32][33];
+// Per-tile, per-channel sum pairs part [tile][2][ld] -> sums[c], sums[C + c] in a fixed order: 32 channels per block,
+// the 32 warps stride the tiles, then a fixed-order sum over the warps.  Used for the dgrad epilogue's sums of g_u and
+// g_u x_hat (float; copy1 / copy2 = gbeta / ggamma, may be null) and for conv1's fp64 statistics of y (count > 0 goes
+// to sums[2 C]).
+constexpr int TS_NT = 1024;
+template <class S>
+__global__ void __launch_bounds__(TS_NT) k_tile_sum(const S* __restrict__ part, int64_t ntiles, int C, int ld,
+                                                    S* __restrict__ sums, S* __restrict__ copy1, S* __restrict__ copy2,
+                                                    double count) {
+  __shared__ S red[2][TS_NT / 32][33];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, c = blockIdx.x * 32 + lane;
-  float s1 = 0.f, s2 = 0.f;
+  S s1 = 0, s2 = 0;
   if (c < C)
-    for (int tile = w; tile < ntiles; tile += GR_NT / 32) {
-      s1 += part[(int64_t)tile * 2 * ldp + c];
-      s2 += part[(int64_t)tile * 2 * ldp + ldp + c];
+    for (int64_t tile = w; tile < ntiles; tile += TS_NT / 32) {
+      s1 += part[tile * 2 * ld + c];
+      s2 += part[(tile * 2 + 1) * ld + c];
     }
   red[0][w][lane] = s1;
   red[1][w][lane] = s2;
   __syncthreads();
   if (w == 0 && c < C) {
-    float r1 = 0.f, r2 = 0.f;
-    for (int k = 0; k < GR_NT / 32; ++k) { r1 += red[0][k][lane]; r2 += red[1][k][lane]; }
-    gsum[c] = r1;
-    gsum[C + c] = r2;
-    if (gbeta) gbeta[c] = r1;
-    if (ggamma) ggamma[c] = r2;
+    S r1 = 0, r2 = 0;
+    for (int k = 0; k < TS_NT / 32; ++k) { r1 += red[0][k][lane]; r2 += red[1][k][lane]; }
+    sums[c] = r1;
+    sums[C + c] = r2;
+    if (copy1) copy1[c] = r1;
+    if (copy2) copy2[c] = r2;
+    if (c == 0 && count > 0) sums[2 * C] = count;
   }
 }
 
@@ -852,22 +871,23 @@ static inline bool shape_ok(int B, int Cin, int64_t HW) {
 // (4) The head's first 1x1 convolution, C -> C, in front of (3) (ProjectionHead(..., fuse_conv1=True)).
 // Replaces lib/models/modules/projection.py:17-19's Conv2d(dim_in, dim_in, 1), its autograd backward and (3)'s
 // statistics pass over y.  bf16 operands, fp32 accumulate, as (2).
-//   k_conv1_pack     W1 (C, C) fp32 -> W1 and W1^T bf16, each (C up to 256 rows, C up to 64 columns), zero-padded
+//   k_pack_bf16      W1 (C, C) fp32 -> W1 and W1^T bf16, each (C up to 256 rows, C up to 64 columns), zero-padded
 //   k_conv1_gemm     out = W . a per pixel: CTA = 128 pixels of one image x one 256-channel band of the output; A = the
-//                    activation tile converted by the threads as in k_proj_fwd, B = the band's 256 rows of W by TMA.
+//                    activation tile converted by the threads, B = the band's 256 rows of W by TMA (k_proj_fwd's loop).
 //                    The bands of one pixel tile are consecutive CTAs, so the tile is read from HBM about once and
 //                    from L2 by its other bands.  The epilogue stages the tile [channel][pixel] in the retired weight
 //                    stages (two halves of 128 channels) and writes it along pixels.
 //                    Forward (W1, x -> y): + b1, and per tile and channel the fp64 sums of the stored y and y^2 (the
 //                    values as rounded to y's type), over 32 lanes by a fixed shuffle tree.
 //                    Data gradient (W1^T, g_y -> gx).
-//   k_conv1_stats    per-tile sums -> sums[2 C + 1] in pcl_proj_bn_stats_dt's layout (fp64, fixed order)
+//   k_tile_sum<double>  per-tile sums -> sums[2 C + 1] in pcl_proj_bn_stats_dt's layout (fp64, fixed order)
 //   k_conv1_gy_pack  g_y -> bf16 in 256-row bands [band][b][256][HW up to 64], zero-padded: the TMA operand of
-//   k_proj_wgrad, k_proj_reduce  run once per band of gW1's rows; the band's gb1 comes from the constant-1 channel.
+//   k_proj_wgrad, k_proj_reduce  run once per band of gW1's rows, reduced straight into the band's rows of gW1; the
+//                    band's gb1 comes from the constant-1 channel.
 struct Conv1Layout {
   int kp, np, nbands, tiles_per_img;             // K padded to 64, rows padded to 256 = nbands x 256
   int64_t ptiles, wt_off, pack_bytes, fwd_bytes;
-  int64_t gy_bytes, part_off, gpad_off, bwd_bytes;
+  int64_t gy_bytes, part_off, bwd_bytes;
   Layout w;                                      // the weight gradient's pixel blocks and split-K partials
 };
 static Conv1Layout conv1_layout(int B, int C, int64_t HW) {
@@ -883,8 +903,7 @@ static Conv1Layout conv1_layout(int B, int C, int64_t HW) {
   L.w = layout(B, C, HW);
   L.gy_bytes = align1k((int64_t)L.np * B * L.w.HWp * 2);
   L.part_off = L.gy_bytes;
-  L.gpad_off = L.part_off + align1k((int64_t)L.w.splits * DOUT * L.w.ldp * 4);
-  L.bwd_bytes = L.gpad_off + align1k((int64_t)DOUT * (C + 1) * 4);
+  L.bwd_bytes = L.part_off + align1k((int64_t)L.w.splits * DOUT * L.w.ldp * 4);
   return L;
 }
 constexpr int GP_NT = 256, GP_UNROLL = 8;
@@ -893,16 +912,6 @@ static inline bool conv1_shape_ok(int B, int C, int64_t HW) {
   const int64_t nb = ceil_div(C, DOUT), HWp = ceil_div64(HW, WB) * WB;
   return ceil_div64(HW, BM) * B * nb < (1ll << 31) && (int64_t)B * nb * DOUT < (1ll << 31) &&
          ceil_div64(HWp, (int64_t)GP_NT * GP_UNROLL) <= 65535;
-}
-
-__global__ void k_conv1_pack(const float* __restrict__ w, int C, int kp, int64_t n, __nv_bfloat16* __restrict__ wk,
-                             __nv_bfloat16* __restrict__ wt) {
-  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= n) return;
-  const int r = (int)(idx / kp), k = (int)(idx % kp);
-  const bool in = r < C && k < C;
-  wk[idx] = __float2bfloat16(in ? w[(int64_t)r * C + k] : 0.f);
-  wt[idx] = __float2bfloat16(in ? w[(int64_t)k * C + r] : 0.f);
 }
 
 template <class T>
@@ -919,58 +928,9 @@ __global__ void __launch_bounds__(NT, 1) k_conv1_gemm(const __grid_constant__ CU
   const int band = blockIdx.x % a.nbands, tile = blockIdx.x / a.nbands;
   const int b = tile / a.tiles_per_img, n0 = band * DOUT;
   const int64_t p0 = (int64_t)(tile - b * a.tiles_per_img) * BM;
-  const T* img = a.a + (int64_t)b * a.C * a.HW;
-  if (t == 0) {
-    ptx::prefetch_tmap(&tmW);
-    for (int s = 0; s < FWD_WSTAGES; ++s) ptx::mbar_init(&sm.full[s], 1);
-    ptx::fence_barrier_init();
-  }
-  sm.bias[t] = (a.bias && n0 + t < a.C) ? a.bias[n0 + t] : 0.f;
-  __syncthreads();
-  if (t == 0)
-    for (int kb = 0; kb < 2 && kb < a.nkb; ++kb) {
-      ptx::mbar_arrive_expect_tx(&sm.full[kb], W_KB);
-      ptx::tma_load_2d(sm.w[kb], &tmW, &sm.full[kb], kb * BK, n0);
-    }
-  // conversion items of this thread: pixel row wt, 16-byte channel chunks g, g + 2, g + 4, g + 6 of each K-block
-  typename Staged<T>::type v[4][8];
-#pragma unroll
-  for (int j = 0; j < 4; ++j) load8(img, a.C, a.HW, 8 * (g + 2 * j), p0 + wt, -1, v[j]);
-#pragma unroll
-  for (int j = 0; j < 4; ++j) store8(sm.a[0], wt, g + 2 * j, v[j]);
-  ptx::fence_proxy_async();
-
   float acc[128];
-  const uint32_t a_off = g * WG_ROWS_BYTES;
-  for (int kb = 0; kb < a.nkb; ++kb) {
-    const int sa = kb & 1, sw = kb % FWD_WSTAGES;
-    __syncthreads();                     // A[sa] complete; every wgmma of K-block kb - 1 retired (stage reuse below)
-    if (t == 0 && kb + 2 < a.nkb) {
-      const int s2 = (kb + 2) % FWD_WSTAGES;
-      ptx::mbar_arrive_expect_tx(&sm.full[s2], W_KB);
-      ptx::tma_load_2d(sm.w[s2], &tmW, &sm.full[s2], (kb + 2) * BK, n0);
-    }
-    const bool more = kb + 1 < a.nkb;
-    if (more) {
-#pragma unroll
-      for (int j = 0; j < 4; ++j) load8(img, a.C, a.HW, (kb + 1) * BK + 8 * (g + 2 * j), p0 + wt, -1, v[j]);
-    }
-    wait_full(&sm.full[sw], (uint32_t)(kb / FWD_WSTAGES) & 1u);
-    const uint32_t abase = ptx::smem_u32(sm.a[sa]) + a_off, wbase = ptx::smem_u32(sm.w[sw]);
-    ptx::wgmma_fence();
-#pragma unroll
-    for (int k = 0; k < BK / 16; ++k)
-      ptx::wgmma_m64n256k16<0>(acc, ptx::make_desc_kmajor_sw128(abase + k * 32), ptx::make_desc_kmajor_sw128(wbase + k * 32),
-                               (kb | k) != 0 ? 1u : 0u);
-    ptx::wgmma_commit();
-    if (more) {
-#pragma unroll
-      for (int j = 0; j < 4; ++j) store8(sm.a[sa ^ 1], wt, g + 2 * j, v[j]);
-      ptx::fence_proxy_async();
-    }
-    ptx::wgmma_wait<0>();
-    ptx::fence_operands(acc);
-  }
+  fwd_mainloop<false>(sm, tmW, a.a + (int64_t)b * a.C * a.HW, a.C, a.HW, p0, n0, a.nkb,
+                      [&](int c) { return (a.bias && n0 + c < a.C) ? a.bias[n0 + c] : 0.f; }, BnPro{}, acc);
 
   // epilogue: acc[4 i + 2 h + e] = pixel g 64 + fr + 8 h of the tile, channel n0 + 8 i + 2 q + e.  Staging pitch LD (in
   // elements): a fragment store's 8 pixel rows x 4 channel pairs fall on distinct banks (132 words; 68 words for 2-byte T).
@@ -1023,30 +983,6 @@ __global__ void __launch_bounds__(NT, 1) k_conv1_gemm(const __grid_constant__ CU
   }
 }
 
-// per-tile sums [tile][2][np] -> sums: 32 channels per block, the 32 warps stride the tiles, then a fixed-order sum
-constexpr int CS_NT = 1024;
-__global__ void __launch_bounds__(CS_NT) k_conv1_stats(const double* __restrict__ part, int64_t ntiles, int C, int np,
-                                                       double count, double* __restrict__ sums) {
-  __shared__ double red[2][CS_NT / 32][33];
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, c = blockIdx.x * 32 + lane;
-  double s1 = 0., s2 = 0.;
-  if (c < C)
-    for (int64_t tile = w; tile < ntiles; tile += CS_NT / 32) {
-      s1 += part[tile * 2 * np + c];
-      s2 += part[(tile * 2 + 1) * np + c];
-    }
-  red[0][w][lane] = s1;
-  red[1][w][lane] = s2;
-  __syncthreads();
-  if (w == 0 && c < C) {
-    double r1 = 0., r2 = 0.;
-    for (int k = 0; k < CS_NT / 32; ++k) { r1 += red[0][k][lane]; r2 += red[1][k][lane]; }
-    sums[c] = r1;
-    sums[C + c] = r2;
-    if (c == 0) sums[2 * C] = count;
-  }
-}
-
 // g_y (B, C, HW) -> bf16 [band][b][256][HWp]: block row = (band B + b) 256 + r, zeros beyond C and HW
 template <class T>
 __global__ void __launch_bounds__(GP_NT) k_conv1_gy_pack(const T* __restrict__ gy, int B, int C, int64_t HW,
@@ -1087,9 +1023,10 @@ extern "C" int pcl_proj_pack(const float* weight, int32_t Cin, void* wpack, void
   PCL_REQUIRE(weight && wpack && Cin > 0 && Cin <= (1 << 20));
   const proj::Layout L = proj::layout(1, Cin, 1);
   uint8_t* base = (uint8_t*)wpack;
-  const int64_t n = (int64_t)proj::DOUT * L.cin256;
-  proj::k_proj_pack<<<(unsigned)ceil_div64(n, 256), 256, 0, (cudaStream_t)stream>>>(
-      weight, Cin, L.cin64, L.cin256, (__nv_bfloat16*)base, (__nv_bfloat16*)(base + L.wt_off));
+  const int64_t n = (int64_t)proj::DOUT * L.cin256;                 // Wt's elements, >= Wk's
+  proj::k_pack_bf16<<<(unsigned)ceil_div64(n, 256), 256, 0, (cudaStream_t)stream>>>(
+      weight, proj::DOUT, Cin, proj::DOUT, L.cin64, L.cin256, proj::DOUT, (__nv_bfloat16*)base,
+      (__nv_bfloat16*)(base + L.wt_off));
   PCL_LAUNCH_CHECK();
   return PCL_OK;
 }
@@ -1128,6 +1065,28 @@ extern "C" int pcl_proj_fwd_dt(const void* x, int32_t dtype, const void* wpack, 
   return PCL_ERR_ARG;                    // fp16 would be rounded to the bf16 GEMM operands: not offered
 }
 
+// Weight gradient of the bf16 gz rows [b][256][HWp] against x (L = layout(B, Cin, HW)): split-K partials, then the
+// fixed-order reduce of their first `rows` rows into gw (rows, Cin) and gb (rows; may be null).
+template <class T, bool BN>
+static int proj_wgrad(const __nv_bfloat16* gz, const T* x, int32_t B, int32_t Cin, int64_t HW, const proj::Layout& L,
+                      float* part, int rows, float* gw, float* gb, proj::BnPro bn, cudaStream_t s) {
+  CUtensorMap tmG;
+  const int st = tc_make_tmap_cols(&tmG, gz, (uint64_t)L.HWp, (uint64_t)B * proj::DOUT, 128);
+  if (st != PCL_OK) return st;
+  proj::ArgsBn<proj::WgradArgs<T>, BN> w;
+  w.x = x; w.partials = part; w.Cin = Cin; w.ldp = L.ldp; w.HW = HW; w.blk_per_img = L.blk_per_img;
+  w.units = L.units; w.splits = L.splits;
+  if constexpr (BN) w.bn = bn;
+  const size_t smem_w = (BN ? sizeof(proj::WgradBnSmem) : sizeof(proj::WgradSmem)) + 1024;
+  PCL_SMEM_OPT_IN((proj::k_proj_wgrad<T, BN>), smem_w);
+  proj::k_proj_wgrad<T, BN><<<dim3(proj::DOUT / 128, L.ctiles, L.splits), proj::NT, smem_w, s>>>(tmG, w);
+  PCL_LAUNCH_CHECK();
+  const int64_t n = (int64_t)rows * (Cin + 1);
+  proj::k_proj_reduce<<<(unsigned)ceil_div64(n, 256), 256, 0, s>>>(part, L.splits, rows, Cin, L.ldp, gw, gb);
+  PCL_LAUNCH_CHECK();
+  return PCL_OK;
+}
+
 template <class T, bool BN = false>
 static int proj_bwd(const T* x, const T* zn, const float* inv_norm, const T* gzn, const void* wpack, int32_t B,
                     int32_t Cin, int64_t HW, void* scratch, T* gx, float* gw, float* gb, void* stream,
@@ -1137,11 +1096,8 @@ static int proj_bwd(const T* x, const T* zn, const float* inv_norm, const T* gzn
   cudaStream_t s = (cudaStream_t)stream;
   uint8_t* sc = (uint8_t*)scratch;
   __nv_bfloat16* gz = (__nv_bfloat16*)sc;
-  float* part = (float*)(sc + L.part_off);
-  CUtensorMap tmWt, tmG;
-  int st = tc_make_tmap_cols(&tmWt, (const uint8_t*)wpack + L.wt_off, proj::DOUT, (uint64_t)L.cin256, proj::DOUT);
-  if (st != PCL_OK) return st;
-  st = tc_make_tmap_cols(&tmG, gz, (uint64_t)L.HWp, (uint64_t)B * proj::DOUT, 128);
+  CUtensorMap tmWt;
+  const int st = tc_make_tmap_cols(&tmWt, (const uint8_t*)wpack + L.wt_off, proj::DOUT, (uint64_t)L.cin256, proj::DOUT);
   if (st != PCL_OK) return st;
 
   proj::ArgsBn<proj::DgradArgs<T>, BN> d;
@@ -1153,20 +1109,7 @@ static int proj_bwd(const T* x, const T* zn, const float* inv_norm, const T* gzn
   PCL_SMEM_OPT_IN((proj::k_proj_dgrad<T, BN>), smem_d);
   proj::k_proj_dgrad<T, BN><<<(unsigned)(B * d.tiles_per_img), proj::NT, smem_d, s>>>(tmWt, d);
   PCL_LAUNCH_CHECK();
-
-  proj::ArgsBn<proj::WgradArgs<T>, BN> w;
-  w.x = x; w.partials = part; w.Cin = Cin; w.ldp = L.ldp; w.HW = HW; w.blk_per_img = L.blk_per_img;
-  w.units = L.units; w.splits = L.splits;
-  if constexpr (BN) w.bn = bn;
-  const size_t smem_w = (BN ? sizeof(proj::WgradBnSmem) : sizeof(proj::WgradSmem)) + 1024;
-  PCL_SMEM_OPT_IN((proj::k_proj_wgrad<T, BN>), smem_w);
-  proj::k_proj_wgrad<T, BN><<<dim3(proj::DOUT / 128, L.ctiles, L.splits), proj::NT, smem_w, s>>>(tmG, w);
-  PCL_LAUNCH_CHECK();
-
-  const int64_t n = (int64_t)proj::DOUT * (Cin + 1);
-  proj::k_proj_reduce<<<(unsigned)ceil_div64(n, 256), 256, 0, s>>>(part, L.splits, Cin, L.ldp, gw, gb);
-  PCL_LAUNCH_CHECK();
-  return PCL_OK;
+  return proj_wgrad<T, BN>(gz, x, B, Cin, HW, L, (float*)(sc + L.part_off), proj::DOUT, gw, gb, bn, s);
 }
 
 extern "C" int pcl_proj_bwd(const float* x, const float* zn, const float* inv_norm, const float* gzn, const void* wpack,
@@ -1194,7 +1137,7 @@ extern "C" int pcl_proj_bwd_dt(const void* x, int32_t dtype, const void* zn, con
 //   k_bn_stats        fp64 sum y, sum y^2 per channel (one CTA per channel, fixed order)
 //   k_bn_finalize     -> scale, shift, mean, invstd (+ running buffers in training)
 //   k_proj_fwd<T, true>, k_proj_dgrad<T, true>, k_proj_wgrad<T, true>   the GEMMs with the BN + ReLU prologue / epilogue
-//   k_bn_grad_reduce  per-tile sums of the dgrad epilogue -> sum g_u, sum g_u x_hat (fixed order)
+//   k_tile_sum<float>  per-tile sums of the dgrad epilogue -> sum g_u, sum g_u x_hat (fixed order)
 //   k_bn_input_grad   g_u -> g_y in place
 extern "C" int64_t pcl_proj_bn_workspace_bytes(int32_t B, int32_t Cin, int64_t HW, int32_t which) {
   if (!proj::shape_ok(B, Cin, HW) || (which != 0 && which != 1)) return PCL_ERR_ARG;
@@ -1262,8 +1205,8 @@ extern "C" int pcl_proj_bn_bwd_dt(const void* y, int32_t dtype, const void* bn_s
                                        (const __nv_bfloat16*)gzn, wpack, B, Cin, HW, scratch, (__nv_bfloat16*)gu, gw,
                                        gb, stream, bn);
   if (st != PCL_OK) return st;
-  proj::k_bn_grad_reduce<<<(unsigned)ceil_div(Cin, 32), proj::GR_NT, 0, (cudaStream_t)stream>>>(
-      part, (int)L.ntiles, Cin, L.ldp, gsum, ggamma, gbeta);
+  proj::k_tile_sum<float><<<(unsigned)ceil_div(Cin, 32), proj::TS_NT, 0, (cudaStream_t)stream>>>(
+      part, L.ntiles, Cin, L.ldp, gsum, gbeta, ggamma, 0.);
   PCL_LAUNCH_CHECK();
   return PCL_OK;
 }
@@ -1297,8 +1240,8 @@ extern "C" int pcl_proj_conv1_pack(const float* w1, int32_t C, void* pack, void*
   const proj::Conv1Layout L = proj::conv1_layout(1, C, 1);
   uint8_t* base = (uint8_t*)pack;
   const int64_t n = (int64_t)L.np * L.kp;
-  proj::k_conv1_pack<<<(unsigned)ceil_div64(n, 256), 256, 0, (cudaStream_t)stream>>>(
-      w1, C, L.kp, n, (__nv_bfloat16*)base, (__nv_bfloat16*)(base + L.wt_off));
+  proj::k_pack_bf16<<<(unsigned)ceil_div64(n, 256), 256, 0, (cudaStream_t)stream>>>(
+      w1, C, C, L.np, L.kp, L.np, L.kp, (__nv_bfloat16*)base, (__nv_bfloat16*)(base + L.wt_off));
   PCL_LAUNCH_CHECK();
   return PCL_OK;
 }
@@ -1326,8 +1269,8 @@ static int conv1_fwd(const T* x, const void* pack, const float* b1, int32_t B, i
   double* part = sums ? (double*)scratch : nullptr;
   const int st = conv1_gemm(x, pack, b1, B, C, HW, y, part, s);
   if (st != PCL_OK || !sums) return st;
-  proj::k_conv1_stats<<<(unsigned)ceil_div(C, 32), proj::CS_NT, 0, s>>>(part, L.ptiles, C, L.np,
-                                                                        (double)B * (double)HW, sums);
+  proj::k_tile_sum<double><<<(unsigned)ceil_div(C, 32), proj::TS_NT, 0, s>>>(part, L.ptiles, C, L.np, sums, nullptr,
+                                                                             nullptr, (double)B * (double)HW);
   PCL_LAUNCH_CHECK();
   return PCL_OK;
 }
@@ -1348,7 +1291,6 @@ static int conv1_bwd(const T* x, const T* gy, const void* pack, int32_t B, int32
   uint8_t* sc = (uint8_t*)scratch;
   __nv_bfloat16* gyb = (__nv_bfloat16*)sc;
   float* part = (float*)(sc + L.part_off);
-  float* gpad = (float*)(sc + L.gpad_off);                    // a last band of fewer than 256 rows: gW1 rows, gb1
   if (gx) {
     const int st = conv1_gemm(gy, (const uint8_t*)pack + L.wt_off, nullptr, B, C, HW, gx, nullptr, s);
     if (st != PCL_OK) return st;
@@ -1356,30 +1298,11 @@ static int conv1_bwd(const T* x, const T* gy, const void* pack, int32_t B, int32
   const dim3 grid((unsigned)((int64_t)B * L.np), (unsigned)ceil_div64(W.HWp, (int64_t)proj::GP_NT * proj::GP_UNROLL));
   proj::k_conv1_gy_pack<T><<<grid, proj::GP_NT, 0, s>>>(gy, B, C, HW, W.HWp, gyb);
   PCL_LAUNCH_CHECK();
-  const size_t smem_w = sizeof(proj::WgradSmem) + 1024;
-  PCL_SMEM_OPT_IN((proj::k_proj_wgrad<T, false>), smem_w);
-  const int64_t nred = (int64_t)proj::DOUT * (C + 1);
   for (int j = 0; j < L.nbands; ++j) {
-    CUtensorMap tmG;
-    const int st = tc_make_tmap_cols(&tmG, gyb + (int64_t)j * B * proj::DOUT * W.HWp, (uint64_t)W.HWp,
-                                     (uint64_t)B * proj::DOUT, 128);
+    const int n0 = j * proj::DOUT, rows = C - n0 < proj::DOUT ? C - n0 : proj::DOUT;
+    const int st = proj_wgrad<T, false>(gyb + (int64_t)n0 * B * W.HWp, x, B, C, HW, W, part, rows,
+                                        gw1 + (int64_t)n0 * C, gb1 ? gb1 + n0 : nullptr, proj::BnPro{}, s);
     if (st != PCL_OK) return st;
-    proj::WgradArgs<T> w;
-    w.x = x; w.partials = part; w.Cin = C; w.ldp = W.ldp; w.HW = HW; w.blk_per_img = W.blk_per_img;
-    w.units = W.units; w.splits = W.splits;
-    proj::k_proj_wgrad<T, false><<<dim3(proj::DOUT / 128, W.ctiles, W.splits), proj::NT, smem_w, s>>>(tmG, w);
-    PCL_LAUNCH_CHECK();
-    const int rows = C - j * proj::DOUT < proj::DOUT ? C - j * proj::DOUT : proj::DOUT;
-    const bool full = rows == proj::DOUT;
-    float* gwj = full ? gw1 + (int64_t)j * proj::DOUT * C : gpad;
-    float* gbj = gb1 ? (full ? gb1 + j * proj::DOUT : gpad + (int64_t)proj::DOUT * C) : nullptr;
-    proj::k_proj_reduce<<<(unsigned)ceil_div64(nred, 256), 256, 0, s>>>(part, W.splits, C, W.ldp, gwj, gbj);
-    PCL_LAUNCH_CHECK();
-    if (!full) {
-      PCL_CUDA(cudaMemcpyAsync(gw1 + (int64_t)j * proj::DOUT * C, gpad, (size_t)rows * C * 4, cudaMemcpyDeviceToDevice,
-                               s));
-      if (gb1) PCL_CUDA(cudaMemcpyAsync(gb1 + j * proj::DOUT, gbj, (size_t)rows * 4, cudaMemcpyDeviceToDevice, s));
-    }
   }
   return PCL_OK;
 }

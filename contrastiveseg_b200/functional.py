@@ -584,6 +584,33 @@ def proj_dtype_code(dtype: torch.dtype, what: str = "project_normalize") -> int:
     return code
 
 
+def _conv1x1_f32(weight, bias, rows, cols, dev):
+    """A 1x1 conv's weight as a contiguous fp32 (rows, cols) matrix on dev, its bias as contiguous fp32 (or None)."""
+    w = weight.detach().to(device=dev, dtype=torch.float32).reshape(rows, cols).contiguous()
+    return w, None if bias is None else bias.detach().to(device=dev, dtype=torch.float32).contiguous()
+
+
+def _proj_pack(lib, x, weight, bias, s):
+    """For the fused last conv on x (B, Cin, H, W): wpack (pcl_proj_pack), the fp32 bias or None, zn and inv_norm."""
+    B, Cin, HW, dev = x.shape[0], x.shape[1], x[0, 0].numel(), x.device
+    w, bc = _conv1x1_f32(weight, bias, PROJ_DIM, Cin, dev)
+    wpack = torch.empty(lib.pcl_proj_workspace_bytes(B, Cin, HW, 0), dtype=torch.uint8, device=dev)
+    zn = torch.empty((B, PROJ_DIM) + tuple(x.shape[2:]), dtype=x.dtype, device=dev)
+    inv = torch.empty(B * HW, dtype=torch.float32, device=dev)
+    _abi.check(lib.pcl_proj_pack(w.data_ptr(), Cin, wpack.data_ptr(), s), "pcl_proj_pack")
+    return wpack, bc, zn, inv
+
+
+def _proj_grad_buffers(x, zn, gzn, scratch_bytes, has_bias):
+    """The fused last conv's backward buffers: gzn in zn's dtype, scratch, x's gradient, gw (256, Cin), gb or None."""
+    dev = x.device
+    g = gzn.to(device=dev, dtype=zn.dtype).contiguous()
+    scratch = torch.empty(scratch_bytes, dtype=torch.uint8, device=dev)
+    gw = torch.empty((PROJ_DIM, x.shape[1]), dtype=torch.float32, device=dev)
+    gb = torch.empty(PROJ_DIM, dtype=torch.float32, device=dev) if has_bias else None
+    return g, scratch, torch.empty_like(x), gw, gb
+
+
 class _ProjNormFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, weight, bias):
@@ -593,20 +620,11 @@ class _ProjNormFn(torch.autograd.Function):
         B, Cin, HW = _proj_dims(x, weight)
         dev = x.device
         xc = x.contiguous()
-        w = weight.detach().to(device=dev, dtype=torch.float32).reshape(PROJ_DIM, Cin).contiguous()
-        bc = None if bias is None else bias.detach().to(device=dev, dtype=torch.float32).contiguous()
-        wpack = torch.empty(lib.pcl_proj_workspace_bytes(B, Cin, HW, 0), dtype=torch.uint8, device=dev)
-        zn = torch.empty((B, PROJ_DIM) + tuple(x.shape[2:]), dtype=x.dtype, device=dev)
-        inv = torch.empty(B * HW, dtype=torch.float32, device=dev)
         with _on_device(dev):
             s = _stream_ptr(dev)
-            _abi.check(lib.pcl_proj_pack(w.data_ptr(), Cin, wpack.data_ptr(), s), "pcl_proj_pack")
-            if dt == _abi.DT_F32:
-                _abi.check(lib.pcl_proj_fwd(xc.data_ptr(), wpack.data_ptr(), _abi.ptr(bc), B, Cin, HW, zn.data_ptr(),
-                                            inv.data_ptr(), s), "pcl_proj_fwd")
-            else:
-                _abi.check(lib.pcl_proj_fwd_dt(xc.data_ptr(), dt, wpack.data_ptr(), _abi.ptr(bc), B, Cin, HW,
-                                               zn.data_ptr(), inv.data_ptr(), s), "pcl_proj_fwd_dt")
+            wpack, bc, zn, inv = _proj_pack(lib, xc, weight, bias, s)
+            _abi.check(lib.pcl_proj_fwd_dt(xc.data_ptr(), dt, wpack.data_ptr(), _abi.ptr(bc), B, Cin, HW, zn.data_ptr(),
+                                           inv.data_ptr(), s), "pcl_proj_fwd_dt")
         ctx.save_for_backward(xc, zn, inv, wpack)
         ctx.dims = (B, Cin, HW, tuple(weight.shape), bias is not None, dt)
         return zn
@@ -617,21 +635,11 @@ class _ProjNormFn(torch.autograd.Function):
         lib = _abi.load()
         xc, zn, inv, wpack = ctx.saved_tensors
         B, Cin, HW, wshape, has_bias, dt = ctx.dims
-        dev = xc.device
-        g = gzn.to(device=dev, dtype=zn.dtype).contiguous()
-        scratch = torch.empty(lib.pcl_proj_workspace_bytes(B, Cin, HW, 1), dtype=torch.uint8, device=dev)
-        gx = torch.empty_like(xc)
-        gw = torch.empty((PROJ_DIM, Cin), dtype=torch.float32, device=dev)
-        gb = torch.empty(PROJ_DIM, dtype=torch.float32, device=dev) if has_bias else None
-        with _on_device(dev):
-            if dt == _abi.DT_F32:
-                _abi.check(lib.pcl_proj_bwd(xc.data_ptr(), zn.data_ptr(), inv.data_ptr(), g.data_ptr(), wpack.data_ptr(),
-                                            B, Cin, HW, scratch.data_ptr(), gx.data_ptr(), gw.data_ptr(), _abi.ptr(gb),
-                                            _stream_ptr(dev)), "pcl_proj_bwd")
-            else:
-                _abi.check(lib.pcl_proj_bwd_dt(xc.data_ptr(), dt, zn.data_ptr(), inv.data_ptr(), g.data_ptr(),
-                                               wpack.data_ptr(), B, Cin, HW, scratch.data_ptr(), gx.data_ptr(),
-                                               gw.data_ptr(), _abi.ptr(gb), _stream_ptr(dev)), "pcl_proj_bwd_dt")
+        g, scratch, gx, gw, gb = _proj_grad_buffers(xc, zn, gzn, lib.pcl_proj_workspace_bytes(B, Cin, HW, 1), has_bias)
+        with _on_device(xc.device):
+            _abi.check(lib.pcl_proj_bwd_dt(xc.data_ptr(), dt, zn.data_ptr(), inv.data_ptr(), g.data_ptr(),
+                                           wpack.data_ptr(), B, Cin, HW, scratch.data_ptr(), gx.data_ptr(),
+                                           gw.data_ptr(), _abi.ptr(gb), _stream_ptr(xc.device)), "pcl_proj_bwd_dt")
         return gx, gw.view(wshape), gb
 
 
@@ -668,19 +676,21 @@ def _check_bn(bn) -> None:
             raise _abi.PclError(f"bn_relu_project_normalize: bn.{name} must be float32")
 
 
+def _check_bn_input(what, name, x, gamma, training) -> None:
+    """bn against its input x (B, C, H, W): C channels, and in training more than one value per channel (as torch)."""
+    if gamma.numel() != x.shape[1]:
+        raise _abi.PclError(f"{what}: bn has {gamma.numel()} channels, {name} has {x.shape[1]}")
+    if training and x.shape[0] * x[0, 0].numel() == 1:
+        raise ValueError(f"Expected more than 1 value per channel when training, got input size {tuple(x.shape)}")
+
+
 def _bn_head_forward(lib, yc, dt, bn, gamma, beta, weight, bias, sums, group, s):
     """From conv1's output y on: (training) the all-reduce of the statistics ``sums`` for a multi-rank SyncBatchNorm and
     the counter, the BN state (batch or running statistics, running buffers updated), the last conv's packed weight
     and the fused GEMM.  Returns zn, inv_norm, wpack, bn_state."""
     B, Cin, HW = yc.shape[0], yc.shape[1], yc[0, 0].numel()
-    dev = yc.device
-    w = weight.detach().to(device=dev, dtype=torch.float32).reshape(PROJ_DIM, Cin).contiguous()
-    bc = None if bias is None else bias.detach().to(device=dev, dtype=torch.float32).contiguous()
     g32, b32 = gamma.detach().contiguous(), beta.detach().contiguous()
-    state = torch.empty(lib.pcl_proj_bn_workspace_bytes(B, Cin, HW, 0), dtype=torch.uint8, device=dev)
-    wpack = torch.empty(lib.pcl_proj_workspace_bytes(B, Cin, HW, 0), dtype=torch.uint8, device=dev)
-    zn = torch.empty((B, PROJ_DIM) + tuple(yc.shape[2:]), dtype=yc.dtype, device=dev)
-    inv = torch.empty(B * HW, dtype=torch.float32, device=dev)
+    state = torch.empty(lib.pcl_proj_bn_workspace_bytes(B, Cin, HW, 0), dtype=torch.uint8, device=yc.device)
     training = sums is not None
     if training:
         if group is not None:                            # fp64 sums and counts add up over the ranks
@@ -689,7 +699,7 @@ def _bn_head_forward(lib, yc, dt, bn, gamma, beta, weight, bias, sums, group, s)
     _abi.check(lib.pcl_proj_bn_finalize(_abi.ptr(sums), g32.data_ptr(), b32.data_ptr(), bn.running_mean.data_ptr(),
                                         bn.running_var.data_ptr(), Cin, bn.eps, bn.momentum, int(training),
                                         state.data_ptr(), s), "pcl_proj_bn_finalize")
-    _abi.check(lib.pcl_proj_pack(w.data_ptr(), Cin, wpack.data_ptr(), s), "pcl_proj_pack")
+    wpack, bc, zn, inv = _proj_pack(lib, yc, weight, bias, s)
     _abi.check(lib.pcl_proj_bn_fwd_dt(yc.data_ptr(), dt, state.data_ptr(), wpack.data_ptr(), _abi.ptr(bc), B, Cin, HW,
                                       zn.data_ptr(), inv.data_ptr(), s), "pcl_proj_bn_fwd_dt")
     return zn, inv, wpack, state
@@ -700,11 +710,7 @@ def _bn_head_backward(lib, yc, dt, zn, inv, wpack, state, gzn, has_bias, trainin
     bias (or None)."""
     B, Cin, HW = yc.shape[0], yc.shape[1], yc[0, 0].numel()
     dev = yc.device
-    g = gzn.to(device=dev, dtype=zn.dtype).contiguous()
-    scratch = torch.empty(lib.pcl_proj_bn_workspace_bytes(B, Cin, HW, 1), dtype=torch.uint8, device=dev)
-    gy = torch.empty_like(yc)
-    gw = torch.empty((PROJ_DIM, Cin), dtype=torch.float32, device=dev)
-    gb = torch.empty(PROJ_DIM, dtype=torch.float32, device=dev) if has_bias else None
+    g, scratch, gy, gw, gb = _proj_grad_buffers(yc, zn, gzn, lib.pcl_proj_bn_workspace_bytes(B, Cin, HW, 1), has_bias)
     gsum = torch.empty(2 * Cin, dtype=torch.float32, device=dev)
     ggamma = torch.empty(Cin, dtype=torch.float32, device=dev)
     gbeta = torch.empty(Cin, dtype=torch.float32, device=dev)
@@ -726,11 +732,8 @@ class _BnProjNormFn(torch.autograd.Function):
         _require_cuda(y, "y")
         dt = proj_dtype_code(y.dtype, "bn_relu_project_normalize")
         B, Cin, HW = _proj_dims(y, weight)
-        if gamma.numel() != Cin:
-            raise _abi.PclError(f"bn_relu_project_normalize: bn has {gamma.numel()} channels, y has {Cin}")
         training = bn.training
-        if training and B * HW == 1:
-            raise ValueError(f"Expected more than 1 value per channel when training, got input size {tuple(y.shape)}")
+        _check_bn_input("bn_relu_project_normalize", "y", y, gamma, training)
         group = _bn_sync_group(bn)
         dev = y.device
         yc = y.contiguous()
@@ -783,16 +786,12 @@ class _ConvBnProjNormFn(torch.autograd.Function):
             raise _abi.PclError(f"conv_bn_relu_project_normalize: w1 must be ({C}, {C}, 1, 1), got {tuple(w1.shape)}")
         if b1 is not None and b1.numel() != C:
             raise _abi.PclError(f"conv_bn_relu_project_normalize: b1 must have {C} elements, got {b1.numel()}")
-        if gamma.numel() != C:
-            raise _abi.PclError(f"conv_bn_relu_project_normalize: bn has {gamma.numel()} channels, x has {C}")
         training = bn.training
-        if training and B * HW == 1:
-            raise ValueError(f"Expected more than 1 value per channel when training, got input size {tuple(x.shape)}")
+        _check_bn_input("conv_bn_relu_project_normalize", "x", x, gamma, training)
         group = _bn_sync_group(bn)
         dev = x.device
         xc = x.contiguous()
-        w = w1.detach().to(device=dev, dtype=torch.float32).reshape(C, C).contiguous()
-        bc = None if b1 is None else b1.detach().to(device=dev, dtype=torch.float32).contiguous()
+        w, bc = _conv1x1_f32(w1, b1, C, C, dev)
         pack = torch.empty(lib.pcl_proj_conv1_workspace_bytes(B, C, HW, 0), dtype=torch.uint8, device=dev)
         y = torch.empty_like(xc)
         with _on_device(dev):

@@ -78,8 +78,8 @@ class ProjectionHead(nn.Module):
                 last, y = self.proj, x
             else:
                 last, y = self.proj[-1], self.proj[:-1](x)
-            # the tensor reaching the fused conv decides zn's dtype: bf16 under autocast for convmlp
-            _fn.proj_dtype_code(y.dtype, "ProjectionHead(fused=True)")
+            # the tensor reaching the fused conv decides zn's dtype (bf16 under autocast for convmlp), and
+            # project_normalize refuses any other than float32 / bfloat16
             return project_normalize(y, last.weight, last.bias)
         y = self.proj(x)
         return l2_normalize(y) if self.normalize else y

@@ -71,7 +71,7 @@ def test_bf16_results_do_not_depend_on_the_schedule_or_uninitialised_memory():
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# host wiring: fp32 inputs make exactly the old calls, bf16 inputs take the _dt entry points with PCL_DT_BF16
+# host wiring: fp32 and bf16 inputs take the _dt entry points with PCL_DT_F32 / PCL_DT_BF16
 # ------------------------------------------------------------------------------------------------------------------
 @pytest.fixture
 def rec(monkeypatch):
@@ -90,33 +90,24 @@ def _run(x, w, b, gzn):
     return xx, zn
 
 
-def test_fp32_inputs_keep_the_fp32_calls_and_bf16_inputs_take_the_typed_calls(rec):
+def test_fp32_and_bf16_inputs_take_the_typed_calls_with_their_dtype_code(rec):
     B, Cin, H, W = 2, 40, 3, 5
     g = torch.Generator().manual_seed(0)
     w = torch.randn(256, Cin, 1, 1, generator=g).requires_grad_(True)
     b = torch.randn(256, generator=g).requires_grad_(True)
     x, gzn = torch.randn(B, Cin, H, W, generator=g), torch.randn(B, 256, H, W, generator=g)
-    for dtype, names in ((torch.float32, ["pcl_proj_pack", "pcl_proj_fwd", "pcl_proj_bwd"]),
-                         (torch.bfloat16, ["pcl_proj_pack", "pcl_proj_fwd_dt", "pcl_proj_bwd_dt"])):
+    for dtype, code in ((torch.float32, _abi.DT_F32), (torch.bfloat16, _abi.DT_BF16)):
         for gdt in (torch.float32, torch.bfloat16):
             rec.calls.clear()
             xx, zn = _run(x.to(dtype), w, b, gzn.to(gdt))
             calls = [(n, a) for n, a in rec.calls if n != "pcl_proj_workspace_bytes"]
-            assert [n for n, _ in calls] == names
+            assert [n for n, _ in calls] == ["pcl_proj_pack", "pcl_proj_fwd_dt", "pcl_proj_bwd_dt"]
             (_, pack), (_, fwd), (_, bwd) = calls
             assert zn.dtype == dtype and xx.grad.dtype == dtype
-            if dtype == torch.float32:
-                # pcl_proj_fwd(x, wpack, bias, B, Cin, HW, zn, inv_norm, stream)
-                assert len(fwd) == 9 and fwd[0] == xx.data_ptr() and fwd[1] == pack[2] and fwd[3:6] == [B, Cin, H * W]
-                assert fwd[6] == zn.data_ptr() and fwd[8] == 0x5EED
-                # pcl_proj_bwd(x, zn, inv_norm, gzn, wpack, B, Cin, HW, scratch, gx, gw, gb, stream)
-                assert len(bwd) == 13 and bwd[0] == xx.data_ptr() and bwd[1] == zn.data_ptr() and bwd[2] == fwd[7]
-                assert bwd[4] == pack[2] and bwd[5:8] == [B, Cin, H * W] and bwd[9] == xx.grad.data_ptr()
-            else:
-                # pcl_proj_fwd_dt(x, dtype, wpack, bias, B, Cin, HW, zn, inv_norm, stream)
-                assert len(fwd) == 10 and fwd[0] == xx.data_ptr() and fwd[1] == _abi.DT_BF16 and fwd[2] == pack[2]
-                assert fwd[4:7] == [B, Cin, H * W] and fwd[7] == zn.data_ptr()
-                # pcl_proj_bwd_dt(x, dtype, zn, inv_norm, gzn, wpack, B, Cin, HW, scratch, gx, gw, gb, stream)
-                assert len(bwd) == 14 and bwd[0] == xx.data_ptr() and bwd[1] == _abi.DT_BF16
-                assert bwd[2] == zn.data_ptr() and bwd[3] == fwd[8] and bwd[5] == pack[2]
-                assert bwd[6:9] == [B, Cin, H * W] and bwd[10] == xx.grad.data_ptr()
+            # pcl_proj_fwd_dt(x, dtype, wpack, bias, B, Cin, HW, zn, inv_norm, stream)
+            assert len(fwd) == 10 and fwd[0] == xx.data_ptr() and fwd[1] == code and fwd[2] == pack[2]
+            assert fwd[4:7] == [B, Cin, H * W] and fwd[7] == zn.data_ptr() and fwd[9] == 0x5EED
+            # pcl_proj_bwd_dt(x, dtype, zn, inv_norm, gzn, wpack, B, Cin, HW, scratch, gx, gw, gb, stream)
+            assert len(bwd) == 14 and bwd[0] == xx.data_ptr() and bwd[1] == code
+            assert bwd[2] == zn.data_ptr() and bwd[3] == fwd[8] and bwd[5] == pack[2]
+            assert bwd[6:9] == [B, Cin, H * W] and bwd[10] == xx.grad.data_ptr()
