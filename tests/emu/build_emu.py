@@ -53,28 +53,33 @@ def _digest() -> str:
     return h.hexdigest()
 
 
-def build(force: bool = False) -> str:
-    stamp = os.path.join(BUILD, "build.sha256")
+def build(force: bool = False, sms: int = 6) -> str:
+    """The emulator library modelling an `sms`-SM device.  6 SMs (the suite's default) is libpcl_emu.so; other counts get
+    a library of their own (libpcl_emu_sm<n>.so), because pcl::num_sms() caches the count per process."""
+    lib = LIB if sms == 6 else os.path.join(BUILD, f"libpcl_emu_sm{sms}.so")
+    stamp = os.path.join(BUILD, "build.sha256" if sms == 6 else f"build_sm{sms}.sha256")
     dig = _digest()
-    if not force and os.path.exists(LIB) and os.path.exists(stamp) and open(stamp).read() == dig:
-        return LIB
+    if not force and os.path.exists(lib) and os.path.exists(stamp) and open(stamp).read() == dig:
+        return lib
     os.makedirs(BUILD, exist_ok=True)
     cpps = []
     for name in SOURCES:
         out = os.path.join(BUILD, name[:-3] + ".emu.cpp")
-        with open(out, "w") as f:
-            f.write(f'#line 1 "{os.path.join(CSRC, name)}"\n' + rewrite(open(os.path.join(CSRC, name)).read()))
+        text = f'#line 1 "{os.path.join(CSRC, name)}"\n' + rewrite(open(os.path.join(CSRC, name)).read())
+        if not (os.path.exists(out) and open(out).read() == text):     # (builds of several counts share these files)
+            with open(out, "w") as f:
+                f.write(text)
         cpps.append(out)
     cpps.append(os.path.join(HERE, "emu_tc_stubs.cpp"))
     cmd = ["g++", "-std=c++17", "-O1", "-g", "-fPIC", "-shared", "-ffp-contract=off", "-fno-strict-aliasing", "-w",
-           "-I", os.path.join(HERE, "shim"), "-I", CSRC, "-I", os.path.join(ROOT, "include"), "-x", "c++"] + cpps + \
-          ["-o", LIB]
+           f"-DPCL_EMU_SMS={int(sms)}", "-I", os.path.join(HERE, "shim"), "-I", CSRC, "-I", os.path.join(ROOT, "include"),
+           "-x", "c++"] + cpps + ["-o", lib]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("emulation build failed:\n" + r.stdout[-4000:] + r.stderr[-8000:])
     with open(stamp, "w") as f:
         f.write(dig)
-    return LIB
+    return lib
 
 
 if __name__ == "__main__":

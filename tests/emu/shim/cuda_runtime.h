@@ -378,8 +378,12 @@ static inline int __float2int_rn(float x) { return (int)lrintf(x); }
 static inline void __trap() { fprintf(stderr, "emu: __trap()\n"); abort(); }
 #define __grid_constant__
 enum cudaDeviceAttr { cudaDevAttrMultiProcessorCount = 16 };
-// a small "GPU" keeps persistent grids short under emulation and still exercises multi-CTA work splitting
-static inline cudaError_t cudaDeviceGetAttribute(int* v, cudaDeviceAttr, int) { *v = 6; return cudaSuccess; }
+// a small "GPU" keeps persistent grids short under emulation and still exercises multi-CTA work splitting; builds with
+// -DPCL_EMU_SMS=n model an n-SM part (132: H100 SXM, 114: H100 PCIe) to reach the work splits of a real device
+#ifndef PCL_EMU_SMS
+#define PCL_EMU_SMS 6
+#endif
+static inline cudaError_t cudaDeviceGetAttribute(int* v, cudaDeviceAttr, int) { *v = PCL_EMU_SMS; return cudaSuccess; }
 enum cudaDriverEntryPointQueryResult { cudaDriverEntryPointSuccess = 0, cudaDriverEntryPointSymbolNotFound = 1 };
 enum { cudaEnableDefault = 0 };
 cudaError_t cudaGetDriverEntryPoint(const char* symbol, void** fn, unsigned long long flags, cudaDriverEntryPointQueryResult* q);

@@ -26,16 +26,16 @@ def _rel(a, b):
     return abs(a - b) / max(abs(b), 1e-9)
 
 
-def fuzz_loss(seed: int, n: int):
+def fuzz_loss(seed: int, n: int, device="cpu", scale: int = 1):
     """PixelContrastLoss (exact path, injected permutations) vs the float64 oracle: random batch / embedding / image
     sizes (divisible and not), class counts, sampling limits, with and without bank, seg logits or predictions.
     Degenerate inputs: the reference raises (no class qualifies, zero views) -> the engine returns an exact zero;
-    rows without positives -> NaN on both sides."""
+    rows without positives -> NaN on both sides.  `scale` multiplies the largest feature map and max_samples."""
     rng = random.Random(seed)
     bad = []
     for it in range(n):
-        B, D, h, w = rng.randint(1, 3), rng.choice([32, 64]), rng.randint(3, 36), rng.randint(3, 36)
-        K, ms, mv = rng.randint(2, 12), rng.randint(4, 160), rng.randint(1, 16)
+        B, D, h, w = rng.randint(1, 3), rng.choice([32, 64]), rng.randint(3, 36 * scale), rng.randint(3, 36 * scale)
+        K, ms, mv = rng.randint(2, 12), rng.randint(4, 160 * scale), rng.randint(1, 16 * scale)
         block, boost = rng.choice([2, 3, 5, 8, 16]), rng.choice([0.0, 1.0, 2.0, 4.0])
         if rng.random() < 0.5:
             st = rng.choice([1, 2, 4])
@@ -63,10 +63,10 @@ def fuzz_loss(seed: int, n: int):
             why = type(ex).__name__
         crit = cs.PixelContrastLoss(_cfg(T, bT, ms, mv, K))
         crit.perm_fn = P.PermReplay(rec.draws) if why is None else (lambda k: torch.randperm(k))
-        embed = data["embed"].clone().requires_grad_(True)
-        queue = (bank["segment_queue"].clone(), bank["pixel_queue"].clone()) if mem else None
-        loss = crit(embed, data["target"], predict=None if use_seg else predict, seg=data["seg"] if use_seg else None,
-                    queue=queue)
+        embed = data["embed"].clone().to(device).requires_grad_(True)
+        queue = (bank["segment_queue"].clone().to(device), bank["pixel_queue"].clone().to(device)) if mem else None
+        loss = crit(embed, data["target"].to(device), predict=None if use_seg else predict.to(device),
+                    seg=data["seg"].to(device) if use_seg else None, queue=queue)
         loss.backward()
         if why == "IndexError":
             continue          # more anchors than bank columns (Q1): the reference crashes, the engine masks nothing
@@ -79,7 +79,7 @@ def fuzz_loss(seed: int, n: int):
             if not math.isnan(lv):
                 bad.append(f"reference NaN, engine {lv}: {desc}")
             continue
-        gerr = (embed.grad.double() - e64.grad).abs().max().item() / max(e64.grad.abs().max().item(), 1e-9)
+        gerr = (embed.grad.double().cpu() - e64.grad).abs().max().item() / max(e64.grad.abs().max().item(), 1e-9)
         if _rel(lv, rv) > 5e-6 or gerr > 2e-5:
             bad.append(f"mismatch rel={_rel(lv, rv):.2e} gerr={gerr:.2e}: {desc}")
     return bad
@@ -170,23 +170,24 @@ def fuzz_segce(seed: int, n: int):
     return bad
 
 
-def fuzz_device_sampling(seed: int, n: int, check_sampling):
+def fuzz_device_sampling(seed: int, n: int, check_sampling, device="cpu", scale: int = 1):
     """Device RNG (keyed bijection, no injected permutations), optional fused normalise: every anchor a valid distinct
-    pixel of its (image, class, hard|easy) group; loss / gradient vs the oracle evaluated on exactly those anchors."""
+    pixel of its (image, class, hard|easy) group; loss / gradient vs the oracle evaluated on exactly those anchors.
+    `scale` multiplies the largest feature map and max_samples."""
     rng = random.Random(seed)
     bad = []
     for it in range(n):
-        B, D, h, w = rng.randint(1, 3), rng.choice([32, 64]), rng.randint(4, 40), rng.randint(4, 40)
-        K, ms, mv = rng.randint(2, 10), rng.randint(4, 200), rng.randint(1, 16)
+        B, D, h, w = rng.randint(1, 3), rng.choice([32, 64]), rng.randint(4, 40 * scale), rng.randint(4, 40 * scale)
+        K, ms, mv = rng.randint(2, 10), rng.randint(4, 200 * scale), rng.randint(1, 16 * scale)
         block, st, boost = rng.choice([2, 4, 8, 16]), rng.choice([1, 2, 4]), rng.choice([0.0, 2.0, 4.0])
         mem, norm, sd = rng.random() < 0.4, rng.random() < 0.4, rng.randint(0, 10 ** 6)
         desc = f"devrng seed={seed} it={it} B={B} D={D} {h}x{w} K={K} ms={ms} mv={mv} block={block} st={st} mem={mem} norm={norm}"
         data = make_contrast_batch(B=B, D=D, h=h, w=w, num_classes=K, img_stride=st, block=block, boost=boost, seed=sd)
         bank = make_bank(K, rng.randint(8, 30), D, sd + 1)
         crit = cs.PixelContrastLoss(_cfg(0.1, 0.07, ms, mv, K))
-        embed = (data["embed_raw"] if norm else data["embed"]).clone().requires_grad_(True)
-        queue = (bank["segment_queue"].clone(), bank["pixel_queue"].clone()) if mem else None
-        loss = crit(embed, data["target"], seg=data["seg"], queue=queue, normalize=norm)
+        embed = (data["embed_raw"] if norm else data["embed"]).clone().to(device).requires_grad_(True)
+        queue = (bank["segment_queue"].clone().to(device), bank["pixel_queue"].clone().to(device)) if mem else None
+        loss = crit(embed, data["target"].to(device), seg=data["seg"].to(device), queue=queue, normalize=norm)
         loss.backward()
         ws = Fn.last_workspace(embed.device)
         TC, V, A = ws.plan_header()[:3]
@@ -219,19 +220,20 @@ def fuzz_device_sampling(seed: int, n: int, check_sampling):
             if not math.isnan(loss.item()):
                 bad.append(f"reference NaN, engine {loss.item()}: {desc}")
             continue
-        gerr = (embed.grad.double() - e64.grad).abs().max().item() / max(e64.grad.abs().max().item(), 1e-9)
+        gerr = (embed.grad.double().cpu() - e64.grad).abs().max().item() / max(e64.grad.abs().max().item(), 1e-9)
         if _rel(loss.item(), lo.item()) > 5e-6 or gerr > 3e-5:
             bad.append(f"mismatch rel={_rel(loss.item(), lo.item()):.2e} gerr={gerr:.2e}: {desc}")
     return bad
 
 
-def fuzz_topk(seed: int, n: int):
+def fuzz_topk(seed: int, n: int, device="cpu", scale: int = 1):
     """a10 top-k kernels vs the sort-based oracle: explicit / self / bank (zero tail) operands; exact dyadic data (ties,
-    strict gradient check) and unit-norm data (near-ties: loss strict, gradient in norm)."""
+    strict gradient check) and unit-norm data (near-ties: loss strict, gradient in norm).  `scale` multiplies the
+    largest A, N and bank size."""
     rng = random.Random(seed)
     bad = []
     for it in range(n):
-        A, N, D, ncls = rng.randint(2, 150), rng.randint(2, 400), rng.choice([32, 64]), rng.randint(2, 8)
+        A, N, D, ncls = rng.randint(2, 150 * scale), rng.randint(2, 400 * scale), rng.choice([32, 64]), rng.randint(2, 8)
         k, exact, mode = rng.randint(1, 60), rng.random() < 0.5, rng.choice(["explicit", "self", "bank"])
         g = torch.Generator().manual_seed(rng.randint(0, 10 ** 6))
         desc = f"topk seed={seed} it={it} A={A} N={N} D={D} classes={ncls} k={k} exact={exact} mode={mode}"
@@ -246,13 +248,15 @@ def fuzz_topk(seed: int, n: int):
         if mode == "explicit":
             c, yc, diag = mk(N, D), torch.randint(0, ncls, (N,), generator=g), torch.arange(A) % N
             o = P.infonce_topk(a, ya, c, yc, T, bT, k, False, diag_cols=diag)
-            loss, rs, st = Fn.infonce_forward(a.float(), ya, contrast=c.float(), contrast_cls=yc, diag_col=diag,
+            loss, rs, st = Fn.infonce_forward(a.float().to(device), ya.to(device), contrast=c.float().to(device),
+                                              contrast_cls=yc.to(device), diag_col=diag.to(device),
                                               temperature=T, base_temperature=bT, topk=k)
         elif mode == "self":
             o = P.infonce_topk(a, ya, a, ya, T, bT, k, True)
-            loss, rs, st = Fn.infonce_forward(a.float(), ya, temperature=T, base_temperature=bT, topk=k)
+            loss, rs, st = Fn.infonce_forward(a.float().to(device), ya.to(device), temperature=T, base_temperature=bT,
+                                              topk=k)
         else:
-            K, M = ncls, rng.randint(1, 12)
+            K, M = ncls, rng.randint(1, 12 * scale)
             if A > K * 2 * M:
                 continue
             segq, pixq = mk(K, M, D), mk(K, M, D)
@@ -261,9 +265,10 @@ def fuzz_topk(seed: int, n: int):
             ya = ya[torch.argsort(torch.where(ya == 0, K, ya), stable=True)]
             contrast, yc = P.flatten_queue(torch.cat((segq, pixq), 1))
             o = P.infonce_topk(a, ya, contrast, yc.long(), T, bT, k, False)
-            loss, rs, st = Fn.infonce_forward(a.float(), ya, queues=(segq.float(), pixq.float()),
-                                              diag_col=torch.arange(A), temperature=T, base_temperature=bT, topk=k)
-        dA = Fn.infonce_backward(st, rs).double()
+            loss, rs, st = Fn.infonce_forward(a.float().to(device), ya.to(device),
+                                              queues=(segq.float().to(device), pixq.float().to(device)),
+                                              diag_col=torch.arange(A).to(device), temperature=T, base_temperature=bT, topk=k)
+        dA = Fn.infonce_backward(st, rs).double().cpu()
         lo = o["loss"].item()
         if math.isnan(lo):
             if not math.isnan(loss.item()):
@@ -282,69 +287,83 @@ def _bf(x):
     return x.to(torch.bfloat16).to(torch.float32)
 
 
-def fuzz_tensor_path(seed: int, n: int):
+def fuzz_tensor_path(seed: int, n: int, device="cpu", scale: int = 1):
     """wgmma sweeps (functional model) on explicit operands: self-contrast, explicit contrast set (sorted / unsorted
     labels), bank through the bf16 shadow; ragged A and N (not multiples of the 128 x 256 tile), few / many classes.
     Loss and positive counts against the float64 closed form on the bf16-rounded operands; gradient within the bf16
-    tolerance of the path (max-abs 6e-3 * max|g|, relative Frobenius 5e-3)."""
-    from contrastiveseg_b200.bank import shadow_rows
+    tolerance of the path (max-abs 6e-3 * max|g|, relative Frobenius 5e-3).  `scale` multiplies the largest A, N and
+    bank size (on a GPU: enough (row tile, column tile) pairs to fill the SMs several times)."""
     rng = random.Random(seed)
     bad = []
-    lib = _abi.load()
     for it in range(n):
-        A, N, ncls = rng.randint(1, 420), rng.randint(1, 1500), rng.randint(1, 20)
+        A, N, ncls = rng.randint(1, 420 * scale), rng.randint(1, 1500 * scale), rng.randint(1, 20)
         T, mode, clustered = rng.choice([0.07, 0.1, 0.5]), rng.choice(["self", "sorted", "unsorted", "bank"]), rng.choice([0.0, 0.5])
         g = torch.Generator().manual_seed(rng.randint(0, 10 ** 6))
-        desc = f"tensor seed={seed} it={it} A={A} N={N} classes={ncls} T={T} mode={mode} clustered={clustered}"
-        centers = F.normalize(torch.randn(ncls + 1, 256, generator=g), dim=1)
-        ya = torch.randint(0, ncls, (A,), generator=g)
-        a = F.normalize(torch.randn(A, 256, generator=g) + clustered * 16 * centers[ya], dim=1)
-        if mode == "self":
-            loss, st, state = Fn.infonce_tc_forward(a, ya, temperature=T, base_temperature=0.07)
-            cf = P.infonce_closed_form(_bf(a).double(), ya, _bf(a).double(), ya, T, 0.07, self_contrast=True)
-        elif mode in ("sorted", "unsorted"):
-            yc = torch.randint(0, ncls, (N,), generator=g)
-            if mode == "sorted":
-                yc = torch.sort(yc).values
-            c = F.normalize(torch.randn(N, 256, generator=g) + clustered * 16 * centers[yc], dim=1)
-            c16 = Fn.to_bf16_rows(c, -(-N // 256) * 256)
-            diag = torch.arange(A) % N
-            loss, st, state = Fn.infonce_tc_forward(a, ya, contrast_bf16=c16, contrast_cls=yc, n_cols=N, diag_col=diag,
-                                                    temperature=T, base_temperature=0.07, sorted_cols=(mode == "sorted"))
-            cf = P.infonce_closed_form(_bf(a).double(), ya, _bf(c).double(), yc, T, 0.07, self_contrast=False, diag_cols=diag)
-        else:
-            K, M = max(ncls, 2), rng.randint(1, 40)
-            if A > K * 2 * M:
-                continue
-            ya = torch.randint(0, K, (A,), generator=g)
-            ya = ya[torch.argsort(torch.where(ya == 0, K, ya), stable=True)]
-            a = F.normalize(torch.randn(A, 256, generator=g) + clustered * 16 * centers[ya], dim=1)
-            segq = F.normalize(torch.randn(K, M, 256, generator=g), dim=2)
-            pixq = F.normalize(torch.randn(K, M, 256, generator=g), dim=2)
-            shadow = torch.empty((shadow_rows(K, M), 256), dtype=torch.bfloat16)
-            _abi.check(lib.pcl_bank_shadow_rebuild(segq.data_ptr(), pixq.data_ptr(), K, M, 256, shadow.data_ptr(), None))
-            loss, st, state = Fn.infonce_tc_forward(a, ya, bank=(shadow, K, 2 * M), diag_col=torch.arange(A),
-                                                    temperature=T, base_temperature=0.07)
-            contrast, yc = P.flatten_queue(torch.cat((_bf(segq), _bf(pixq)), 1).double())
-            cf = P.infonce_closed_form(_bf(a).double(), ya, contrast, yc.long(), T, 0.07, self_contrast=False)
-        dA = Fn.infonce_tc_backward(state, st).double()
-        lo = cf["loss"].item()
-        if math.isnan(lo):
-            if not math.isnan(loss.item()):
-                bad.append(f"reference NaN, engine {loss.item()}: {desc}")
-            continue
-        if not torch.equal(st[4].double(), cf["npos"]):
-            bad.append(f"positive counts differ: {desc}")
-            continue
-        # the gradient reference uses the same bf16-rounded operands (the rounding of the operands is not under test)
-        gmax = cf["dA"].abs().max().item()
-        gabs = (dA - cf["dA"]).abs().max().item() / max(gmax, 1e-9)
-        gfro = ((dA - cf["dA"]).norm() / max(cf["dA"].norm().item(), 1e-9)).item()
-        # (a loss that is exactly 0 in real arithmetic — a single class, no negatives — comes out as ~1e-8 of ex2/lg2
-        # approximation noise on the tensor path: absolute floor next to the relative bound)
-        if abs(loss.item() - lo) > 5e-5 * abs(lo) + 1e-6 or gabs > 6e-3 or gfro > 5e-3:   # (tiny contrast sets average less)
-            bad.append(f"mismatch rel={_rel(loss.item(), lo):.2e} gabs={gabs:.2e} gfro={gfro:.2e}: {desc}")
+        M = rng.randint(1, 40 * scale) if mode == "bank" else None
+        why = tensor_case(A, N, ncls, T, mode, clustered, g, M=M, device=device, ref_device=device)
+        if why:
+            bad.append(f"{why}: tensor seed={seed} it={it} A={A} N={N} classes={ncls} T={T} mode={mode} clustered={clustered}")
     return bad
+
+
+def tensor_case(A, N, ncls, T, mode, clustered, g, M=None, device="cpu", ref_device="cpu"):
+    """One tensor-path call (forward + backward) against the float64 closed form (fuzz_tensor_path's bounds), operands
+    drawn from `g`.  mode "bank": K = max(ncls, 2) classes of M rows in each queue (A > 2 K M is skipped: the closed
+    form needs a contrast column per anchor).  Returns None, or what differs."""
+    from contrastiveseg_b200.bank import shadow_rows
+    lib = _abi.load()
+    centers = F.normalize(torch.randn(ncls + 1, 256, generator=g), dim=1)
+    ya = torch.randint(0, ncls, (A,), generator=g)
+    a = F.normalize(torch.randn(A, 256, generator=g) + clustered * 16 * centers[ya], dim=1)
+    if mode == "self":
+        loss, st, state = Fn.infonce_tc_forward(a.to(device), ya.to(device), temperature=T, base_temperature=0.07)
+        cf = P.infonce_closed_form(_bf(a).double().to(ref_device), ya.to(ref_device), _bf(a).double().to(ref_device),
+                                   ya.to(ref_device), T, 0.07, self_contrast=True)
+    elif mode in ("sorted", "unsorted"):
+        yc = torch.randint(0, ncls, (N,), generator=g)
+        if mode == "sorted":
+            yc = torch.sort(yc).values
+        c = F.normalize(torch.randn(N, 256, generator=g) + clustered * 16 * centers[yc], dim=1)
+        c16 = Fn.to_bf16_rows(c.to(device), -(-N // 256) * 256)
+        diag = torch.arange(A) % N
+        loss, st, state = Fn.infonce_tc_forward(a.to(device), ya.to(device), contrast_bf16=c16, contrast_cls=yc.to(device),
+                                                n_cols=N, diag_col=diag.to(device), temperature=T, base_temperature=0.07,
+                                                sorted_cols=(mode == "sorted"))
+        cf = P.infonce_closed_form(_bf(a).double().to(ref_device), ya.to(ref_device), _bf(c).double().to(ref_device),
+                                   yc.to(ref_device), T, 0.07, self_contrast=False, diag_cols=diag)
+    else:
+        K = max(ncls, 2)
+        if A > K * 2 * M:
+            return None
+        ya = torch.randint(0, K, (A,), generator=g)
+        ya = ya[torch.argsort(torch.where(ya == 0, K, ya), stable=True)]
+        a = F.normalize(torch.randn(A, 256, generator=g) + clustered * 16 * centers[ya], dim=1)
+        segq = F.normalize(torch.randn(K, M, 256, generator=g), dim=2)
+        pixq = F.normalize(torch.randn(K, M, 256, generator=g), dim=2)
+        shadow = torch.empty((shadow_rows(K, M), 256), dtype=torch.bfloat16, device=device)
+        segq_d, pixq_d = segq.to(device), pixq.to(device)
+        _abi.check(lib.pcl_bank_shadow_rebuild(segq_d.data_ptr(), pixq_d.data_ptr(), K, M, 256, shadow.data_ptr(), None))
+        loss, st, state = Fn.infonce_tc_forward(a.to(device), ya.to(device), bank=(shadow, K, 2 * M),
+                                                diag_col=torch.arange(A).to(device), temperature=T, base_temperature=0.07)
+        contrast, yc = P.flatten_queue(torch.cat((_bf(segq), _bf(pixq)), 1).double())
+        cf = P.infonce_closed_form(_bf(a).double().to(ref_device), ya.to(ref_device), contrast.to(ref_device),
+                                   yc.long().to(ref_device), T, 0.07, self_contrast=False)
+    dA = Fn.infonce_tc_backward(state, st).double().cpu()
+    cf = {k: cf[k].cpu() for k in ("loss", "npos", "dA")}
+    lo = cf["loss"].item()
+    if math.isnan(lo):
+        return None if math.isnan(loss.item()) else f"reference NaN, engine {loss.item()}"
+    if not torch.equal(st[4].double().cpu(), cf["npos"]):
+        return "positive counts differ"
+    # the gradient reference uses the same bf16-rounded operands (the rounding of the operands is not under test)
+    gmax = cf["dA"].abs().max().item()
+    gabs = (dA - cf["dA"]).abs().max().item() / max(gmax, 1e-9)
+    gfro = ((dA - cf["dA"]).norm() / max(cf["dA"].norm().item(), 1e-9)).item()
+    # (a loss that is exactly 0 in real arithmetic — a single class, no negatives — comes out as ~1e-8 of ex2/lg2
+    # approximation noise on the tensor path: absolute floor next to the relative bound)
+    if abs(loss.item() - lo) > 5e-5 * abs(lo) + 1e-6 or gabs > 6e-3 or gfro > 5e-3:   # (tiny contrast sets average less)
+        return f"mismatch rel={_rel(loss.item(), lo):.2e} gabs={gabs:.2e} gfro={gfro:.2e}"
+    return None
 
 
 def fuzz_graphed_step(seed: int, n: int):

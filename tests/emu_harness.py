@@ -12,19 +12,19 @@ from contrastiveseg_b200 import _abi, bank as bank_mod, functional as Fn
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "emu"))
 import build_emu  # noqa: E402
 
-_lib = None
+_libs = {}
 
 
-def emu_library():
-    global _lib
-    if _lib is None:
-        lib = C.CDLL(build_emu.build())
+def emu_library(sms: int = 6):
+    """The emulator library for an `sms`-SM device, loaded once per count (each count is a library of its own)."""
+    if sms not in _libs:
+        lib = C.CDLL(build_emu.build() if sms == 6 else build_emu.build(sms=sms))
         for name, (res, args) in _abi.SIGNATURES.items():
             fn = getattr(lib, name)
             fn.restype, fn.argtypes = res, args
         assert lib.pcl_emulated() == 1
-        _lib = lib
-    return _lib
+        _libs[sms] = lib
+    return _libs[sms]
 
 
 class _NoCtx:
@@ -38,8 +38,8 @@ class _NoCtx:
         return False
 
 
-def use_emulation(monkeypatch):
-    lib = emu_library()
+def use_emulation(monkeypatch, sms: int = 6):
+    lib = emu_library(sms)
     monkeypatch.setattr(_abi, "load", lambda *a, **k: lib)
     monkeypatch.setattr(Fn, "_require_cuda", lambda t, name: None)
     monkeypatch.setattr(Fn, "_stream_ptr", lambda device: 0)
