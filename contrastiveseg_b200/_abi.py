@@ -126,6 +126,9 @@ SIGNATURES = {
     "pcl_rmi_scratch_bytes": (c_i64, [c_i32] * 9),
     "pcl_rmi_fwd": (c_i32, [c_vp, c_vp] + [c_i32] * 9 + [c_f32, c_i32, c_f32, c_vp, c_vp, c_vp]),
     "pcl_rmi_bwd": (c_i32, [c_vp, c_vp] + [c_i32] * 9 + [c_f32, c_i32, c_f32, c_vp, c_vp, c_vp, c_vp]),
+    "pcl_lovasz_scratch_bytes": (c_i64, [c_i32] * 6),
+    "pcl_lovasz_fwd": (c_i32, [c_vp, c_vp] + [c_i32] * 7 + [c_vp, c_vp, c_vp]),
+    "pcl_lovasz_bwd": (c_i32, [c_vp, c_vp] + [c_i32] * 7 + [c_vp, c_vp, c_vp, c_vp]),
     "pcl_bank_packet_floats": (c_i64, [C.POINTER(BankGeom)]),
     "pcl_bank_scratch_floats": (c_i64, [C.POINTER(BankGeom)]),
     "pcl_bank_packet": (c_i32, [C.POINTER(BankGeom), c_vp, c_vp, c_vp, c_u64, c_vp, c_vp, c_vp]),

@@ -1,6 +1,6 @@
-// Fused segmentation losses of the contrast wrappers: the plain CE (first part of this file) and the RMI loss of
-// contrast.use_rmi (second part).  Both up-sample the logits bilinearly inside the kernels and share the tile geometry
-// and transposed bilinear map of pcl_upsample.cuh.
+// Fused segmentation losses of the contrast wrappers: the plain CE (first part of this file), the RMI loss of
+// contrast.use_rmi (second part) and the Lovasz-softmax term of FSCELOVASZLoss (third part).  All up-sample the logits
+// bilinearly inside the kernels and share the tile geometry and transposed bilinear map of pcl_upsample.cuh.
 //
 // Fused segmentation cross-entropy of ContrastCELoss.forward (SURVEY §8f row 1, the next row after the contrast path):
 // replaces  F.interpolate(seg, (Himg,Wimg), bilinear, align_corners=True)  +  nn.CrossEntropyLoss(weight, ignore_index,
@@ -943,6 +943,597 @@ extern "C" int pcl_rmi_bwd(const float* seg, const int64_t* target, int32_t B, i
   PCL_SMEM_OPT_IN(k_rmi_bwd_tile, 200 * 1024);
   k_rmi_bwd_tile<<<dim3((unsigned)ceil_div(Wimg, BT), (unsigned)ceil_div(Himg, BTY), B), BT * BTY, smem, s>>>(
       a, (const float*)(sc + l.dP), (const uint8_t*)(sc + l.A), (const double*)(sc + l.fin), grad_loss, dseg, kc, pitch);
+  PCL_LAUNCH_CHECK();
+  return PCL_OK;
+}
+
+// ==================================================================================================================
+// Fused Lovasz-softmax segmentation loss of the contrast wrappers (FSCELOVASZLoss, lib/loss/loss_helper.py:77-124,
+// built by lib/loss/loss_contrast_mem.py:187-194 with contrast.use_lovasz): replaces
+//   F.interpolate(seg, (Himg,Wimg), bilinear, align_corners=True) + softmax + flatten_probas + lovasz_softmax_flat(
+//   only_present=True)  (lib/loss/lovasz_loss.py:216-267)
+// and its autograd backward without materialising the (B,K,Himg,Wimg) up-sampled logits, their softmax, the permuted
+// copy or the masked gather, and without a host sync per class.  N = B*Himg*Wimg label pixels, q = (b*Himg + y)*Wimg + x.
+//   k_lov_keys      tile kernel (pcl_upsample.cuh geometry): bilinear logits, softmax, per class the key
+//                   d = bits(1.0f) - bits(e), e = |fg - p_c| (e in [0, 1]: the bit order is the value order, so an
+//                   ascending sort of d is a descending sort of e); an ignored pixel gets LOV_SENT, which sorts last.
+//                   Also the pixel's (max, sum of exp) for the backward and a u8 label copy.
+//   sort            per class, stable LSD radix sort of (d, q) in 4 passes of 8 bits, classes in chunks chosen from the
+//                   shapes.  Each pass: k_lov_hist (per-tile digit counts), k_lov_scan (exclusive scan per class, fixed
+//                   order), k_lov_scatter (stable in-tile rank by warp ballots).  No CTA waits on another: the result
+//                   does not depend on scheduling.  Ties in e keep ascending q (the input order).
+//   k_lov_fgcount   fg count per tile of the sorted order, scanned by k_lov_scan (the class's gts is its total)
+//   k_lov_loss      per sorted position i with cumfg F and cumbg i-F before it (exact integers): I = gts - F,
+//                   U = gts + i - F, g = 1/U for a fg step, I/(U(U+1)) for a bg step (the reference's J_i - J_{i-1} in
+//                   closed form, free of its fp32 cancellation); loss_c partials sum e*g in fp64, g is scattered to ge[c][q]
+//   k_lov_finalize  mean of loss_c over the present classes (gts > 0), in a fixed order: the loss is bit-reproducible
+//   k_lov_bwd_tile  recomputes p from the staged patch; dp_c = grad * ge_c * sgn(p_c - fg_c) / n_present, dz = p (dp - <p, dp>),
+//                   then the transposed bilinear map into dseg (up_tile_flush: <= 4-way fp32 atomics, dseg reproducible to
+//                   the last ulp or two)
+// First-order HBM bytes at B=8, K=19, 128x256 -> 512x1024 (N = 4.19 M, K*N = 79.7 M keys): the keys kernel writes 318 MB;
+// each sort pass reads the keys twice and the payload once and writes both (~20 B per key, 1.6 GB per pass); the loss
+// reads the sorted pairs twice and scatters ge (~1 GB); the backward reads ge (318 MB) and seg, and writes dseg (DESIGN §4).
+namespace pcl {
+
+constexpr uint32_t LOV_ONE = 0x3F800000u;     // bits of 1.0f
+constexpr uint32_t LOV_SENT = 0x3FFFFFFFu;    // ignored pixel: above every d = LOV_ONE - bits(e) <= LOV_ONE
+constexpr int LOV_THREADS = 256;
+constexpr int LOV_ITEMS = 8;
+constexpr int LOV_TILE = LOV_THREADS * LOV_ITEMS;   // keys per sort / loss tile
+constexpr int LOV_RADIX = 256;
+constexpr int LOV_PASSES = 4;                       // 4 x 8 bits cover the 30 live bits of d
+constexpr int LOV_KC = 32;                          // classes staged per pass in the keys kernel
+constexpr int LOV_KC_BWD = 24;
+
+struct LovArgs {
+  const float* seg; const int64_t* target;
+  int B, K, h, w, H, W, ignore_index;
+  float ry, rx;
+  int64_t N;                    // B*H*W
+};
+
+// bilinear weights / patch offsets of this thread's label pixel inside the staged patch
+struct LovPix {
+  float w00, w01, w10, w11;
+  int i00, i01, i10, i11;
+};
+
+__device__ __forceinline__ LovPix lov_pix(const UpTile& g, int tx, int ty, const int* s_y0, const int* s_y1,
+                                          const float* s_ly, const int* s_x0, const int* s_x1, const float* s_lx) {
+  LovPix p;
+  const int ly0 = s_y0[ty] - g.ys_base, ly1 = s_y1[ty] - g.ys_base, lx0 = s_x0[tx] - g.xs_base, lx1 = s_x1[tx] - g.xs_base;
+  const float ly = s_ly[ty], lx = s_lx[tx];
+  p.w00 = (1.f - ly) * (1.f - lx); p.w01 = (1.f - ly) * lx; p.w10 = ly * (1.f - lx); p.w11 = ly * lx;
+  p.i00 = ly0 * g.xs_n + lx0; p.i01 = ly0 * g.xs_n + lx1; p.i10 = ly1 * g.xs_n + lx0; p.i11 = ly1 * g.xs_n + lx1;
+  return p;
+}
+
+__device__ __forceinline__ float lov_logit(const LovPix& p, const float* s) {
+  return p.w00 * s[p.i00] + p.w01 * s[p.i01] + p.w10 * s[p.i10] + p.w11 * s[p.i11];
+}
+
+__device__ __forceinline__ void lov_stage(const LovArgs& a, const UpTile& g, int b, int c0, int cn, int pitch, float* S) {
+  const int patch = g.ys_n * g.xs_n;
+  const int64_t hw = (int64_t)a.h * a.w;
+  for (int i = threadIdx.x; i < cn * patch; i += BT * BTY) {
+    const int cc = i / patch, r = i - cc * patch;
+    const int yy = r / g.xs_n, xx = r - yy * g.xs_n;
+    S[cc * pitch + r] = a.seg[((int64_t)b * a.K + c0 + cc) * hw + (int64_t)(g.ys_base + yy) * a.w + g.xs_base + xx];
+  }
+}
+
+// the label of pixel (b, y, x) if it counts (not ignore_index, inside [0, K)), else -1
+__device__ __forceinline__ int lov_label(const LovArgs& a, int64_t q) {
+  const int64_t t = a.target[q];
+  return (t != (int64_t)a.ignore_index && t >= 0 && t < a.K) ? (int)t : -1;
+}
+
+// ---- keys --------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(BT * BTY)
+k_lov_keys(LovArgs a, uint32_t* __restrict__ keys, float2* __restrict__ ms, uint8_t* __restrict__ lab, int pitch, int kc) {
+  extern __shared__ float sm[];                    // [kc][pitch] source patch
+  __shared__ int s_y0[BTY], s_y1[BTY], s_x0[BT], s_x1[BT];
+  __shared__ float s_ly[BTY], s_lx[BT];
+  const int tx = threadIdx.x & (BT - 1), ty = threadIdx.x >> 5;
+  const int b = blockIdx.z;
+  const int X0 = blockIdx.x * BT, Y0 = blockIdx.y * BTY;
+  const int x = X0 + tx, y = Y0 + ty;
+  const UpTile g = up_tile_coords(X0, Y0, a.H, a.W, a.h, a.w, a.ry, a.rx, s_y0, s_y1, s_ly, s_x0, s_x1, s_lx);
+  const LovPix px = lov_pix(g, tx, ty, s_y0, s_y1, s_ly, s_x0, s_x1, s_lx);
+  const bool inside = x < a.W && y < a.H;
+  const int64_t q = ((int64_t)b * a.H + y) * a.W + x;
+  const int t = inside ? lov_label(a, q) : -1;
+  float m = -CUDART_INF_F, se = 0.f;
+  const bool one = a.K <= kc;                      // one staged chunk: the second sweep reuses it
+  for (int c0 = 0; c0 < a.K; c0 += kc) {
+    const int cn = min(kc, a.K - c0);
+    lov_stage(a, g, b, c0, cn, pitch, sm);
+    __syncthreads();
+    for (int cc = 0; cc < cn; ++cc) {
+      const float v = lov_logit(px, sm + cc * pitch);
+      if (v > m) { se = se * __expf(m - v) + 1.f; m = v; }     // online sum of exp
+      else       { se += __expf(v - m); }
+    }
+    if (!one) __syncthreads();
+  }
+  if (inside) {
+    ms[q] = make_float2(m, se);
+    lab[q] = (uint8_t)(t >= 0 ? t : 0);
+  }
+  for (int c0 = 0; c0 < a.K; c0 += kc) {
+    const int cn = min(kc, a.K - c0);
+    if (!one) {
+      lov_stage(a, g, b, c0, cn, pitch, sm);
+      __syncthreads();
+    }
+    if (inside) {
+      for (int cc = 0; cc < cn; ++cc) {
+        const int c = c0 + cc;
+        uint32_t d = LOV_SENT;
+        if (t >= 0) {
+          const float p = __expf(lov_logit(px, sm + cc * pitch) - m) / se;
+          const float e = fabsf((t == c ? 1.f : 0.f) - p);
+          d = LOV_ONE - __float_as_uint(e);
+        }
+        keys[(int64_t)c * a.N + q] = d;
+      }
+    }
+    if (!one) __syncthreads();
+  }
+}
+
+// ---- sort ----------------------------------------------------------------------------------------------
+// hist[c][digit][tile]: digit counts of each tile (shared-memory atomics: integer counts, order-free)
+__global__ void __launch_bounds__(LOV_THREADS)
+k_lov_hist(const uint32_t* __restrict__ keys, int64_t N, int shift, int ntiles, int* __restrict__ hist) {
+  __shared__ int s_h[LOV_RADIX];
+  const int c = blockIdx.y;
+  s_h[threadIdx.x] = 0;
+  __syncthreads();
+  const uint32_t* k = keys + (int64_t)c * N;
+  const int64_t base = (int64_t)blockIdx.x * LOV_TILE;
+  for (int r = 0; r < LOV_ITEMS; ++r) {
+    const int64_t i = base + r * LOV_THREADS + threadIdx.x;
+    if (i < N) atomicAdd(&s_h[(k[i] >> shift) & (LOV_RADIX - 1)], 1);
+  }
+  __syncthreads();
+  hist[((int64_t)c * LOV_RADIX + threadIdx.x) * ntiles + blockIdx.x] = s_h[threadIdx.x];
+}
+
+// In-place exclusive scan of len ints per class (blockIdx.x = class, row stride `stride`); the total goes to total[c]
+// when total is given.  One CTA per class, sequential over chunks: a fixed order, no inter-CTA dependency.
+__global__ void __launch_bounds__(1024)
+k_lov_scan(int* __restrict__ data, int64_t len, int64_t stride, int* __restrict__ total) {
+  __shared__ int s_w[32];
+  int* d = data + (int64_t)blockIdx.x * stride;
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  int carry = 0;
+  for (int64_t base = 0; base < len; base += 4 * 1024) {
+    int v[4], s = 0;
+    const int64_t i0 = base + 4 * (int64_t)threadIdx.x;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) { v[j] = i0 + j < len ? d[i0 + j] : 0; s += v[j]; }
+    int incl = s;                                                    // warp inclusive scan
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int u = __shfl_up_sync(0xffffffffu, incl, o);
+      if (lane >= o) incl += u;
+    }
+    if (lane == 31) s_w[wid] = incl;
+    __syncthreads();
+    if (wid == 0) {
+      const int wv = s_w[lane];
+      int wi = wv;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const int u = __shfl_up_sync(0xffffffffu, wi, o);
+        if (lane >= o) wi += u;
+      }
+      s_w[lane] = wi - wv;                                           // exclusive warp offsets
+    }
+    __syncthreads();
+    int run = carry + s_w[wid] + incl - s;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      if (i0 + j < len) d[i0 + j] = run;
+      run += v[j];
+    }
+    __syncthreads();
+    if (threadIdx.x == 1023) s_w[0] = s_w[31] + incl;             // chunk total: last warp's offset + its total
+    __syncthreads();
+    carry += s_w[0];
+    __syncthreads();
+  }
+  if (total && threadIdx.x == 0) total[blockIdx.x] = carry;
+}
+
+// One stable LSD pass: keys_in / vals_in (vals_in null on the first pass: the payload is the index q) -> keys_out /
+// vals_out at offs[c][digit][tile] + the item's rank among the tile's items of its digit.  Items go in index order: round
+// r, warp w, lane l holds index r*256 + 32 w + l; within a warp the peers of a digit come from 8 ballots.
+__global__ void __launch_bounds__(LOV_THREADS)
+k_lov_scatter(const uint32_t* __restrict__ keys_in, const uint32_t* __restrict__ vals_in, int64_t N, int shift,
+              int ntiles, const int* __restrict__ offs, uint32_t* __restrict__ keys_out, uint32_t* __restrict__ vals_out) {
+  __shared__ int s_cnt[2 * LOV_RADIX * (LOV_THREADS / 32)];         // [buffer][digit][warp]
+  __shared__ int s_base[LOV_RADIX];                                  // global offset of the tile's digit + running count
+  const int c = blockIdx.y;
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  constexpr int NW = LOV_THREADS / 32;
+  const int64_t cN = (int64_t)c * N;
+  for (int i = threadIdx.x; i < 2 * LOV_RADIX * NW; i += LOV_THREADS) s_cnt[i] = 0;
+  s_base[threadIdx.x] = offs[((int64_t)c * LOV_RADIX + threadIdx.x) * ntiles + blockIdx.x];
+  __syncthreads();
+  const int64_t base = (int64_t)blockIdx.x * LOV_TILE;
+  const unsigned lt = (1u << lane) - 1u;
+  for (int r = 0; r < LOV_ITEMS; ++r) {
+    int* cnt = s_cnt + (r & 1) * LOV_RADIX * NW;
+    const int64_t i = base + r * LOV_THREADS + threadIdx.x;
+    const bool valid = i < N;
+    uint32_t key = 0, val = 0;
+    if (valid) {
+      key = keys_in[cN + i];
+      val = vals_in ? vals_in[cN + i] : (uint32_t)i;
+    }
+    const int dg = (int)((key >> shift) & (LOV_RADIX - 1));
+    unsigned peers = __ballot_sync(0xffffffffu, valid);
+#pragma unroll
+    for (int bit = 0; bit < 8; ++bit) {
+      const int on = (dg >> bit) & 1;
+      const unsigned bb = __ballot_sync(0xffffffffu, on);
+      peers &= on ? bb : ~bb;
+    }
+    const int rank = __popc(peers & lt);
+    if (valid && rank == 0) cnt[dg * NW + wid] = __popc(peers);
+    __syncthreads();
+    {                                                                // thread = digit: warp counts -> offsets
+      int* row = cnt + threadIdx.x * NW;
+      int run = s_base[threadIdx.x];
+#pragma unroll
+      for (int w = 0; w < NW; ++w) { const int n = row[w]; row[w] = run; run += n; }
+      s_base[threadIdx.x] = run;
+      int* nxt = s_cnt + ((r + 1) & 1) * LOV_RADIX * NW + threadIdx.x * NW;
+#pragma unroll
+      for (int w = 0; w < NW; ++w) nxt[w] = 0;
+    }
+    __syncthreads();
+    if (valid) {
+      const int64_t o = cN + cnt[dg * NW + wid] + rank;
+      keys_out[o] = key;
+      vals_out[o] = val;
+    }
+  }
+}
+
+// ---- scan and loss -----------------------------------------------------------------------------------------
+__device__ __forceinline__ bool lov_fg(uint32_t key, uint32_t q, const uint8_t* lab, int c) {
+  return key != LOV_SENT && (int)lab[q] == c;
+}
+
+__global__ void __launch_bounds__(LOV_THREADS)
+k_lov_fgcount(const uint32_t* __restrict__ keys, const uint32_t* __restrict__ vals, const uint8_t* __restrict__ lab,
+              int64_t N, int c0, int ntiles, int* __restrict__ tilefg) {
+  __shared__ int s_w[LOV_THREADS / 32];
+  const int c = blockIdx.y;
+  const int64_t cN = (int64_t)c * N;
+  const int64_t base = (int64_t)blockIdx.x * LOV_TILE;
+  int n = 0;
+  for (int r = 0; r < LOV_ITEMS; ++r) {
+    const int64_t i = base + r * LOV_THREADS + threadIdx.x;
+    if (i < N) n += lov_fg(keys[cN + i], vals[cN + i], lab, c0 + c);
+  }
+  n = warp_sum_i(n);
+  if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = n;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int s = 0;
+    for (int w = 0; w < LOV_THREADS / 32; ++w) s += s_w[w];
+    tilefg[(int64_t)(c0 + c) * ntiles + blockIdx.x] = s;
+  }
+}
+
+// Thread t of a tile owns the LOV_ITEMS consecutive sorted positions base + t*LOV_ITEMS + j.
+__global__ void __launch_bounds__(LOV_THREADS)
+k_lov_loss(const uint32_t* __restrict__ keys, const uint32_t* __restrict__ vals, const uint8_t* __restrict__ lab,
+           int64_t N, int c0, int ntiles, const int* __restrict__ tilefg, const int* __restrict__ gts_all,
+           float* __restrict__ ge, double* __restrict__ part) {
+  __shared__ int s_w[LOV_THREADS / 32];
+  __shared__ double s_d[LOV_THREADS / 32];
+  const int c = blockIdx.y, cg = c0 + c;
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const int64_t cN = (int64_t)c * N;
+  const int64_t i0 = (int64_t)blockIdx.x * LOV_TILE + (int64_t)threadIdx.x * LOV_ITEMS;
+  const int64_t gts = gts_all[cg];
+  float* gec = ge + (int64_t)cg * N;
+  uint32_t key[LOV_ITEMS], q[LOV_ITEMS];
+  int nfg = 0;
+#pragma unroll
+  for (int j = 0; j < LOV_ITEMS; ++j) {
+    key[j] = LOV_SENT; q[j] = 0;
+    if (i0 + j < N) { key[j] = keys[cN + i0 + j]; q[j] = vals[cN + i0 + j]; }
+    nfg += lov_fg(key[j], q[j], lab, cg);
+  }
+  int incl = nfg;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int u = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += u;
+  }
+  if (lane == 31) s_w[wid] = incl;
+  __syncthreads();
+  int wbase = 0;
+  for (int w = 0; w < wid; ++w) wbase += s_w[w];
+  int64_t F = (int64_t)tilefg[(int64_t)cg * ntiles + blockIdx.x] + wbase + incl - nfg;   // fg before position i0
+  double acc = 0.0;
+#pragma unroll
+  for (int j = 0; j < LOV_ITEMS; ++j) {
+    const int64_t i = i0 + j;
+    if (i >= N) break;
+    if (key[j] == LOV_SENT || gts == 0) { gec[q[j]] = 0.f; continue; }
+    const bool fg = (int)lab[q[j]] == cg;
+    const double I = (double)(gts - F), U = (double)(gts + (i - F));
+    const double gv = fg ? 1.0 / U : I / (U * (U + 1.0));
+    acc += (double)__uint_as_float(LOV_ONE - key[j]) * gv;
+    gec[q[j]] = (float)gv;
+    F += fg;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  if (lane == 0) s_d[wid] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double s = 0.0;
+    for (int w = 0; w < LOV_THREADS / 32; ++w) s += s_d[w];                      // fixed order
+    part[(int64_t)cg * ntiles + blockIdx.x] = s;
+  }
+}
+
+// loss = sum over present classes of loss_c / n_present (0 when no pixel counts); fin = {loss, n_present}
+__global__ void __launch_bounds__(256)
+k_lov_finalize(const double* __restrict__ part, const int* __restrict__ gts, int K, int ntiles, float* __restrict__ fin,
+               float* __restrict__ out) {
+  __shared__ double s_d[256];
+  double tot = 0.0;
+  int npres = 0;
+  for (int c = 0; c < K; ++c) {
+    double s = 0.0;
+    for (int t = threadIdx.x; t < ntiles; t += 256) s += part[(int64_t)c * ntiles + t];
+    s_d[threadIdx.x] = s;
+    __syncthreads();
+    for (int o = 128; o > 0; o >>= 1) {
+      if (threadIdx.x < o) s_d[threadIdx.x] += s_d[threadIdx.x + o];
+      __syncthreads();
+    }
+    if (gts[c] > 0) { tot += s_d[0]; ++npres; }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    const float loss = npres ? (float)(tot / (double)npres) : 0.f;
+    fin[0] = loss;
+    fin[1] = (float)npres;
+    out[0] = loss;
+  }
+}
+
+// ---- backward ----------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(BT * BTY, 4)     // 4 CTAs per SM: 64 registers, no spill
+k_lov_bwd_tile(LovArgs a, const float2* __restrict__ ms, const float* __restrict__ ge, const float* __restrict__ fin,
+               const float* __restrict__ grad_out, float* __restrict__ dseg, int kc, int pitch) {
+  extern __shared__ float sm[];
+  float* G = sm;                                   // [kc][BTY][BT]
+  float* Hx = G + (size_t)kc * BTY * BT;           // [kc][BTY][SRC_MAX]
+  float* S = Hx + (size_t)kc * BTY * SRC_MAX;      // [kc][pitch] source patch
+  __shared__ int s_y0[BTY], s_y1[BTY], s_x0[BT], s_x1[BT];
+  __shared__ float s_ly[BTY], s_lx[BT];
+  __shared__ float s_wx[SRC_MAX * (BT + 1)], s_wy[SRC_MAX * (BTY + 1)];
+  __shared__ short s_xlo[SRC_MAX], s_xhi[SRC_MAX], s_ylo[SRC_MAX], s_yhi[SRC_MAX];
+  const int tx = threadIdx.x & (BT - 1), ty = threadIdx.x >> 5;
+  const int b = blockIdx.z;
+  const int X0 = blockIdx.x * BT, Y0 = blockIdx.y * BTY;
+  const int x = X0 + tx, y = Y0 + ty;
+  const int64_t hw = (int64_t)a.h * a.w;
+  const UpTile g = up_tile_coords(X0, Y0, a.H, a.W, a.h, a.w, a.ry, a.rx, s_y0, s_y1, s_ly, s_x0, s_x1, s_lx);
+  const LovPix px = lov_pix(g, tx, ty, s_y0, s_y1, s_ly, s_x0, s_x1, s_lx);
+  const int64_t q = ((int64_t)b * a.H + y) * a.W + x;
+  const float npres = fin[1];
+  const float scale = npres > 0.f ? (grad_out ? grad_out[0] : 1.f) / npres : 0.f;
+  int t = -1;
+  float m = 0.f, se = 1.f;
+  if (x < a.W && y < a.H) {
+    t = lov_label(a, q);
+    const float2 v = ms[q];
+    m = v.x; se = v.y;
+  }
+  up_tile_tables(g, a.ry, a.rx, s_y0, s_y1, s_ly, s_x0, s_x1, s_lx, s_wx, s_wy, s_xlo, s_xhi, s_ylo, s_yhi);
+  const bool one = a.K <= kc;
+  float dot = 0.f;                                 // <p, dp>
+  if (!one) {                                      // several chunks: <p, dp> first
+    for (int c0 = 0; c0 < a.K; c0 += kc) {
+      const int cn = min(kc, a.K - c0);
+      __syncthreads();
+      lov_stage(a, g, b, c0, cn, pitch, S);
+      __syncthreads();
+      if (t >= 0) {
+        for (int cc = 0; cc < cn; ++cc) {
+          const int c = c0 + cc;
+          const float p = __expf(lov_logit(px, S + cc * pitch) - m) / se;
+          const float f = t == c ? 1.f : 0.f;
+          const float dp = p > f ? ge[(int64_t)c * a.N + q] : (p < f ? -ge[(int64_t)c * a.N + q] : 0.f);
+          dot += p * dp;
+        }
+      }
+    }
+  }
+  __syncthreads();
+  for (int c0 = 0; c0 < a.K; c0 += kc) {
+    const int cn = min(kc, a.K - c0);
+    lov_stage(a, g, b, c0, cn, pitch, S);
+    __syncthreads();
+    for (int cc = 0; cc < cn; ++cc) {              // dp (and <p, dp> when one chunk holds every class)
+      float dp = 0.f;
+      if (t >= 0) {
+        const int c = c0 + cc;
+        const float p = __expf(lov_logit(px, S + cc * pitch) - m) / se;
+        const float f = t == c ? 1.f : 0.f;
+        dp = p > f ? ge[(int64_t)c * a.N + q] : (p < f ? -ge[(int64_t)c * a.N + q] : 0.f);
+        if (one) dot += p * dp;
+      }
+      G[((size_t)cc * BTY + ty) * BT + tx] = dp;
+    }
+    for (int cc = 0; cc < cn; ++cc) {              // dz = scale * p (dp - <p, dp>)
+      float gv = 0.f;
+      if (t >= 0) {
+        const float p = __expf(lov_logit(px, S + cc * pitch) - m) / se;
+        gv = scale * p * (G[((size_t)cc * BTY + ty) * BT + tx] - dot);
+      }
+      G[((size_t)cc * BTY + ty) * BT + tx] = gv;
+    }
+    __syncthreads();
+    up_tile_flush(g, cn, G, Hx, s_wx, s_wy, s_xlo, s_xhi, s_ylo, s_yhi, dseg + ((int64_t)b * a.K + c0) * hw, hw, a.w);
+    __syncthreads();
+  }
+}
+
+}  // namespace pcl
+
+using namespace pcl;
+
+namespace {
+
+struct LovLayout {
+  size_t keys, vals, keys2, vals2, ge, ms, lab, hist, tilefg, gts, part, fin, total;
+  int ntiles, cc;
+};
+
+size_t lov_align(size_t x) { return (x + 255) & ~(size_t)255; }
+
+// Refuses (PCL_ERR_UNSUPPORTED) a label grid smaller than the logits, more than 256 classes and N >= 2^31.
+int lov_geometry(int B, int K, int h, int w, int H, int W, LovArgs* a) {
+  if (B <= 0 || K <= 0 || h <= 0 || w <= 0 || H <= 0 || W <= 0) return PCL_ERR_ARG;
+  if (H < h || W < w || K > 256) return PCL_ERR_UNSUPPORTED;
+  const int64_t N = (int64_t)B * H * W;
+  if (N >= ((int64_t)1 << 31)) return PCL_ERR_UNSUPPORTED;
+  a->B = B; a->K = K; a->h = h; a->w = w; a->H = H; a->W = W; a->N = N;
+  a->ry = H > 1 ? (float)(h - 1) / (float)(H - 1) : 0.f;
+  a->rx = W > 1 ? (float)(w - 1) / (float)(W - 1) : 0.f;
+  return PCL_OK;
+}
+
+// Classes sorted together: a quarter of them (rounded up), so the sort's three extra key / payload buffers stay at
+// about 3/4 of the keys buffer.
+LovLayout lov_layout(const LovArgs& a) {
+  LovLayout l;
+  l.ntiles = (int)ceil_div64(a.N, LOV_TILE);
+  l.cc = (a.K + 3) / 4;
+  const size_t kn = (size_t)a.K * a.N, cn = (size_t)l.cc * a.N;
+  size_t o = 0;
+  l.keys = o;   o = lov_align(o + kn * 4);
+  l.ge = o;     o = lov_align(o + kn * 4);
+  l.vals = o;   o = lov_align(o + cn * 4);
+  l.keys2 = o;  o = lov_align(o + cn * 4);
+  l.vals2 = o;  o = lov_align(o + cn * 4);
+  l.ms = o;     o = lov_align(o + (size_t)a.N * 8);
+  l.lab = o;    o = lov_align(o + (size_t)a.N);
+  l.hist = o;   o = lov_align(o + (size_t)l.cc * LOV_RADIX * l.ntiles * 4);
+  l.tilefg = o; o = lov_align(o + (size_t)a.K * l.ntiles * 4);
+  l.gts = o;    o = lov_align(o + (size_t)a.K * 4);
+  l.part = o;   o = lov_align(o + (size_t)a.K * l.ntiles * 8);
+  l.fin = o;    o = lov_align(o + 4 * sizeof(float));
+  l.total = o;
+  return l;
+}
+
+int lov_make(const float* seg, const int64_t* target, int B, int K, int h, int w, int H, int W, int ignore_index,
+             LovArgs* a) {
+  if (!seg || !target) return PCL_ERR_ARG;
+  const int st = lov_geometry(B, K, h, w, H, W, a);
+  if (st != PCL_OK) return st;
+  a->seg = seg; a->target = target; a->ignore_index = ignore_index;
+  return PCL_OK;
+}
+
+}  // namespace
+
+extern "C" int64_t pcl_lovasz_scratch_bytes(int32_t B, int32_t K, int32_t h, int32_t w, int32_t Himg, int32_t Wimg) {
+  LovArgs a;
+  const int st = lov_geometry(B, K, h, w, Himg, Wimg, &a);
+  if (st != PCL_OK) return st;
+  return (int64_t)lov_layout(a).total;
+}
+
+extern "C" int pcl_lovasz_fwd(const float* seg, const int64_t* target, int32_t B, int32_t K, int32_t h, int32_t w,
+                              int32_t Himg, int32_t Wimg, int32_t ignore_index, void* scratch, float* loss, void* stream) {
+  LovArgs a;
+  const int st = lov_make(seg, target, B, K, h, w, Himg, Wimg, ignore_index, &a);
+  if (st != PCL_OK) return st;
+  PCL_REQUIRE(scratch && loss);
+  cudaStream_t s = (cudaStream_t)stream;
+  const LovLayout l = lov_layout(a);
+  char* sc = (char*)scratch;
+  uint32_t* keys = (uint32_t*)(sc + l.keys);
+  uint32_t* vals = (uint32_t*)(sc + l.vals);
+  uint32_t* keys2 = (uint32_t*)(sc + l.keys2);
+  uint32_t* vals2 = (uint32_t*)(sc + l.vals2);
+  const uint8_t* lab = (const uint8_t*)(sc + l.lab);
+  int* hist = (int*)(sc + l.hist);
+  int* tilefg = (int*)(sc + l.tilefg);
+  int* gts = (int*)(sc + l.gts);
+  const int pitch = up_patch_pitch(h, w, a.ry, a.rx);
+  int kc = K < LOV_KC ? K : LOV_KC;
+  while (kc > 1 && (size_t)kc * pitch * sizeof(float) > 96 * 1024) --kc;
+  const size_t smem = (size_t)kc * pitch * sizeof(float);
+  if (smem > 200 * 1024) return PCL_ERR_UNSUPPORTED;
+  PCL_SMEM_OPT_IN(k_lov_keys, 200 * 1024);
+  k_lov_keys<<<dim3((unsigned)ceil_div(Wimg, BT), (unsigned)ceil_div(Himg, BTY), B), BT * BTY, smem, s>>>(
+      a, keys, (float2*)(sc + l.ms), (uint8_t*)(sc + l.lab), pitch, kc);
+  PCL_LAUNCH_CHECK();
+  const int nt = l.ntiles;
+  for (int c0 = 0; c0 < K; c0 += l.cc) {
+    const int cn = min(l.cc, K - c0);
+    uint32_t* kA = keys + (int64_t)c0 * a.N;
+    const dim3 grid((unsigned)nt, (unsigned)cn);
+    for (int p = 0; p < LOV_PASSES; ++p) {               // A -> B -> A -> B -> A
+      const uint32_t* kin = p & 1 ? keys2 : kA;
+      const uint32_t* vin = p == 0 ? nullptr : (p & 1 ? vals2 : vals);
+      uint32_t* kout = p & 1 ? kA : keys2;
+      uint32_t* vout = p & 1 ? vals : vals2;
+      k_lov_hist<<<grid, LOV_THREADS, 0, s>>>(kin, a.N, 8 * p, nt, hist);
+      PCL_LAUNCH_CHECK();
+      k_lov_scan<<<cn, 1024, 0, s>>>(hist, (int64_t)LOV_RADIX * nt, (int64_t)LOV_RADIX * nt, nullptr);
+      PCL_LAUNCH_CHECK();
+      k_lov_scatter<<<grid, LOV_THREADS, 0, s>>>(kin, vin, a.N, 8 * p, nt, hist, kout, vout);
+      PCL_LAUNCH_CHECK();
+    }
+    k_lov_fgcount<<<grid, LOV_THREADS, 0, s>>>(kA, vals, lab, a.N, c0, nt, tilefg);
+    PCL_LAUNCH_CHECK();
+    k_lov_scan<<<cn, 1024, 0, s>>>(tilefg + (int64_t)c0 * nt, nt, nt, gts + c0);
+    PCL_LAUNCH_CHECK();
+    k_lov_loss<<<grid, LOV_THREADS, 0, s>>>(kA, vals, lab, a.N, c0, nt, tilefg, gts, (float*)(sc + l.ge),
+                                            (double*)(sc + l.part));
+    PCL_LAUNCH_CHECK();
+  }
+  k_lov_finalize<<<1, 256, 0, s>>>((const double*)(sc + l.part), gts, K, nt, (float*)(sc + l.fin), loss);
+  PCL_LAUNCH_CHECK();
+  return PCL_OK;
+}
+
+extern "C" int pcl_lovasz_bwd(const float* seg, const int64_t* target, int32_t B, int32_t K, int32_t h, int32_t w,
+                              int32_t Himg, int32_t Wimg, int32_t ignore_index, void* scratch, const float* grad_loss,
+                              float* dseg, void* stream) {
+  LovArgs a;
+  const int st = lov_make(seg, target, B, K, h, w, Himg, Wimg, ignore_index, &a);
+  if (st != PCL_OK) return st;
+  PCL_REQUIRE(scratch && dseg);
+  cudaStream_t s = (cudaStream_t)stream;
+  const LovLayout l = lov_layout(a);
+  const char* sc = (const char*)scratch;
+  PCL_CUDA(cudaMemsetAsync(dseg, 0, (size_t)B * K * h * w * sizeof(float), s));
+  const int pitch = up_patch_pitch(h, w, a.ry, a.rx);
+  int kc = K < LOV_KC_BWD ? K : LOV_KC_BWD;
+  while (kc > 1 && (size_t)kc * (BTY * BT + BTY * SRC_MAX + pitch) * sizeof(float) > 200 * 1024) --kc;
+  const size_t smem = (size_t)kc * (BTY * BT + BTY * SRC_MAX + pitch) * sizeof(float);
+  if (smem > 200 * 1024) return PCL_ERR_UNSUPPORTED;
+  PCL_SMEM_OPT_IN(k_lov_bwd_tile, 200 * 1024);
+  k_lov_bwd_tile<<<dim3((unsigned)ceil_div(Wimg, BT), (unsigned)ceil_div(Himg, BTY), B), BT * BTY, smem, s>>>(
+      a, (const float2*)(sc + l.ms), (const float*)(sc + l.ge), (const float*)(sc + l.fin), grad_loss, dseg, kc, pitch);
   PCL_LAUNCH_CHECK();
   return PCL_OK;
 }

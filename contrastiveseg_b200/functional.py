@@ -1085,3 +1085,63 @@ def upsample_rmi_loss(seg: torch.Tensor, target: torch.Tensor, *, num_classes: i
     params = (int(radius), int(pool_way), int(pool_stride), float(weight_lambda), 1 if lambda_way else 0,
               float(loss_weight))
     return _RmiFn.apply(seg, target, params)
+
+
+# ------------------------------------------------------------------------------------------------
+# §8f row f6: fused bilinear up-sampling (align_corners=True) + Lovasz-softmax, only present classes
+# (lib/loss/lovasz_loss.py:216-267 via FSCELOVASZLoss, lib/loss/loss_helper.py:77-124)
+# ------------------------------------------------------------------------------------------------
+class _LovaszFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, seg, target, ignore_index):
+        lib = _abi.load()
+        _require_cuda(seg, "seg")
+        dev = seg.device
+        seg_c = seg if (seg.dtype == torch.float32 and seg.is_contiguous()) else seg.to(torch.float32).contiguous()
+        tgt = target
+        if tgt.device != dev or tgt.dtype != torch.int64 or not tgt.is_contiguous():
+            tgt = tgt.to(device=dev, dtype=torch.int64).contiguous()
+        B, K, h, w = seg_c.shape
+        H, W = tgt.shape[1], tgt.shape[2]
+        n = lib.pcl_lovasz_scratch_bytes(B, K, h, w, H, W)
+        if n < 0:
+            _abi.check(n, "pcl_lovasz_scratch_bytes")
+        scratch = torch.empty(n, dtype=torch.uint8, device=dev)
+        out = torch.empty((), dtype=torch.float32, device=dev)
+        with _on_device(dev):
+            _abi.check(lib.pcl_lovasz_fwd(seg_c.data_ptr(), tgt.data_ptr(), B, K, h, w, H, W, int(ignore_index),
+                                          scratch.data_ptr(), out.data_ptr(), _stream_ptr(dev)), "pcl_lovasz_fwd")
+        ctx.keep = (seg_c, tgt, scratch)
+        ctx.dims = (B, K, h, w, H, W, int(ignore_index))
+        ctx.seg_dtype = seg.dtype
+        return out
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out):
+        lib = _abi.load()
+        seg_c, tgt, scratch = ctx.keep
+        dev = seg_c.device
+        go = grad_out
+        if go.device != dev or go.dtype != torch.float32 or not go.is_contiguous():
+            go = go.detach().to(device=dev, dtype=torch.float32).contiguous()
+        dseg = torch.empty_like(seg_c)
+        with _on_device(dev):
+            _abi.check(lib.pcl_lovasz_bwd(seg_c.data_ptr(), tgt.data_ptr(), *ctx.dims, scratch.data_ptr(),
+                                          go.data_ptr(), dseg.data_ptr(), _stream_ptr(dev)), "pcl_lovasz_bwd")
+        ctx.keep = None
+        return dseg.to(ctx.seg_dtype), None, None
+
+
+def upsample_lovasz_softmax(seg: torch.Tensor, target: torch.Tensor, ignore_index: int = -1) -> torch.Tensor:
+    """Lovasz-softmax loss of bilinearly (align_corners=True) up-sampled logits against a full-resolution label map,
+    fused: == lovasz_softmax_flat(*flatten_probas(softmax(F.interpolate(seg, target.shape[1:], mode='bilinear',
+    align_corners=True), 1), target, ignore_index), only_present=True) without the (B,K,Himg,Wimg) intermediates or a
+    host sync.  Pixels are pooled over the batch; labels outside [0, K) count as ignored; every pixel ignored gives 0
+    with a zero gradient.  Equal errors are ordered by ascending pixel index (a stable sort), which fixes the per-pixel
+    gradient where the reference leaves it unspecified.  seg fp32, bf16 or fp16 (read as fp32); the gradient comes back
+    in seg's dtype; ``target`` is not modified.  A label grid smaller than seg, more than 256 classes or 2^31 label
+    pixels raise PclError."""
+    if seg.dim() != 4 or target.dim() != 3 or seg.shape[0] != target.shape[0]:
+        raise ValueError(f"seg (B,K,h,w) and target (B,H,W) expected, got {tuple(seg.shape)} and {tuple(target.shape)}")
+    return _LovaszFn.apply(seg, target, ignore_index)

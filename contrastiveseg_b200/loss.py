@@ -3,9 +3,11 @@ as the reference (lib/loss/loss_contrast.py, lib/loss/loss_contrast_mem.py, lib/
 
 The contrast term runs on the H100 engine (functional.pixel_contrast_loss); the plain segmentation CE runs on
 the fused up-sample + CE kernels (``contrast.fused_seg_ce``, default on), and with ``contrast.use_rmi`` the RMI seg
-loss runs on the fused up-sample + RMI kernels (same switch: off, F.interpolate runs first).  Engine-only knobs are read from
-optional config keys under ``contrast``: ``rng`` ("device" | "torch_cpu"), ``nan_safe``, ``precision``
-("fp32" | "bf16"), ``skip_warmup_contrast``, ``topk_negatives`` (a10 extension, default off).
+loss runs on the fused up-sample + RMI kernels (same switch: off, F.interpolate runs first); a
+``seg_criterion=FSCELOVASZLoss(configer)`` runs its Lovasz term on the fused up-sample + Lovasz kernels (same
+switch).  Engine-only knobs are read from optional config keys under ``contrast``: ``rng`` ("device" |
+"torch_cpu"), ``nan_safe``, ``precision`` ("fp32" | "bf16"), ``skip_warmup_contrast``, ``topk_negatives`` (a10
+extension, default off).
 """
 from __future__ import annotations
 
@@ -15,8 +17,8 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from .functional import ContrastOptions, pixel_contrast_loss, upsample_cross_entropy
-from .loss_helper import FSAuxCELoss, FSAuxRMILoss, FSCELoss, FSRMILoss
+from .functional import ContrastOptions, pixel_contrast_loss, upsample_cross_entropy, upsample_lovasz_softmax
+from .loss_helper import FSAuxCELoss, FSAuxRMILoss, FSCELOVASZLoss, FSCELoss, FSRMILoss
 
 
 def _opt(configer, key, default):
@@ -106,8 +108,8 @@ class ContrastCELoss(nn.Module):
             if self.use_rmi:
                 seg_criterion = self._rmi_seg_criterion(configer)
             elif self.use_lovasz:
-                raise NotImplementedError("the Lovasz seg loss (contrast.use_lovasz) is not implemented; pass the "
-                                          "reference module via seg_criterion=")
+                raise NotImplementedError("contrast.use_lovasz does not build the Lovasz seg loss by itself; pass "
+                                          "seg_criterion=cs.FSCELOVASZLoss(configer) to run it on the engine")
             else:
                 seg_criterion = self._default_seg_criterion(configer)
         self.seg_criterion = seg_criterion
@@ -122,7 +124,7 @@ class ContrastCELoss(nn.Module):
         return upsample_cross_entropy(seg, target, ce.weight, ce.ignore_index)
 
     def _can_fuse(self, ce_module, seg):
-        return (self.fused_seg_ce and isinstance(ce_module, FSCELoss) and seg.is_cuda and
+        return (self.fused_seg_ce and isinstance(ce_module, (FSCELoss, FSCELOVASZLoss)) and seg.is_cuda and
                 ce_module.ce_loss.reduction == "mean" and getattr(ce_module.ce_loss, "label_smoothing", 0.0) == 0.0)
 
     @staticmethod
@@ -146,11 +148,25 @@ class ContrastCELoss(nn.Module):
     def _seg_loss(self, preds, target):
         if isinstance(self.seg_criterion, FSRMILoss):
             return self.seg_criterion(self._rmi_input(preds["seg"], target), target)
+        if isinstance(self.seg_criterion, FSCELOVASZLoss):
+            return self._lovasz_seg_loss(preds["seg"], target, self.seg_criterion)
         if self._can_fuse(self.seg_criterion, preds["seg"]):
             return self._fused_ce(preds["seg"], target, self.seg_criterion)
         h, w = target.size(1), target.size(2)
         pred = F.interpolate(input=preds["seg"], size=(h, w), mode="bilinear", align_corners=True)
         return self.seg_criterion(pred, target)
+
+    def _lovasz_seg_loss(self, seg, target, crit):
+        """CE + Lovasz of FSCELOVASZLoss on the up-sampled logits: the CE on the fused seg CE kernels when it can run
+        there, the Lovasz term on the fused up-sample + Lovasz kernels (F.interpolate first with fused_seg_ce off)."""
+        h, w = target.size(1), target.size(2)
+        up = None
+        if self._can_fuse(crit, seg):
+            ce = self._fused_ce(seg, target, crit)
+        else:
+            up = F.interpolate(input=seg, size=(h, w), mode="bilinear", align_corners=True)
+            ce = crit.ce_loss(up, target)
+        return ce + upsample_lovasz_softmax(seg if up is None else up, target, crit.ignore_index)
 
     def _queues(self, preds):
         return None

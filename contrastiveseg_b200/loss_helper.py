@@ -2,8 +2,8 @@
 
 The CE modules are plain PyTorch ops so the wrappers are drop-in (the wrappers run the fused up-sample + CE kernels
 instead when they can, SURVEY §8f row 1).  The RMI modules (contrast.use_rmi) run the fused RMI kernels
-(functional.upsample_rmi_loss, §8f row f5).  The Lovasz variant (contrast.use_lovasz) is not re-implemented: pass the
-reference's own module through ``seg_criterion=`` if needed.
+(functional.upsample_rmi_loss, §8f row f5).  FSCELOVASZLoss adds the Lovasz-softmax term of the fused up-sample +
+Lovasz kernels (functional.upsample_lovasz_softmax, §8f row f6) to the CE.
 """
 from __future__ import annotations
 
@@ -11,7 +11,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from .functional import upsample_rmi_loss
+from .functional import upsample_lovasz_softmax, upsample_rmi_loss
 
 
 def _ce_params(configer):
@@ -118,3 +118,31 @@ class FSAuxRMILoss(nn.Module):
         aux_out, seg_out = inputs
         w = self.configer.get("network", "loss_weights")
         return w["seg_loss"] * self.rmi_loss(seg_out, targets) + w["aux_loss"] * self.ce_loss(aux_out, targets)
+
+
+class FSCELOVASZLoss(nn.Module):
+    """CE + Lovasz-softmax  (lib/loss/loss_helper.py:77-124).  Reads ce_weight, ce_reduction and ce_ignore_index.  A
+    single tensor gives CE + Lovasz at the input's resolution (the target nearest-scaled to it); a list or tuple gives
+    the weighted CE sum of the reference's list branch, without the Lovasz term.  The Lovasz term runs on the engine
+    (upsample_lovasz_softmax with the identity geometry); the contrast wrappers hand it the low-resolution logits
+    instead, with the up-sampling fused."""
+
+    def __init__(self, configer=None):
+        super().__init__()
+        self.configer = configer
+        weight, reduction, ignore_index = _ce_params(configer)
+        self.ignore_index = ignore_index
+        self.ce_loss = nn.CrossEntropyLoss(weight=weight, ignore_index=ignore_index, reduction=reduction)
+
+    def forward(self, inputs, *targets, weights=None, **kwargs):
+        if isinstance(inputs, dict) and "seg" in inputs:
+            inputs = inputs["seg"]
+        if isinstance(inputs, (tuple, list)):
+            weights = weights or [1.0] * len(inputs)
+            loss = 0.0
+            for i, x in enumerate(inputs):
+                tgt = targets[i] if len(targets) > 1 else targets[0]
+                loss = loss + weights[i] * self.ce_loss(x, _scale_target(tgt, (x.size(2), x.size(3))))
+            return loss
+        target = _scale_target(targets[0], (inputs.size(2), inputs.size(3)))
+        return self.ce_loss(inputs, target) + upsample_lovasz_softmax(inputs, target, self.ignore_index)

@@ -319,6 +319,27 @@ int pcl_rmi_bwd(const float* seg, const int64_t* target, int32_t B, int32_t K, i
                 int32_t lambda_way, float loss_weight, void* scratch, const float* grad_loss, float* dseg, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * §8f row f6: the Lovasz-softmax term of FSCELOVASZLoss (lib/loss/loss_helper.py:77-124, selected by
+ * contrast.use_lovasz in lib/loss/loss_contrast_mem.py:187-194), fused.  Replaces F.interpolate(seg, (Himg,Wimg),
+ * bilinear, align_corners=True) + softmax + lovasz_softmax_flat(*flatten_probas(...), only_present=True)
+ * (lib/loss/lovasz_loss.py:216-267) and its autograd backward; the (B,K,Himg,Wimg) logits and probabilities are never
+ * materialised and no call syncs with the host (capturable).
+ *   seg (B,K,h,w) fp32 with Himg >= h, Wimg >= w; target (B,Himg,Wimg) int64 (read only).  A pixel counts when its label
+ *   is not ignore_index and lies in [0, K); the others are ignored (the reference's CE raises on them).  Pixels are
+ *   pooled over the whole batch; the loss is the mean over the classes present among them, 0 (zero gradient) when none.
+ *   Equal errors are ordered by ascending pixel index (b*Himg + y)*Wimg + x, i.e. a stable descending sort; the loss
+ *   does not depend on that order, the per-pixel gradient does.  p exactly 0 or 1 gets a zero gradient (abs').
+ *   A label grid smaller than seg, K > 256 or B*Himg*Wimg >= 2^31 return PCL_ERR_UNSUPPORTED.
+ *   scratch: pcl_lovasz_scratch_bytes (host only; a negative PCL_ERR_* for a refused request).  pcl_lovasz_bwd reads the
+ *   scratch its pcl_lovasz_fwd wrote.  The loss is bit-reproducible; dseg to the last ulp or two (fp32 atomics).
+ * ----------------------------------------------------------------------------------------------*/
+int64_t pcl_lovasz_scratch_bytes(int32_t B, int32_t K, int32_t h, int32_t w, int32_t Himg, int32_t Wimg);
+int pcl_lovasz_fwd(const float* seg, const int64_t* target, int32_t B, int32_t K, int32_t h, int32_t w, int32_t Himg,
+                   int32_t Wimg, int32_t ignore_index, void* scratch, float* loss, void* stream);
+int pcl_lovasz_bwd(const float* seg, const int64_t* target, int32_t B, int32_t K, int32_t h, int32_t w, int32_t Himg,
+                   int32_t Wimg, int32_t ignore_index, void* scratch, const float* grad_loss, float* dseg, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * a7 + a8: memory bank.  Replaces segmentor/trainer_contrastive.py:102-138 (_dequeue_and_enqueue).
  * Step 1 (parallel): build this rank's enqueue packet.  Step 2 (ordered): apply the packets of all
  * ranks in rank order — world 1 reproduces the reference exactly, world > 1 is the allgather merge
