@@ -10,10 +10,12 @@ from .functional import ContrastOptions, l2_normalize, pixel_contrast_loss, proj
 from .functional import bn_relu_project_normalize                     # noqa: F401
 from .functional import upsample_rmi_loss                             # noqa: F401
 from .functional import upsample_lovasz_softmax                       # noqa: F401
+from .functional import upsample_ohem_cross_entropy                   # noqa: F401
 from .functional import conv_bn_relu_project_normalize                # noqa: F401
 from .loss import (ContrastAuxCELoss, ContrastCELoss, MemContrastCELoss, PixelContrastLoss, SEG_LOSS_DICT,  # noqa: F401
                    get_seg_loss)
 from .loss_helper import FSCELOVASZLoss                               # noqa: F401
+from .loss_helper import FSAuxOhemCELoss, FSOhemCELoss                # noqa: F401
 from .bank import MemoryBank, dequeue_and_enqueue, gather_packets      # noqa: F401
 from .projection import ProjectionHead                                  # noqa: F401
 from .trainer_hook import ContrastTrainerHook, LossStepTimer            # noqa: F401

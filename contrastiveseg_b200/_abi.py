@@ -129,6 +129,9 @@ SIGNATURES = {
     "pcl_lovasz_scratch_bytes": (c_i64, [c_i32] * 6),
     "pcl_lovasz_fwd": (c_i32, [c_vp, c_vp] + [c_i32] * 7 + [c_vp, c_vp, c_vp]),
     "pcl_lovasz_bwd": (c_i32, [c_vp, c_vp] + [c_i32] * 7 + [c_vp, c_vp, c_vp, c_vp]),
+    "pcl_ohem_ce_scratch_bytes": (c_i64, [c_i32] * 6),
+    "pcl_ohem_ce_fwd": (c_i32, [c_vp, c_vp, c_vp] + [c_i32] * 7 + [c_f32, c_i64, c_i32, c_vp, c_vp, c_vp]),
+    "pcl_ohem_ce_bwd": (c_i32, [c_vp, c_vp, c_vp] + [c_i32] * 7 + [c_vp, c_vp, c_vp, c_vp]),
     "pcl_bank_packet_floats": (c_i64, [C.POINTER(BankGeom)]),
     "pcl_bank_scratch_floats": (c_i64, [C.POINTER(BankGeom)]),
     "pcl_bank_packet": (c_i32, [C.POINTER(BankGeom), c_vp, c_vp, c_vp, c_u64, c_vp, c_vp, c_vp]),

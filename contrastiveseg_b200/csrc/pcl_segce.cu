@@ -1,6 +1,7 @@
 // Fused segmentation losses of the contrast wrappers: the plain CE (first part of this file), the RMI loss of
-// contrast.use_rmi (second part) and the Lovasz-softmax term of FSCELOVASZLoss (third part).  All up-sample the logits
-// bilinearly inside the kernels and share the tile geometry and transposed bilinear map of pcl_upsample.cuh.
+// contrast.use_rmi (second part), the Lovasz-softmax term of FSCELOVASZLoss (third part) and the OHEM cross-entropy of
+// FSOhemCELoss (fourth part, which runs the first part's tile kernels with their OHEM flag set).  All up-sample the
+// logits bilinearly inside the kernels and share the tile geometry and transposed bilinear map of pcl_upsample.cuh.
 //
 // Fused segmentation cross-entropy of ContrastCELoss.forward (SURVEY §8f row 1, the next row after the contrast path):
 // replaces  F.interpolate(seg, (Himg,Wimg), bilinear, align_corners=True)  +  nn.CrossEntropyLoss(weight, ignore_index,
@@ -30,11 +31,21 @@ struct SegCeArgs {
 constexpr int CE_THREADS = 256;
 constexpr int KC_FWD_MAX = 32;         // classes staged per pass in the forward (one pass for K <= 32: one exposed load latency)
 
+// Per-pixel outputs of the OHEM forward (OHEM = true, fourth part of this file); the plain CE leaves them unused.
+struct OhemPix {
+  float* p;                     // p_t = softmax of the target class; NaN at a pixel that does not count
+  float* wnll;                  // w_t * nll
+  int* counts;                  // {counted pixels n, pixels with p_t < thresh}
+  float thresh;                 // fp32(thresh)
+};
+
 // Forward, tile formulation: the <= (32*ry+2) x (32*rx+2) source logits of the tile are staged in shared memory per class
-// chunk; every thread (one label pixel) runs an online log-sum-exp over the classes from shared memory.
+// chunk; every thread (one label pixel) runs an online log-sum-exp over the classes from shared memory.  With OHEM the
+// per-CTA partial sums give way to the per-pixel p_t and w_t * nll, and the two counts go to integer atomics.
+template <bool OHEM>
 __global__ void __launch_bounds__(BT * BTY)
 k_segce_fwd(SegCeArgs a, float* __restrict__ lse_out, float* __restrict__ part_nll, float* __restrict__ part_w, int pitch,
-            int kc) {
+            int kc, OhemPix o) {
   extern __shared__ float sm[];                    // [kc][pitch] source patch
   __shared__ float s_n[BT * BTY / 32], s_w[BT * BTY / 32];
   __shared__ int s_y0[BTY], s_y1[BTY], s_x0[BT], s_x1[BT];
@@ -81,6 +92,15 @@ k_segce_fwd(SegCeArgs a, float* __restrict__ lse_out, float* __restrict__ part_n
       nll = wc * (lse - vt);
       wt = wc;
     }
+    if constexpr (OHEM) {
+      const int64_t q = (int64_t)b * HWo + (int64_t)y * a.W + x;
+      const bool counted = t != (int64_t)a.ignore_index && t >= 0 && t < a.K;
+      const float p = counted ? __expf(vt - m) / se : CUDART_NAN_F;
+      o.p[q] = p;
+      o.wnll[q] = nll;
+      nll = counted ? 1.f : 0.f;                   // the two counts take the partial sums' place (exact in fp32)
+      wt = p < o.thresh ? 1.f : 0.f;
+    }
   }
   nll = warp_sum(nll); wt = warp_sum(wt);
   if ((threadIdx.x & 31) == 0) { s_n[threadIdx.x >> 5] = nll; s_w[threadIdx.x >> 5] = wt; }
@@ -88,9 +108,13 @@ k_segce_fwd(SegCeArgs a, float* __restrict__ lse_out, float* __restrict__ part_n
   if (threadIdx.x == 0) {
     float an = 0.f, aw = 0.f;
     for (int i = 0; i < BT * BTY / 32; ++i) { an += s_n[i]; aw += s_w[i]; }      // fixed order
-    const int64_t blk = ((int64_t)blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
-    part_nll[blk] = an;
-    part_w[blk] = aw;
+    if constexpr (OHEM) {
+      if (an > 0.f) { atomicAdd(&o.counts[0], (int)an); atomicAdd(&o.counts[1], (int)aw); }
+    } else {
+      const int64_t blk = ((int64_t)blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
+      part_nll[blk] = an;
+      part_w[blk] = aw;
+    }
   }
 }
 
@@ -116,9 +140,13 @@ k_segce_finalize(const float* __restrict__ part_nll, const float* __restrict__ p
 //   B, C  the transposed bilinear map into dseg (up_tile_flush, pcl_upsample.cuh)
 // Each (pixel, class) softmax is evaluated once (the per-logit gather below needs 16x as many); B and C only visit the
 // label columns / rows inside the footprint of their source cell.
+// With OHEM, fin is the OHEM state (fin[1] the denominator, fin[2] the threshold) and only the pixels whose stored
+// p_t (ohem_p) lies below the threshold carry a gradient: the forward's selection, read back rather than recomputed.
+template <bool OHEM>
 __global__ void __launch_bounds__(BT * BTY, 5)     // 5 CTAs per SM: holds the kernel at 48 registers
 k_segce_bwd_tile(SegCeArgs a, const float* __restrict__ lse, const float* __restrict__ fin,
-                 const float* __restrict__ grad_out, float* __restrict__ dseg, int kc, int pitch) {
+                 const float* __restrict__ grad_out, float* __restrict__ dseg, int kc, int pitch,
+                 const float* __restrict__ ohem_p) {
   extern __shared__ float sm[];
   float* G = sm;                                   // [kc][BTY][BT]
   float* Hx = G + (size_t)kc * BTY * BT;           // [kc][BTY][SRC_MAX]
@@ -141,7 +169,8 @@ k_segce_bwd_tile(SegCeArgs a, const float* __restrict__ lse, const float* __rest
   float lse_p = 0.f, coef = 0.f;
   if (inside) {
     t = a.target[(int64_t)b * HWo + (int64_t)y * a.W + x];
-    if (t != (int64_t)a.ignore_index && t >= 0 && t < a.K) {
+    if (t != (int64_t)a.ignore_index && t >= 0 && t < a.K &&
+        (!OHEM || ohem_p[(int64_t)b * HWo + (int64_t)y * a.W + x] < fin[2])) {
       coef = scale * (a.weight ? a.weight[t] : 1.f);
       lse_p = lse[(int64_t)b * HWo + (int64_t)y * a.W + x];
     } else {
@@ -249,6 +278,38 @@ static int make_ce(const float* seg, const int64_t* target, const float* weight,
 
 static int patch_pitch(const SegCeArgs& a) { return up_patch_pitch(a.h, a.w, a.ry, a.rx); }
 
+template <bool OHEM>
+static int segce_fwd_launch(const SegCeArgs& a, float* lse, float* pn, float* pw, OhemPix o, cudaStream_t s) {
+  const int pitch = patch_pitch(a);
+  int kc = a.K < KC_FWD_MAX ? a.K : KC_FWD_MAX;
+  while (kc > 1 && (size_t)kc * pitch * sizeof(float) > 96 * 1024) --kc;
+  const size_t smem = (size_t)kc * pitch * sizeof(float);
+  if (smem > 200 * 1024) return PCL_ERR_UNSUPPORTED;
+  PCL_SMEM_OPT_IN(k_segce_fwd<OHEM>, 200 * 1024);
+  k_segce_fwd<OHEM><<<dim3((unsigned)ceil_div(a.W, BT), (unsigned)ceil_div(a.H, BTY), a.B), BT * BTY, smem, s>>>(
+      a, lse, pn, pw, pitch, kc, o);
+  PCL_LAUNCH_CHECK();
+  return PCL_OK;
+}
+
+// dseg is zeroed here; the tile kernel accumulates into it
+template <bool OHEM>
+static int segce_bwd_tile_launch(const SegCeArgs& a, const float* lse, const float* fin, const float* grad_loss,
+                                 float* dseg, const float* ohem_p, cudaStream_t s) {
+  PCL_CUDA(cudaMemsetAsync(dseg, 0, (size_t)a.B * a.K * a.h * a.w * sizeof(float), s));
+  // classes per pass: G (kc*32*32) + Hx (kc*32*34) + source patch (kc*pitch) floats, two CTAs per SM when possible
+  const int pitch = patch_pitch(a);
+  int kc = a.K < 24 ? a.K : 24;              // one pass for K <= 24 (fewer bulk-synchronous phases per CTA)
+  while (kc > 1 && (size_t)kc * (BTY * BT + BTY * SRC_MAX + pitch) * sizeof(float) > 200 * 1024) --kc;
+  const size_t smem = (size_t)kc * (BTY * BT + BTY * SRC_MAX + pitch) * sizeof(float);
+  if (smem > 200 * 1024) return PCL_ERR_UNSUPPORTED;
+  PCL_SMEM_OPT_IN(k_segce_bwd_tile<OHEM>, 200 * 1024);
+  k_segce_bwd_tile<OHEM><<<dim3((unsigned)ceil_div(a.W, BT), (unsigned)ceil_div(a.H, BTY), a.B), BT * BTY, smem, s>>>(
+      a, lse, fin, grad_loss, dseg, kc, pitch, ohem_p);
+  PCL_LAUNCH_CHECK();
+  return PCL_OK;
+}
+
 extern "C" int64_t pcl_seg_ce_scratch_floats(int32_t B, int32_t H, int32_t W) {
   const int64_t blocks = (int64_t)ceil_div(H, BTY) * ceil_div(W, BT) * B;
   return (int64_t)B * H * W + 2 * blocks + 2;            // lse | partial nll | partial weight | (loss, weight sum)
@@ -268,14 +329,8 @@ extern "C" int pcl_seg_ce_fwd(const float* seg, const int64_t* target, const flo
   float* pn = scratch + (int64_t)B * HWo;
   float* pw = pn + blocks;
   float* fin = pw + blocks;
-  const int pitch = patch_pitch(a);
-  int kc = K < KC_FWD_MAX ? K : KC_FWD_MAX;
-  while (kc > 1 && (size_t)kc * pitch * sizeof(float) > 96 * 1024) --kc;
-  const size_t smem = (size_t)kc * pitch * sizeof(float);
-  if (smem > 200 * 1024) return PCL_ERR_UNSUPPORTED;
-  PCL_SMEM_OPT_IN(k_segce_fwd, 200 * 1024);
-  k_segce_fwd<<<dim3((unsigned)ceil_div(W, BT), (unsigned)ceil_div(H, BTY), B), BT * BTY, smem, s>>>(a, lse, pn, pw, pitch, kc);
-  PCL_LAUNCH_CHECK();
+  st = segce_fwd_launch<false>(a, lse, pn, pw, OhemPix{}, s);
+  if (st != PCL_OK) return st;
   k_segce_finalize<<<1, 1024, 0, s>>>(pn, pw, blocks, fin);
   PCL_LAUNCH_CHECK();
   PCL_CUDA(cudaMemcpyAsync(loss, fin, sizeof(float), cudaMemcpyDeviceToDevice, s));
@@ -300,18 +355,7 @@ extern "C" int pcl_seg_ce_bwd(const float* seg, const int64_t* target, const flo
     PCL_LAUNCH_CHECK();
     return PCL_OK;
   }
-  PCL_CUDA(cudaMemsetAsync(dseg, 0, (size_t)B * K * hw * sizeof(float), s));
-  // classes per pass: G (kc*32*32) + Hx (kc*32*34) + source patch (kc*pitch) floats, two CTAs per SM when possible
-  const int pitch = patch_pitch(a);
-  int kc = K < 24 ? K : 24;                  // one pass for K <= 24 (fewer bulk-synchronous phases per CTA)
-  while (kc > 1 && (size_t)kc * (BTY * BT + BTY * SRC_MAX + pitch) * sizeof(float) > 200 * 1024) --kc;
-  const size_t smem = (size_t)kc * (BTY * BT + BTY * SRC_MAX + pitch) * sizeof(float);
-  if (smem > 200 * 1024) return PCL_ERR_UNSUPPORTED;
-  PCL_SMEM_OPT_IN(k_segce_bwd_tile, 200 * 1024);
-  k_segce_bwd_tile<<<dim3((unsigned)ceil_div(W, BT), (unsigned)ceil_div(H, BTY), B), BT * BTY, smem, s>>>(a, lse, fin, grad_loss,
-                                                                                                     dseg, kc, pitch);
-  PCL_LAUNCH_CHECK();
-  return PCL_OK;
+  return segce_bwd_tile_launch<false>(a, lse, fin, grad_loss, dseg, nullptr, s);
 }
 
 // ==================================================================================================================
@@ -1536,4 +1580,275 @@ extern "C" int pcl_lovasz_bwd(const float* seg, const int64_t* target, int32_t B
       a, (const float2*)(sc + l.ms), (const float*)(sc + l.ge), (const float*)(sc + l.fin), grad_loss, dseg, kc, pitch);
   PCL_LAUNCH_CHECK();
   return PCL_OK;
+}
+
+// ==================================================================================================================
+// Fused OHEM cross-entropy of the contrast wrappers (FSOhemCELoss, and the seg term of FSAuxOhemCELoss,
+// lib/loss/loss_helper.py:215-281): replaces
+//   F.interpolate(seg, (Himg,Wimg), bilinear, align_corners=True) + softmax + gather of the target probability + sort of
+//   the labelled pixels' p_t + nn.CrossEntropyLoss(weight, reduction='none') + the selection p_t < threshold
+// and its autograd backward, without materialising the (B,K,Himg,Wimg) logits or probabilities and without a host sync.
+// m = min(min_kept, n - 1) over the n counted pixels; threshold = max(kth, fp32(thresh)), kth the m-th smallest p_t
+// (0-based); the loss sums w_t * nll over the pixels with p_t < threshold (strict: a tie at the threshold is all out).
+//   k_segce_fwd<true>  the seg CE tile pass: per label pixel lse (kept for the backward), p_t and w_t * nll; integer
+//                      counts of n and of p_t < thresh
+//   k_ohem_decide      count(p_t < thresh) > m means kth < thresh: threshold = fp32(thresh), exact, and the select levels
+//                      below exit at once (the usual training case); n = 0 takes the same exit
+//   k_ohem_hist/scan   otherwise an exact radix select of the m-th smallest key over three levels of 11/11/10 bits of
+//                      the p_t bits (p_t >= 0: the raw fp32 bits sort in value order); per level an integer histogram of
+//                      the pixels matching the prefix so far, and a one-CTA scan that picks the digit holding rank m.
+//                      State on the device, integer atomics only: the result does not depend on scheduling.
+//   k_ohem_sum         per-CTA sums of w_t * nll (fp64) and counts over p_t < threshold, fixed tiles of OHEM_TILE pixels
+//   k_ohem_finalize    fixed-order fp64 sum of the partials: sum / count ('mean', NaN for an empty selection, as the
+//                      reference's mean of nothing) or the sum; 0 when no pixel counts.  Bit-reproducible.
+//   k_segce_bwd_tile<true>  the seg CE backward with coefficient grad * w_t / count ('mean') or grad * w_t ('sum') at
+//                      the pixels whose stored p_t < threshold, 0 elsewhere (dseg to the last ulp or two, fp32 atomics)
+// First-order HBM bytes at B=8, K=19, 128x256 -> 512x1024 (N = 4.19 M): the tile pass reads seg (19.9 MB) and the labels
+// (33.6 MB) and writes lse, p_t and w_t * nll (50.3 MB); each select level re-reads p_t (16.8 MB); the sum reads p_t and
+// w_t * nll (33.6 MB); the backward reads the labels, lse, p_t and seg and writes dseg (DESIGN §4).
+namespace pcl {
+
+constexpr int OHEM_BINS = 2048;                      // 11-bit digits (the last level uses 10 of them)
+constexpr int OHEM_THREADS = 256;
+constexpr int OHEM_ITEMS = 8;
+constexpr int OHEM_TILE = OHEM_THREADS * OHEM_ITEMS;  // pixels per k_ohem_sum CTA
+constexpr int OHEM_HIST_CTAS = 1024;
+
+// At byte 0 of the scratch (layout documented in pcl.h): the first four words are the finished forward's result.
+struct OhemState {
+  float loss, denom, threshold;   // loss; the backward's denominator (selected count for 'mean', 1 for 'sum'); threshold
+  int select;                     // 1 when the select levels ran (count(p_t < thresh) <= m)
+  int n, below, count, rank;      // counted pixels; p_t < thresh; selected pixels; rank still to find in the select
+  uint32_t prefix;                // key bits found so far
+};
+static_assert(sizeof(OhemState) <= 256, "p_t starts at byte 256 of the scratch (pcl.h)");
+
+__global__ void __launch_bounds__(32)
+k_ohem_decide(OhemState* __restrict__ st, int64_t min_kept, float thresh) {
+  if (threadIdx.x != 0) return;
+  const int64_t n = st->n;
+  const int64_t m = min(min_kept, n - 1);
+  const bool sel = n > 0 && (int64_t)st->below <= m;
+  st->select = sel ? 1 : 0;
+  st->rank = sel ? (int)m : 0;
+  st->prefix = 0u;
+  st->threshold = thresh;                          // the select overwrites it with max(kth, thresh)
+}
+
+// level 0: bits 31..21 of every counted key; level 1: bits 20..10 of the keys whose bits 31..21 equal the prefix;
+// level 2: bits 9..0 of the keys whose bits 31..10 equal the prefix
+__global__ void __launch_bounds__(OHEM_THREADS)
+k_ohem_hist(const float* __restrict__ p, int64_t N, int level, const OhemState* __restrict__ st, int* __restrict__ hist) {
+  __shared__ int s_h[OHEM_BINS];
+  if (!st->select) return;                         // uniform over the grid: the threshold decided
+  const uint32_t prefix = st->prefix;
+  const int shift = level == 0 ? 21 : (level == 1 ? 10 : 0);
+  const int hi = level == 1 ? 21 : 10;
+  const uint32_t mask = level == 2 ? 1023u : 2047u;
+  for (int i = threadIdx.x; i < OHEM_BINS; i += OHEM_THREADS) s_h[i] = 0;
+  __syncthreads();
+  for (int64_t i = (int64_t)blockIdx.x * OHEM_THREADS + threadIdx.x; i < N; i += (int64_t)gridDim.x * OHEM_THREADS) {
+    const float v = p[i];
+    if (v != v) continue;                          // NaN: the pixel does not count
+    const uint32_t key = __float_as_uint(v);
+    if (level == 0 || (key >> hi) == prefix) atomicAdd(&s_h[(key >> shift) & mask], 1);
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < OHEM_BINS; i += OHEM_THREADS)
+    if (s_h[i]) atomicAdd(&hist[level * OHEM_BINS + i], s_h[i]);
+}
+
+// One CTA: exclusive scan of the level's 2048 counts (two per thread); the thread whose bins hold rank r appends the
+// digit to the prefix and keeps the rank within it.  After level 2 the prefix is the key of the m-th smallest p_t.
+__global__ void __launch_bounds__(1024)
+k_ohem_scan(int level, float thresh, OhemState* __restrict__ st, const int* __restrict__ hist) {
+  __shared__ int s_w[32];
+  if (!st->select) return;
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const int a0 = hist[level * OHEM_BINS + 2 * threadIdx.x], a1 = hist[level * OHEM_BINS + 2 * threadIdx.x + 1];
+  const int s = a0 + a1;
+  int incl = s;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int u = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += u;
+  }
+  if (lane == 31) s_w[wid] = incl;
+  __syncthreads();
+  if (wid == 0) {
+    const int wv = s_w[lane];
+    int wi = wv;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int u = __shfl_up_sync(0xffffffffu, wi, o);
+      if (lane >= o) wi += u;
+    }
+    s_w[lane] = wi - wv;
+  }
+  __syncthreads();
+  const int excl = s_w[wid] + incl - s;
+  const int r = st->rank;
+  int d = -1, nr = 0;
+  if (r >= excl && r < excl + a0) { d = 2 * threadIdx.x; nr = r - excl; }
+  else if (r >= excl + a0 && r < excl + s) { d = 2 * threadIdx.x + 1; nr = r - excl - a0; }
+  __syncthreads();                                 // every thread has read the rank
+  if (d >= 0) {
+    const uint32_t prefix = (st->prefix << (level == 2 ? 10 : 11)) | (uint32_t)d;
+    st->prefix = prefix;
+    st->rank = nr;
+    if (level == 2) st->threshold = fmaxf(__uint_as_float(prefix), thresh);
+  }
+}
+
+__global__ void __launch_bounds__(OHEM_THREADS)
+k_ohem_sum(const float* __restrict__ p, const float* __restrict__ wnll, int64_t N, const OhemState* __restrict__ st,
+           double* __restrict__ part_s, int* __restrict__ part_c) {
+  __shared__ double s_d[OHEM_THREADS / 32];
+  __shared__ int s_c[OHEM_THREADS / 32];
+  const float thr = st->threshold;
+  const int64_t base = (int64_t)blockIdx.x * OHEM_TILE;
+  double acc = 0.0;
+  int c = 0;
+  for (int r = 0; r < OHEM_ITEMS; ++r) {
+    const int64_t i = base + r * OHEM_THREADS + threadIdx.x;
+    if (i < N && p[i] < thr) { acc += (double)wnll[i]; ++c; }     // NaN (not counted) compares false
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  c = warp_sum_i(c);
+  if ((threadIdx.x & 31) == 0) { s_d[threadIdx.x >> 5] = acc; s_c[threadIdx.x >> 5] = c; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double sd = 0.0;
+    int sc = 0;
+    for (int w = 0; w < OHEM_THREADS / 32; ++w) { sd += s_d[w]; sc += s_c[w]; }    // fixed order
+    part_s[blockIdx.x] = sd;
+    part_c[blockIdx.x] = sc;
+  }
+}
+
+__global__ void __launch_bounds__(1024)
+k_ohem_finalize(const double* __restrict__ part_s, const int* __restrict__ part_c, int64_t nt, int reduction,
+                OhemState* __restrict__ st, float* __restrict__ out) {
+  __shared__ double s_d[1024];
+  __shared__ int64_t s_c[1024];
+  double acc = 0.0;
+  int64_t c = 0;
+  for (int64_t i = threadIdx.x; i < nt; i += 1024) { acc += part_s[i]; c += part_c[i]; }
+  s_d[threadIdx.x] = acc; s_c[threadIdx.x] = c;
+  __syncthreads();
+  for (int o = 512; o > 0; o >>= 1) {
+    if (threadIdx.x < o) { s_d[threadIdx.x] += s_d[threadIdx.x + o]; s_c[threadIdx.x] += s_c[threadIdx.x + o]; }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    const int64_t cnt = s_c[0];
+    float loss;
+    if (st->n == 0) loss = 0.f;                                   // no labelled pixel: 0, zero gradient
+    else if (reduction == 0) loss = (float)(s_d[0] / (double)cnt);  // 0 / 0 = NaN: the mean of an empty selection
+    else loss = (float)s_d[0];
+    st->loss = loss;
+    st->denom = reduction == 0 ? (float)cnt : 1.f;
+    st->count = (int)cnt;
+    out[0] = loss;
+  }
+}
+
+}  // namespace pcl
+
+namespace {
+
+struct OhemLayout {
+  size_t p, lse, wnll, hist, part_s, part_c, total;
+  int64_t ntiles;
+};
+
+// state (byte 0) | p_t (byte 256, as pcl.h documents) | lse | w_t * nll | 3 histograms | partial sums, counts
+OhemLayout ohem_layout(int64_t N) {
+  OhemLayout l;
+  l.ntiles = ceil_div64(N, OHEM_TILE);
+  size_t o = lov_align(sizeof(OhemState));
+  l.p = o;      o = lov_align(o + (size_t)N * 4);
+  l.lse = o;    o = lov_align(o + (size_t)N * 4);
+  l.wnll = o;   o = lov_align(o + (size_t)N * 4);
+  l.hist = o;   o = lov_align(o + (size_t)3 * OHEM_BINS * 4);
+  l.part_s = o; o = lov_align(o + (size_t)l.ntiles * 8);
+  l.part_c = o; o = lov_align(o + (size_t)l.ntiles * 4);
+  l.total = o;
+  return l;
+}
+
+// Refuses (PCL_ERR_UNSUPPORTED) a label grid smaller than the logits, more than 256 classes and B*Himg*Wimg >= 2^31.
+int ohem_geometry(int B, int K, int h, int w, int H, int W) {
+  if (B <= 0 || K <= 0 || h <= 0 || w <= 0 || H <= 0 || W <= 0) return PCL_ERR_ARG;
+  if (H < h || W < w || K > 256) return PCL_ERR_UNSUPPORTED;
+  if ((int64_t)B * H * W >= ((int64_t)1 << 31)) return PCL_ERR_UNSUPPORTED;
+  return PCL_OK;
+}
+
+int ohem_make(const float* seg, const int64_t* target, const float* weight, int B, int K, int h, int w, int H, int W,
+              int ignore_index, SegCeArgs* a) {
+  if (!seg || !target) return PCL_ERR_ARG;
+  const int st = ohem_geometry(B, K, h, w, H, W);
+  if (st != PCL_OK) return st;
+  return make_ce(seg, target, weight, B, K, h, w, H, W, ignore_index, a);
+}
+
+}  // namespace
+
+extern "C" int64_t pcl_ohem_ce_scratch_bytes(int32_t B, int32_t K, int32_t h, int32_t w, int32_t Himg, int32_t Wimg) {
+  const int st = ohem_geometry(B, K, h, w, Himg, Wimg);
+  if (st != PCL_OK) return st;
+  return (int64_t)ohem_layout((int64_t)B * Himg * Wimg).total;
+}
+
+extern "C" int pcl_ohem_ce_fwd(const float* seg, const int64_t* target, const float* class_weight, int32_t B, int32_t K,
+                               int32_t h, int32_t w, int32_t Himg, int32_t Wimg, int32_t ignore_index, float thresh,
+                               int64_t min_kept, int32_t reduction, void* scratch, float* loss, void* stream) {
+  SegCeArgs a;
+  int st = ohem_make(seg, target, class_weight, B, K, h, w, Himg, Wimg, ignore_index, &a);
+  if (st != PCL_OK) return st;
+  PCL_REQUIRE(scratch && loss && min_kept >= 1 && (reduction == 0 || reduction == 1));
+  cudaStream_t s = (cudaStream_t)stream;
+  const int64_t N = (int64_t)B * Himg * Wimg;
+  const OhemLayout l = ohem_layout(N);
+  char* sc = (char*)scratch;
+  OhemState* state = (OhemState*)sc;
+  float* p = (float*)(sc + l.p);
+  float* wnll = (float*)(sc + l.wnll);
+  int* hist = (int*)(sc + l.hist);
+  PCL_CUDA(cudaMemsetAsync(state, 0, sizeof(OhemState), s));
+  PCL_CUDA(cudaMemsetAsync(hist, 0, (size_t)3 * OHEM_BINS * sizeof(int), s));
+  st = segce_fwd_launch<true>(a, (float*)(sc + l.lse), nullptr, nullptr, OhemPix{p, wnll, &state->n, thresh}, s);
+  if (st != PCL_OK) return st;
+  k_ohem_decide<<<1, 32, 0, s>>>(state, min_kept, thresh);
+  PCL_LAUNCH_CHECK();
+  const int64_t tiles = ceil_div64(N, OHEM_TILE);
+  const unsigned hist_ctas = (unsigned)(tiles < OHEM_HIST_CTAS ? tiles : OHEM_HIST_CTAS);
+  for (int level = 0; level < 3; ++level) {
+    k_ohem_hist<<<hist_ctas, OHEM_THREADS, 0, s>>>(p, N, level, state, hist);
+    PCL_LAUNCH_CHECK();
+    k_ohem_scan<<<1, 1024, 0, s>>>(level, thresh, state, hist);
+    PCL_LAUNCH_CHECK();
+  }
+  k_ohem_sum<<<(unsigned)l.ntiles, OHEM_THREADS, 0, s>>>(p, wnll, N, state, (double*)(sc + l.part_s),
+                                                         (int*)(sc + l.part_c));
+  PCL_LAUNCH_CHECK();
+  k_ohem_finalize<<<1, 1024, 0, s>>>((const double*)(sc + l.part_s), (const int*)(sc + l.part_c), l.ntiles, reduction,
+                                     state, loss);
+  PCL_LAUNCH_CHECK();
+  return PCL_OK;
+}
+
+extern "C" int pcl_ohem_ce_bwd(const float* seg, const int64_t* target, const float* class_weight, int32_t B, int32_t K,
+                               int32_t h, int32_t w, int32_t Himg, int32_t Wimg, int32_t ignore_index,
+                               const void* scratch, const float* grad_loss, float* dseg, void* stream) {
+  SegCeArgs a;
+  const int st = ohem_make(seg, target, class_weight, B, K, h, w, Himg, Wimg, ignore_index, &a);
+  if (st != PCL_OK) return st;
+  PCL_REQUIRE(scratch && dseg);
+  const OhemLayout l = ohem_layout((int64_t)B * Himg * Wimg);
+  const char* sc = (const char*)scratch;
+  return segce_bwd_tile_launch<true>(a, (const float*)(sc + l.lse), (const float*)sc, grad_loss, dseg,
+                                     (const float*)(sc + l.p), (cudaStream_t)stream);
 }

@@ -1145,3 +1145,106 @@ def upsample_lovasz_softmax(seg: torch.Tensor, target: torch.Tensor, ignore_inde
     if seg.dim() != 4 or target.dim() != 3 or seg.shape[0] != target.shape[0]:
         raise ValueError(f"seg (B,K,h,w) and target (B,H,W) expected, got {tuple(seg.shape)} and {tuple(target.shape)}")
     return _LovaszFn.apply(seg, target, ignore_index)
+
+
+# ------------------------------------------------------------------------------------------------
+# §8f row f7: fused bilinear up-sampling (align_corners=True) + OHEM cross-entropy
+# (FSOhemCELoss, lib/loss/loss_helper.py:215-261)
+# ------------------------------------------------------------------------------------------------
+_OHEM_REDUCTIONS = {"mean": 0, "elementwise_mean": 0, "sum": 1}
+
+
+def _ohem_forward(seg, target, weight, ignore_index, thresh, min_kept, reduction):
+    """Runs pcl_ohem_ce_fwd; returns (loss, the kept tensors, dims, scratch)."""
+    lib = _abi.load()
+    _require_cuda(seg, "seg")
+    dev = seg.device
+    seg_c = seg if (seg.dtype == torch.float32 and seg.is_contiguous()) else seg.to(torch.float32).contiguous()
+    tgt = target
+    if tgt.device != dev or tgt.dtype != torch.int64 or not tgt.is_contiguous():
+        tgt = tgt.to(device=dev, dtype=torch.int64).contiguous()
+    wt = None if weight is None else weight.to(device=dev, dtype=torch.float32).contiguous()
+    B, K, h, w = seg_c.shape
+    H, W = tgt.shape[1], tgt.shape[2]
+    n = lib.pcl_ohem_ce_scratch_bytes(B, K, h, w, H, W)
+    if n < 0:
+        _abi.check(n, "pcl_ohem_ce_scratch_bytes")
+    scratch = torch.empty(n, dtype=torch.uint8, device=dev)
+    out = torch.empty((), dtype=torch.float32, device=dev)
+    dims = (B, K, h, w, H, W, int(ignore_index))
+    with _on_device(dev):
+        _abi.check(lib.pcl_ohem_ce_fwd(seg_c.data_ptr(), tgt.data_ptr(), _abi.ptr(wt), *dims, float(thresh),
+                                       int(min_kept), reduction, scratch.data_ptr(), out.data_ptr(), _stream_ptr(dev)),
+                   "pcl_ohem_ce_fwd")
+    return out, (seg_c, tgt, wt, scratch), dims
+
+
+class _OhemCeFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, seg, target, weight, ignore_index, thresh, min_kept, reduction):
+        out, ctx.keep, ctx.dims = _ohem_forward(seg, target, weight, ignore_index, thresh, min_kept, reduction)
+        ctx.seg_dtype = seg.dtype
+        return out
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out):
+        lib = _abi.load()
+        seg_c, tgt, wt, scratch = ctx.keep
+        dev = seg_c.device
+        go = grad_out
+        if go.device != dev or go.dtype != torch.float32 or not go.is_contiguous():
+            go = go.detach().to(device=dev, dtype=torch.float32).contiguous()
+        dseg = torch.empty_like(seg_c)
+        with _on_device(dev):
+            _abi.check(lib.pcl_ohem_ce_bwd(seg_c.data_ptr(), tgt.data_ptr(), _abi.ptr(wt), *ctx.dims, scratch.data_ptr(),
+                                           go.data_ptr(), dseg.data_ptr(), _stream_ptr(dev)), "pcl_ohem_ce_bwd")
+        ctx.keep = None
+        return dseg.to(ctx.seg_dtype), None, None, None, None, None, None
+
+
+def _ohem_args(seg, target, reduction, min_kept):
+    if seg.dim() != 4 or target.dim() != 3 or seg.shape[0] != target.shape[0]:
+        raise ValueError(f"seg (B,K,h,w) and target (B,H,W) expected, got {tuple(seg.shape)} and {tuple(target.shape)}")
+    if reduction not in _OHEM_REDUCTIONS:
+        raise NotImplementedError(f"Reduction Error! OHEM CE reduction {reduction!r} (mean, elementwise_mean or sum)")
+    return _OHEM_REDUCTIONS[reduction], max(1, int(min_kept))
+
+
+def upsample_ohem_cross_entropy(seg: torch.Tensor, target: torch.Tensor, weight: Optional[torch.Tensor] = None,
+                                ignore_index: int = -1, thresh: float = 0.9, min_kept: int = 100000,
+                                reduction: str = "mean") -> torch.Tensor:
+    """OHEM cross-entropy of bilinearly (align_corners=True) up-sampled logits against a full-resolution label map,
+    fused: == FSOhemCELoss.forward(F.interpolate(seg, target.shape[1:], mode='bilinear', align_corners=True), target)
+    without the (B,K,Himg,Wimg) intermediates, the sort or a host sync (the defaults of thresh and min_kept are the
+    contrast configs' ohem_thresh and ohem_minkeep).  Over the counted pixels (label not
+    ignore_index and inside [0, K)) of the whole batch, p_t is the softmax of the target class; the pixels with
+    p_t < max(kth, thresh) are kept, kth the min(max(1, min_kept), n - 1)-th smallest p_t (0-based), thresh compared in
+    fp32.  reduction 'mean' (or 'elementwise_mean') divides the weighted NLL sum by the kept count (not by the sum of the
+    weights), 'sum' does not; anything else raises NotImplementedError.  No counted pixel gives 0 with a zero gradient;
+    an empty selection gives NaN ('mean') or 0 ('sum') with a zero gradient.  seg fp32, bf16 or fp16 (read as fp32); the
+    gradient comes back in seg's dtype; ``target`` is not modified.  A label grid smaller than seg, more than 256
+    classes or 2^31 label pixels raise PclError."""
+    red, mk = _ohem_args(seg, target, reduction, min_kept)
+    return _OhemCeFn.apply(seg, target, weight, ignore_index, float(thresh), mk, red)
+
+
+def ohem_selection(seg: torch.Tensor, target: torch.Tensor, weight: Optional[torch.Tensor] = None,
+                   ignore_index: int = -1, thresh: float = 0.9, min_kept: int = 100000,
+                   reduction: str = "mean") -> dict:
+    """The forward of upsample_ohem_cross_entropy with what it decided, for tests and measurement: the loss, the
+    threshold, which branch set it ("select": the exact select of the kth value ran; "threshold": fp32(thresh) decided
+    without it), the counted pixels n, the selected count and the (B,Himg,Wimg) bool mask of the selected pixels (the
+    stored p_t < threshold, exactly the pixels the backward reads as selected).  Synchronises with the device."""
+    red, mk = _ohem_args(seg, target, reduction, min_kept)
+    with torch.no_grad():
+        out, keep, dims = _ohem_forward(seg, target, weight, ignore_index, float(thresh), mk, red)
+    scratch = keep[3]
+    B, H, W = dims[0], dims[4], dims[5]
+    head = scratch[:28].cpu()
+    f = head[:12].view(torch.float32)
+    i = head[12:28].view(torch.int32)
+    p = scratch[256:256 + 4 * B * H * W].view(torch.float32).view(B, H, W)
+    thr = float(f[2])
+    return {"loss": out, "threshold": thr, "branch": "select" if int(i[0]) else "threshold", "n": int(i[1]),
+            "count": int(i[3]), "selected": p < thr, "p": p}

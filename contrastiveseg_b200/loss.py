@@ -5,7 +5,8 @@ The contrast term runs on the H100 engine (functional.pixel_contrast_loss); the 
 the fused up-sample + CE kernels (``contrast.fused_seg_ce``, default on), and with ``contrast.use_rmi`` the RMI seg
 loss runs on the fused up-sample + RMI kernels (same switch: off, F.interpolate runs first); a
 ``seg_criterion=FSCELOVASZLoss(configer)`` runs its Lovasz term on the fused up-sample + Lovasz kernels (same
-switch).  Engine-only knobs are read from optional config keys under ``contrast``: ``rng`` ("device" |
+switch); ``seg_criterion=FSOhemCELoss(configer)`` (``FSAuxOhemCELoss`` for contrast_auxce_loss) runs the OHEM CE on
+the fused up-sample + OHEM CE kernels (same switch).  Engine-only knobs are read from optional config keys under ``contrast``: ``rng`` ("device" |
 "torch_cpu"), ``nan_safe``, ``precision`` ("fp32" | "bf16"), ``skip_warmup_contrast``, ``topk_negatives`` (a10
 extension, default off).
 """
@@ -18,7 +19,8 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from .functional import ContrastOptions, pixel_contrast_loss, upsample_cross_entropy, upsample_lovasz_softmax
-from .loss_helper import FSAuxCELoss, FSAuxRMILoss, FSCELOVASZLoss, FSCELoss, FSRMILoss
+from .loss_helper import (FSAuxCELoss, FSAuxOhemCELoss, FSAuxRMILoss, FSCELOVASZLoss, FSCELoss, FSOhemCELoss,
+                          FSRMILoss)
 
 
 def _opt(configer, key, default):
@@ -146,7 +148,7 @@ class ContrastCELoss(nn.Module):
         return F.interpolate(input=seg, size=(target.size(1), target.size(2)), mode="bilinear", align_corners=True)
 
     def _seg_loss(self, preds, target):
-        if isinstance(self.seg_criterion, FSRMILoss):
+        if isinstance(self.seg_criterion, (FSRMILoss, FSOhemCELoss)):
             return self.seg_criterion(self._rmi_input(preds["seg"], target), target)
         if isinstance(self.seg_criterion, FSCELOVASZLoss):
             return self._lovasz_seg_loss(preds["seg"], target, self.seg_criterion)
@@ -202,14 +204,15 @@ class ContrastAuxCELoss(ContrastCELoss):
     def _seg_loss(self, preds, target):
         assert "seg_aux" in preds
         crit = self.seg_criterion
-        if isinstance(crit, FSAuxRMILoss):
+        if isinstance(crit, (FSAuxRMILoss, FSAuxOhemCELoss)):
             lw = crit.configer.get("network", "loss_weights")
             if self._can_fuse(crit.ce_loss, preds["seg_aux"]):
                 aux = self._fused_ce(preds["seg_aux"], target, crit.ce_loss)
             else:
                 aux = crit.ce_loss(F.interpolate(input=preds["seg_aux"], size=(target.size(1), target.size(2)),
                                                  mode="bilinear", align_corners=True), target)
-            return lw["seg_loss"] * crit.rmi_loss(self._rmi_input(preds["seg"], target), target) + lw["aux_loss"] * aux
+            seg_term = crit.rmi_loss if isinstance(crit, FSAuxRMILoss) else crit.ohem_ce_loss
+            return lw["seg_loss"] * seg_term(self._rmi_input(preds["seg"], target), target) + lw["aux_loss"] * aux
         if isinstance(crit, FSAuxCELoss) and self._can_fuse(crit.ce_loss, preds["seg"]):
             lw = crit.configer.get("network", "loss_weights")
             return (lw["seg_loss"] * self._fused_ce(preds["seg"], target, crit.ce_loss) +

@@ -3,7 +3,8 @@
 The CE modules are plain PyTorch ops so the wrappers are drop-in (the wrappers run the fused up-sample + CE kernels
 instead when they can, SURVEY §8f row 1).  The RMI modules (contrast.use_rmi) run the fused RMI kernels
 (functional.upsample_rmi_loss, §8f row f5).  FSCELOVASZLoss adds the Lovasz-softmax term of the fused up-sample +
-Lovasz kernels (functional.upsample_lovasz_softmax, §8f row f6) to the CE.
+Lovasz kernels (functional.upsample_lovasz_softmax, §8f row f6) to the CE.  FSOhemCELoss and the seg term of
+FSAuxOhemCELoss run the fused up-sample + OHEM CE kernels (functional.upsample_ohem_cross_entropy, §8f row f7).
 """
 from __future__ import annotations
 
@@ -11,7 +12,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from .functional import upsample_lovasz_softmax, upsample_rmi_loss
+from .functional import upsample_lovasz_softmax, upsample_ohem_cross_entropy, upsample_rmi_loss
 
 
 def _ce_params(configer):
@@ -146,3 +147,42 @@ class FSCELOVASZLoss(nn.Module):
             return loss
         target = _scale_target(targets[0], (inputs.size(2), inputs.size(3)))
         return self.ce_loss(inputs, target) + upsample_lovasz_softmax(inputs, target, self.ignore_index)
+
+
+class FSOhemCELoss(nn.Module):
+    """OHEM cross-entropy  (lib/loss/loss_helper.py:215-261) on the engine (upsample_ohem_cross_entropy).  Reads
+    ohem_thresh, ohem_minkeep (min_kept = max(1, ohem_minkeep)), ce_weight, ce_reduction ('elementwise_mean' by default,
+    'mean' accepted as its alias, 'sum'; anything else raises NotImplementedError in forward) and ce_ignore_index.
+    ``predict`` may be the logits at label resolution (the reference's call) or below it: the bilinear up-sampling
+    (align_corners=True) is fused.  Labels outside [0, K) count as ignored; no labelled pixel gives 0."""
+
+    def __init__(self, configer=None):
+        super().__init__()
+        self.configer = configer
+        p = configer.get("loss", "params")
+        self.thresh = p["ohem_thresh"]
+        self.min_kept = max(1, p["ohem_minkeep"])
+        weight, reduction, ignore_index = _ce_params(configer)
+        self.register_buffer("weight", weight, persistent=False)
+        self.reduction = reduction
+        self.ignore_label = ignore_index
+
+    def forward(self, predict, target, **kwargs):
+        return upsample_ohem_cross_entropy(predict, target, self.weight, self.ignore_label, self.thresh, self.min_kept,
+                                           self.reduction)
+
+
+class FSAuxOhemCELoss(nn.Module):
+    """seg_loss_weight * OHEM CE(seg) + aux_loss_weight * CE(aux)  (lib/loss/loss_helper.py:264-281).  Always the OHEM
+    CE: unlike the reference, loss.loss_type is not asserted, so the module can be built from a contrast config."""
+
+    def __init__(self, configer=None):
+        super().__init__()
+        self.configer = configer
+        self.ce_loss = FSCELoss(configer)
+        self.ohem_ce_loss = FSOhemCELoss(configer)
+
+    def forward(self, inputs, targets, **kwargs):
+        aux_out, seg_out = inputs
+        w = self.configer.get("network", "loss_weights")
+        return w["seg_loss"] * self.ohem_ce_loss(seg_out, targets) + w["aux_loss"] * self.ce_loss(aux_out, targets)

@@ -340,6 +340,41 @@ int pcl_lovasz_bwd(const float* seg, const int64_t* target, int32_t B, int32_t K
                    int32_t Wimg, int32_t ignore_index, void* scratch, const float* grad_loss, float* dseg, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * §8f row f7: the OHEM cross-entropy of FSOhemCELoss and of the seg term of FSAuxOhemCELoss
+ * (lib/loss/loss_helper.py:215-261), fused.  Replaces F.interpolate(seg, (Himg,Wimg), bilinear, align_corners=True) +
+ * softmax + gather of the target probability + sort of the labelled pixels + CrossEntropyLoss(weight,
+ * reduction='none') + the selection, and its autograd backward; the (B,K,Himg,Wimg) logits and probabilities are never
+ * materialised and no call syncs with the host (capturable).
+ *   seg (B,K,h,w) fp32 with Himg >= h, Wimg >= w; target (B,Himg,Wimg) int64 (read only); class_weight (K) fp32 or NULL.
+ *   A pixel counts when its label is not ignore_index and lies in [0, K); the others are ignored (the reference raises
+ *   on labels outside [0, K)).  Over the n counted pixels of the whole batch, p_t = softmax(up(seg))[t]:
+ *     kth = the m-th smallest p_t, 0-based, m = min(min_kept, n - 1)   (min_kept >= 1: the module passes
+ *           max(1, ohem_minkeep));
+ *     threshold = max(kth, thresh), compared in fp32 (thresh is passed as a float, as torch compares it);
+ *     the selected pixels are those with p_t < threshold (strict: pixels tied at the threshold are all left out);
+ *     loss_i = w[t_i] * nll_i; reduction 0 ('mean' / 'elementwise_mean'): sum(loss_i) / count (not divided by the
+ *     sum of the weights); reduction 1 ('sum'): the plain sum.  Any other reduction is PCL_ERR_ARG.
+ *   The selection carries no gradient: a selected pixel's gradient is s * w_t * (softmax - onehot_t), s = grad / count
+ *   ('mean') or grad ('sum').  No counted pixel (n = 0): the loss is 0 with a zero gradient (the reference raises on the
+ *   empty sort).  n > 0 with an empty selection (e.g. n = 1, or every p_t equal): NaN for 'mean', 0 for 'sum', with a
+ *   zero gradient, as in the reference.
+ *   A label grid smaller than seg, K > 256 or B*Himg*Wimg >= 2^31 return PCL_ERR_UNSUPPORTED.
+ *   scratch: pcl_ohem_ce_scratch_bytes (host only; a negative PCL_ERR_* for a refused request), 256-byte aligned.  After
+ *   pcl_ohem_ce_fwd its first 32 bytes hold float loss, float denominator, float threshold, int32 select (1 when the
+ *   exact select ran, 0 when fp32(thresh) decided), int32 n, int32 count(p_t < thresh), int32 selected count; from byte
+ *   256 on the B*Himg*Wimg floats p_t in (b, y, x) order, NaN at the pixels that do not count.
+ *   pcl_ohem_ce_bwd reads the scratch its pcl_ohem_ce_fwd wrote.  The loss is bit-reproducible; dseg to the last ulp or
+ *   two (fp32 atomics).
+ * ----------------------------------------------------------------------------------------------*/
+int64_t pcl_ohem_ce_scratch_bytes(int32_t B, int32_t K, int32_t h, int32_t w, int32_t Himg, int32_t Wimg);
+int pcl_ohem_ce_fwd(const float* seg, const int64_t* target, const float* class_weight, int32_t B, int32_t K, int32_t h,
+                    int32_t w, int32_t Himg, int32_t Wimg, int32_t ignore_index, float thresh, int64_t min_kept,
+                    int32_t reduction, void* scratch, float* loss, void* stream);
+int pcl_ohem_ce_bwd(const float* seg, const int64_t* target, const float* class_weight, int32_t B, int32_t K, int32_t h,
+                    int32_t w, int32_t Himg, int32_t Wimg, int32_t ignore_index, const void* scratch,
+                    const float* grad_loss, float* dseg, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * a7 + a8: memory bank.  Replaces segmentor/trainer_contrastive.py:102-138 (_dequeue_and_enqueue).
  * Step 1 (parallel): build this rank's enqueue packet.  Step 2 (ordered): apply the packets of all
  * ranks in rank order — world 1 reproduces the reference exactly, world > 1 is the allgather merge
