@@ -22,14 +22,92 @@
 
 namespace pcl {
 
-struct SegCeArgs {
+struct SegCeArgs : UpGeom {
   const float* seg; const int64_t* target; const float* weight;
-  int B, K, h, w, H, W, ignore_index;
-  float ry, rx;                 // (h-1)/(H-1), (w-1)/(W-1)   (align_corners=True)
+  int ignore_index;
 };
 
 constexpr int CE_THREADS = 256;
-constexpr int KC_FWD_MAX = 32;         // classes staged per pass in the forward (one pass for K <= 32: one exposed load latency)
+
+// Fixed-order sums of two per-CTA partial arrays by a 1024-thread CTA: thread i accumulates entries i, i + 1024, ... in
+// TA / TB, then a 512 -> 1 tree; thread 0 then runs done(total_a, total_b).  The totals reach done as references to
+// shared memory, so they are read where done uses them.  The finalisers built on it are bit-reproducible.
+template <class TA, class TB, class PA, class PB, class Done>
+__device__ __forceinline__ void block_sum2_1024(const PA* pa, const PB* pb, int64_t n, Done done) {
+  __shared__ TA s_a[1024];
+  __shared__ TB s_b[1024];
+  TA va = 0;
+  TB vb = 0;
+  for (int64_t i = threadIdx.x; i < n; i += 1024) { va += pa[i]; vb += pb[i]; }
+  s_a[threadIdx.x] = va; s_b[threadIdx.x] = vb;
+  __syncthreads();
+  for (int o = 512; o > 0; o >>= 1) {
+    if (threadIdx.x < o) { s_a[threadIdx.x] += s_a[threadIdx.x + o]; s_b[threadIdx.x] += s_b[threadIdx.x + o]; }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) done(s_a[0], s_b[0]);
+}
+
+// Exclusive scan of one int per thread of a 1024-thread CTA, in a fixed order: warp shuffle-up scans, then one warp over
+// the 32 warp totals (s_w: 32 ints of shared memory).  Every thread calls it (it contains barriers).
+__device__ __forceinline__ int block_exclusive_scan_1024(int v, int* s_w) {
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  int incl = v;                                                      // warp inclusive scan
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int u = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += u;
+  }
+  if (lane == 31) s_w[wid] = incl;
+  __syncthreads();
+  if (wid == 0) {
+    const int wv = s_w[lane];
+    int wi = wv;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int u = __shfl_up_sync(0xffffffffu, wi, o);
+      if (lane >= o) wi += u;
+    }
+    s_w[lane] = wi - wv;                                             // exclusive warp offsets
+  }
+  __syncthreads();
+  return s_w[wid] + incl - v;
+}
+
+// Backward tile skeleton of the up-sampling losses: one CTA = a 32 x 8 tile of label pixels of one image, classes in
+// chunks of kc.  Dynamic shared memory: G [kc][BTY][BT] | Hx [kc][BTY][SRC_MAX] | S [kc][pitch] source patch.
+//   pre(g, px, S)             once, after the tile tables (a pass over the classes that the chunks need first)
+//   per chunk: the source patch is staged; fill(c0, cn, px, S, G) writes G[cc][ty][tx], the gradient w.r.t. the
+//   (virtual) up-sampled logits of the chunk; the transposed bilinear map takes it into dseg (up_tile_flush)
+template <class Pre, class Fill>
+__device__ __forceinline__ void up_bwd_tile(const UpGeom& a, const float* seg, float* dseg, int kc, int pitch, Pre pre,
+                                            Fill fill) {
+  extern __shared__ float sm[];
+  float* G = sm;                                   // [kc][BTY][BT]
+  float* Hx = G + (size_t)kc * BTY * BT;           // [kc][BTY][SRC_MAX]
+  float* S = Hx + (size_t)kc * BTY * SRC_MAX;      // [kc][pitch] source patch
+  __shared__ int s_y0[BTY], s_y1[BTY], s_x0[BT], s_x1[BT];
+  __shared__ float s_ly[BTY], s_lx[BT];
+  __shared__ float s_wx[SRC_MAX * (BT + 1)], s_wy[SRC_MAX * (BTY + 1)];
+  __shared__ short s_xlo[SRC_MAX], s_xhi[SRC_MAX], s_ylo[SRC_MAX], s_yhi[SRC_MAX];
+  const int b = blockIdx.z;
+  const int64_t hw = (int64_t)a.h * a.w;
+  const UpTile g = up_tile_coords(blockIdx.x * BT, blockIdx.y * BTY, a.H, a.W, a.h, a.w, a.ry, a.rx, s_y0, s_y1, s_ly,
+                                  s_x0, s_x1, s_lx);
+  const UpPix px = up_pix(g, threadIdx.x & (BT - 1), threadIdx.x >> 5, s_y0, s_y1, s_ly, s_x0, s_x1, s_lx);
+  up_tile_tables(g, a.ry, a.rx, s_y0, s_y1, s_ly, s_x0, s_x1, s_lx, s_wx, s_wy, s_xlo, s_xhi, s_ylo, s_yhi);
+  pre(g, px, S);
+  __syncthreads();
+  for (int c0 = 0; c0 < a.K; c0 += kc) {
+    const int cn = min(kc, a.K - c0);
+    up_stage(a, seg, b, c0, cn, g.ys_base, g.xs_base, g.ys_n, g.xs_n, pitch, S);
+    __syncthreads();
+    fill(c0, cn, px, S, G);
+    __syncthreads();
+    up_tile_flush(g, cn, G, Hx, s_wx, s_wy, s_xlo, s_xhi, s_ylo, s_yhi, dseg + ((int64_t)b * a.K + c0) * hw, hw, a.w);
+    __syncthreads();
+  }
+}
 
 // Per-pixel outputs of the OHEM forward (OHEM = true, fourth part of this file); the plain CE leaves them unused.
 struct OhemPix {
@@ -54,29 +132,19 @@ k_segce_fwd(SegCeArgs a, float* __restrict__ lse_out, float* __restrict__ part_n
   const int b = blockIdx.z;
   const int X0 = blockIdx.x * BT, Y0 = blockIdx.y * BTY;
   const int x = X0 + tx, y = Y0 + ty;
-  const int64_t hw = (int64_t)a.h * a.w, HWo = (int64_t)a.H * a.W;
+  const int64_t HWo = (int64_t)a.H * a.W;
   const UpTile g = up_tile_coords(X0, Y0, a.H, a.W, a.h, a.w, a.ry, a.rx, s_y0, s_y1, s_ly, s_x0, s_x1, s_lx);
-  const int ys_base = g.ys_base, xs_base = g.xs_base, ys_n = g.ys_n, xs_n = g.xs_n;
+  const UpPix px = up_pix(g, tx, ty, s_y0, s_y1, s_ly, s_x0, s_x1, s_lx);
   const bool inside = x < a.W && y < a.H;
-  const int ly0 = s_y0[ty] - ys_base, ly1 = s_y1[ty] - ys_base, lx0 = s_x0[tx] - xs_base, lx1 = s_x1[tx] - xs_base;
-  const float ly = s_ly[ty], lx = s_lx[tx];
-  const float w00 = (1.f - ly) * (1.f - lx), w01 = (1.f - ly) * lx, w10 = ly * (1.f - lx), w11 = ly * lx;
-  const int i00 = ly0 * xs_n + lx0, i01 = ly0 * xs_n + lx1, i10 = ly1 * xs_n + lx0, i11 = ly1 * xs_n + lx1;
   int64_t t = -1;
   if (inside) t = a.target[(int64_t)b * HWo + (int64_t)y * a.W + x];
   float m = -CUDART_INF_F, se = 0.f, vt = 0.f;
   for (int c0 = 0; c0 < a.K; c0 += kc) {
     const int cn = min(kc, a.K - c0);
-    const int patch = ys_n * xs_n;
-    for (int i = threadIdx.x; i < cn * patch; i += BT * BTY) {
-      const int cc = i / patch, r = i - cc * patch;
-      const int yy = r / xs_n, xx = r - yy * xs_n;
-      sm[cc * pitch + r] = a.seg[((int64_t)b * a.K + c0 + cc) * hw + (int64_t)(ys_base + yy) * a.w + xs_base + xx];
-    }
+    up_stage(a, a.seg, b, c0, cn, g.ys_base, g.xs_base, g.ys_n, g.xs_n, pitch, sm);
     __syncthreads();
     for (int cc = 0; cc < cn; ++cc) {
-      const float* p = sm + cc * pitch;
-      const float v = w00 * p[i00] + w01 * p[i01] + w10 * p[i10] + w11 * p[i11];
+      const float v = up_logit(px, sm + cc * pitch);
       if (v > m) { se = se * __expf(m - v) + 1.f; m = v; }     // online log-sum-exp
       else       { se += __expf(v - m); }
       if (c0 + cc == (int)t) vt = v;
@@ -120,54 +188,31 @@ k_segce_fwd(SegCeArgs a, float* __restrict__ lse_out, float* __restrict__ part_n
 
 __global__ void __launch_bounds__(1024)
 k_segce_finalize(const float* __restrict__ part_nll, const float* __restrict__ part_w, int64_t n, float* __restrict__ out) {
-  __shared__ double s_n[1024], s_w[1024];
-  double an = 0.0, aw = 0.0;
-  for (int64_t i = threadIdx.x; i < n; i += 1024) { an += part_nll[i]; aw += part_w[i]; }
-  s_n[threadIdx.x] = an; s_w[threadIdx.x] = aw;
-  __syncthreads();
-  for (int o = 512; o > 0; o >>= 1) {
-    if (threadIdx.x < o) { s_n[threadIdx.x] += s_n[threadIdx.x + o]; s_w[threadIdx.x] += s_w[threadIdx.x + o]; }
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) {
-    out[0] = (float)(s_n[0] / s_w[0]);          // 'mean' reduction: sum(w_t * nll) / sum(w_t) over non-ignored pixels
-    out[1] = (float)s_w[0];
-  }
+  block_sum2_1024<double, double>(part_nll, part_w, n, [&](const double& an, const double& aw) {
+    out[0] = (float)(an / aw);                  // 'mean' reduction: sum(w_t * nll) / sum(w_t) over non-ignored pixels
+    out[1] = (float)aw;
+  });
 }
 
-// Backward, tile formulation: one CTA = a 32 x 8 tile of label pixels of one image, classes in chunks of kc.
-//   A  a thread per label pixel: G[c] = coef * w_t * (softmax_c - [c == t]) from the staged source patch -> shared memory
-//   B, C  the transposed bilinear map into dseg (up_tile_flush, pcl_upsample.cuh)
-// Each (pixel, class) softmax is evaluated once (the per-logit gather below needs 16x as many); B and C only visit the
+// Backward, tile formulation (up_bwd_tile): per chunk, a thread per label pixel computes
+// G[c] = coef * w_t * (softmax_c - [c == t]) from the staged source patch; then the transposed bilinear map into dseg.
+// Each (pixel, class) softmax is evaluated once (the per-logit gather below needs 16x as many); the map only visits the
 // label columns / rows inside the footprint of their source cell.
 // With OHEM, fin is the OHEM state (fin[1] the denominator, fin[2] the threshold) and only the pixels whose stored
 // p_t (ohem_p) lies below the threshold carry a gradient: the forward's selection, read back rather than recomputed.
 template <bool OHEM>
 __global__ void __launch_bounds__(BT * BTY, 5)     // 5 CTAs per SM: holds the kernel at 48 registers
 k_segce_bwd_tile(SegCeArgs a, const float* __restrict__ lse, const float* __restrict__ fin,
-                 const float* __restrict__ grad_out, float* __restrict__ dseg, int kc, int pitch,
-                 const float* __restrict__ ohem_p) {
-  extern __shared__ float sm[];
-  float* G = sm;                                   // [kc][BTY][BT]
-  float* Hx = G + (size_t)kc * BTY * BT;           // [kc][BTY][SRC_MAX]
-  float* S = Hx + (size_t)kc * BTY * SRC_MAX;      // [kc][pitch] source patch
-  __shared__ int s_y0[BTY], s_y1[BTY], s_x0[BT], s_x1[BT];
-  __shared__ float s_ly[BTY], s_lx[BT];
-  __shared__ float s_wx[SRC_MAX * (BT + 1)], s_wy[SRC_MAX * (BTY + 1)];
-  __shared__ short s_xlo[SRC_MAX], s_xhi[SRC_MAX], s_ylo[SRC_MAX], s_yhi[SRC_MAX];
+                 const float* __restrict__ grad_out, const float* __restrict__ ohem_p, float* __restrict__ dseg, int kc,
+                 int pitch) {
   const int tx = threadIdx.x & (BT - 1), ty = threadIdx.x >> 5;
   const int b = blockIdx.z;
-  const int X0 = blockIdx.x * BT, Y0 = blockIdx.y * BTY;
-  const int x = X0 + tx, y = Y0 + ty;
-  const int64_t hw = (int64_t)a.h * a.w, HWo = (int64_t)a.H * a.W;
-  const UpTile g = up_tile_coords(X0, Y0, a.H, a.W, a.h, a.w, a.ry, a.rx, s_y0, s_y1, s_ly, s_x0, s_x1, s_lx);
-  const int ys_base = g.ys_base, xs_base = g.xs_base, xs_n = g.xs_n;
-  const int patch = g.ys_n * xs_n;
-  const bool inside = x < a.W && y < a.H;
+  const int x = blockIdx.x * BT + tx, y = blockIdx.y * BTY + ty;
+  const int64_t HWo = (int64_t)a.H * a.W;
   const float scale = (grad_out ? grad_out[0] : 1.f) / fin[1];
   int64_t t = -1;
   float lse_p = 0.f, coef = 0.f;
-  if (inside) {
+  if (x < a.W && y < a.H) {
     t = a.target[(int64_t)b * HWo + (int64_t)y * a.W + x];
     if (t != (int64_t)a.ignore_index && t >= 0 && t < a.K &&
         (!OHEM || ohem_p[(int64_t)b * HWo + (int64_t)y * a.W + x] < fin[2])) {
@@ -177,35 +222,17 @@ k_segce_bwd_tile(SegCeArgs a, const float* __restrict__ lse, const float* __rest
       t = -1;
     }
   }
-  const int ly0 = s_y0[ty] - ys_base, ly1 = s_y1[ty] - ys_base, lx0 = s_x0[tx] - xs_base, lx1 = s_x1[tx] - xs_base;
-  const float ly = s_ly[ty], lx = s_lx[tx];
-  const float w00 = (1.f - ly) * (1.f - lx), w01 = (1.f - ly) * lx, w10 = ly * (1.f - lx), w11 = ly * lx;
-  const int i00 = ly0 * xs_n + lx0, i01 = ly0 * xs_n + lx1, i10 = ly1 * xs_n + lx0, i11 = ly1 * xs_n + lx1;
-  up_tile_tables(g, a.ry, a.rx, s_y0, s_y1, s_ly, s_x0, s_x1, s_lx, s_wx, s_wy, s_xlo, s_xhi, s_ylo, s_yhi);
-  __syncthreads();
-  for (int c0 = 0; c0 < a.K; c0 += kc) {
-    const int cn = min(kc, a.K - c0);
-    for (int i = threadIdx.x; i < cn * patch; i += BT * BTY) {
-      const int cc = i / patch, r = i - cc * patch;
-      const int yy = r / xs_n, xx = r - yy * xs_n;
-      S[cc * pitch + r] = a.seg[((int64_t)b * a.K + c0 + cc) * hw + (int64_t)(ys_base + yy) * a.w + xs_base + xx];
-    }
-    __syncthreads();
-    // ---- A: gradient w.r.t. the (virtual) up-sampled logits ----
+  up_bwd_tile(a, a.seg, dseg, kc, pitch, [](const UpTile&, const UpPix&, float*) {},
+              [&](int c0, int cn, const UpPix& px, const float* S, float* G) {
     for (int cc = 0; cc < cn; ++cc) {
       float gv = 0.f;
       if (t >= 0) {
-        const float* p = S + cc * pitch;
-        const float v = w00 * p[i00] + w01 * p[i01] + w10 * p[i10] + w11 * p[i11];
+        const float v = up_logit(px, S + cc * pitch);
         gv = coef * (__expf(v - lse_p) - ((c0 + cc) == (int)t ? 1.f : 0.f));
       }
       G[((size_t)cc * BTY + ty) * BT + tx] = gv;
     }
-    __syncthreads();
-    // ---- B, C: transposed bilinear map, flush ----
-    up_tile_flush(g, cn, G, Hx, s_wx, s_wy, s_xlo, s_xhi, s_ylo, s_yhi, dseg + ((int64_t)b * a.K + c0) * hw, hw, a.w);
-    __syncthreads();
-  }
+  });
 }
 
 // General backward (any scale, e.g. label grid smaller than the logits): one thread per logit gathers over the label
@@ -268,44 +295,40 @@ using namespace pcl;
 
 static int make_ce(const float* seg, const int64_t* target, const float* weight, int B, int K, int h, int w, int H, int W,
                    int ignore_index, SegCeArgs* a) {
-  if (!seg || !target || B <= 0 || K <= 0 || h <= 0 || w <= 0 || H <= 0 || W <= 0) return PCL_ERR_ARG;
-  a->seg = seg; a->target = target; a->weight = weight;
-  a->B = B; a->K = K; a->h = h; a->w = w; a->H = H; a->W = W; a->ignore_index = ignore_index;
-  a->ry = H > 1 ? (float)(h - 1) / (float)(H - 1) : 0.f;
-  a->rx = W > 1 ? (float)(w - 1) / (float)(W - 1) : 0.f;
+  if (!seg || !target) return PCL_ERR_ARG;
+  const int st = up_geometry(B, K, h, w, H, W, a);
+  if (st != PCL_OK) return st;
+  a->seg = seg; a->target = target; a->weight = weight; a->ignore_index = ignore_index;
   return PCL_OK;
 }
 
-static int patch_pitch(const SegCeArgs& a) { return up_patch_pitch(a.h, a.w, a.ry, a.rx); }
-
 template <bool OHEM>
 static int segce_fwd_launch(const SegCeArgs& a, float* lse, float* pn, float* pw, OhemPix o, cudaStream_t s) {
-  const int pitch = patch_pitch(a);
-  int kc = a.K < KC_FWD_MAX ? a.K : KC_FWD_MAX;
-  while (kc > 1 && (size_t)kc * pitch * sizeof(float) > 96 * 1024) --kc;
-  const size_t smem = (size_t)kc * pitch * sizeof(float);
-  if (smem > 200 * 1024) return PCL_ERR_UNSUPPORTED;
+  UpPlan pl;
+  const int st = up_fwd_plan(a, up_patch_pitch(a, BTY, BT), 0, &pl);
+  if (st != PCL_OK) return st;
   PCL_SMEM_OPT_IN(k_segce_fwd<OHEM>, 200 * 1024);
-  k_segce_fwd<OHEM><<<dim3((unsigned)ceil_div(a.W, BT), (unsigned)ceil_div(a.H, BTY), a.B), BT * BTY, smem, s>>>(
-      a, lse, pn, pw, pitch, kc, o);
+  k_segce_fwd<OHEM><<<dim3((unsigned)ceil_div(a.W, BT), (unsigned)ceil_div(a.H, BTY), a.B), BT * BTY, pl.smem, s>>>(
+      a, lse, pn, pw, pl.pitch, pl.kc, o);
   PCL_LAUNCH_CHECK();
   return PCL_OK;
 }
 
-// dseg is zeroed here; the tile kernel accumulates into it
-template <bool OHEM>
-static int segce_bwd_tile_launch(const SegCeArgs& a, const float* lse, const float* fin, const float* grad_loss,
-                                 float* dseg, const float* ohem_p, cudaStream_t s) {
+// Launch plan of the backward tile kernels (up_bwd_tile): dseg is zeroed here (the kernel accumulates into it); kc
+// classes per pass, at most KC_BWD_MAX, fewer while G + Hx + the source patch (kc * (BTY*BT + BTY*SRC_MAX + pitch)
+// floats) exceed 200 KB.  The kernel is a template argument because PCL_SMEM_OPT_IN keeps one flag per instantiation:
+// every kernel opts in on its own, k_segce_bwd_tile<false> and <true> included (they have the same type).
+template <auto Kernel, class Args, class... P>
+static int up_bwd_launch(const Args& a, cudaStream_t s, float* dseg, P... p) {
   PCL_CUDA(cudaMemsetAsync(dseg, 0, (size_t)a.B * a.K * a.h * a.w * sizeof(float), s));
-  // classes per pass: G (kc*32*32) + Hx (kc*32*34) + source patch (kc*pitch) floats, two CTAs per SM when possible
-  const int pitch = patch_pitch(a);
-  int kc = a.K < 24 ? a.K : 24;              // one pass for K <= 24 (fewer bulk-synchronous phases per CTA)
+  const int pitch = up_patch_pitch(a, BTY, BT);
+  int kc = a.K < KC_BWD_MAX ? a.K : KC_BWD_MAX;
   while (kc > 1 && (size_t)kc * (BTY * BT + BTY * SRC_MAX + pitch) * sizeof(float) > 200 * 1024) --kc;
   const size_t smem = (size_t)kc * (BTY * BT + BTY * SRC_MAX + pitch) * sizeof(float);
   if (smem > 200 * 1024) return PCL_ERR_UNSUPPORTED;
-  PCL_SMEM_OPT_IN(k_segce_bwd_tile<OHEM>, 200 * 1024);
-  k_segce_bwd_tile<OHEM><<<dim3((unsigned)ceil_div(a.W, BT), (unsigned)ceil_div(a.H, BTY), a.B), BT * BTY, smem, s>>>(
-      a, lse, fin, grad_loss, dseg, kc, pitch, ohem_p);
+  PCL_SMEM_OPT_IN(Kernel, 200 * 1024);
+  Kernel<<<dim3((unsigned)ceil_div(a.W, BT), (unsigned)ceil_div(a.H, BTY), a.B), BT * BTY, smem, s>>>(a, p..., dseg, kc,
+                                                                                                      pitch);
   PCL_LAUNCH_CHECK();
   return PCL_OK;
 }
@@ -355,7 +378,7 @@ extern "C" int pcl_seg_ce_bwd(const float* seg, const int64_t* target, const flo
     PCL_LAUNCH_CHECK();
     return PCL_OK;
   }
-  return segce_bwd_tile_launch<false>(a, lse, fin, grad_loss, dseg, nullptr, s);
+  return up_bwd_launch<k_segce_bwd_tile<false>>(a, s, dseg, lse, fin, grad_loss, (const float*)nullptr);
 }
 
 // ==================================================================================================================
@@ -388,10 +411,10 @@ constexpr int MB_PITCH = MB_X + RMI_R_MAX - 1;
 constexpr double RMI_ALPHA = 1e-3;                       // _POS_ALPHA
 constexpr float RMI_CLIP_MIN = 1e-6f;                    // _CLIP_MIN
 
-struct RmiArgs {
+static_assert(PT_X * PT_Y == BT * BTY, "k_rmi_pool stages its patch with up_stage (256 threads)");
+
+struct RmiArgs : UpGeom {
   const float* seg; const int64_t* target;
-  int B, K, h, w, H, W;
-  float ry, rx;                 // (h-1)/(H-1), (w-1)/(W-1)   (align_corners=True)
   int r, way, s, pad;           // radius, pool way (0 max, 1 avg), pool size == stride, padding s/2
   int Hp, Wp, nY, nX;           // pooled map, neighbour-vector points (Hp-r+1) x (Wp-r+1)
   float lw, wb, wr;             // loss_weight, BCE weight, RMI weight (lambda_way: lambda, 1-lambda; else 1, lambda)
@@ -436,7 +459,7 @@ k_rmi_pool(RmiArgs a, float* __restrict__ P, uint8_t* __restrict__ L, uint8_t* _
     src_coord(C0 + i, a.rx, a.w, i0, i1, l);
     s_x0[i] = i0; s_x1[i] = i1; s_lx[i] = l;
   }
-  const int64_t HWo = (int64_t)a.H * a.W, hw = (int64_t)a.h * a.w;
+  const int64_t HWo = (int64_t)a.H * a.W;
   for (int i = threadIdx.x; i < nr * nc; i += PT_X * PT_Y) {
     const int lr = i / nc, lc = i - lr * nc;
     int64_t t = a.target[(int64_t)b * HWo + (int64_t)(R0 + lr) * a.W + C0 + lc];
@@ -445,7 +468,7 @@ k_rmi_pool(RmiArgs a, float* __restrict__ P, uint8_t* __restrict__ L, uint8_t* _
   }
   __syncthreads();
   const int ys_base = s_y0[0], xs_base = s_x0[0];
-  const int xs_n = s_x1[nc - 1] - xs_base + 1, patch = (s_y1[nr - 1] - ys_base + 1) * xs_n;
+  const int ys_n = s_y1[nr - 1] - ys_base + 1, xs_n = s_x1[nc - 1] - xs_base + 1;
   const bool active = oy < a.Hp && ox < a.Wp;
   const int wy0 = oy * s - pad, wx0 = ox * s - pad;                  // window origin (may lie in the padding)
   int ylo = 0, yhi = 0, xlo = 0, xhi = 0;
@@ -461,11 +484,7 @@ k_rmi_pool(RmiArgs a, float* __restrict__ P, uint8_t* __restrict__ L, uint8_t* _
   const int64_t HWp = (int64_t)a.Hp * a.Wp;
   for (int c0 = 0; c0 < a.K; c0 += kc) {
     const int cn = min(kc, a.K - c0);
-    for (int i = threadIdx.x; i < cn * patch; i += PT_X * PT_Y) {
-      const int cc = i / patch, r = i - cc * patch;
-      const int yy = r / xs_n, xx = r - yy * xs_n;
-      S[cc * pitch + r] = a.seg[((int64_t)b * a.K + c0 + cc) * hw + (int64_t)(ys_base + yy) * a.w + xs_base + xx];
-    }
+    up_stage(a, a.seg, b, c0, cn, ys_base, xs_base, ys_n, xs_n, pitch, S);
     __syncthreads();
     if (active) {
       for (int cc = 0; cc < cn; ++cc) {
@@ -690,18 +709,8 @@ k_rmi_solve(RmiArgs a, const double* __restrict__ part, int nbands, double* __re
 __global__ void __launch_bounds__(1024)
 k_rmi_finalize(RmiArgs a, const float* __restrict__ part_bce, const int* __restrict__ part_cnt, int64_t n,
                const double* __restrict__ rmi_bc, double* __restrict__ fin, float* __restrict__ out) {
-  __shared__ double s_b[1024];
-  __shared__ long long s_c[1024];
-  double ab = 0.0; long long ac = 0;
-  for (int64_t i = threadIdx.x; i < n; i += 1024) { ab += part_bce[i]; ac += part_cnt[i]; }
-  s_b[threadIdx.x] = ab; s_c[threadIdx.x] = ac;
-  __syncthreads();
-  for (int o = 512; o > 0; o >>= 1) {
-    if (threadIdx.x < o) { s_b[threadIdx.x] += s_b[threadIdx.x + o]; s_c[threadIdx.x] += s_c[threadIdx.x + o]; }
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) {
-    const double inv_n = 1.0 / ((double)s_c[0] + 1.0);
+  block_sum2_1024<double, long long>(part_bce, part_cnt, n, [&](const double& ab, const long long& ac) {
+    const double inv_n = 1.0 / ((double)ac + 1.0);
     double rmi = 0.0;
     for (int c = 0; c < a.K; ++c) {                           // sum_c mean_b(rmi_bc) / half_d
       double m = 0.0;
@@ -709,13 +718,13 @@ k_rmi_finalize(RmiArgs a, const float* __restrict__ part_bce, const int* __restr
       rmi += m / (double)a.B;
     }
     rmi /= (double)(a.r * a.r);
-    const double loss = (double)a.lw * ((double)a.wb * s_b[0] * inv_n + (double)a.wr * rmi);
+    const double loss = (double)a.lw * ((double)a.wb * ab * inv_n + (double)a.wr * rmi);
     fin[0] = loss;
     fin[1] = (double)a.lw * (double)a.wb * inv_n;             // d loss / d (sum of the BCE terms)
     fin[2] = rmi;
-    fin[3] = (double)s_c[0];
+    fin[3] = (double)ac;
     out[0] = (float)loss;
-  }
+  });
 }
 
 // ---- backward ----------------------------------------------------------------------------------------
@@ -755,22 +764,10 @@ k_rmi_dpool(RmiArgs a, const float* __restrict__ P, const uint8_t* __restrict__ 
 __global__ void __launch_bounds__(BT * BTY)
 k_rmi_bwd_tile(RmiArgs a, const float* __restrict__ dP, const uint8_t* __restrict__ Am, const double* __restrict__ fin,
                const float* __restrict__ grad_out, float* __restrict__ dseg, int kc, int pitch) {
-  extern __shared__ float sm[];
-  float* G = sm;                                   // [kc][BTY][BT]
-  float* Hx = G + (size_t)kc * BTY * BT;           // [kc][BTY][SRC_MAX]
-  float* S = Hx + (size_t)kc * BTY * SRC_MAX;      // [kc][pitch] source patch
-  __shared__ int s_y0[BTY], s_y1[BTY], s_x0[BT], s_x1[BT];
-  __shared__ float s_ly[BTY], s_lx[BT];
-  __shared__ float s_wx[SRC_MAX * (BT + 1)], s_wy[SRC_MAX * (BTY + 1)];
-  __shared__ short s_xlo[SRC_MAX], s_xhi[SRC_MAX], s_ylo[SRC_MAX], s_yhi[SRC_MAX];
   const int tx = threadIdx.x & (BT - 1), ty = threadIdx.x >> 5;
   const int b = blockIdx.z;
-  const int X0 = blockIdx.x * BT, Y0 = blockIdx.y * BTY;
-  const int x = X0 + tx, y = Y0 + ty;
-  const int64_t hw = (int64_t)a.h * a.w, HWo = (int64_t)a.H * a.W, HWp = (int64_t)a.Hp * a.Wp;
-  const UpTile g = up_tile_coords(X0, Y0, a.H, a.W, a.h, a.w, a.ry, a.rx, s_y0, s_y1, s_ly, s_x0, s_x1, s_lx);
-  const int ys_base = g.ys_base, xs_base = g.xs_base, xs_n = g.xs_n;
-  const int patch = g.ys_n * xs_n;
+  const int x = blockIdx.x * BT + tx, y = blockIdx.y * BTY + ty;
+  const int64_t HWo = (int64_t)a.H * a.W, HWp = (int64_t)a.Hp * a.Wp;
   const float cb = (float)fin[1] * (grad_out ? grad_out[0] : 1.f);
   int tv = -1;
   int64_t u = -1;                                  // pooled pixel whose window holds this label pixel
@@ -786,25 +783,17 @@ k_rmi_bwd_tile(RmiArgs a, const float* __restrict__ dP, const uint8_t* __restric
     }
   }
   const float inv_s2 = 1.f / (float)(a.s * a.s);
-  const int ly0 = s_y0[ty] - ys_base, ly1 = s_y1[ty] - ys_base, lx0 = s_x0[tx] - xs_base, lx1 = s_x1[tx] - xs_base;
-  const float ly = s_ly[ty], lx = s_lx[tx];
-  const int i00 = ly0 * xs_n + lx0, i01 = ly0 * xs_n + lx1, i10 = ly1 * xs_n + lx0, i11 = ly1 * xs_n + lx1;
-  up_tile_tables(g, a.ry, a.rx, s_y0, s_y1, s_ly, s_x0, s_x1, s_lx, s_wx, s_wy, s_xlo, s_xhi, s_ylo, s_yhi);
-  __syncthreads();
-  for (int c0 = 0; c0 < a.K; c0 += kc) {
-    const int cn = min(kc, a.K - c0);
-    for (int i = threadIdx.x; i < cn * patch; i += BT * BTY) {
-      const int cc = i / patch, r = i - cc * patch;
-      const int yy = r / xs_n, xx = r - yy * xs_n;
-      S[cc * pitch + r] = a.seg[((int64_t)b * a.K + c0 + cc) * hw + (int64_t)(ys_base + yy) * a.w + xs_base + xx];
-    }
-    __syncthreads();
+  up_bwd_tile(a, a.seg, dseg, kc, pitch, [](const UpTile&, const UpPix&, float*) {},
+              [&](int c0, int cn, const UpPix& px, const float* S, float* G) {
+    const float ly = px.ly, lx = px.lx;
     for (int cc = 0; cc < cn; ++cc) {
       float gv = 0.f;
       if (tv >= 0) {
         const int c = c0 + cc;
         const float* p = S + cc * pitch;
-        const float z = (1.f - ly) * ((1.f - lx) * p[i00] + lx * p[i01]) + ly * ((1.f - lx) * p[i10] + lx * p[i11]);
+        // the nested form of k_rmi_pool: its FMA chain, so the forward and backward see the same z
+        const float z = (1.f - ly) * ((1.f - lx) * p[px.i00] + lx * p[px.i01]) +
+                        ly * ((1.f - lx) * p[px.i10] + lx * p[px.i11]);
         const float sg = 1.f / (1.f + expf(-z));
         gv = cb * (sg - (tv == c ? 1.f : 0.f));                                  // BCE with logits
         if (u >= 0) {
@@ -815,10 +804,7 @@ k_rmi_bwd_tile(RmiArgs a, const float* __restrict__ dP, const uint8_t* __restric
       }
       G[((size_t)cc * BTY + ty) * BT + tx] = gv;
     }
-    __syncthreads();
-    up_tile_flush(g, cn, G, Hx, s_wx, s_wy, s_xlo, s_xhi, s_ylo, s_yhi, dseg + ((int64_t)b * a.K + c0) * hw, hw, a.w);
-    __syncthreads();
-  }
+  });
 }
 
 }  // namespace pcl
@@ -833,18 +819,14 @@ struct RmiLayout {
   int nbands;
 };
 
-size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 // Validates the geometry and parameters; fills the pooled-map sizes.  Refuses (PCL_ERR_UNSUPPORTED) what the reference
 // accepts but the engine does not implement: radius 5-10, pool way 2, stride > 4, down-sampling, a pooled map smaller
 // than the radius, more than 256 classes.
 int rmi_geometry(int B, int K, int h, int w, int H, int W, int radius, int way, int stride, RmiArgs* a) {
-  if (B <= 0 || K <= 0 || h <= 0 || w <= 0 || H <= 0 || W <= 0) return PCL_ERR_ARG;
+  const int st = up_geometry(B, K, h, w, H, W, a);
+  if (st != PCL_OK) return st;
   if (radius < 1 || radius > 10 || way < 0 || way > 3 || stride < 1) return PCL_ERR_ARG;
   if (radius > RMI_R_MAX || way > 1 || stride > RMI_S_MAX || K > 256 || H < h || W < w) return PCL_ERR_UNSUPPORTED;
-  a->B = B; a->K = K; a->h = h; a->w = w; a->H = H; a->W = W;
-  a->ry = H > 1 ? (float)(h - 1) / (float)(H - 1) : 0.f;
-  a->rx = W > 1 ? (float)(w - 1) / (float)(W - 1) : 0.f;
   a->r = radius; a->way = way; a->s = stride; a->pad = stride / 2;
   a->Hp = (H + 2 * a->pad - stride) / stride + 1;
   a->Wp = (W + 2 * a->pad - stride) / stride + 1;
@@ -931,20 +913,15 @@ extern "C" int pcl_rmi_fwd(const float* seg, const int64_t* target, int32_t B, i
   cudaStream_t s = (cudaStream_t)stream;
   const RmiLayout l = rmi_layout(a);
   char* sc = (char*)scratch;
-  // source patch of a pool tile: label rows / columns of REG_ROWS x REG_COLS at most
-  const int py = (int)((float)(REG_ROWS - 1) * a.ry) + 3, px = (int)((float)(REG_COLS - 1) * a.rx) + 3;
-  const int pitch = (py < h + 1 ? py : h + 1) * (px < w + 1 ? px : w + 1) + 1;
-  const size_t lab_bytes = (size_t)REG_ROWS * REG_COLS * sizeof(short);
-  int kc = K < 32 ? K : 32;
-  while (kc > 1 && lab_bytes + (size_t)kc * pitch * sizeof(float) > 96 * 1024) --kc;
-  const size_t smem = lab_bytes + (size_t)kc * pitch * sizeof(float);
-  if (smem > 200 * 1024) return PCL_ERR_UNSUPPORTED;
+  // source patch of a pool tile: label rows / columns of REG_ROWS x REG_COLS at most, after its label region
+  UpPlan pl;
+  int rc = up_fwd_plan(a, up_patch_pitch(a, REG_ROWS, REG_COLS), (size_t)REG_ROWS * REG_COLS * sizeof(short), &pl);
+  if (rc != PCL_OK) return rc;
   PCL_SMEM_OPT_IN(k_rmi_pool, 200 * 1024);
-  k_rmi_pool<<<dim3((unsigned)ceil_div(a.Wp, PT_X), (unsigned)ceil_div(a.Hp, PT_Y), B), PT_X * PT_Y, smem, s>>>(
+  k_rmi_pool<<<dim3((unsigned)ceil_div(a.Wp, PT_X), (unsigned)ceil_div(a.Hp, PT_Y), B), PT_X * PT_Y, pl.smem, s>>>(
       a, (float*)(sc + l.P), (uint8_t*)(sc + l.L), (uint8_t*)(sc + l.A), (float*)(sc + l.bce), (int*)(sc + l.cnt),
-      pitch, kc);
+      pl.pitch, pl.kc);
   PCL_LAUNCH_CHECK();
-  int rc = PCL_OK;
   switch (radius) {
     case 1: rc = rmi_moments_solve<1>(a, l, sc, s); break;
     case 2: rc = rmi_moments_solve<2>(a, l, sc, s); break;
@@ -978,17 +955,8 @@ extern "C" int pcl_rmi_bwd(const float* seg, const int64_t* target, int32_t B, i
     default: rc = rmi_dpool<4>(a, l, sc, grad_loss, s); break;
   }
   if (rc != PCL_OK) return rc;
-  PCL_CUDA(cudaMemsetAsync(dseg, 0, (size_t)B * K * h * w * sizeof(float), s));
-  const int pitch = up_patch_pitch(h, w, a.ry, a.rx);
-  int kc = K < 24 ? K : 24;
-  while (kc > 1 && (size_t)kc * (BTY * BT + BTY * SRC_MAX + pitch) * sizeof(float) > 200 * 1024) --kc;
-  const size_t smem = (size_t)kc * (BTY * BT + BTY * SRC_MAX + pitch) * sizeof(float);
-  if (smem > 200 * 1024) return PCL_ERR_UNSUPPORTED;
-  PCL_SMEM_OPT_IN(k_rmi_bwd_tile, 200 * 1024);
-  k_rmi_bwd_tile<<<dim3((unsigned)ceil_div(Wimg, BT), (unsigned)ceil_div(Himg, BTY), B), BT * BTY, smem, s>>>(
-      a, (const float*)(sc + l.dP), (const uint8_t*)(sc + l.A), (const double*)(sc + l.fin), grad_loss, dseg, kc, pitch);
-  PCL_LAUNCH_CHECK();
-  return PCL_OK;
+  return up_bwd_launch<k_rmi_bwd_tile>(a, s, dseg, (const float*)(sc + l.dP), (const uint8_t*)(sc + l.A),
+                                       (const double*)(sc + l.fin), grad_loss);
 }
 
 // ==================================================================================================================
@@ -1026,45 +994,12 @@ constexpr int LOV_ITEMS = 8;
 constexpr int LOV_TILE = LOV_THREADS * LOV_ITEMS;   // keys per sort / loss tile
 constexpr int LOV_RADIX = 256;
 constexpr int LOV_PASSES = 4;                       // 4 x 8 bits cover the 30 live bits of d
-constexpr int LOV_KC = 32;                          // classes staged per pass in the keys kernel
-constexpr int LOV_KC_BWD = 24;
 
-struct LovArgs {
+struct LovArgs : UpGeom {
   const float* seg; const int64_t* target;
-  int B, K, h, w, H, W, ignore_index;
-  float ry, rx;
+  int ignore_index;
   int64_t N;                    // B*H*W
 };
-
-// bilinear weights / patch offsets of this thread's label pixel inside the staged patch
-struct LovPix {
-  float w00, w01, w10, w11;
-  int i00, i01, i10, i11;
-};
-
-__device__ __forceinline__ LovPix lov_pix(const UpTile& g, int tx, int ty, const int* s_y0, const int* s_y1,
-                                          const float* s_ly, const int* s_x0, const int* s_x1, const float* s_lx) {
-  LovPix p;
-  const int ly0 = s_y0[ty] - g.ys_base, ly1 = s_y1[ty] - g.ys_base, lx0 = s_x0[tx] - g.xs_base, lx1 = s_x1[tx] - g.xs_base;
-  const float ly = s_ly[ty], lx = s_lx[tx];
-  p.w00 = (1.f - ly) * (1.f - lx); p.w01 = (1.f - ly) * lx; p.w10 = ly * (1.f - lx); p.w11 = ly * lx;
-  p.i00 = ly0 * g.xs_n + lx0; p.i01 = ly0 * g.xs_n + lx1; p.i10 = ly1 * g.xs_n + lx0; p.i11 = ly1 * g.xs_n + lx1;
-  return p;
-}
-
-__device__ __forceinline__ float lov_logit(const LovPix& p, const float* s) {
-  return p.w00 * s[p.i00] + p.w01 * s[p.i01] + p.w10 * s[p.i10] + p.w11 * s[p.i11];
-}
-
-__device__ __forceinline__ void lov_stage(const LovArgs& a, const UpTile& g, int b, int c0, int cn, int pitch, float* S) {
-  const int patch = g.ys_n * g.xs_n;
-  const int64_t hw = (int64_t)a.h * a.w;
-  for (int i = threadIdx.x; i < cn * patch; i += BT * BTY) {
-    const int cc = i / patch, r = i - cc * patch;
-    const int yy = r / g.xs_n, xx = r - yy * g.xs_n;
-    S[cc * pitch + r] = a.seg[((int64_t)b * a.K + c0 + cc) * hw + (int64_t)(g.ys_base + yy) * a.w + g.xs_base + xx];
-  }
-}
 
 // the label of pixel (b, y, x) if it counts (not ignore_index, inside [0, K)), else -1
 __device__ __forceinline__ int lov_label(const LovArgs& a, int64_t q) {
@@ -1083,7 +1018,7 @@ k_lov_keys(LovArgs a, uint32_t* __restrict__ keys, float2* __restrict__ ms, uint
   const int X0 = blockIdx.x * BT, Y0 = blockIdx.y * BTY;
   const int x = X0 + tx, y = Y0 + ty;
   const UpTile g = up_tile_coords(X0, Y0, a.H, a.W, a.h, a.w, a.ry, a.rx, s_y0, s_y1, s_ly, s_x0, s_x1, s_lx);
-  const LovPix px = lov_pix(g, tx, ty, s_y0, s_y1, s_ly, s_x0, s_x1, s_lx);
+  const UpPix px = up_pix(g, tx, ty, s_y0, s_y1, s_ly, s_x0, s_x1, s_lx);
   const bool inside = x < a.W && y < a.H;
   const int64_t q = ((int64_t)b * a.H + y) * a.W + x;
   const int t = inside ? lov_label(a, q) : -1;
@@ -1091,10 +1026,10 @@ k_lov_keys(LovArgs a, uint32_t* __restrict__ keys, float2* __restrict__ ms, uint
   const bool one = a.K <= kc;                      // one staged chunk: the second sweep reuses it
   for (int c0 = 0; c0 < a.K; c0 += kc) {
     const int cn = min(kc, a.K - c0);
-    lov_stage(a, g, b, c0, cn, pitch, sm);
+    up_stage(a, a.seg, b, c0, cn, g.ys_base, g.xs_base, g.ys_n, g.xs_n, pitch, sm);
     __syncthreads();
     for (int cc = 0; cc < cn; ++cc) {
-      const float v = lov_logit(px, sm + cc * pitch);
+      const float v = up_logit(px, sm + cc * pitch);
       if (v > m) { se = se * __expf(m - v) + 1.f; m = v; }     // online sum of exp
       else       { se += __expf(v - m); }
     }
@@ -1107,7 +1042,7 @@ k_lov_keys(LovArgs a, uint32_t* __restrict__ keys, float2* __restrict__ ms, uint
   for (int c0 = 0; c0 < a.K; c0 += kc) {
     const int cn = min(kc, a.K - c0);
     if (!one) {
-      lov_stage(a, g, b, c0, cn, pitch, sm);
+      up_stage(a, a.seg, b, c0, cn, g.ys_base, g.xs_base, g.ys_n, g.xs_n, pitch, sm);
       __syncthreads();
     }
     if (inside) {
@@ -1115,7 +1050,7 @@ k_lov_keys(LovArgs a, uint32_t* __restrict__ keys, float2* __restrict__ ms, uint
         const int c = c0 + cc;
         uint32_t d = LOV_SENT;
         if (t >= 0) {
-          const float p = __expf(lov_logit(px, sm + cc * pitch) - m) / se;
+          const float p = __expf(up_logit(px, sm + cc * pitch) - m) / se;
           const float e = fabsf((t == c ? 1.f : 0.f) - p);
           d = LOV_ONE - __float_as_uint(e);
         }
@@ -1150,40 +1085,21 @@ __global__ void __launch_bounds__(1024)
 k_lov_scan(int* __restrict__ data, int64_t len, int64_t stride, int* __restrict__ total) {
   __shared__ int s_w[32];
   int* d = data + (int64_t)blockIdx.x * stride;
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   int carry = 0;
   for (int64_t base = 0; base < len; base += 4 * 1024) {
     int v[4], s = 0;
     const int64_t i0 = base + 4 * (int64_t)threadIdx.x;
 #pragma unroll
     for (int j = 0; j < 4; ++j) { v[j] = i0 + j < len ? d[i0 + j] : 0; s += v[j]; }
-    int incl = s;                                                    // warp inclusive scan
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int u = __shfl_up_sync(0xffffffffu, incl, o);
-      if (lane >= o) incl += u;
-    }
-    if (lane == 31) s_w[wid] = incl;
-    __syncthreads();
-    if (wid == 0) {
-      const int wv = s_w[lane];
-      int wi = wv;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const int u = __shfl_up_sync(0xffffffffu, wi, o);
-        if (lane >= o) wi += u;
-      }
-      s_w[lane] = wi - wv;                                           // exclusive warp offsets
-    }
-    __syncthreads();
-    int run = carry + s_w[wid] + incl - s;
+    const int excl = block_exclusive_scan_1024(s, s_w);
+    int run = carry + excl;
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       if (i0 + j < len) d[i0 + j] = run;
       run += v[j];
     }
     __syncthreads();
-    if (threadIdx.x == 1023) s_w[0] = s_w[31] + incl;             // chunk total: last warp's offset + its total
+    if (threadIdx.x == 1023) s_w[0] = excl + s;                   // chunk total: the last thread's inclusive sum
     __syncthreads();
     carry += s_w[0];
     __syncthreads();
@@ -1361,21 +1277,9 @@ k_lov_finalize(const double* __restrict__ part, const int* __restrict__ gts, int
 __global__ void __launch_bounds__(BT * BTY, 4)     // 4 CTAs per SM: 64 registers, no spill
 k_lov_bwd_tile(LovArgs a, const float2* __restrict__ ms, const float* __restrict__ ge, const float* __restrict__ fin,
                const float* __restrict__ grad_out, float* __restrict__ dseg, int kc, int pitch) {
-  extern __shared__ float sm[];
-  float* G = sm;                                   // [kc][BTY][BT]
-  float* Hx = G + (size_t)kc * BTY * BT;           // [kc][BTY][SRC_MAX]
-  float* S = Hx + (size_t)kc * BTY * SRC_MAX;      // [kc][pitch] source patch
-  __shared__ int s_y0[BTY], s_y1[BTY], s_x0[BT], s_x1[BT];
-  __shared__ float s_ly[BTY], s_lx[BT];
-  __shared__ float s_wx[SRC_MAX * (BT + 1)], s_wy[SRC_MAX * (BTY + 1)];
-  __shared__ short s_xlo[SRC_MAX], s_xhi[SRC_MAX], s_ylo[SRC_MAX], s_yhi[SRC_MAX];
   const int tx = threadIdx.x & (BT - 1), ty = threadIdx.x >> 5;
   const int b = blockIdx.z;
-  const int X0 = blockIdx.x * BT, Y0 = blockIdx.y * BTY;
-  const int x = X0 + tx, y = Y0 + ty;
-  const int64_t hw = (int64_t)a.h * a.w;
-  const UpTile g = up_tile_coords(X0, Y0, a.H, a.W, a.h, a.w, a.ry, a.rx, s_y0, s_y1, s_ly, s_x0, s_x1, s_lx);
-  const LovPix px = lov_pix(g, tx, ty, s_y0, s_y1, s_ly, s_x0, s_x1, s_lx);
+  const int x = blockIdx.x * BT + tx, y = blockIdx.y * BTY + ty;
   const int64_t q = ((int64_t)b * a.H + y) * a.W + x;
   const float npres = fin[1];
   const float scale = npres > 0.f ? (grad_out ? grad_out[0] : 1.f) / npres : 0.f;
@@ -1386,36 +1290,31 @@ k_lov_bwd_tile(LovArgs a, const float2* __restrict__ ms, const float* __restrict
     const float2 v = ms[q];
     m = v.x; se = v.y;
   }
-  up_tile_tables(g, a.ry, a.rx, s_y0, s_y1, s_ly, s_x0, s_x1, s_lx, s_wx, s_wy, s_xlo, s_xhi, s_ylo, s_yhi);
   const bool one = a.K <= kc;
   float dot = 0.f;                                 // <p, dp>
-  if (!one) {                                      // several chunks: <p, dp> first
+  up_bwd_tile(a, a.seg, dseg, kc, pitch, [&](const UpTile& g, const UpPix& px, float* S) {
+    if (one) return;                               // several chunks: <p, dp> first
     for (int c0 = 0; c0 < a.K; c0 += kc) {
       const int cn = min(kc, a.K - c0);
       __syncthreads();
-      lov_stage(a, g, b, c0, cn, pitch, S);
+      up_stage(a, a.seg, b, c0, cn, g.ys_base, g.xs_base, g.ys_n, g.xs_n, pitch, S);
       __syncthreads();
       if (t >= 0) {
         for (int cc = 0; cc < cn; ++cc) {
           const int c = c0 + cc;
-          const float p = __expf(lov_logit(px, S + cc * pitch) - m) / se;
+          const float p = __expf(up_logit(px, S + cc * pitch) - m) / se;
           const float f = t == c ? 1.f : 0.f;
           const float dp = p > f ? ge[(int64_t)c * a.N + q] : (p < f ? -ge[(int64_t)c * a.N + q] : 0.f);
           dot += p * dp;
         }
       }
     }
-  }
-  __syncthreads();
-  for (int c0 = 0; c0 < a.K; c0 += kc) {
-    const int cn = min(kc, a.K - c0);
-    lov_stage(a, g, b, c0, cn, pitch, S);
-    __syncthreads();
+  }, [&](int c0, int cn, const UpPix& px, const float* S, float* G) {
     for (int cc = 0; cc < cn; ++cc) {              // dp (and <p, dp> when one chunk holds every class)
       float dp = 0.f;
       if (t >= 0) {
         const int c = c0 + cc;
-        const float p = __expf(lov_logit(px, S + cc * pitch) - m) / se;
+        const float p = __expf(up_logit(px, S + cc * pitch) - m) / se;
         const float f = t == c ? 1.f : 0.f;
         dp = p > f ? ge[(int64_t)c * a.N + q] : (p < f ? -ge[(int64_t)c * a.N + q] : 0.f);
         if (one) dot += p * dp;
@@ -1425,15 +1324,12 @@ k_lov_bwd_tile(LovArgs a, const float2* __restrict__ ms, const float* __restrict
     for (int cc = 0; cc < cn; ++cc) {              // dz = scale * p (dp - <p, dp>)
       float gv = 0.f;
       if (t >= 0) {
-        const float p = __expf(lov_logit(px, S + cc * pitch) - m) / se;
+        const float p = __expf(up_logit(px, S + cc * pitch) - m) / se;
         gv = scale * p * (G[((size_t)cc * BTY + ty) * BT + tx] - dot);
       }
       G[((size_t)cc * BTY + ty) * BT + tx] = gv;
     }
-    __syncthreads();
-    up_tile_flush(g, cn, G, Hx, s_wx, s_wy, s_xlo, s_xhi, s_ylo, s_yhi, dseg + ((int64_t)b * a.K + c0) * hw, hw, a.w);
-    __syncthreads();
-  }
+  });
 }
 
 }  // namespace pcl
@@ -1447,18 +1343,20 @@ struct LovLayout {
   int ntiles, cc;
 };
 
-size_t lov_align(size_t x) { return (x + 255) & ~(size_t)255; }
-
-// Refuses (PCL_ERR_UNSUPPORTED) a label grid smaller than the logits, more than 256 classes and N >= 2^31.
-int lov_geometry(int B, int K, int h, int w, int H, int W, LovArgs* a) {
-  if (B <= 0 || K <= 0 || h <= 0 || w <= 0 || H <= 0 || W <= 0) return PCL_ERR_ARG;
+// Geometry of the losses that sort or select over the label pixels (Lovasz, OHEM): refuses (PCL_ERR_UNSUPPORTED) a label
+// grid smaller than the logits, more than 256 classes and N = B*H*W >= 2^31 (pixel indices are 32-bit).
+int sort_geometry(int B, int K, int h, int w, int H, int W, UpGeom* g) {
+  const int st = up_geometry(B, K, h, w, H, W, g);
+  if (st != PCL_OK) return st;
   if (H < h || W < w || K > 256) return PCL_ERR_UNSUPPORTED;
-  const int64_t N = (int64_t)B * H * W;
-  if (N >= ((int64_t)1 << 31)) return PCL_ERR_UNSUPPORTED;
-  a->B = B; a->K = K; a->h = h; a->w = w; a->H = H; a->W = W; a->N = N;
-  a->ry = H > 1 ? (float)(h - 1) / (float)(H - 1) : 0.f;
-  a->rx = W > 1 ? (float)(w - 1) / (float)(W - 1) : 0.f;
+  if ((int64_t)B * H * W >= ((int64_t)1 << 31)) return PCL_ERR_UNSUPPORTED;
   return PCL_OK;
+}
+
+int lov_geometry(int B, int K, int h, int w, int H, int W, LovArgs* a) {
+  const int st = sort_geometry(B, K, h, w, H, W, a);
+  a->N = (int64_t)B * H * W;
+  return st;
 }
 
 // Classes sorted together: a quarter of them (rounded up), so the sort's three extra key / payload buffers stay at
@@ -1469,18 +1367,18 @@ LovLayout lov_layout(const LovArgs& a) {
   l.cc = (a.K + 3) / 4;
   const size_t kn = (size_t)a.K * a.N, cn = (size_t)l.cc * a.N;
   size_t o = 0;
-  l.keys = o;   o = lov_align(o + kn * 4);
-  l.ge = o;     o = lov_align(o + kn * 4);
-  l.vals = o;   o = lov_align(o + cn * 4);
-  l.keys2 = o;  o = lov_align(o + cn * 4);
-  l.vals2 = o;  o = lov_align(o + cn * 4);
-  l.ms = o;     o = lov_align(o + (size_t)a.N * 8);
-  l.lab = o;    o = lov_align(o + (size_t)a.N);
-  l.hist = o;   o = lov_align(o + (size_t)l.cc * LOV_RADIX * l.ntiles * 4);
-  l.tilefg = o; o = lov_align(o + (size_t)a.K * l.ntiles * 4);
-  l.gts = o;    o = lov_align(o + (size_t)a.K * 4);
-  l.part = o;   o = lov_align(o + (size_t)a.K * l.ntiles * 8);
-  l.fin = o;    o = lov_align(o + 4 * sizeof(float));
+  l.keys = o;   o = align256(o + kn * 4);
+  l.ge = o;     o = align256(o + kn * 4);
+  l.vals = o;   o = align256(o + cn * 4);
+  l.keys2 = o;  o = align256(o + cn * 4);
+  l.vals2 = o;  o = align256(o + cn * 4);
+  l.ms = o;     o = align256(o + (size_t)a.N * 8);
+  l.lab = o;    o = align256(o + (size_t)a.N);
+  l.hist = o;   o = align256(o + (size_t)l.cc * LOV_RADIX * l.ntiles * 4);
+  l.tilefg = o; o = align256(o + (size_t)a.K * l.ntiles * 4);
+  l.gts = o;    o = align256(o + (size_t)a.K * 4);
+  l.part = o;   o = align256(o + (size_t)a.K * l.ntiles * 8);
+  l.fin = o;    o = align256(o + 4 * sizeof(float));
   l.total = o;
   return l;
 }
@@ -1520,14 +1418,12 @@ extern "C" int pcl_lovasz_fwd(const float* seg, const int64_t* target, int32_t B
   int* hist = (int*)(sc + l.hist);
   int* tilefg = (int*)(sc + l.tilefg);
   int* gts = (int*)(sc + l.gts);
-  const int pitch = up_patch_pitch(h, w, a.ry, a.rx);
-  int kc = K < LOV_KC ? K : LOV_KC;
-  while (kc > 1 && (size_t)kc * pitch * sizeof(float) > 96 * 1024) --kc;
-  const size_t smem = (size_t)kc * pitch * sizeof(float);
-  if (smem > 200 * 1024) return PCL_ERR_UNSUPPORTED;
+  UpPlan pl;
+  const int rc = up_fwd_plan(a, up_patch_pitch(a, BTY, BT), 0, &pl);
+  if (rc != PCL_OK) return rc;
   PCL_SMEM_OPT_IN(k_lov_keys, 200 * 1024);
-  k_lov_keys<<<dim3((unsigned)ceil_div(Wimg, BT), (unsigned)ceil_div(Himg, BTY), B), BT * BTY, smem, s>>>(
-      a, keys, (float2*)(sc + l.ms), (uint8_t*)(sc + l.lab), pitch, kc);
+  k_lov_keys<<<dim3((unsigned)ceil_div(Wimg, BT), (unsigned)ceil_div(Himg, BTY), B), BT * BTY, pl.smem, s>>>(
+      a, keys, (float2*)(sc + l.ms), (uint8_t*)(sc + l.lab), pl.pitch, pl.kc);
   PCL_LAUNCH_CHECK();
   const int nt = l.ntiles;
   for (int c0 = 0; c0 < K; c0 += l.cc) {
@@ -1569,17 +1465,8 @@ extern "C" int pcl_lovasz_bwd(const float* seg, const int64_t* target, int32_t B
   cudaStream_t s = (cudaStream_t)stream;
   const LovLayout l = lov_layout(a);
   const char* sc = (const char*)scratch;
-  PCL_CUDA(cudaMemsetAsync(dseg, 0, (size_t)B * K * h * w * sizeof(float), s));
-  const int pitch = up_patch_pitch(h, w, a.ry, a.rx);
-  int kc = K < LOV_KC_BWD ? K : LOV_KC_BWD;
-  while (kc > 1 && (size_t)kc * (BTY * BT + BTY * SRC_MAX + pitch) * sizeof(float) > 200 * 1024) --kc;
-  const size_t smem = (size_t)kc * (BTY * BT + BTY * SRC_MAX + pitch) * sizeof(float);
-  if (smem > 200 * 1024) return PCL_ERR_UNSUPPORTED;
-  PCL_SMEM_OPT_IN(k_lov_bwd_tile, 200 * 1024);
-  k_lov_bwd_tile<<<dim3((unsigned)ceil_div(Wimg, BT), (unsigned)ceil_div(Himg, BTY), B), BT * BTY, smem, s>>>(
-      a, (const float2*)(sc + l.ms), (const float*)(sc + l.ge), (const float*)(sc + l.fin), grad_loss, dseg, kc, pitch);
-  PCL_LAUNCH_CHECK();
-  return PCL_OK;
+  return up_bwd_launch<k_lov_bwd_tile>(a, s, dseg, (const float2*)(sc + l.ms), (const float*)(sc + l.ge),
+                                       (const float*)(sc + l.fin), grad_loss);
 }
 
 // ==================================================================================================================
@@ -1664,29 +1551,9 @@ __global__ void __launch_bounds__(1024)
 k_ohem_scan(int level, float thresh, OhemState* __restrict__ st, const int* __restrict__ hist) {
   __shared__ int s_w[32];
   if (!st->select) return;
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const int a0 = hist[level * OHEM_BINS + 2 * threadIdx.x], a1 = hist[level * OHEM_BINS + 2 * threadIdx.x + 1];
   const int s = a0 + a1;
-  int incl = s;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int u = __shfl_up_sync(0xffffffffu, incl, o);
-    if (lane >= o) incl += u;
-  }
-  if (lane == 31) s_w[wid] = incl;
-  __syncthreads();
-  if (wid == 0) {
-    const int wv = s_w[lane];
-    int wi = wv;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int u = __shfl_up_sync(0xffffffffu, wi, o);
-      if (lane >= o) wi += u;
-    }
-    s_w[lane] = wi - wv;
-  }
-  __syncthreads();
-  const int excl = s_w[wid] + incl - s;
+  const int excl = block_exclusive_scan_1024(s, s_w);
   const int r = st->rank;
   int d = -1, nr = 0;
   if (r >= excl && r < excl + a0) { d = 2 * threadIdx.x; nr = r - excl; }
@@ -1730,28 +1597,16 @@ k_ohem_sum(const float* __restrict__ p, const float* __restrict__ wnll, int64_t 
 __global__ void __launch_bounds__(1024)
 k_ohem_finalize(const double* __restrict__ part_s, const int* __restrict__ part_c, int64_t nt, int reduction,
                 OhemState* __restrict__ st, float* __restrict__ out) {
-  __shared__ double s_d[1024];
-  __shared__ int64_t s_c[1024];
-  double acc = 0.0;
-  int64_t c = 0;
-  for (int64_t i = threadIdx.x; i < nt; i += 1024) { acc += part_s[i]; c += part_c[i]; }
-  s_d[threadIdx.x] = acc; s_c[threadIdx.x] = c;
-  __syncthreads();
-  for (int o = 512; o > 0; o >>= 1) {
-    if (threadIdx.x < o) { s_d[threadIdx.x] += s_d[threadIdx.x + o]; s_c[threadIdx.x] += s_c[threadIdx.x + o]; }
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) {
-    const int64_t cnt = s_c[0];
+  block_sum2_1024<double, int64_t>(part_s, part_c, nt, [&](const double& sum, const int64_t& cnt) {
     float loss;
     if (st->n == 0) loss = 0.f;                                   // no labelled pixel: 0, zero gradient
-    else if (reduction == 0) loss = (float)(s_d[0] / (double)cnt);  // 0 / 0 = NaN: the mean of an empty selection
-    else loss = (float)s_d[0];
+    else if (reduction == 0) loss = (float)(sum / (double)cnt);   // 0 / 0 = NaN: the mean of an empty selection
+    else loss = (float)sum;
     st->loss = loss;
     st->denom = reduction == 0 ? (float)cnt : 1.f;
     st->count = (int)cnt;
     out[0] = loss;
-  }
+  });
 }
 
 }  // namespace pcl
@@ -1767,29 +1622,21 @@ struct OhemLayout {
 OhemLayout ohem_layout(int64_t N) {
   OhemLayout l;
   l.ntiles = ceil_div64(N, OHEM_TILE);
-  size_t o = lov_align(sizeof(OhemState));
-  l.p = o;      o = lov_align(o + (size_t)N * 4);
-  l.lse = o;    o = lov_align(o + (size_t)N * 4);
-  l.wnll = o;   o = lov_align(o + (size_t)N * 4);
-  l.hist = o;   o = lov_align(o + (size_t)3 * OHEM_BINS * 4);
-  l.part_s = o; o = lov_align(o + (size_t)l.ntiles * 8);
-  l.part_c = o; o = lov_align(o + (size_t)l.ntiles * 4);
+  size_t o = align256(sizeof(OhemState));
+  l.p = o;      o = align256(o + (size_t)N * 4);
+  l.lse = o;    o = align256(o + (size_t)N * 4);
+  l.wnll = o;   o = align256(o + (size_t)N * 4);
+  l.hist = o;   o = align256(o + (size_t)3 * OHEM_BINS * 4);
+  l.part_s = o; o = align256(o + (size_t)l.ntiles * 8);
+  l.part_c = o; o = align256(o + (size_t)l.ntiles * 4);
   l.total = o;
   return l;
-}
-
-// Refuses (PCL_ERR_UNSUPPORTED) a label grid smaller than the logits, more than 256 classes and B*Himg*Wimg >= 2^31.
-int ohem_geometry(int B, int K, int h, int w, int H, int W) {
-  if (B <= 0 || K <= 0 || h <= 0 || w <= 0 || H <= 0 || W <= 0) return PCL_ERR_ARG;
-  if (H < h || W < w || K > 256) return PCL_ERR_UNSUPPORTED;
-  if ((int64_t)B * H * W >= ((int64_t)1 << 31)) return PCL_ERR_UNSUPPORTED;
-  return PCL_OK;
 }
 
 int ohem_make(const float* seg, const int64_t* target, const float* weight, int B, int K, int h, int w, int H, int W,
               int ignore_index, SegCeArgs* a) {
   if (!seg || !target) return PCL_ERR_ARG;
-  const int st = ohem_geometry(B, K, h, w, H, W);
+  const int st = sort_geometry(B, K, h, w, H, W, a);
   if (st != PCL_OK) return st;
   return make_ce(seg, target, weight, B, K, h, w, H, W, ignore_index, a);
 }
@@ -1797,7 +1644,8 @@ int ohem_make(const float* seg, const int64_t* target, const float* weight, int 
 }  // namespace
 
 extern "C" int64_t pcl_ohem_ce_scratch_bytes(int32_t B, int32_t K, int32_t h, int32_t w, int32_t Himg, int32_t Wimg) {
-  const int st = ohem_geometry(B, K, h, w, Himg, Wimg);
+  UpGeom g;
+  const int st = sort_geometry(B, K, h, w, Himg, Wimg, &g);
   if (st != PCL_OK) return st;
   return (int64_t)ohem_layout((int64_t)B * Himg * Wimg).total;
 }
@@ -1849,6 +1697,6 @@ extern "C" int pcl_ohem_ce_bwd(const float* seg, const int64_t* target, const fl
   PCL_REQUIRE(scratch && dseg);
   const OhemLayout l = ohem_layout((int64_t)B * Himg * Wimg);
   const char* sc = (const char*)scratch;
-  return segce_bwd_tile_launch<true>(a, (const float*)(sc + l.lse), (const float*)sc, grad_loss, dseg,
-                                     (const float*)(sc + l.p), (cudaStream_t)stream);
+  return up_bwd_launch<k_segce_bwd_tile<true>>(a, (cudaStream_t)stream, dseg, (const float*)(sc + l.lse),
+                                                (const float*)sc, grad_loss, (const float*)(sc + l.p));
 }

@@ -1,7 +1,8 @@
 // Tile geometry of the fused bilinear up-sampling kernels (F.interpolate(..., mode='bilinear', align_corners=True)),
-// shared by the seg CE and the RMI loss (both in pcl_segce.cu).  A CTA owns a BT x BTY tile of label pixels of one
-// image; the source logits the tile reads form a ys_n x xs_n patch starting at (ys_base, xs_base).  The backward maps a
-// per-pixel gradient G[class][row][col] of the tile through the transposed bilinear map into dseg (up_tile_flush).
+// shared by the seg CE, the RMI, the Lovasz-softmax and the OHEM CE losses (all in pcl_segce.cu).  A CTA owns a BT x BTY
+// tile of label pixels of one image; the source logits the tile reads form a ys_n x xs_n patch starting at
+// (ys_base, xs_base), staged per class chunk (up_stage).  The backward maps a per-pixel gradient G[class][row][col] of the
+// tile through the transposed bilinear map into dseg (up_tile_flush).
 #pragma once
 #include "pcl_common.cuh"
 
@@ -11,6 +12,25 @@ constexpr int BT = 32;                 // tile width  (label pixels)
 constexpr int BTY = 8;                 // tile height: 32 x 8 = 256 threads per CTA -> several CTAs per SM hide the
                                        // load latency of the bulk-synchronous phases (a 32 x 32 tile ran 1 CTA/SM)
 constexpr int SRC_MAX = 34;            // source cells per tile edge (scale >= 1: up to 32 + 2)
+constexpr int KC_FWD_MAX = 32;         // classes staged per forward pass (one pass for K <= 32: one exposed load latency)
+constexpr int KC_BWD_MAX = 24;         // classes per backward pass (one pass for K <= 24: fewer bulk-synchronous phases)
+
+// Logits (B, K, h, w) up-sampled to the label grid (B, H, W).
+struct UpGeom {
+  int B, K, h, w, H, W;
+  float ry, rx;                 // (h-1)/(H-1), (w-1)/(W-1)   (align_corners=True)
+};
+
+// PCL_ERR_ARG on a non-positive dimension; otherwise fills g.
+static inline int up_geometry(int B, int K, int h, int w, int H, int W, UpGeom* g) {
+  if (B <= 0 || K <= 0 || h <= 0 || w <= 0 || H <= 0 || W <= 0) return PCL_ERR_ARG;
+  g->B = B; g->K = K; g->h = h; g->w = w; g->H = H; g->W = W;
+  g->ry = H > 1 ? (float)(h - 1) / (float)(H - 1) : 0.f;
+  g->rx = W > 1 ? (float)(w - 1) / (float)(W - 1) : 0.f;
+  return PCL_OK;
+}
+
+static inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
 
 __device__ __forceinline__ void src_coord(int o, float r, int in_size, int& i0, int& i1, float& l1) {
   const float s = r * (float)o;                       // ATen area_pixel_compute_source_index, align_corners=True
@@ -46,6 +66,42 @@ __device__ __forceinline__ UpTile up_tile_coords(int X0, int Y0, int H, int W, i
   g.ys_base = s_y0[0]; g.xs_base = s_x0[0];
   g.ys_n = s_y1[g.ny - 1] - g.ys_base + 1; g.xs_n = s_x1[g.nx - 1] - g.xs_base + 1;
   return g;
+}
+
+// Bilinear weights and patch offsets of this thread's label pixel (column tx, row ty of the tile) in the staged patch
+struct UpPix {
+  float w00, w01, w10, w11;
+  int i00, i01, i10, i11;
+  float ly, lx;                        // the row / column weights the four above are built from
+};
+
+__device__ __forceinline__ UpPix up_pix(const UpTile& g, int tx, int ty, const int* s_y0, const int* s_y1,
+                                        const float* s_ly, const int* s_x0, const int* s_x1, const float* s_lx) {
+  UpPix p;
+  const int ly0 = s_y0[ty] - g.ys_base, ly1 = s_y1[ty] - g.ys_base, lx0 = s_x0[tx] - g.xs_base, lx1 = s_x1[tx] - g.xs_base;
+  const float ly = s_ly[ty], lx = s_lx[tx];
+  p.ly = ly; p.lx = lx;
+  p.w00 = (1.f - ly) * (1.f - lx); p.w01 = (1.f - ly) * lx; p.w10 = ly * (1.f - lx); p.w11 = ly * lx;
+  p.i00 = ly0 * g.xs_n + lx0; p.i01 = ly0 * g.xs_n + lx1; p.i10 = ly1 * g.xs_n + lx0; p.i11 = ly1 * g.xs_n + lx1;
+  return p;
+}
+
+// The up-sampled logit of the pixel from one staged class plane s
+__device__ __forceinline__ float up_logit(const UpPix& p, const float* s) {
+  return p.w00 * s[p.i00] + p.w01 * s[p.i01] + p.w10 * s[p.i10] + p.w11 * s[p.i11];
+}
+
+// Copies the ys_n x xs_n source patch at (ys_base, xs_base) of classes [c0, c0 + cn) of image b into S[cc][pitch], by
+// every thread of the 256-thread CTA.  The caller syncs before reading S.
+__device__ __forceinline__ void up_stage(const UpGeom& a, const float* seg, int b, int c0, int cn, int ys_base,
+                                         int xs_base, int ys_n, int xs_n, int pitch, float* S) {
+  const int patch = ys_n * xs_n;
+  const int64_t hw = (int64_t)a.h * a.w;
+  for (int i = threadIdx.x; i < cn * patch; i += BT * BTY) {
+    const int cc = i / patch, r = i - cc * patch;
+    const int yy = r / xs_n, xx = r - yy * xs_n;
+    S[cc * pitch + r] = seg[((int64_t)b * a.K + c0 + cc) * hw + (int64_t)(ys_base + yy) * a.w + xs_base + xx];
+  }
 }
 
 // The transposed bilinear map of the tile, once per CTA (it is the same for every class and row): weight of label
@@ -126,10 +182,26 @@ __device__ __forceinline__ void up_tile_flush(const UpTile& g, int cn, const flo
   }
 }
 
-// Upper bound of the source cells a BT x BTY label tile touches (ys_n * xs_n), + 1 to de-phase the class planes.
-static inline int up_patch_pitch(int h, int w, float ry, float rx) {
-  const int py = (int)((float)(BTY - 1) * ry) + 3, px = (int)((float)(BT - 1) * rx) + 3;
-  return (py < h + 1 ? py : h + 1) * (px < w + 1 ? px : w + 1) + 1;
+// Upper bound of the source cells a rows x cols block of label pixels touches (ys_n * xs_n), + 1 to de-phase the class
+// planes.
+static inline int up_patch_pitch(const UpGeom& a, int rows, int cols) {
+  const int py = (int)((float)(rows - 1) * a.ry) + 3, px = (int)((float)(cols - 1) * a.rx) + 3;
+  return (py < a.h + 1 ? py : a.h + 1) * (px < a.w + 1 ? px : a.w + 1) + 1;
+}
+
+// Forward launch plan: kc classes staged per pass (at most KC_FWD_MAX), fewer while the kc source patches of `pitch`
+// floats and `extra` bytes exceed 96 KB (two CTAs per SM).
+struct UpPlan {
+  int pitch, kc;
+  size_t smem;
+};
+
+static inline int up_fwd_plan(const UpGeom& a, int pitch, size_t extra, UpPlan* p) {
+  int kc = a.K < KC_FWD_MAX ? a.K : KC_FWD_MAX;
+  while (kc > 1 && extra + (size_t)kc * pitch * sizeof(float) > 96 * 1024) --kc;
+  p->pitch = pitch; p->kc = kc;
+  p->smem = extra + (size_t)kc * pitch * sizeof(float);
+  return p->smem > 200 * 1024 ? PCL_ERR_UNSUPPORTED : PCL_OK;
 }
 
 }  // namespace pcl

@@ -968,6 +968,37 @@ def infonce_tc_backward(state, rowstats: torch.Tensor, grad_loss: Optional[torch
 
 
 # ------------------------------------------------------------------------------------------------
+# Operands of the fused up-sampling segmentation losses below (seg CE, RMI, Lovasz, OHEM CE)
+# ------------------------------------------------------------------------------------------------
+def _seg_operands(seg, target, weight=None):
+    """(seg as contiguous fp32, target as contiguous int64 on seg's device, class weights as contiguous fp32 there or
+    None, (B, K, h, w, H, W))."""
+    _require_cuda(seg, "seg")
+    dev = seg.device
+    seg_c = seg if (seg.dtype == torch.float32 and seg.is_contiguous()) else seg.to(torch.float32).contiguous()
+    tgt = target
+    if tgt.device != dev or tgt.dtype != torch.int64 or not tgt.is_contiguous():
+        tgt = tgt.to(device=dev, dtype=torch.int64).contiguous()
+    wt = None if weight is None else weight.to(device=dev, dtype=torch.float32).contiguous()
+    B, K, h, w = seg_c.shape
+    return seg_c, tgt, wt, (B, K, h, w, tgt.shape[1], tgt.shape[2])
+
+
+def _byte_scratch(n: int, name: str, dev) -> torch.Tensor:
+    """The uint8 scratch of a *_scratch_bytes query; a negative n is the query's error code."""
+    if n < 0:
+        _abi.check(n, name)
+    return torch.empty(n, dtype=torch.uint8, device=dev)
+
+
+def _grad_scalar(grad_out: torch.Tensor, dev) -> torch.Tensor:
+    """The incoming loss gradient as a contiguous fp32 scalar on dev."""
+    if grad_out.device != dev or grad_out.dtype != torch.float32 or not grad_out.is_contiguous():
+        grad_out = grad_out.detach().to(device=dev, dtype=torch.float32).contiguous()
+    return grad_out
+
+
+# ------------------------------------------------------------------------------------------------
 # §8f row 1: fused bilinear up-sampling (align_corners=True) + weighted cross-entropy with ignore_index
 # (lib/loss/loss_contrast.py:180-181 + lib/loss/loss_helper.py:169-212)
 # ------------------------------------------------------------------------------------------------
@@ -975,17 +1006,8 @@ class _SegCeFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, seg, target, weight, ignore_index):
         lib = _abi.load()
-        _require_cuda(seg, "seg")
-        dev = seg.device
-        seg_c = seg if (seg.dtype == torch.float32 and seg.is_contiguous()) else seg.to(torch.float32).contiguous()
-        tgt = target
-        if tgt.device != dev or tgt.dtype != torch.int64 or not tgt.is_contiguous():
-            tgt = tgt.to(device=dev, dtype=torch.int64).contiguous()
-        B, K, h, w = seg_c.shape
-        H, W = tgt.shape[1], tgt.shape[2]
-        wt = None
-        if weight is not None:
-            wt = weight.to(device=dev, dtype=torch.float32).contiguous()
+        seg_c, tgt, wt, (B, K, h, w, H, W) = _seg_operands(seg, target, weight)
+        dev = seg_c.device
         scratch = torch.empty(lib.pcl_seg_ce_scratch_floats(B, H, W), dtype=torch.float32, device=dev)
         out = torch.empty((), dtype=torch.float32, device=dev)
         with _on_device(dev):
@@ -1002,9 +1024,7 @@ class _SegCeFn(torch.autograd.Function):
         seg_c, tgt, wt, scratch = ctx.keep
         B, K, h, w, H, W, ign = ctx.dims
         dev = seg_c.device
-        go = grad_out
-        if go.device != dev or go.dtype != torch.float32 or not go.is_contiguous():
-            go = go.detach().to(device=dev, dtype=torch.float32).contiguous()
+        go = _grad_scalar(grad_out, dev)
         dseg = torch.empty_like(seg_c)
         with _on_device(dev):
             _abi.check(lib.pcl_seg_ce_bwd(seg_c.data_ptr(), tgt.data_ptr(), _abi.ptr(wt), B, K, h, w, H, W, ign,
@@ -1030,18 +1050,10 @@ class _RmiFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, seg, target, params):
         lib = _abi.load()
-        _require_cuda(seg, "seg")
-        dev = seg.device
-        seg_c = seg if (seg.dtype == torch.float32 and seg.is_contiguous()) else seg.to(torch.float32).contiguous()
-        tgt = target
-        if tgt.device != dev or tgt.dtype != torch.int64 or not tgt.is_contiguous():
-            tgt = tgt.to(device=dev, dtype=torch.int64).contiguous()
-        B, K, h, w = seg_c.shape
-        H, W = tgt.shape[1], tgt.shape[2]
-        n = lib.pcl_rmi_scratch_bytes(B, K, h, w, H, W, params[0], params[1], params[2])
-        if n < 0:
-            _abi.check(n, "pcl_rmi_scratch_bytes")
-        scratch = torch.empty(n, dtype=torch.uint8, device=dev)
+        seg_c, tgt, _, (B, K, h, w, H, W) = _seg_operands(seg, target)
+        dev = seg_c.device
+        scratch = _byte_scratch(lib.pcl_rmi_scratch_bytes(B, K, h, w, H, W, params[0], params[1], params[2]),
+                                "pcl_rmi_scratch_bytes", dev)
         out = torch.empty((), dtype=torch.float32, device=dev)
         with _on_device(dev):
             _abi.check(lib.pcl_rmi_fwd(seg_c.data_ptr(), tgt.data_ptr(), B, K, h, w, H, W, *params, scratch.data_ptr(),
@@ -1058,9 +1070,7 @@ class _RmiFn(torch.autograd.Function):
         lib = _abi.load()
         seg_c, tgt, scratch = ctx.keep
         dev = seg_c.device
-        go = grad_out
-        if go.device != dev or go.dtype != torch.float32 or not go.is_contiguous():
-            go = go.detach().to(device=dev, dtype=torch.float32).contiguous()
+        go = _grad_scalar(grad_out, dev)
         dseg = torch.empty_like(seg_c)
         with _on_device(dev):
             _abi.check(lib.pcl_rmi_bwd(seg_c.data_ptr(), tgt.data_ptr(), *ctx.dims, *ctx.params, scratch.data_ptr(),
@@ -1095,18 +1105,9 @@ class _LovaszFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, seg, target, ignore_index):
         lib = _abi.load()
-        _require_cuda(seg, "seg")
-        dev = seg.device
-        seg_c = seg if (seg.dtype == torch.float32 and seg.is_contiguous()) else seg.to(torch.float32).contiguous()
-        tgt = target
-        if tgt.device != dev or tgt.dtype != torch.int64 or not tgt.is_contiguous():
-            tgt = tgt.to(device=dev, dtype=torch.int64).contiguous()
-        B, K, h, w = seg_c.shape
-        H, W = tgt.shape[1], tgt.shape[2]
-        n = lib.pcl_lovasz_scratch_bytes(B, K, h, w, H, W)
-        if n < 0:
-            _abi.check(n, "pcl_lovasz_scratch_bytes")
-        scratch = torch.empty(n, dtype=torch.uint8, device=dev)
+        seg_c, tgt, _, (B, K, h, w, H, W) = _seg_operands(seg, target)
+        dev = seg_c.device
+        scratch = _byte_scratch(lib.pcl_lovasz_scratch_bytes(B, K, h, w, H, W), "pcl_lovasz_scratch_bytes", dev)
         out = torch.empty((), dtype=torch.float32, device=dev)
         with _on_device(dev):
             _abi.check(lib.pcl_lovasz_fwd(seg_c.data_ptr(), tgt.data_ptr(), B, K, h, w, H, W, int(ignore_index),
@@ -1122,9 +1123,7 @@ class _LovaszFn(torch.autograd.Function):
         lib = _abi.load()
         seg_c, tgt, scratch = ctx.keep
         dev = seg_c.device
-        go = grad_out
-        if go.device != dev or go.dtype != torch.float32 or not go.is_contiguous():
-            go = go.detach().to(device=dev, dtype=torch.float32).contiguous()
+        go = _grad_scalar(grad_out, dev)
         dseg = torch.empty_like(seg_c)
         with _on_device(dev):
             _abi.check(lib.pcl_lovasz_bwd(seg_c.data_ptr(), tgt.data_ptr(), *ctx.dims, scratch.data_ptr(),
@@ -1157,19 +1156,9 @@ _OHEM_REDUCTIONS = {"mean": 0, "elementwise_mean": 0, "sum": 1}
 def _ohem_forward(seg, target, weight, ignore_index, thresh, min_kept, reduction):
     """Runs pcl_ohem_ce_fwd; returns (loss, the kept tensors, dims, scratch)."""
     lib = _abi.load()
-    _require_cuda(seg, "seg")
-    dev = seg.device
-    seg_c = seg if (seg.dtype == torch.float32 and seg.is_contiguous()) else seg.to(torch.float32).contiguous()
-    tgt = target
-    if tgt.device != dev or tgt.dtype != torch.int64 or not tgt.is_contiguous():
-        tgt = tgt.to(device=dev, dtype=torch.int64).contiguous()
-    wt = None if weight is None else weight.to(device=dev, dtype=torch.float32).contiguous()
-    B, K, h, w = seg_c.shape
-    H, W = tgt.shape[1], tgt.shape[2]
-    n = lib.pcl_ohem_ce_scratch_bytes(B, K, h, w, H, W)
-    if n < 0:
-        _abi.check(n, "pcl_ohem_ce_scratch_bytes")
-    scratch = torch.empty(n, dtype=torch.uint8, device=dev)
+    seg_c, tgt, wt, (B, K, h, w, H, W) = _seg_operands(seg, target, weight)
+    dev = seg_c.device
+    scratch = _byte_scratch(lib.pcl_ohem_ce_scratch_bytes(B, K, h, w, H, W), "pcl_ohem_ce_scratch_bytes", dev)
     out = torch.empty((), dtype=torch.float32, device=dev)
     dims = (B, K, h, w, H, W, int(ignore_index))
     with _on_device(dev):
@@ -1192,9 +1181,7 @@ class _OhemCeFn(torch.autograd.Function):
         lib = _abi.load()
         seg_c, tgt, wt, scratch = ctx.keep
         dev = seg_c.device
-        go = grad_out
-        if go.device != dev or go.dtype != torch.float32 or not go.is_contiguous():
-            go = go.detach().to(device=dev, dtype=torch.float32).contiguous()
+        go = _grad_scalar(grad_out, dev)
         dseg = torch.empty_like(seg_c)
         with _on_device(dev):
             _abi.check(lib.pcl_ohem_ce_bwd(seg_c.data_ptr(), tgt.data_ptr(), _abi.ptr(wt), *ctx.dims, scratch.data_ptr(),

@@ -1,9 +1,10 @@
 """Mutation check of the many-class tests (tests/test_emu_many_classes.py) on the CPU emulator.
 
-Each mutant changes ONE source text in a scratch copy of a kernel file (a class-chunk offset dropped from the seg-CE
-kernels, the K > 32 argmax turned into a last-maximum, the plan's shared-memory table bound raised past its size), is
-built for the emulator with tests/emu/build_emu.py and must make the emulated many-class tests fail or abort.  Nothing
-in the tree is modified.  The last mutant (the plan keeps 9 x 512 totals in its 4096-entry shared table) is caught by
+Each mutant changes ONE source text in a scratch copy of a kernel file or header (a class-chunk offset dropped from the
+seg-CE kernels or from the patch staging every up-sampling loss shares, the K > 32 argmax turned into a last-maximum, the
+plan's shared-memory table bound raised past its size), is built for the emulator with tests/emu/build_emu.py and must
+make the emulated many-class tests fail or abort.  A mutated header is written to the mutant's build directory, which
+comes first on the include path.  Nothing in the tree is modified.  The last mutant (the plan keeps 9 x 512 totals in its 4096-entry shared table) is caught by
 the emulator's index check of fixed-size __shared__ arrays (emu::SharedArray): the B = 9, K = 256 plan case aborts at
 the first write past the table.  Emulator only: a mutant is a deliberately wrong kernel and is never run on a GPU.
 
@@ -26,9 +27,8 @@ MUTANTS = [   # (name, source file, exact text, replacement, which occurrence)
      "((c0 + cc) == (int)t ? 1.f : 0.f)", "(cc == (int)t ? 1.f : 0.f)", 0),
     ("segce bwd tile: dseg flush without the chunk offset", "pcl_segce.cu",
      "dseg + ((int64_t)b * a.K + c0) * hw", "dseg + ((int64_t)b * a.K) * hw", 0),
-    ("segce fwd: staged load without the chunk offset", "pcl_segce.cu",
-     "sm[cc * pitch + r] = a.seg[((int64_t)b * a.K + c0 + cc) * hw", "sm[cc * pitch + r] = a.seg[((int64_t)b * a.K + cc) * hw",
-     0),
+    ("up_stage: staged load without the chunk offset", "pcl_upsample.cuh",
+     "S[cc * pitch + r] = seg[((int64_t)b * a.K + c0 + cc) * hw", "S[cc * pitch + r] = seg[((int64_t)b * a.K + cc) * hw", 0),
     ("select k_keys K > 32: last maximum wins", "pcl_select.cu",
      "if (v[u] > best) { best = v[u]; pred = c0 + u; }", "if (v[u] >= best) { best = v[u]; pred = c0 + u; }", 0),
     ("select fused tail: shared totals past the 4096-entry table", "pcl_select.cu",
@@ -38,17 +38,27 @@ NEW = os.path.join(ROOT, "tests", "test_emu_many_classes.py")
 EXISTING = [os.path.join(ROOT, "tests", "test_emu_kernels.py"), os.path.join(ROOT, "tests", "test_emu_fuzz.py")]
 
 
+def mutate(idx, text, needle, repl, occ):
+    assert text.count(needle) > occ, f"mutant {idx}: occurrence {occ} of the source text not found: {needle}"
+    at = -1
+    for _ in range(occ + 1):
+        at = text.index(needle, at + 1)
+    return text[:at] + repl + text[at + len(needle):]
+
+
 def build_mutant(idx, src, needle, repl, occ, out):
     os.makedirs(out, exist_ok=True)
+    for f in os.listdir(out):          # a header mutated by an earlier run must not shadow csrc/
+        if f.endswith(".cuh"):
+            os.remove(os.path.join(out, f))
+    if src.endswith(".cuh"):           # out comes first on the include path
+        with open(os.path.join(out, src), "w") as f:
+            f.write(mutate(idx, open(os.path.join(b.CSRC, src)).read(), needle, repl, occ))
     cpps = []
     for name in b.SOURCES:
         text = open(os.path.join(b.CSRC, name)).read()
         if name == src:
-            assert text.count(needle) > occ, f"mutant {idx}: occurrence {occ} of the source text not found: {needle}"
-            at = -1
-            for _ in range(occ + 1):
-                at = text.index(needle, at + 1)
-            text = text[:at] + repl + text[at + len(needle):]
+            text = mutate(idx, text, needle, repl, occ)
         p = os.path.join(out, name[:-3] + ".emu.cpp")
         with open(p, "w") as f:
             f.write(b.rewrite(text))
@@ -56,7 +66,7 @@ def build_mutant(idx, src, needle, repl, occ, out):
     cpps.append(os.path.join(b.HERE, "emu_tc_stubs.cpp"))
     lib = os.path.join(out, "libpcl_emu.so")
     subprocess.run(["g++", "-std=c++17", "-O1", "-fPIC", "-shared", "-ffp-contract=off", "-fno-strict-aliasing", "-w", "-Wno-psabi",
-                    "-I", os.path.join(b.HERE, "shim"), "-I", b.CSRC, "-I", os.path.join(b.ROOT, "include"), "-x", "c++"] + cpps +
+                    "-I", out, "-I", os.path.join(b.HERE, "shim"), "-I", b.CSRC, "-I", os.path.join(b.ROOT, "include"), "-x", "c++"] + cpps +
                    ["-o", lib], check=True)
     return lib
 
