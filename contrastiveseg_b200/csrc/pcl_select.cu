@@ -682,6 +682,8 @@ int pcl::scatter_rows(const pcl_geom* g, const int32_t* plan, const int32_t* anc
 static int check_geom(const pcl_geom* g) {
   if (!g) return PCL_ERR_ARG;
   if (g->B <= 0 || g->D <= 0 || g->h <= 0 || g->w <= 0 || g->Himg <= 0 || g->Wimg <= 0) return PCL_ERR_ARG;
+  // the widths the sweeps take: refused here, before the scan and the selection run, not after them
+  if (g->D % 32 != 0 || g->D > 256) return PCL_ERR_UNSUPPORTED;
   if (g->K <= 0 || g->K > PCL_MAX_CLASSES) return PCL_ERR_ARG;
   if (g->max_samples <= 0 || g->max_views <= 0) return PCL_ERR_ARG;
   if ((int64_t)g->B * g->K > (1 << 20)) return PCL_ERR_ARG;

@@ -189,7 +189,12 @@ def _get_workspace(device, key, geom, mode, bank_K, bank_M0, bank_M1) -> Contras
         if not ws.busy:
             _LAST_WS[device.index] = ws
             return ws
-    ws = ContrastWorkspace(device, geom, mode, bank_K, bank_M0, bank_M1)
+    try:
+        ws = ContrastWorkspace(device, geom, mode, bank_K, bank_M0, bank_M1)
+    except _abi.PclError:
+        if not lst:                      # a refused geometry leaves no cache entry behind
+            del _WS_CACHE[ck]
+        raise
     lst.append(ws)
     _LAST_WS[device.index] = ws
     return ws

@@ -66,7 +66,7 @@ uint64_t    pcl_launch_count(void);
  * Geometry of one loss call (host struct, passed by pointer).
  * ----------------------------------------------------------------------------------------------*/
 typedef struct {
-  int32_t B, D, h, w;          /* embedding (B,D,h,w) fp32 NCHW                                  */
+  int32_t B, D, h, w;          /* embedding (B,D,h,w) fp32 NCHW; D % 32 == 0 and D <= 256        */
   int32_t Himg, Wimg;          /* label map (B,Himg,Wimg) int64                                  */
   int32_t K;                   /* number of class ids, labels outside [0,K) count as ignored     */
   int32_t max_samples;         /* contrast.max_samples                                            */
