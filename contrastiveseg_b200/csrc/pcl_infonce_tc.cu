@@ -15,31 +15,21 @@
 #include "pcl_common.cuh"
 #include "pcl_sweep.cuh"
 #include "ptx_sm90.cuh"
+#include "pcl_wgmma.cuh"
 #include "pcl_topk.cuh"
-#include <stdlib.h>
 #include <mutex>
 
 namespace pcl {
-int tc_make_tmap(CUtensorMap* m, const void* base, uint64_t rows, uint32_t box_rows);
-int tc_make_tmap_cols(CUtensorMap* m, const void* base, uint64_t cols, uint64_t rows, uint32_t box_rows);
 namespace tc {
+using namespace cta;
 
 // Forward tile = 128 rows x 256 columns: each consumer warpgroup runs M64 x N256 x K16 wgmmas on its 64 rows, so both
 // read the same contrast box once per K step (the widest N wgmma has, the fewest operand bytes per MMA).
-constexpr int BM = 128, BN = 256, BK = 64, NKB = 4, DDIM = 256;
 constexpr int STAGES = 3;
-constexpr int A_KB_BYTES = BM * BK * 2;          // 16 KB
 constexpr int B_STAGE_BYTES = BN * BK * 2;       // 32 KB
-constexpr int WG_ROW_BYTES = 64 * 128;           // offset of warpgroup 1's 64 rows inside a [rows x 64] K-block
-constexpr int NUM_THREADS = 384;                 // warps 0-7: two consumer warpgroups, warps 8-11: producer warpgroup
-constexpr int PRODUCER_WARP = 8;                 // (its first warp issues the TMA loads)
-// Registers per thread after setmaxnreg: 2 x 128 x 232 + 128 x 40 fit the 64 K register file; the consumers hold the
-// wgmma accumulators (128 floats for an m64n256 tile).
-constexpr uint32_t CONSUMER_REGS = 232, PRODUCER_REGS = 40;
-constexpr int EPI_THREADS = 256;                 // the consumer warpgroups (named barrier 1; barriers 2, 3: one warpgroup)
 constexpr int CONSUMER_WARPS = 8;                // arrivals on an "empty" barrier: every consumer warp after its wgmma wait
 constexpr int SPITCH = 36;                       // staging row pitch in floats (32 columns + 4: conflict-free row reads)
-constexpr float LOG2E = 1.4426950408889634f, LN2 = 0.6931471805599453f;
+constexpr float LOG2E = 1.4426950408889634f;
 
 struct TcArgs {
   const int32_t* acls; const int32_t* diag; const int32_t* plan; const int32_t* ccls;
@@ -79,7 +69,7 @@ static inline void make_div(uint32_t d, uint32_t* mul, uint32_t* sh) {
 
 struct SmemLayout {
   uint8_t a[NKB * A_KB_BYTES];
-  uint8_t b[STAGES * B_STAGE_BYTES];
+  uint8_t c[STAGES * B_STAGE_BYTES];
   float stage[2][2][64][SPITCH];                 // [warpgroup][column half][row]: one 32-column chunk of each half
   uint64_t full[STAGES], empty[STAGES], a_full, a_empty;
   float comb[3][2][BM];
@@ -162,8 +152,6 @@ __device__ __forceinline__ void chunk_labels(const TcArgs& a, int base, bool en,
 enum { TC_NEG = 0, TC_POS = 1, TC_DUMP = 2,     // DUMP: raw logit tiles to global (descriptor self-test)
        TC_H1 = 3, TC_H2 = 4, TC_H3 = 5,         // a10: radix-select histogram sweeps (11 + 11 + 10 bits of the logit key)
        TC_NEGW = 6 };                           // a10: negative sum with the selection weights
-// modes that walk ALL columns persistently and (NEG, NEGW) leave a partial negative sum per (slot, row)
-#define TC_IS_NEGLIKE(M) ((M) == TC_NEG || (M) == TC_NEGW || (M) == TC_H1 || (M) == TC_H2 || (M) == TC_H3)
 
 // A segment = consecutive column tiles [ct0, ct1) of one row tile, whose partial row sums go to slot `slot`.
 struct Seg { int r, ct0, ct1, slot; };
@@ -196,27 +184,76 @@ struct SegWalker {
   }
 };
 
-// 2^x for x <= ~0 on the FMA/ALU pipes (Cody-Waite + degree-5 polynomial, max rel. error 2.3e-7): takes a share of
-// the exponentials off the 16/clk/SM MUFU pipe, which is co-critical with the tensor pipe in this kernel.
-__device__ __forceinline__ float exp2_poly(float x) {
-  x = fmaxf(x, -126.f);
-  const float t = x + 12582912.f;                  // 1.5 * 2^23: integer part lands in the low mantissa bits
-  const float f = x - (t - 12582912.f);            // f in [-0.5, 0.5]
-  float p = 0.0013266970636323094f;
-  p = fmaf(p, f, 0.009675459936261177f);
-  p = fmaf(p, f, 0.05550742521882057f);
-  p = fmaf(p, f, 0.24022121727466583f);
-  p = fmaf(p, f, 0.6931469440460205f);
-  p = fmaf(p, f, 1.0000001192092896f);
-  return __int_as_float(__float_as_int(p) + (__float_as_int(t) << 23));
+// Partial slots of the persistent NEG walk that can hold sums of one row tile: G CTAs walk the row_tiles x col_tiles
+// pairs in contiguous ranges of U = P / G >= 1 pairs, so a row tile's col_tiles pairs meet at most col_tiles / U + 2 CTAs.
+__host__ __device__ __forceinline__ long long neg_slot_bound(long long row_tiles, long long col_tiles, int grid) {
+  const long long P = row_tiles * col_tiles;
+  const long long U = P / (grid > 1 ? grid : 1);
+  return col_tiles / (U > 1 ? U : 1) + 2;
 }
 
+// Row prologue of the POS sweeps: the sum over negatives of `row` = fixed-order sum of the NEG sweep's partial slots
+// (unwritten slots hold 0) + the analytic zero tail of the flattened bank (Q3).  `publish`: the CTA of split 0 writes
+// (m, Neg) to the row statistics for the backward.
+__device__ __forceinline__ float pos_row_neg(const TcArgs& a, const float* partials, int A, int col_tiles, int row,
+                                             int rcls, float m2, bool publish, float* rowstats_out) {
+  const int64_t stride = (int64_t)a.slots * a.a_pad;
+  const int used = (int)min((long long)a.slots, neg_slot_bound((A + BM - 1) / BM, col_tiles, a.neg_grid));
+  float n = 0.f;
+#pragma unroll 8
+  for (int pslot = 0; pslot < used; ++pslot) n += __ldcg(partials + stride + (int64_t)pslot * a.a_pad + row);
+  if (a.tail_count > 0 && rcls != 0) {
+    // the zero tail takes part in the a10 selection with the key of +0.0
+    const float wt = a.tk_sel ? topk_weight(KEY_ZERO, a.tk_sel[row], __uint_as_float(a.tk_sel[a.a_rows + row])) : 1.f;
+    n += wt * (float)a.tail_count * ptx::ex2_approx(-m2);
+  }
+  if (publish && rowstats_out != nullptr) {
+    rowstats_out[row] = m2 * LN2;
+    rowstats_out[a.a_rows + row] = n;
+  }
+  return n;
+}
 
-template <int MODE, bool POLY>
+// Barriers of a ring pipeline (full / empty per stage, a_full / a_empty for the operand that stays), by one thread.
+template <int STAGES_, class Smem>
+__device__ __forceinline__ void init_ring_barriers(Smem& sm, const CUtensorMap* tm0, const CUtensorMap* tm1) {
+  ptx::prefetch_tmap(tm0);
+  ptx::prefetch_tmap(tm1);
+  for (int s = 0; s < STAGES_; ++s) { ptx::mbar_init(&sm.full[s], 1); ptx::mbar_init(&sm.empty[s], CONSUMER_WARPS); }
+  ptx::mbar_init(&sm.a_full, 1);
+  ptx::mbar_init(&sm.a_empty, CONSUMER_WARPS);
+  ptx::fence_barrier_init();
+}
+
+// The TMA producer of a ring pipeline, one work item with tiles [t0, t1) (t1 > t0): once the previous item's MMAs have
+// retired, the operand that stays (NKB boxes of FIXED_KB bytes from row `fixed_row`, into sm.a), then NKB boxes of
+// RING_KB bytes per tile of TILE_ROWS rows through the ring (sm.c).  `item` counts the items loaded so far.
+struct ProducerState { uint32_t stage = 0, phase = 0; int item = 0; };
+template <int STAGES_, int FIXED_KB, int RING_KB, int TILE_ROWS, class Smem>
+__device__ __forceinline__ void produce_item(Smem& sm, ProducerState& p, const CUtensorMap* tm_fixed,
+                                             const CUtensorMap* tm_ring, int fixed_row, int t0, int t1) {
+  if (p.item > 0) ptx::mbar_wait(&sm.a_empty, (p.item - 1) & 1);
+  ptx::mbar_arrive_expect_tx(&sm.a_full, NKB * FIXED_KB);
+  for (int kb = 0; kb < NKB; ++kb) ptx::tma_load_2d(sm.a + kb * FIXED_KB, tm_fixed, &sm.a_full, kb * BK, fixed_row);
+  for (int t = t0; t < t1; ++t) {
+    for (int kb = 0; kb < NKB; ++kb) {
+      ptx::mbar_wait(&sm.empty[p.stage], p.phase ^ 1);
+      ptx::mbar_arrive_expect_tx(&sm.full[p.stage], RING_KB);
+      ptx::tma_load_2d(sm.c + p.stage * RING_KB, tm_ring, &sm.full[p.stage], kb * BK, t * TILE_ROWS);
+      if (++p.stage == STAGES_) { p.stage = 0; p.phase ^= 1; }
+    }
+  }
+  ++p.item;
+}
+
+template <int MODE>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 k_tc_fwd(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, TcArgs a,
          float* __restrict__ partials, float* __restrict__ rowstats_out) {
   extern __shared__ uint8_t smem_raw[];
+  // Rounded through an integer, unlike aligned_smem: the staging buffer is then reached by generic loads and stores,
+  // and the NEG sweep at A = 65536 x N = 131072 ran 10.49 - 10.68 ms that way against 10.69 - 11.00 ms with LDS / STS
+  // (H100 SXM, 700 W).
   SmemLayout& sm = *reinterpret_cast<SmemLayout*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int A = a.plan ? min(a.plan[PCL_PLAN_A], a.a_rows) : a.a_rows;
@@ -306,14 +343,7 @@ k_tc_fwd(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtens
   }
 
   // ---- one-time setup ----
-  if (warp == PRODUCER_WARP && lane == 0) {
-    ptx::prefetch_tmap(&tmA);
-    ptx::prefetch_tmap(&tmB);
-    for (int s = 0; s < STAGES; ++s) { ptx::mbar_init(&sm.full[s], 1); ptx::mbar_init(&sm.empty[s], CONSUMER_WARPS); }
-    ptx::mbar_init(&sm.a_full, 1);
-    ptx::mbar_init(&sm.a_empty, CONSUMER_WARPS);
-    ptx::fence_barrier_init();
-  }
+  if (warp == PRODUCER_WARP && lane == 0) init_ring_barriers<STAGES>(sm, &tmA, &tmB);
   __syncthreads();
 
   if (warp >= PRODUCER_WARP) {
@@ -322,23 +352,9 @@ k_tc_fwd(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtens
     if (warp == PRODUCER_WARP && lane == 0) {
       SegWalker w = w0;
       Seg sg;
-      uint32_t stage = 0, phase = 0;
-      int seg_idx = 0;
-      while (w.next(sg)) {
-        if (sg.ct1 <= sg.ct0) continue;
-        if (seg_idx > 0) ptx::mbar_wait(&sm.a_empty, (seg_idx - 1) & 1);     // previous segment's MMAs retired
-        ptx::mbar_arrive_expect_tx(&sm.a_full, NKB * A_KB_BYTES);
-        for (int kb = 0; kb < NKB; ++kb) ptx::tma_load_2d(sm.a + kb * A_KB_BYTES, &tmA, &sm.a_full, kb * BK, sg.r * BM);
-        for (int ct = sg.ct0; ct < sg.ct1; ++ct) {
-          for (int kb = 0; kb < NKB; ++kb) {
-            ptx::mbar_wait(&sm.empty[stage], phase ^ 1);
-            ptx::mbar_arrive_expect_tx(&sm.full[stage], B_STAGE_BYTES);
-            ptx::tma_load_2d(sm.b + stage * B_STAGE_BYTES, &tmB, &sm.full[stage], kb * BK, ct * BN);
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
-          }
-        }
-        ++seg_idx;
-      }
+      ProducerState ps;
+      while (w.next(sg))
+        if (sg.ct1 > sg.ct0) produce_item<STAGES, A_KB_BYTES, B_STAGE_BYTES, BN>(sm, ps, &tmA, &tmB, sg.r * BM, sg.ct0, sg.ct1);
     }
   } else {
     // =========================== consumer warpgroups: wgmma + epilogue ===========================
@@ -346,7 +362,7 @@ k_tc_fwd(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtens
     const int g = threadIdx.x >> 7, t = threadIdx.x & 127;
     const int half = t >> 6;                          // which 128 columns of the 256-column tile
     const int r_in = g * 64 + (t & 63);
-    const uint32_t a_base = ptx::smem_u32(sm.a) + g * WG_ROW_BYTES, b_base = ptx::smem_u32(sm.b);
+    const uint32_t a_base = ptx::smem_u32(sm.a) + g * WG_ROW_BYTES, b_base = ptx::smem_u32(sm.c);
     Ring ring;
     SegWalker w = w0;
     Seg sg;
@@ -358,29 +374,7 @@ k_tc_fwd(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtens
       const int rdiag = valid ? (a.mode == 0 ? row : (a.diag ? a.diag[row] : -1)) : -1;
       const float m2 = valid ? a.row_m2[row] : 0.f;
       float neg_i = 1.f;
-      if (MODE == TC_POS) {
-        // Sum over negatives = fixed-order sum of the NEG sweep's partial slots (unwritten slots hold 0) + the analytic
-        // zero tail of the flattened bank (Q3).  The CTA of split 0 publishes (m, Neg) for the backward.
-        if (valid) {
-          const int64_t stride = (int64_t)a.slots * a.a_pad;
-          // a row tile is touched by at most T/U + 2 CTAs of the persistent NEG walk (U = pairs per CTA)
-          const long long Pn = (long long)((A + BM - 1) / BM) * T_all;
-          const long long Un = max(1LL, Pn / max(1, a.neg_grid));
-          const int used = (int)min((long long)a.slots, T_all / Un + 2);
-          float n = 0.f;
-          for (int pslot = 0; pslot < used; ++pslot) n += partials[stride + (int64_t)pslot * a.a_pad + row];
-          if (a.tail_count > 0 && rcls != 0) {
-            // the zero tail takes part in the a10 selection with the key of +0.0
-            const float wt = a.tk_sel ? topk_weight(KEY_ZERO, a.tk_sel[row], __uint_as_float(a.tk_sel[a.a_rows + row])) : 1.f;
-            n += wt * (float)a.tail_count * ptx::ex2_approx(-m2);
-          }
-          neg_i = n;
-          if (sg.slot == 0 && rowstats_out != nullptr) {
-            rowstats_out[row] = m2 * LN2;
-            rowstats_out[a.a_rows + row] = n;
-          }
-        }
-      }
+      if (MODE == TC_POS && valid) neg_i = pos_row_neg(a, partials, A, T_all, row, rcls, m2, sg.slot == 0, rowstats_out);
       // a10 selection state of this row: key prefix (H2, H3) / tau key and tie weight (NEGW)
       uint32_t tk_pref = TK_ALL;
       float tk_tw = 0.f;
@@ -475,8 +469,7 @@ k_tc_fwd(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtens
                   acc0 += ptx::ex2_approx(fmaf(__uint_as_float(v[j + 0]), a.k1, -m2));
                   acc1 += ptx::ex2_approx(fmaf(__uint_as_float(v[j + 1]), a.k1, -m2));
                   acc2 += ptx::ex2_approx(fmaf(__uint_as_float(v[j + 2]), a.k1, -m2));
-                  if (POLY) acc3 += exp2_poly(fmaf(__uint_as_float(v[j + 3]), a.k1, -m2));   // 1 in 4 off the MUFU pipe
-                  else      acc3 += ptx::ex2_approx(fmaf(__uint_as_float(v[j + 3]), a.k1, -m2));
+                  acc3 += ptx::ex2_approx(fmaf(__uint_as_float(v[j + 3]), a.k1, -m2));
                 }
               }
             } else {
@@ -628,7 +621,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
 k_tc_pos_t(const __grid_constant__ CUtensorMap tmA64, const __grid_constant__ CUtensorMap tmC128, TcArgs a,
            float* __restrict__ partials, float* __restrict__ rowstats_out) {
   extern __shared__ uint8_t smem_raw[];
-  SmemPosT& sm = *reinterpret_cast<SmemPosT*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  SmemPosT& sm = aligned_smem<SmemPosT>(smem_raw);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int A = a.plan ? min(a.plan[PCL_PLAN_A], a.a_rows) : a.a_rows;
   if (A <= 0) return;
@@ -668,12 +661,7 @@ k_tc_pos_t(const __grid_constant__ CUtensorMap tmA64, const __grid_constant__ CU
     int U = (P + (int)gridDim.x - 1) / (int)gridDim.x;
     const int u_slots = a.splits >= 2 ? (tmax + a.splits - 2) / (a.splits - 1) : max(P, 1);
     sm.U = max(1, max(U, u_slots));
-    ptx::prefetch_tmap(&tmA64);
-    ptx::prefetch_tmap(&tmC128);
-    for (int s = 0; s < PT_STAGES; ++s) { ptx::mbar_init(&sm.full[s], 1); ptx::mbar_init(&sm.empty[s], CONSUMER_WARPS); }
-    ptx::mbar_init(&sm.a_full, 1);
-    ptx::mbar_init(&sm.a_empty, CONSUMER_WARPS);
-    ptx::fence_barrier_init();
+    init_ring_barriers<PT_STAGES>(sm, &tmA64, &tmC128);
   }
   __syncthreads();
 
@@ -681,26 +669,12 @@ k_tc_pos_t(const __grid_constant__ CUtensorMap tmA64, const __grid_constant__ CU
     // =========================== TMA producer ===========================
     ptx::setmaxnreg_dec<PRODUCER_REGS>();
     if (warp == PRODUCER_WARP && lane == 0) {
-      uint32_t stage = 0, phase = 0;
-      int seq = 0;
+      ProducerState ps;
       PosWalk w;
       PosItem it;
       w.init(sm, blockIdx.x, gridDim.x);
-      while (w.next(sm, a, it)) {
-        if (it.t1 <= it.t0) continue;
-        if (seq > 0) ptx::mbar_wait(&sm.a_empty, (seq - 1) & 1);             // previous block's MMAs retired
-        ptx::mbar_arrive_expect_tx(&sm.a_full, NKB * PT_A_KB);
-        for (int kb = 0; kb < NKB; ++kb) ptx::tma_load_2d(sm.a + kb * PT_A_KB, &tmA64, &sm.a_full, kb * BK, it.r0);
-        for (int t = it.t0; t < it.t1; ++t) {
-          for (int kb = 0; kb < NKB; ++kb) {
-            ptx::mbar_wait(&sm.empty[stage], phase ^ 1);
-            ptx::mbar_arrive_expect_tx(&sm.full[stage], PT_C_KB);
-            ptx::tma_load_2d(sm.c + stage * PT_C_KB, &tmC128, &sm.full[stage], kb * BK, t * PT_BM);
-            if (++stage == PT_STAGES) { stage = 0; phase ^= 1; }
-          }
-        }
-        ++seq;
-      }
+      while (w.next(sm, a, it))
+        if (it.t1 > it.t0) produce_item<PT_STAGES, PT_A_KB, PT_C_KB, PT_BM>(sm, ps, &tmA64, &tmC128, it.r0, it.t0, it.t1);
     }
   } else {
     // =========================== consumer warpgroups: wgmma (M = 64 bank columns each, N = 64 anchors) + epilogue ====
@@ -723,21 +697,8 @@ k_tc_pos_t(const __grid_constant__ CUtensorMap tmA64, const __grid_constant__ CU
         if (et < it.nv && it.r0 + et < A) {
           const int row = it.r0 + et;
           const float m2 = a.row_m2[row];
-          const long long Pn = (long long)((A + BM - 1) / BM) * (long long)((a.n_cols + BN - 1) / BN);
-          const long long Un = max(1LL, Pn / max(1, a.neg_grid));
-          const int used = (int)min((long long)a.slots, (long long)((a.n_cols + BN - 1) / BN) / Un + 2);
-          float ng = 0.f;
-#pragma unroll 8
-          for (int pslot = 0; pslot < used; ++pslot) ng += __ldcg(partials + stride + (int64_t)pslot * a.a_pad + row);
-          const int rcls = a.acls[row];
-          if (a.tail_count > 0 && rcls != 0) {
-            const float wt = a.tk_sel ? topk_weight(KEY_ZERO, a.tk_sel[row], __uint_as_float(a.tk_sel[a.a_rows + row])) : 1.f;
-            ng += wt * (float)a.tail_count * ptx::ex2_approx(-m2);
-          }
-          if (it.split == 0 && rowstats_out != nullptr) {
-            rowstats_out[row] = m2 * LN2;
-            rowstats_out[a.a_rows + row] = ng;
-          }
+          const int col_tiles = (int)((a.n_cols + BN - 1) / BN);
+          const float ng = pos_row_neg(a, partials, A, col_tiles, row, a.acls[row], m2, it.split == 0, rowstats_out);
           pr = make_float4(m2, ng, __int_as_float(a.diag ? a.diag[row] : -1), 0.f);
         }
         sm.par[et] = pr;
@@ -842,17 +803,12 @@ struct TcBwdArgs {
   int nan_safe;
 };
 
-__device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
-  __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
-  return *reinterpret_cast<uint32_t*>(&v);
-}
-
 template <bool TOPK>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 k_tc_bwd(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmC, TcBwdArgs ba,
          float* __restrict__ dpartials) {
   extern __shared__ uint8_t smem_raw[];
-  SmemBwd& sm = *reinterpret_cast<SmemBwd*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  SmemBwd& sm = aligned_smem<SmemBwd>(smem_raw);
   const TcArgs& a = ba.t;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int A = a.plan ? min(a.plan[PCL_PLAN_A], a.a_rows) : a.a_rows;
@@ -1158,16 +1114,15 @@ static bool has_current_context() {
   return fn != nullptr && fn(&ctx) == CUDA_SUCCESS && ctx != nullptr;
 }
 
-// bf16 row-major (rows, cols) matrix (cols a multiple of 8), box = 64 columns (128 B) x box_rows, 128-byte swizzle, OOB
-// rows read as zero.  Encoding costs ~2 us of host time and the step re-uses the same few (pointer, shape, box) keys
-// every call, so a small read-mostly cache keeps them (a tensor map only describes addresses/shapes: no lifetime coupling).
+// Encoding a tensor map costs ~2 us of host time and the step re-uses the same few (pointer, shape, box) keys every
+// call, so a small read-mostly cache keeps them (a tensor map only describes addresses/shapes: no lifetime coupling).
 struct TmapKey { const void* base; uint64_t cols; uint64_t rows; uint32_t box_rows; };
 struct TmapEntry { TmapKey k; CUtensorMap m; bool used; };
 static TmapEntry g_tmaps[16];
 static unsigned g_tmap_next = 0;
 static std::mutex g_tmap_mu;
 
-static int make_tmap_cols(CUtensorMap* m, const void* base, uint64_t cols, uint64_t rows, uint32_t box_rows) {
+int pcl::tc_make_tmap(CUtensorMap* m, const void* base, uint64_t cols, uint64_t rows, uint32_t box_rows) {
   {
     std::lock_guard<std::mutex> lk(g_tmap_mu);
     for (auto& e : g_tmaps)
@@ -1205,31 +1160,11 @@ static int make_tmap_cols(CUtensorMap* m, const void* base, uint64_t cols, uint6
   return PCL_OK;
 }
 
-static int make_tmap(CUtensorMap* m, const void* base, uint64_t rows, uint32_t box_rows) {
-  return make_tmap_cols(m, base, tc::DDIM, rows, box_rows);
-}
-
-int pcl::tc_make_tmap(CUtensorMap* m, const void* base, uint64_t rows, uint32_t box_rows) {
-  return make_tmap(m, base, rows, box_rows);
-}
-int pcl::tc_make_tmap_cols(CUtensorMap* m, const void* base, uint64_t cols, uint64_t rows, uint32_t box_rows) {
-  return make_tmap_cols(m, base, cols, rows, box_rows);
-}
-
 struct TcPlan {
   tc::TcArgs a;
   SweepArgs sw;         // for the shared combine / finalize kernels
   int row_tiles, grid_persistent, splits_bwd;
 };
-
-// Tuning knobs for profiling runs (env PCL_TC_VARIANT, bit 0: polynomial exp2 for 1 in 4 logits, bit 1: 2-D grid
-// NEG sweep, bit 3: NEG sweep only, bit 4: row-tile POS sweep for small bank-mode anchor sets).  Default 0 = the
-// shipped configuration (all-MUFU exp2, persistent walk).
-static int tc_variant() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("PCL_TC_VARIANT"); v = e ? atoi(e) : 0; }
-  return v;
-}
 
 int pcl::num_sms() {
   static int cache[64] = {0};     // per device (a process may drive several GPUs)
@@ -1281,8 +1216,8 @@ static int make_tc_plan(const pcl_tc_desc* d, TcPlan* p) {
   const long long P = (long long)p->row_tiles * col_tiles;
   p->grid_persistent = (int)(P < sms ? P : sms);
   a.neg_grid = p->grid_persistent;
-  const long long U = P / p->grid_persistent;                      // pairs per CTA (floor, >= 1)
-  long long slots_neg = d->plan ? (long long)p->grid_persistent : (col_tiles / U + 2);   // live A unknown on the host
+  long long slots_neg = d->plan ? (long long)p->grid_persistent                            // live A unknown on the host
+                                : tc::neg_slot_bound(p->row_tiles, col_tiles, p->grid_persistent);
   if (slots_neg > p->grid_persistent) slots_neg = p->grid_persistent;
   if (slots_neg > col_tiles) slots_neg = col_tiles;
   if (slots_neg < 1) slots_neg = 1;
@@ -1337,6 +1272,29 @@ int pcl::tc_query(const pcl_tc_desc* d, int64_t* n_slot_rows, float* m2_scale) {
   return PCL_OK;
 }
 
+// The contrast operand of a descriptor as a tensor map of box_rows-row boxes: the anchors themselves in self-contrast
+// mode, else the bf16 contrast rows (as many as allocated, or the real columns).
+static int contrast_tmap(CUtensorMap* m, const pcl_tc_desc* d, const tc::TcArgs& a, uint32_t box_rows) {
+  if (d->mode == 0) return tc_make_tmap(m, d->anchors_bf16, tc::DDIM, (uint64_t)a.a_pad, box_rows);
+  return tc_make_tmap(m, d->contrast_bf16, tc::DDIM,
+                      (uint64_t)(d->contrast_rows_alloc > 0 ? d->contrast_rows_alloc : a.n_cols), box_rows);
+}
+
+// Set-up of the row-tile forward sweeps: with `prep`, the bf16 anchors (if fp32 given) and the row stabilisers row_m2
+// (contrast norm bound `cbound`), and the partial slots initialised when `partials` is given; then the tensor maps of the
+// anchor tiles and of the contrast tiles.
+static int fwd_setup(const pcl_tc_desc* d, const tc::TcArgs& a, bool prep, float cbound, float* row_m2, float* partials,
+                     cudaStream_t s, CUtensorMap* tmA, CUtensorMap* tmB) {
+  if (prep) {
+    tc::k_tc_prep<<<ceil_div(a.a_pad, 8), 256, 0, s>>>(d->anchors_f32, d->anchors_f32 ? (__nv_bfloat16*)d->anchors_bf16 : nullptr,
+                                                       (const __nv_bfloat16*)d->anchors_bf16, d->a_rows, a.a_pad, cbound,
+                                                       a.k1, row_m2, partials, (int64_t)a.slots * a.a_pad);
+    PCL_LAUNCH_CHECK();
+  }
+  const int st = tc_make_tmap(tmA, d->anchors_bf16, tc::DDIM, (uint64_t)a.a_pad, tc::BM);
+  return st != PCL_OK ? st : contrast_tmap(tmB, d, a, tc::BN);
+}
+
 extern "C" int pcl_infonce_tc_fwd(const pcl_tc_desc* d, float* row_m2, float* partials, float* rowstats, float* loss,
                                   void* stream) {
   return pcl::tc_fwd_ex(d, row_m2, partials, rowstats, loss, stream, false, nullptr);
@@ -1372,15 +1330,11 @@ int pcl::tc_fwd_topk_ex(const pcl_tc_desc* d, int k, uint32_t* scratch, float* r
   cudaStream_t s = (cudaStream_t)stream;
   tc::TcArgs& a = p.a;
   a.row_m2 = row_m2;
-  // 1. bf16 anchors (if fp32 given) + row stabilisers
+  // (the step path has the anchor selection kernel write row_m2 and initialise the partial slots: skip_prep)
   const float cbound = d->contrast_norm_bound > 0.f ? d->contrast_norm_bound : 1.0f;
-  const int64_t n_slot_rows = (int64_t)a.slots * a.a_pad;
-  if (!skip_prep) {       // (the step path has the anchor selection kernel write row_m2 and initialise the partial slots)
-    tc::k_tc_prep<<<ceil_div(a.a_pad, 8), 256, 0, s>>>(d->anchors_f32, d->anchors_f32 ? (__nv_bfloat16*)d->anchors_bf16 : nullptr,
-                                                       (const __nv_bfloat16*)d->anchors_bf16, d->a_rows, a.a_pad, cbound,
-                                                       a.k1, row_m2, partials, n_slot_rows);
-    PCL_LAUNCH_CHECK();
-  }
+  CUtensorMap tmA, tmB;
+  st = fwd_setup(d, a, !skip_prep, cbound, row_m2, partials, s, &tmA, &tmB);
+  if (st != PCL_OK) return st;
   if (d->mode == 2 && a.sorted) {
     int32_t* cls_start = reinterpret_cast<int32_t*>(row_m2 + a.a_pad);       // scratch tail: PCL_MAX_CLASSES + 1 ints
     tc::k_cls_bounds_init<<<2, 256, 0, s>>>(cls_start, (int)a.n_cols);
@@ -1389,24 +1343,15 @@ int pcl::tc_fwd_topk_ex(const pcl_tc_desc* d, int k, uint32_t* scratch, float* r
     PCL_LAUNCH_CHECK();
     a.cls_start = cls_start;
   }
-  // 2. tensor maps
-  CUtensorMap tmA, tmB;
-  st = make_tmap(&tmA, d->anchors_bf16, (uint64_t)a.a_pad, tc::BM);
-  if (st != PCL_OK) return st;
-  if (d->mode == 0) st = make_tmap(&tmB, d->anchors_bf16, (uint64_t)a.a_pad, tc::BN);
-  else st = make_tmap(&tmB, d->contrast_bf16, (uint64_t)(d->contrast_rows_alloc > 0 ? d->contrast_rows_alloc : a.n_cols), tc::BN);
-  if (st != PCL_OK) return st;
   const size_t smem = sizeof(tc::SmemLayout) + 1024;
-  PCL_SMEM_OPT_IN((tc::k_tc_fwd<tc::TC_NEG, true>), smem);
-  PCL_SMEM_OPT_IN((tc::k_tc_fwd<tc::TC_NEG, false>), smem);
-  PCL_SMEM_OPT_IN((tc::k_tc_fwd<tc::TC_POS, false>), smem);
-  dim3 grid(p.row_tiles, a.splits);
-  const int variant = tc_variant();
+  PCL_SMEM_OPT_IN(tc::k_tc_fwd<tc::TC_NEG>, smem);
+  PCL_SMEM_OPT_IN(tc::k_tc_fwd<tc::TC_POS>, smem);
+  a.persistent = 1;
   if (k >= 1) {
-    PCL_SMEM_OPT_IN((tc::k_tc_fwd<tc::TC_H1, false>), smem);
-    PCL_SMEM_OPT_IN((tc::k_tc_fwd<tc::TC_H2, false>), smem);
-    PCL_SMEM_OPT_IN((tc::k_tc_fwd<tc::TC_H3, false>), smem);
-    PCL_SMEM_OPT_IN((tc::k_tc_fwd<tc::TC_NEGW, false>), smem);
+    PCL_SMEM_OPT_IN(tc::k_tc_fwd<tc::TC_H1>, smem);
+    PCL_SMEM_OPT_IN(tc::k_tc_fwd<tc::TC_H2>, smem);
+    PCL_SMEM_OPT_IN(tc::k_tc_fwd<tc::TC_H3>, smem);
+    PCL_SMEM_OPT_IN(tc::k_tc_fwd<tc::TC_NEGW>, smem);
     TopkArgs tk;
     tk.k = k;
     tk.hist = scratch;
@@ -1415,45 +1360,38 @@ int pcl::tc_fwd_topk_ex(const pcl_tc_desc* d, int k, uint32_t* scratch, float* r
     a.tk_sel = tk.sel;
     PCL_CUDA(cudaMemsetAsync(tk.hist, 0, (size_t)a.a_pad * TK_BINS * sizeof(uint32_t), s));
     const int scan_blocks = ceil_div(d->a_rows, 8);          // 8 warps (rows) per 256-thread block
-    a.persistent = 1;
-    tc::k_tc_fwd<tc::TC_H1, false><<<p.grid_persistent, tc::NUM_THREADS, smem, s>>>(tmA, tmB, a, partials, nullptr);
+    tc::k_tc_fwd<tc::TC_H1><<<p.grid_persistent, tc::NUM_THREADS, smem, s>>>(tmA, tmB, a, partials, nullptr);
     PCL_LAUNCH_CHECK();
     k_topk_scan<1><<<scan_blocks, 256, 0, s>>>(p.sw, tk);
     PCL_LAUNCH_CHECK();
-    tc::k_tc_fwd<tc::TC_H2, false><<<p.grid_persistent, tc::NUM_THREADS, smem, s>>>(tmA, tmB, a, partials, nullptr);
+    tc::k_tc_fwd<tc::TC_H2><<<p.grid_persistent, tc::NUM_THREADS, smem, s>>>(tmA, tmB, a, partials, nullptr);
     PCL_LAUNCH_CHECK();
     k_topk_scan<2><<<scan_blocks, 256, 0, s>>>(p.sw, tk);
     PCL_LAUNCH_CHECK();
-    tc::k_tc_fwd<tc::TC_H3, false><<<p.grid_persistent, tc::NUM_THREADS, smem, s>>>(tmA, tmB, a, partials, nullptr);
+    tc::k_tc_fwd<tc::TC_H3><<<p.grid_persistent, tc::NUM_THREADS, smem, s>>>(tmA, tmB, a, partials, nullptr);
     PCL_LAUNCH_CHECK();
     k_topk_scan<3><<<scan_blocks, 256, 0, s>>>(p.sw, tk);
     PCL_LAUNCH_CHECK();
-    tc::k_tc_fwd<tc::TC_NEGW, false><<<p.grid_persistent, tc::NUM_THREADS, smem, s>>>(tmA, tmB, a, partials, nullptr);
-  } else if (variant & 2) {                            // tuning knob: 2-D grid instead of the persistent walk
-    a.persistent = 0;
-    if (variant & 1) tc::k_tc_fwd<tc::TC_NEG, true><<<grid, tc::NUM_THREADS, smem, s>>>(tmA, tmB, a, partials, nullptr);
-    else             tc::k_tc_fwd<tc::TC_NEG, false><<<grid, tc::NUM_THREADS, smem, s>>>(tmA, tmB, a, partials, nullptr);
+    tc::k_tc_fwd<tc::TC_NEGW><<<p.grid_persistent, tc::NUM_THREADS, smem, s>>>(tmA, tmB, a, partials, nullptr);
   } else {
-    a.persistent = 1;
-    if (variant & 1) tc::k_tc_fwd<tc::TC_NEG, true><<<p.grid_persistent, tc::NUM_THREADS, smem, s>>>(tmA, tmB, a, partials, nullptr);
-    else             tc::k_tc_fwd<tc::TC_NEG, false><<<p.grid_persistent, tc::NUM_THREADS, smem, s>>>(tmA, tmB, a, partials, nullptr);
+    tc::k_tc_fwd<tc::TC_NEG><<<p.grid_persistent, tc::NUM_THREADS, smem, s>>>(tmA, tmB, a, partials, nullptr);
   }
   PCL_LAUNCH_CHECK();
   a.persistent = 0;
-  if ((variant & 8) || d->neg_only) return PCL_OK;     // similarity + negative-sum sweep only (roofline measurement)
+  if (d->neg_only) return PCL_OK;     // similarity + negative-sum sweep only (roofline measurement)
   // (the NEG partials are combined by the POS sweep's row prologue: no separate pass)
-  if (d->mode == 1 && d->a_rows <= tc::PT_MAX_ROWS && !(variant & 16)) {
+  if (d->mode == 1 && d->a_rows <= tc::PT_MAX_ROWS) {
     // small anchor sets against the bank: the transposed POS sweep (work list by class, every epilogue lane busy)
     CUtensorMap tmA64, tmC128;
-    st = make_tmap(&tmA64, d->anchors_bf16, (uint64_t)a.a_pad, tc::PT_NB);
+    st = tc_make_tmap(&tmA64, d->anchors_bf16, tc::DDIM, (uint64_t)a.a_pad, tc::PT_NB);
     if (st != PCL_OK) return st;
-    st = make_tmap(&tmC128, d->contrast_bf16, (uint64_t)(d->contrast_rows_alloc > 0 ? d->contrast_rows_alloc : a.n_cols), tc::PT_BM);
+    st = contrast_tmap(&tmC128, d, a, tc::PT_BM);
     if (st != PCL_OK) return st;
     const size_t smem_pt = sizeof(tc::SmemPosT) + 1024;
     PCL_SMEM_OPT_IN(tc::k_tc_pos_t, smem_pt);
     tc::k_tc_pos_t<<<num_sms(), tc::NUM_THREADS, smem_pt, s>>>(tmA64, tmC128, a, partials, rowstats);
   } else {
-    tc::k_tc_fwd<tc::TC_POS, false><<<grid, tc::NUM_THREADS, smem, s>>>(tmA, tmB, a, partials, rowstats);
+    tc::k_tc_fwd<tc::TC_POS><<<dim3(p.row_tiles, a.splits), tc::NUM_THREADS, smem, s>>>(tmA, tmB, a, partials, rowstats);
   }
   PCL_LAUNCH_CHECK();
   k_finalize<<<1, 1024, 0, s>>>(p.sw, partials, rowstats, loss, step_counter);
@@ -1471,20 +1409,12 @@ extern "C" int pcl_tc_dump_logits(const pcl_tc_desc* d, float* row_m2, float* du
   cudaStream_t s = (cudaStream_t)stream;
   tc::TcArgs& a = p.a;
   a.row_m2 = row_m2;
-  tc::k_tc_prep<<<ceil_div(a.a_pad, 8), 256, 0, s>>>(d->anchors_f32, d->anchors_f32 ? (__nv_bfloat16*)d->anchors_bf16 : nullptr,
-                                                     (const __nv_bfloat16*)d->anchors_bf16, d->a_rows, a.a_pad, 1.f, a.k1,
-                                                     row_m2, nullptr, 0);
-  PCL_LAUNCH_CHECK();
   CUtensorMap tmA, tmB;
-  st = make_tmap(&tmA, d->anchors_bf16, (uint64_t)a.a_pad, tc::BM);
-  if (st != PCL_OK) return st;
-  if (d->mode == 0) st = make_tmap(&tmB, d->anchors_bf16, (uint64_t)a.a_pad, tc::BN);
-  else st = make_tmap(&tmB, d->contrast_bf16, (uint64_t)(d->contrast_rows_alloc > 0 ? d->contrast_rows_alloc : a.n_cols), tc::BN);
+  st = fwd_setup(d, a, true, 1.f, row_m2, nullptr, s, &tmA, &tmB);
   if (st != PCL_OK) return st;
   const size_t smem = sizeof(tc::SmemLayout) + 1024;
-  PCL_SMEM_OPT_IN((tc::k_tc_fwd<tc::TC_DUMP, false>), smem);
-  dim3 grid(p.row_tiles, a.splits);
-  tc::k_tc_fwd<tc::TC_DUMP, false><<<grid, tc::NUM_THREADS, smem, s>>>(tmA, tmB, a, dump, nullptr);
+  PCL_SMEM_OPT_IN(tc::k_tc_fwd<tc::TC_DUMP>, smem);
+  tc::k_tc_fwd<tc::TC_DUMP><<<dim3(p.row_tiles, a.splits), tc::NUM_THREADS, smem, s>>>(tmA, tmB, a, dump, nullptr);
   PCL_LAUNCH_CHECK();
   return PCL_OK;
 }
@@ -1521,10 +1451,9 @@ int pcl::tc_bwd_ex(const pcl_tc_desc* d, const float* row_m2, const float* rowst
   ba.t.splits = splits;
   p.sw.splits = splits;
   CUtensorMap tmA, tmC;
-  st = make_tmap(&tmA, d->anchors_bf16, (uint64_t)ba.t.a_pad, tc::BM);
+  st = tc_make_tmap(&tmA, d->anchors_bf16, tc::DDIM, (uint64_t)ba.t.a_pad, tc::BM);
   if (st != PCL_OK) return st;
-  if (d->mode == 0) st = make_tmap(&tmC, d->anchors_bf16, (uint64_t)ba.t.a_pad, tc::BNB);
-  else st = make_tmap(&tmC, d->contrast_bf16, (uint64_t)(d->contrast_rows_alloc > 0 ? d->contrast_rows_alloc : ba.t.n_cols), tc::BNB);
+  st = contrast_tmap(&tmC, d, ba.t, tc::BNB);
   if (st != PCL_OK) return st;
   const size_t smem = sizeof(tc::SmemBwd) + 1024;
   PCL_SMEM_OPT_IN((tc::k_tc_bwd<false>), smem);

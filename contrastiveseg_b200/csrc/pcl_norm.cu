@@ -8,6 +8,7 @@
 
 #include "pcl_common.cuh"
 #include "ptx_sm90.cuh"
+#include "pcl_wgmma.cuh"
 
 namespace pcl {
 
@@ -161,21 +162,6 @@ struct DgradBnSmem : DgradSmem {
   float bnred[2][NT / 32][DOUT];                 // per-warp channel sums of g_u and g_u x_hat, one 256-channel pass
 };
 static_assert(sizeof(DgradBnSmem) + 1024 <= 227 * 1024, "shared memory of one H100 block");
-
-template <class T>
-__device__ __forceinline__ T& aligned_smem(uint8_t* raw) {
-  return *reinterpret_cast<T*>(raw + ((1024u - (ptx::smem_u32(raw) & 1023u)) & 1023u));
-}
-
-__device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
-  __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
-  return *reinterpret_cast<uint32_t*>(&v);
-}
-
-__device__ __forceinline__ float quad_sum(float v) {
-  v += __shfl_xor_sync(0xffffffffu, v, 1);
-  return v + __shfl_xor_sync(0xffffffffu, v, 2);
-}
 
 // mbarrier wait without ptx::mbar_wait's timeout printf: a call in the kernel serialises every wgmma
 __device__ __forceinline__ void wait_full(uint64_t* bar, uint32_t parity) {
@@ -1011,8 +997,6 @@ __global__ void __launch_bounds__(GP_NT) k_conv1_gy_pack(const T* __restrict__ g
 
 using namespace pcl;
 
-namespace pcl { int tc_make_tmap_cols(CUtensorMap* m, const void* base, uint64_t cols, uint64_t rows, uint32_t box_rows); }
-
 extern "C" int64_t pcl_proj_workspace_bytes(int32_t B, int32_t Cin, int64_t HW, int32_t which) {
   if (!proj::shape_ok(B, Cin, HW) || (which != 0 && which != 1)) return PCL_ERR_ARG;
   const proj::Layout L = proj::layout(B, Cin, HW);
@@ -1037,7 +1021,7 @@ static int proj_fwd(const T* x, const void* wpack, const float* bias, int32_t B,
   PCL_REQUIRE(x && wpack && zn && inv_norm && proj::shape_ok(B, Cin, HW));
   const proj::Layout L = proj::layout(B, Cin, HW);
   CUtensorMap tmW;
-  int st = tc_make_tmap_cols(&tmW, wpack, (uint64_t)L.cin64, proj::DOUT, proj::DOUT);
+  int st = tc_make_tmap(&tmW, wpack, (uint64_t)L.cin64, proj::DOUT, proj::DOUT);
   if (st != PCL_OK) return st;
   proj::ArgsBn<proj::FwdArgs<T>, BN> a;
   a.x = x; a.bias = bias; a.zn = zn; a.inv_norm = inv_norm;
@@ -1071,7 +1055,7 @@ template <class T, bool BN>
 static int proj_wgrad(const __nv_bfloat16* gz, const T* x, int32_t B, int32_t Cin, int64_t HW, const proj::Layout& L,
                       float* part, int rows, float* gw, float* gb, proj::BnPro bn, cudaStream_t s) {
   CUtensorMap tmG;
-  const int st = tc_make_tmap_cols(&tmG, gz, (uint64_t)L.HWp, (uint64_t)B * proj::DOUT, 128);
+  const int st = tc_make_tmap(&tmG, gz, (uint64_t)L.HWp, (uint64_t)B * proj::DOUT, 128);
   if (st != PCL_OK) return st;
   proj::ArgsBn<proj::WgradArgs<T>, BN> w;
   w.x = x; w.partials = part; w.Cin = Cin; w.ldp = L.ldp; w.HW = HW; w.blk_per_img = L.blk_per_img;
@@ -1097,7 +1081,7 @@ static int proj_bwd(const T* x, const T* zn, const float* inv_norm, const T* gzn
   uint8_t* sc = (uint8_t*)scratch;
   __nv_bfloat16* gz = (__nv_bfloat16*)sc;
   CUtensorMap tmWt;
-  const int st = tc_make_tmap_cols(&tmWt, (const uint8_t*)wpack + L.wt_off, proj::DOUT, (uint64_t)L.cin256, proj::DOUT);
+  const int st = tc_make_tmap(&tmWt, (const uint8_t*)wpack + L.wt_off, proj::DOUT, (uint64_t)L.cin256, proj::DOUT);
   if (st != PCL_OK) return st;
 
   proj::ArgsBn<proj::DgradArgs<T>, BN> d;
@@ -1252,7 +1236,7 @@ static int conv1_gemm(const T* a, const void* wmat, const float* bias, int32_t B
                       double* part, cudaStream_t s) {
   const proj::Conv1Layout L = proj::conv1_layout(B, C, HW);
   CUtensorMap tmW;
-  int st = tc_make_tmap_cols(&tmW, wmat, (uint64_t)L.kp, (uint64_t)L.np, proj::DOUT);
+  int st = tc_make_tmap(&tmW, wmat, (uint64_t)L.kp, (uint64_t)L.np, proj::DOUT);
   if (st != PCL_OK) return st;
   proj::Conv1Args<T> g{a, bias, out, part, C, L.kp / proj::BK, L.nbands, L.np, HW, L.tiles_per_img};
   const size_t smem = sizeof(proj::FwdSmem) + 1024;

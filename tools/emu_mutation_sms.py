@@ -20,7 +20,8 @@ import build_emu as b  # noqa: E402
 TC, NORM = "pcl_infonce_tc.cu", "pcl_norm.cu"
 MUTANTS = [   # (name, source file, exact text, replacement)
     ("k_tc_fwd: no clamp of the grid to the live pairs", TC, "if (w0.G > w0.P) w0.G = (int)w0.P;", ""),
-    ("make_tc_plan: slots_neg without the + 2", TC, "(col_tiles / U + 2)", "(col_tiles / U)"),
+    ("neg_slot_bound: without the + 2 (host slots and POS prologues)", TC, "col_tiles / (U > 1 ? U : 1) + 2;",
+     "col_tiles / (U > 1 ? U : 1);"),
     ("make_tc_plan: splits not capped by col_tiles", TC, "  if (splits > col_tiles) splits = col_tiles;\n", ""),
     ("layout(): ctiles from Cin instead of Cin + 1", NORM, "L.ctiles = ceil_div(Cin + 1, DOUT);",
      "L.ctiles = ceil_div(Cin, DOUT);"),

@@ -1,6 +1,8 @@
-"""S4 sweep (BASELINE configs[4]): tcgen05 InfoNCE forward / backward throughput at anchor x bank sizes.
+"""S4 sweep (BASELINE configs[4]): tensor-core (wgmma) InfoNCE forward / backward throughput at anchor x bank sizes.
 Prints one JSON line per point: ms (CUDA events, median of iters after warm-up), algorithmic TFLOP/s
-(fwd 2*A*N*D; bwd 2*A*N*D, recompute not counted) and the fraction of the measured bf16 peak."""
+(fwd 2*A*N*D; bwd 2*A*N*D, recompute not counted) and the fraction of the measured bf16 peak.
+
+    python tools/sweep_bench.py [AxN ...] [--neg-only]     # --neg-only: similarity + negative-sum sweep, no backward"""
 import json
 import os
 import sys
@@ -19,8 +21,7 @@ points = [(1024, 190000), (4096, 32768), (16384, 65536), (65536, 131072)]
 args = [x for x in sys.argv[1:] if "x" in x]
 if args:
     points = [tuple(int(x) for x in p.split("x")) for p in args]
-variant = int(os.environ.get("PCL_TC_VARIANT", "0"))
-neg_only = bool(variant & 8)
+neg_only = "--neg-only" in sys.argv[1:]
 iters = 5
 
 
@@ -51,7 +52,7 @@ for A, N in points:
 
     def fwd():
         loss, st, state = Fn.infonce_tc_forward(a, ya, contrast_bf16=c16, contrast_cls=yc, n_cols=N, diag_col=diag,
-                                                temperature=0.07, base_temperature=0.07)
+                                                temperature=0.07, base_temperature=0.07, neg_only=neg_only)
         state_box["s"] = (loss, st, state)
 
     def bwd():
@@ -63,5 +64,5 @@ for A, N in points:
     fl = 2.0 * A * N * 256
     out = {"A": A, "N": N, "fwd_ms": t_f, "bwd_ms": t_b, "fwd_tflops": fl / t_f / 1e9, "bwd_tflops": fl / t_b / 1e9,
            "fwd_frac_of_measured_peak": fl / t_f / 1e9 / peaks["bf16_tflops"],
-           "bwd_frac_of_measured_peak": fl / t_b / 1e9 / peaks["bf16_tflops"], "loss": state_box["s"][0].item(), "variant": variant}
+           "bwd_frac_of_measured_peak": fl / t_b / 1e9 / peaks["bf16_tflops"], "loss": state_box["s"][0].item(), "neg_only": neg_only}
     print(json.dumps(out), flush=True)
