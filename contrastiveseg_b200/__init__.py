@@ -20,5 +20,6 @@ from .bank import MemoryBank, dequeue_and_enqueue, gather_packets      # noqa: F
 from .projection import ProjectionHead                                  # noqa: F401
 from .trainer_hook import ContrastTrainerHook, LossStepTimer            # noqa: F401
 from .graph_step import GraphedContrastStep                             # noqa: F401
+from .graph_criterion import GraphedContrastCriterion                   # noqa: F401
 
 __version__ = "0.1.0"

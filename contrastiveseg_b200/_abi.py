@@ -123,6 +123,8 @@ SIGNATURES = {
     "pcl_seg_ce_fwd": (c_i32, [c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_vp, c_vp, c_vp]),
     "pcl_seg_ce_bwd": (c_i32, [c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_vp, c_vp, c_vp,
                                c_vp]),
+    "pcl_seg_ce_fwd_bwd_scratch_floats": (c_i64, [c_i32] * 4),
+    "pcl_seg_ce_fwd_bwd": (c_i32, [c_vp, c_vp, c_vp] + [c_i32] * 7 + [c_vp, c_vp, c_vp, c_vp, c_vp]),
     "pcl_rmi_scratch_bytes": (c_i64, [c_i32] * 9),
     "pcl_rmi_fwd": (c_i32, [c_vp, c_vp] + [c_i32] * 9 + [c_f32, c_i32, c_f32, c_vp, c_vp, c_vp]),
     "pcl_rmi_bwd": (c_i32, [c_vp, c_vp] + [c_i32] * 9 + [c_f32, c_i32, c_f32, c_vp, c_vp, c_vp, c_vp]),

@@ -15,8 +15,12 @@
 //                geometries; the default up-sampling geometry runs k_segce_bwd_tile, which accumulates the source
 //                cells shared by up to 4 neighbouring tiles with fp32 global atomics: its dseg is reproducible only to
 //                the last ulp or two (summation order of <= 4 addends), which the parity tolerance (1e-5 max|g|) covers
+//   k_segce_fwd_bwd_tile  both in one tile pass, when the upstream gradient is a device scalar that exists before the
+//                pass (a captured terminal loss): the forward's lse and partials in the backward tile's pre, the unscaled
+//                gradient in its fill, then k_segce_finalize and k_segce_scale (dseg *= grad / sum(w))
 // HBM: reads seg (B*K*h*w*4) + labels (B*Himg*Wimg*8), writes lse (B*Himg*Wimg*4); backward re-reads them and writes
-// dseg.  Everything else stays in L1/L2 (a 4x4 block of label pixels shares its 4 source logits).
+// dseg (the one-pass form writes no lse and reads the labels once, then reads and writes dseg once more to scale it).
+// Everything else stays in L1/L2 (a 4x4 block of label pixels shares its 4 source logits).
 #include "pcl_upsample.cuh"
 #include <math_constants.h>
 
@@ -79,7 +83,9 @@ __device__ __forceinline__ int block_exclusive_scan_1024(int v, int* s_w) {
 //   pre(g, px, S)             once, after the tile tables (a pass over the classes that the chunks need first)
 //   per chunk: the source patch is staged; fill(c0, cn, px, S, G) writes G[cc][ty][tx], the gradient w.r.t. the
 //   (virtual) up-sampled logits of the chunk; the transposed bilinear map takes it into dseg (up_tile_flush)
-template <class Pre, class Fill>
+// PRE_STAGES: when one chunk holds every class (K <= kc), pre leaves that chunk staged in S and the loop does not stage
+// it again.
+template <bool PRE_STAGES = false, class Pre, class Fill>
 __device__ __forceinline__ void up_bwd_tile(const UpGeom& a, const float* seg, float* dseg, int kc, int pitch, Pre pre,
                                             Fill fill) {
   extern __shared__ float sm[];
@@ -100,8 +106,10 @@ __device__ __forceinline__ void up_bwd_tile(const UpGeom& a, const float* seg, f
   __syncthreads();
   for (int c0 = 0; c0 < a.K; c0 += kc) {
     const int cn = min(kc, a.K - c0);
-    up_stage(a, seg, b, c0, cn, g.ys_base, g.xs_base, g.ys_n, g.xs_n, pitch, S);
-    __syncthreads();
+    if (!PRE_STAGES || cn < a.K) {
+      up_stage(a, seg, b, c0, cn, g.ys_base, g.xs_base, g.ys_n, g.xs_n, pitch, S);
+      __syncthreads();
+    }
     fill(c0, cn, px, S, G);
     __syncthreads();
     up_tile_flush(g, cn, G, Hx, s_wx, s_wy, s_xlo, s_xhi, s_ylo, s_yhi, dseg + ((int64_t)b * a.K + c0) * hw, hw, a.w);
@@ -233,6 +241,90 @@ k_segce_bwd_tile(SegCeArgs a, const float* __restrict__ lse, const float* __rest
       G[((size_t)cc * BTY + ty) * BT + tx] = gv;
     }
   });
+}
+
+// Forward and backward in one tile pass (up_bwd_tile), for a caller whose upstream gradient is a device scalar that
+// exists when the pass runs (a captured terminal loss).  pre runs k_segce_fwd's online log-sum-exp over every class
+// (same class order, same up_logit, same __expf / __logf), so the lse, nll and w_t of every pixel and the per-CTA
+// partials, written in k_segce_fwd's order and layout, are its bits; fill writes the unscaled w_t * (softmax_c - [c == t]).
+// k_segce_finalize sums the partials and k_segce_scale applies grad / sum(w).  No per-pixel lse goes to HBM and the
+// labels are read once; at K <= kc the patch pre stages serves the fill too.
+__global__ void __launch_bounds__(BT * BTY, 4)     // 4 CTAs per SM: 64 registers
+k_segce_fwd_bwd_tile(SegCeArgs a, float* __restrict__ part_nll, float* __restrict__ part_w, float* __restrict__ dseg,
+                     int kc, int pitch) {
+  __shared__ float s_n[BT * BTY / 32], s_w[BT * BTY / 32];
+  const int tx = threadIdx.x & (BT - 1), ty = threadIdx.x >> 5;
+  const int b = blockIdx.z;
+  const int x = blockIdx.x * BT + tx, y = blockIdx.y * BTY + ty;
+  const int64_t HWo = (int64_t)a.H * a.W;
+  const bool inside = x < a.W && y < a.H;
+  int64_t t = -1;
+  if (inside) t = a.target[(int64_t)b * HWo + (int64_t)y * a.W + x];
+  float lse = 0.f, wt = 0.f;
+  up_bwd_tile<true>(a, a.seg, dseg, kc, pitch, [&](const UpTile& g, const UpPix& px, float* S) {
+    float m = -CUDART_INF_F, se = 0.f, vt = 0.f;
+    for (int c0 = 0; c0 < a.K; c0 += kc) {
+      const int cn = min(kc, a.K - c0);
+      if (c0 > 0) __syncthreads();                 // the previous chunk is read
+      up_stage(a, a.seg, b, c0, cn, g.ys_base, g.xs_base, g.ys_n, g.xs_n, pitch, S);
+      __syncthreads();
+      for (int cc = 0; cc < cn; ++cc) {
+        const float v = up_logit(px, S + cc * pitch);
+        if (v > m) { se = se * __expf(m - v) + 1.f; m = v; }     // online log-sum-exp
+        else       { se += __expf(v - m); }
+        if (c0 + cc == (int)t) vt = v;
+      }
+    }
+    float nll = 0.f;
+    bool counted = false;
+    if (inside) {
+      lse = m + __logf(se);
+      if (t != (int64_t)a.ignore_index && t >= 0 && t < a.K) {
+        const float wc = a.weight ? a.weight[t] : 1.f;
+        nll = wc * (lse - vt);
+        wt = wc;
+        counted = true;
+      }
+    }
+    if (!counted) t = -1;                          // no gradient
+    float an = warp_sum(nll), aw = warp_sum(wt);
+    if ((threadIdx.x & 31) == 0) { s_n[threadIdx.x >> 5] = an; s_w[threadIdx.x >> 5] = aw; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      an = 0.f; aw = 0.f;
+      for (int i = 0; i < BT * BTY / 32; ++i) { an += s_n[i]; aw += s_w[i]; }      // fixed order
+      const int64_t blk = ((int64_t)blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
+      part_nll[blk] = an;
+      part_w[blk] = aw;
+    }
+  }, [&](int c0, int cn, const UpPix& px, const float* S, float* G) {
+    for (int cc = 0; cc < cn; ++cc) {
+      float gv = 0.f;
+      if (t >= 0) {
+        const float v = up_logit(px, S + cc * pitch);
+        gv = wt * (__expf(v - lse) - ((c0 + cc) == (int)t ? 1.f : 0.f));
+      }
+      G[((size_t)cc * BTY + ty) * BT + tx] = gv;
+    }
+  });
+}
+
+// dseg *= grad / sum(w) after k_segce_fwd_bwd_tile.  Every pixel ignored (sum(w) == 0, the loss is NaN): dseg stays the
+// zeros the tile pass left, as the two-kernel backward leaves it (no 0 * inf).
+__global__ void __launch_bounds__(CE_THREADS)
+k_segce_scale(float* __restrict__ dseg, int64_t n, const float* __restrict__ fin, const float* __restrict__ grad_out) {
+  const float aw = fin[1];
+  if (aw == 0.f) return;
+  const float scale = (grad_out ? grad_out[0] : 1.f) / aw;
+  const int64_t stride = (int64_t)gridDim.x * CE_THREADS;
+  const int64_t n4 = (reinterpret_cast<uintptr_t>(dseg) & 15) ? 0 : n >> 2;    // float4 when 16-byte aligned
+  float4* d4 = reinterpret_cast<float4*>(dseg);
+  for (int64_t i = (int64_t)blockIdx.x * CE_THREADS + threadIdx.x; i < n4; i += stride) {
+    float4 v = d4[i];
+    v.x *= scale; v.y *= scale; v.z *= scale; v.w *= scale;
+    d4[i] = v;
+  }
+  for (int64_t i = 4 * n4 + (int64_t)blockIdx.x * CE_THREADS + threadIdx.x; i < n; i += stride) dseg[i] *= scale;
 }
 
 // General backward (any scale, e.g. label grid smaller than the logits): one thread per logit gathers over the label
@@ -379,6 +471,54 @@ extern "C" int pcl_seg_ce_bwd(const float* seg, const int64_t* target, const flo
     return PCL_OK;
   }
   return up_bwd_launch<k_segce_bwd_tile<false>>(a, s, dseg, lse, fin, grad_loss, (const float*)nullptr);
+}
+
+// One tile pass where one class chunk holds every class (K <= KC_BWD_MAX): the pass then stages the patch once instead of
+// twice and the labels and the lse stay out of HBM.  With several chunks both passes stage every chunk anyway, and the
+// scale pass over dseg made the one-pass form slower than the two kernels (DESIGN §4, ADE20K shape): pcl_seg_ce_fwd's
+// and pcl_seg_ce_bwd's kernels run there, with the lse in front of the partials in the scratch.
+static bool segce_one_pass(int K) { return K <= KC_BWD_MAX; }
+
+extern "C" int64_t pcl_seg_ce_fwd_bwd_scratch_floats(int32_t B, int32_t K, int32_t H, int32_t W) {
+  const int64_t blocks = (int64_t)ceil_div(H, BTY) * ceil_div(W, BT) * B;
+  return (segce_one_pass(K) ? 0 : (int64_t)B * H * W) + 2 * blocks + 2;     // [lse] | partial nll | partial w | fin
+}
+
+extern "C" int pcl_seg_ce_fwd_bwd(const float* seg, const int64_t* target, const float* class_weight, int32_t B,
+                                  int32_t K, int32_t h, int32_t w, int32_t H, int32_t W, int32_t ignore_index,
+                                  float* scratch, const float* grad_scale, float* loss, float* dseg, void* stream) {
+  SegCeArgs a;
+  int st = make_ce(seg, target, class_weight, B, K, h, w, H, W, ignore_index, &a);
+  if (st != PCL_OK) return st;
+  PCL_REQUIRE(scratch && loss && dseg);
+  if (H < h || W < w) return PCL_ERR_UNSUPPORTED;          // down-sampling: pcl_seg_ce_fwd + pcl_seg_ce_bwd
+  cudaStream_t s = (cudaStream_t)stream;
+  const int64_t blocks = (int64_t)ceil_div(H, BTY) * ceil_div(W, BT) * B;
+  const bool one = segce_one_pass(K);
+  float* lse = scratch;
+  float* pn = scratch + (one ? 0 : (int64_t)B * H * W);
+  float* pw = pn + blocks;
+  float* fin = pw + blocks;
+  if (!one) {
+    st = segce_fwd_launch<false>(a, lse, pn, pw, OhemPix{}, s);
+    if (st != PCL_OK) return st;
+    k_segce_finalize<<<1, 1024, 0, s>>>(pn, pw, blocks, fin);
+    PCL_LAUNCH_CHECK();
+    PCL_CUDA(cudaMemcpyAsync(loss, fin, sizeof(float), cudaMemcpyDeviceToDevice, s));
+    return up_bwd_launch<k_segce_bwd_tile<false>>(a, s, dseg, (const float*)lse, (const float*)fin, grad_scale,
+                                                  (const float*)nullptr);
+  }
+  st = up_bwd_launch<k_segce_fwd_bwd_tile>(a, s, dseg, pn, pw);
+  if (st != PCL_OK) return st;
+  k_segce_finalize<<<1, 1024, 0, s>>>(pn, pw, blocks, fin);
+  PCL_LAUNCH_CHECK();
+  const int64_t n = (int64_t)B * K * h * w;
+  const int64_t want = ceil_div64(ceil_div64(n, 4), CE_THREADS);
+  const int cap = 8 * num_sms();
+  k_segce_scale<<<(unsigned)(want < cap ? (want > 0 ? want : 1) : cap), CE_THREADS, 0, s>>>(dseg, n, fin, grad_scale);
+  PCL_LAUNCH_CHECK();
+  PCL_CUDA(cudaMemcpyAsync(loss, fin, sizeof(float), cudaMemcpyDeviceToDevice, s));
+  return PCL_OK;
 }
 
 // ==================================================================================================================

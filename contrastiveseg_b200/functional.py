@@ -1047,6 +1047,30 @@ def upsample_cross_entropy(seg: torch.Tensor, target: torch.Tensor, weight: Opti
     return _SegCeFn.apply(seg, target, weight, ignore_index)
 
 
+def seg_ce_loss_and_grad(seg: torch.Tensor, target: torch.Tensor, weight: Optional[torch.Tensor] = None,
+                         ignore_index: int = -1, grad_scale=None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """(loss, dseg) of upsample_cross_entropy in one tile pass (pcl_seg_ce_fwd_bwd), outside autograd, for tests and
+    tools: loss is the forward's to the bit, dseg = grad_scale * d loss / d seg (grad_scale: None for 1, a float, or a
+    device scalar read when the kernels run).  seg fp32, bf16 or fp16 (read as fp32); dseg comes back in seg's dtype.
+    Every pixel ignored gives a NaN loss and a zero dseg.  A label grid smaller than seg raises PclError."""
+    if seg.dim() != 4 or target.dim() != 3 or seg.shape[0] != target.shape[0]:
+        raise ValueError(f"seg (B,K,h,w) and target (B,H,W) expected, got {tuple(seg.shape)} and {tuple(target.shape)}")
+    lib = _abi.load()
+    seg_c, tgt, wt, (B, K, h, w, H, W) = _seg_operands(seg.detach(), target, weight)
+    dev = seg_c.device
+    gs = None
+    if grad_scale is not None:
+        gs = _grad_scalar(grad_scale if torch.is_tensor(grad_scale) else torch.tensor(float(grad_scale)), dev)
+    scratch = torch.empty(lib.pcl_seg_ce_fwd_bwd_scratch_floats(B, K, H, W), dtype=torch.float32, device=dev)
+    loss = torch.empty((), dtype=torch.float32, device=dev)
+    dseg = torch.empty_like(seg_c)
+    with _on_device(dev):
+        _abi.check(lib.pcl_seg_ce_fwd_bwd(seg_c.data_ptr(), tgt.data_ptr(), _abi.ptr(wt), B, K, h, w, H, W,
+                                          int(ignore_index), scratch.data_ptr(), _abi.ptr(gs), loss.data_ptr(),
+                                          dseg.data_ptr(), _stream_ptr(dev)), "pcl_seg_ce_fwd_bwd")
+    return loss, dseg.to(seg.dtype)
+
+
 # ------------------------------------------------------------------------------------------------
 # §8f row f5: fused bilinear up-sampling (align_corners=True) + RMI loss, sigmoid path
 # (lib/loss/rmi_loss.py:200-402 via lib/loss/loss_helper.py:316-369)

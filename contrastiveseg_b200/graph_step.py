@@ -31,7 +31,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
-from typing import Optional, Tuple
+from typing import Callable, Optional, Tuple
 
 import torch
 
@@ -71,11 +71,16 @@ class GraphedContrastStep:
                  pixel_queue: Optional[torch.Tensor] = None, bank_shadow: Optional[torch.Tensor] = None,
                  options: Optional[ContrastOptions] = None, grad_scale: float = 1.0, capture: bool = True,
                  warmup: int = 2, overlap_zero_fill: bool = True, enqueue: Optional[dict] = None,
-                 fused: Optional[bool] = None, sparse_reset: bool = False):
+                 fused: Optional[bool] = None, sparse_reset: bool = False,
+                 prologue: Optional[Callable[[int], None]] = None, epilogue: Optional[Callable[[int], None]] = None):
         """embed and seg may be fp32, bf16 or fp16 (each independently); ``grad`` has embed's dtype.
         enqueue (bank steps): dict(bank=MemoryBank, keys=(B,D,h,w) fp32/bf16/fp16 [default: embed], labels=(B,Himg,Wimg) int64
-        [default: labels], network_stride=int, pixel_update_freq=int, seed=int, group=process group or None)."""
+        [default: labels], network_stride=int, pixel_update_freq=int, seed=int, group=process group or None).
+        prologue / epilogue: work of the caller launched on the step's stream (its handle is the argument) before the
+        step's first kernel and after its last, captured into the first and the last graph (GraphedContrastCriterion's
+        seg half and total loss)."""
         self.lib = _abi.load()
+        self.prologue, self.epilogue = prologue, epilogue
         opts = options or ContrastOptions()
         _fn._require_cuda(embed, "embed")
         device = embed.device
@@ -257,6 +262,8 @@ class GraphedContrastStep:
     def _enqueue_a(self, stream: int) -> None:
         """First half: (zero-fill branch ||) stats -> forward -> this rank's enqueue packet."""
         lib, d = self.lib, self.ws.desc
+        if self.prologue is not None:
+            self.prologue(stream)
         if self.fused:
             early = bool(os.environ.get("PCL_FILL_FORK_EARLY")) and not self.sparse_reset      # tuning runs
             if early:
@@ -315,6 +322,8 @@ class GraphedContrastStep:
         self._enqueue_b(stream)
         if self._apply_separately:
             self._enqueue_apply(stream)
+        if self.epilogue is not None:
+            self.epilogue(stream)
 
     def _capture(self, warmup: int) -> None:
         dev = self.device
@@ -341,6 +350,8 @@ class GraphedContrastStep:
                 s = torch.cuda.current_stream(dev).cuda_stream
                 self._enqueue_a(s)
                 self._enqueue_b(s)
+                if self.epilogue is not None:
+                    self.epilogue(s)
             self.graph = graph
         else:
             graph_b = torch.cuda.CUDAGraph()
@@ -348,10 +359,14 @@ class GraphedContrastStep:
                 self._enqueue_a(torch.cuda.current_stream(dev).cuda_stream)
             with torch.cuda.device(dev), torch.cuda.graph(graph_b, stream=cap, capture_error_mode="thread_local"):
                 self._enqueue_b(torch.cuda.current_stream(dev).cuda_stream)
+                if self.epilogue is not None and not self._apply_separately:
+                    self.epilogue(torch.cuda.current_stream(dev).cuda_stream)
             if self._apply_separately:         # third graph: the bank write, after the all_gather that ran under graph_b
                 graph_c = torch.cuda.CUDAGraph()
                 with torch.cuda.device(dev), torch.cuda.graph(graph_c, stream=cap, capture_error_mode="thread_local"):
                     self._enqueue_apply(torch.cuda.current_stream(dev).cuda_stream)
+                    if self.epilogue is not None:
+                        self.epilogue(torch.cuda.current_stream(dev).cuda_stream)
                 self.graph_c = graph_c
                 self._gather_stream = torch.cuda.Stream(dev)
             self.graph, self.graph_b = graph, graph_b

@@ -12,7 +12,7 @@ extension, default off).
 """
 from __future__ import annotations
 
-from typing import Optional
+from typing import NamedTuple, Optional
 
 import torch
 import torch.nn as nn
@@ -21,6 +21,15 @@ import torch.nn.functional as F
 from .functional import ContrastOptions, pixel_contrast_loss, upsample_cross_entropy, upsample_lovasz_softmax
 from .loss_helper import (FSAuxCELoss, FSAuxOhemCELoss, FSAuxRMILoss, FSCELOVASZLoss, FSCELoss, FSOhemCELoss,
                           FSRMILoss)
+
+
+class SegTerm(NamedTuple):
+    """One engine term of a wrapper's seg loss: kind 'ce' (module: the nn.CrossEntropyLoss), 'rmi' (RMILoss), 'lovasz'
+    (FSCELOVASZLoss) or 'ohem' (FSOhemCELoss), on preds[head], entering the seg loss as coef * term (None: 1)."""
+    kind: str
+    head: str
+    module: nn.Module
+    coef: Optional[float]
 
 
 def _opt(configer, key, default):
@@ -121,10 +130,6 @@ class ContrastCELoss(nn.Module):
         # the seg criterion is the plain mean-reduced CE of the reference configs
         self.fused_seg_ce = bool(_opt(configer, "fused_seg_ce", True))
 
-    def _fused_ce(self, seg, target, ce_module):
-        ce = ce_module.ce_loss
-        return upsample_cross_entropy(seg, target, ce.weight, ce.ignore_index)
-
     def _can_fuse(self, ce_module, seg):
         return (self.fused_seg_ce and isinstance(ce_module, (FSCELoss, FSCELOVASZLoss)) and seg.is_cuda and
                 ce_module.ce_loss.reduction == "mean" and getattr(ce_module.ce_loss, "label_smoothing", 0.0) == 0.0)
@@ -147,28 +152,50 @@ class ContrastCELoss(nn.Module):
             return seg
         return F.interpolate(input=seg, size=(target.size(1), target.size(2)), mode="bilinear", align_corners=True)
 
+    def seg_terms(self, preds):
+        """The seg loss as engine terms, in launch order: [SegTerm(kind, head, module, coef)], the seg loss being the
+        sum of coef * term (coef None: the term itself).  None when part of it runs in torch (contrast.fused_seg_ce off,
+        a CE the kernels do not fuse, a custom seg_criterion).  The eager forward and GraphedContrastCriterion both run
+        what this returns."""
+        crit, seg = self.seg_criterion, preds["seg"]
+        if isinstance(crit, (FSRMILoss, FSOhemCELoss)):
+            if not self.fused_seg_ce:
+                return None
+            return [SegTerm("rmi", "seg", crit.rmi_loss, None) if isinstance(crit, FSRMILoss) else
+                    SegTerm("ohem", "seg", crit, None)]
+        if not (isinstance(crit, (FSCELoss, FSCELOVASZLoss)) and self._can_fuse(crit, seg)):
+            return None
+        if isinstance(crit, FSCELOVASZLoss):
+            return [SegTerm("ce", "seg", crit.ce_loss, None), SegTerm("lovasz", "seg", crit, None)]
+        return [SegTerm("ce", "seg", crit.ce_loss, None)]
+
+    def _run_seg_terms(self, preds, target, terms):
+        loss = None
+        for kind, head, mod, coef in terms:
+            x = preds[head]
+            if kind == "ce":
+                v = upsample_cross_entropy(x, target, mod.weight, mod.ignore_index)
+            elif kind == "lovasz":
+                v = upsample_lovasz_softmax(x, target, mod.ignore_index)
+            else:                                               # RMILoss, FSOhemCELoss
+                v = mod(x, target)
+            if coef is not None:
+                v = coef * v
+            loss = v if loss is None else loss + v
+        return loss
+
     def _seg_loss(self, preds, target):
+        terms = self.seg_terms(preds)
+        if terms is not None:
+            return self._run_seg_terms(preds, target, terms)
         if isinstance(self.seg_criterion, (FSRMILoss, FSOhemCELoss)):
             return self.seg_criterion(self._rmi_input(preds["seg"], target), target)
-        if isinstance(self.seg_criterion, FSCELOVASZLoss):
-            return self._lovasz_seg_loss(preds["seg"], target, self.seg_criterion)
-        if self._can_fuse(self.seg_criterion, preds["seg"]):
-            return self._fused_ce(preds["seg"], target, self.seg_criterion)
         h, w = target.size(1), target.size(2)
         pred = F.interpolate(input=preds["seg"], size=(h, w), mode="bilinear", align_corners=True)
+        if isinstance(self.seg_criterion, FSCELOVASZLoss):
+            return self.seg_criterion.ce_loss(pred, target) + upsample_lovasz_softmax(pred, target,
+                                                                                       self.seg_criterion.ignore_index)
         return self.seg_criterion(pred, target)
-
-    def _lovasz_seg_loss(self, seg, target, crit):
-        """CE + Lovasz of FSCELOVASZLoss on the up-sampled logits: the CE on the fused seg CE kernels when it can run
-        there, the Lovasz term on the fused up-sample + Lovasz kernels (F.interpolate first with fused_seg_ce off)."""
-        h, w = target.size(1), target.size(2)
-        up = None
-        if self._can_fuse(crit, seg):
-            ce = self._fused_ce(seg, target, crit)
-        else:
-            up = F.interpolate(input=seg, size=(h, w), mode="bilinear", align_corners=True)
-            ce = crit.ce_loss(up, target)
-        return ce + upsample_lovasz_softmax(seg if up is None else up, target, crit.ignore_index)
 
     def _queues(self, preds):
         return None
@@ -201,22 +228,33 @@ class ContrastAuxCELoss(ContrastCELoss):
     def _rmi_seg_criterion(configer):
         return FSAuxRMILoss(configer)
 
-    def _seg_loss(self, preds, target):
+    def seg_terms(self, preds):
         assert "seg_aux" in preds
         crit = self.seg_criterion
         if isinstance(crit, (FSAuxRMILoss, FSAuxOhemCELoss)):
+            if not self._can_fuse(crit.ce_loss, preds["seg_aux"]):
+                return None
             lw = crit.configer.get("network", "loss_weights")
-            if self._can_fuse(crit.ce_loss, preds["seg_aux"]):
-                aux = self._fused_ce(preds["seg_aux"], target, crit.ce_loss)
-            else:
-                aux = crit.ce_loss(F.interpolate(input=preds["seg_aux"], size=(target.size(1), target.size(2)),
-                                                 mode="bilinear", align_corners=True), target)
-            seg_term = crit.rmi_loss if isinstance(crit, FSAuxRMILoss) else crit.ohem_ce_loss
-            return lw["seg_loss"] * seg_term(self._rmi_input(preds["seg"], target), target) + lw["aux_loss"] * aux
+            head = (SegTerm("rmi", "seg", crit.rmi_loss, lw["seg_loss"]) if isinstance(crit, FSAuxRMILoss) else
+                    SegTerm("ohem", "seg", crit.ohem_ce_loss, lw["seg_loss"]))
+            return [SegTerm("ce", "seg_aux", crit.ce_loss.ce_loss, lw["aux_loss"]), head]
         if isinstance(crit, FSAuxCELoss) and self._can_fuse(crit.ce_loss, preds["seg"]):
             lw = crit.configer.get("network", "loss_weights")
-            return (lw["seg_loss"] * self._fused_ce(preds["seg"], target, crit.ce_loss) +
-                    lw["aux_loss"] * self._fused_ce(preds["seg_aux"], target, crit.ce_loss))
+            return [SegTerm("ce", "seg", crit.ce_loss.ce_loss, lw["seg_loss"]),
+                    SegTerm("ce", "seg_aux", crit.ce_loss.ce_loss, lw["aux_loss"])]
+        return None
+
+    def _seg_loss(self, preds, target):
+        terms = self.seg_terms(preds)
+        if terms is not None:
+            return self._run_seg_terms(preds, target, terms)
+        crit = self.seg_criterion
+        if isinstance(crit, (FSAuxRMILoss, FSAuxOhemCELoss)):
+            lw = crit.configer.get("network", "loss_weights")
+            aux = crit.ce_loss(F.interpolate(input=preds["seg_aux"], size=(target.size(1), target.size(2)),
+                                             mode="bilinear", align_corners=True), target)
+            seg_term = crit.rmi_loss if isinstance(crit, FSAuxRMILoss) else crit.ohem_ce_loss
+            return lw["seg_loss"] * seg_term(self._rmi_input(preds["seg"], target), target) + lw["aux_loss"] * aux
         h, w = target.size(1), target.size(2)
         pred = F.interpolate(input=preds["seg"], size=(h, w), mode="bilinear", align_corners=True)
         pred_aux = F.interpolate(input=preds["seg_aux"], size=(h, w), mode="bilinear", align_corners=True)

@@ -295,6 +295,18 @@ int pcl_seg_ce_fwd(const float* seg, const int64_t* target, const float* class_w
 int pcl_seg_ce_bwd(const float* seg, const int64_t* target, const float* class_weight, int32_t B, int32_t K, int32_t h,
                    int32_t w, int32_t Himg, int32_t Wimg, int32_t ignore_index, const float* scratch,
                    const float* grad_loss, float* dseg, void* stream);
+/* The same forward and backward in one call, for a terminal loss whose upstream gradient is a device scalar that exists
+ * when the call runs (a captured criterion): replaces the same lines (loss_contrast.py:180-181 + loss_helper.py:169-212
+ * and their autograd backward).  With K <= 24 (one class chunk of the backward tile) it is one tile pass that keeps no
+ * per-pixel log-sum-exp between forward and backward, stages the logit patch once and reads the labels once; with more
+ * classes it runs the kernels of pcl_seg_ce_fwd and pcl_seg_ce_bwd.  loss (1 float) is pcl_seg_ce_fwd's to the bit;
+ * dseg = grad_scale[0] (1 when NULL) * d loss / d seg, pcl_seg_ce_bwd's to the last ulp or two (fp32 atomics in both).
+ * Every pixel ignored: loss NaN, dseg zero.  A label grid smaller than the logits (Himg < h or Wimg < w):
+ * PCL_ERR_UNSUPPORTED.  scratch: pcl_seg_ce_fwd_bwd_scratch_floats floats. */
+int64_t pcl_seg_ce_fwd_bwd_scratch_floats(int32_t B, int32_t K, int32_t Himg, int32_t Wimg);
+int pcl_seg_ce_fwd_bwd(const float* seg, const int64_t* target, const float* class_weight, int32_t B, int32_t K,
+                       int32_t h, int32_t w, int32_t Himg, int32_t Wimg, int32_t ignore_index, float* scratch,
+                       const float* grad_scale, float* loss, float* dseg, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * §8f row f5: the RMI segmentation loss of the contrast wrappers with contrast.use_rmi, fused.  Replaces
