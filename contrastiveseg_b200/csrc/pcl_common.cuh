@@ -58,12 +58,26 @@ static inline size_t dtype_size(int dt) { return dt == PCL_DT_F32 ? sizeof(float
 
 // internal (not part of the C ABI): fused variants used by pcl_step_forward / pcl_step_backward.  `embed_dtype` /
 // `seg_dtype` / `grad_dtype`: element type of embed and grad_clear / seg / grad_embed (PCL_DT_*).
-int select_gather_ex(const pcl_geom* g, const void* embed, const uint16_t* keys, const int32_t* chunk_pref,
-                     const int32_t* plan, const int32_t* ranks, uint64_t seed, int normalize, int32_t* anchor_meta,
-                     float* anchors_f32, void* anchors_bf16, float* inv_norm, float* norm_max, float* row_m2,
-                     float m2_scale, float* partials, int64_t n_slot_rows, void* stream,
-                     const unsigned long long* seed_ctr = nullptr, unsigned int* dbg = nullptr,
-                     const int32_t* prev_rows = nullptr, void* grad_clear = nullptr, int embed_dtype = PCL_DT_F32);
+
+// Arguments of the selection kernel (pcl_select_gather): the stabiliser and slot initialisation of the tensor path
+// (row_m2 .. n_slot_rows), the captured step's counter and timeline (seed_ctr, dbg) and the sparse reset (prev_rows,
+// grad_clear) are optional.
+struct select_args {
+  const pcl_geom* g;
+  const void* embed;
+  int embed_dtype, normalize;
+  uint64_t seed;
+  const uint16_t* keys;
+  const int32_t *chunk_pref, *plan, *ranks, *prev_rows;
+  int32_t* anchor_meta;
+  float *anchors_f32, *inv_norm, *norm_max, *row_m2, *partials;
+  void *anchors_bf16, *grad_clear;
+  float m2_scale;
+  int64_t n_slot_rows;
+  const unsigned long long* seed_ctr;
+  unsigned int* dbg;
+};
+int select_gather(const select_args& a, void* stream);
 int tc_fwd_ex(const pcl_tc_desc* d, float* row_m2, float* partials, float* rowstats, float* loss, void* stream,
               bool skip_prep, unsigned long long* step_counter = nullptr);
 int simt_fwd_ex(const pcl_sweep_desc* d, int k, uint32_t* scratch, float* partials, float* rowstats, float* loss,
@@ -75,27 +89,32 @@ int tc_fwd_topk_ex(const pcl_tc_desc* d, int k, uint32_t* scratch, float* row_m2
 int tc_query(const pcl_tc_desc* d, int64_t* n_slot_rows, float* m2_scale);
 int tc_bwd_ex(const pcl_tc_desc* d, const float* row_m2, const float* rowstats, const float* grad_loss, float* dpartials,
               float* dA, void* stream, int* splits_out, int* a_pad_out, const uint32_t* topk_scratch = nullptr);
-int zero_scatter_reduce(const pcl_geom* g, const int32_t* plan, const int32_t* anchor_meta, const float* dpartials,
-                        int splits, int a_pad, float inv_T, const float* grad_loss, void* grad_embed, void* stream,
-                        int grad_dtype = PCL_DT_F32);
 
 int self_fused_supported(const pcl_tc_desc* d);
+// layout of the fused kernel's partial gradient rows, dpartials [splits][a_pad][256]: split p holds the contrast
+// columns [p * split_cols, (p + 1) * split_cols)
+void self_fused_splits(int a_rows, int* a_pad, int* splits, int* split_cols);
 int self_fused(const pcl_tc_desc* d, const float* row_m2, float* partials, float* rowstats, float* loss, float* dpartials,
                unsigned int* sync, void* stream);
 int class_stats(const pcl_geom* g, const int64_t* labels, const void* seg, const int64_t* predict, uint16_t* keys,
-                int32_t* chunk_pref, int32_t* counts, void* stream, int seg_dtype);
-int class_stats_plan(const pcl_geom* g, const int64_t* labels, const void* seg, const int64_t* predict, uint16_t* keys,
-                     int32_t* chunk_pref, int32_t* counts, int32_t* plan, unsigned int* done_ctr, void* stream,
-                     int seg_dtype = PCL_DT_F32);
-int scatter_reduce_rows(const pcl_geom* g, const int32_t* plan, const int32_t* anchor_meta, const float* dpartials, int splits,
-                        int split_cols, int a_pad, float inv_T, const float* grad_scale, void* grad_embed, unsigned long long* step_counter,
-                        void* stream, unsigned int* dbg = nullptr, int32_t* prev_rows = nullptr, int grad_dtype = PCL_DT_F32);
+                int32_t* chunk_pref, int32_t* counts, int32_t* plan, unsigned int* done_ctr, void* stream, int seg_dtype);
 int fill_zero(void* ptr, uint64_t bytes, void* stream, unsigned int* dbg, int reserve_sms);
-int scatter_rows(const pcl_geom* g, const int32_t* plan, const int32_t* anchor_meta, const float* dA,
-                 const float* anchors_f32, const float* inv_norm, int normalize, void* grad_embed, void* stream,
-                 int grad_dtype = PCL_DT_F32);
-int scatter_grad(const pcl_geom* g, const int32_t* plan, const int32_t* anchor_meta, const float* dA, const float* anchors_f32,
-                 const float* inv_norm, int normalize, void* grad_embed, void* stream, int grad_dtype);
+
+// Where the dense gradient's anchor rows come from: the (A, D) matrix dA (with the projection of the L2 normalise when
+// `normalize`: anchors_f32, inv_norm), or, when dpartials is set, the backward sweep's per-split partial rows (dpartials
+// [splits][a_pad][D]; split_cols > 0: split p covers the contrast columns [p * split_cols, (p + 1) * split_cols) and only
+// the live ones were written), summed in fixed order and scaled by inv_T * grad_scale[0].
+struct grad_rows {
+  const float *dA, *anchors_f32, *inv_norm, *dpartials, *grad_scale;
+  int normalize, splits, split_cols, a_pad;
+  float inv_T;
+};
+// Writes the dense (B, D, h, w) gradient; `zeroed`: the caller has zero-filled it already.  The captured fused step's
+// extras (dbg: its timeline, step_counter, prev_rows: what the next step's sparse reset clears) serve partial rows into a
+// zeroed buffer.
+int dense_grad(const pcl_geom* g, const int32_t* plan, const int32_t* anchor_meta, const grad_rows& r, bool zeroed,
+               void* grad_embed, int grad_dtype, void* stream, unsigned int* dbg = nullptr,
+               unsigned long long* step_counter = nullptr, int32_t* prev_rows = nullptr);
 
 // ---- per-device kernel attributes ----------------------------------------------------------------
 // cudaFuncAttributeMaxDynamicSharedMemorySize is a property of (function, device) and SETS the limit (a later call with

@@ -7,10 +7,9 @@
 //   k_plan    class filter, TC, V, hard/easy split, class-sorted row layout (one block, integer only)
 //   k_select  one warp per anchor: rank -> pixel (chunk prefix search + in-chunk ordered scan), gather
 //             of the pixel's D channels from NCHW, optional L2-normalise, fp32 + bf16 rows
-//   k_scatter dense-gradient writer (after a memset): one warp per anchor row
+//   k_zero_scatter, k_scatter_reduce, k_scatter   the dense-gradient writers (dense_grad picks one)
 #include "pcl_common.cuh"
 #include <math_constants.h>
-#include <stdlib.h>
 
 namespace pcl {
 
@@ -472,63 +471,63 @@ k_scatter(pcl_geom g, const int32_t* __restrict__ plan, const int32_t* __restric
 }
 
 // ------------------------------------------------------------------------------------------------
+// Anchor rows of the dense gradient: the (A, D) matrix dA, or (step path: the matrix is never written) the backward
+// sweep's per-split partial rows, value = scale * sum_p dpartials[p][s][d].
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ float split_sum(const float* dpartials, int splits, int a_pad, int D, int s, int d) {
+  float v = 0.f;
+  for (int p = 0; p < splits; ++p) v += __ldg(dpartials + ((int64_t)p * a_pad + s) * D + d);     // fixed order
+  return v;
+}
+
+struct DaRows {                      // dA's value as it is: a zero-gradient row may hold -0, which 0.f + x would lose
+  const float* dA;
+  __device__ float scale() const { return 1.f; }
+  __device__ float at(int s, int d, int D, float) const { return __ldg(dA + (int64_t)s * D + d); }
+};
+
+struct SplitRows {
+  const float* dpartials;
+  int splits, a_pad;
+  float inv_T;
+  const float* grad_scale;           // device scalar (captured steps rescale it between replays), null = 1
+  __device__ float scale() const { return inv_T * (grad_scale ? __ldg(grad_scale) : 1.f); }
+  __device__ float at(int s, int d, int D, float scale) const { return split_sum(dpartials, splits, a_pad, D, s, d) * scale; }
+};
+
+// Zero-fills one (image, channel) plane of HW elements, with 16-byte stores when the plane allows them.
+template <typename T>
+__device__ __forceinline__ void zero_plane(T* dst, int64_t HW) {
+  constexpr int E = 16 / sizeof(T);                // elements per 16-byte store
+  if (HW % E == 0) {
+    uint4* d4 = reinterpret_cast<uint4*>(dst);
+    const uint4 z = make_uint4(0u, 0u, 0u, 0u);
+    for (int64_t i = threadIdx.x; i < HW / E; i += blockDim.x) d4[i] = z;
+  } else {
+    for (int64_t i = threadIdx.x; i < HW; i += blockDim.x) dst[i] = from_f32<T>(0.f);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // k_zero_scatter: the dense gradient in ONE pass — each CTA owns one (image, channel) plane of h*w floats, zero-fills
 // it with 16-byte stores and then drops in the gradient entries of the anchors sampled from that image.
 // HBM-bound: writes B*D*h*w*4 bytes once (the floor of the backward: autograd needs the dense tensor).
 // ------------------------------------------------------------------------------------------------
-template <typename T>
+template <typename T, typename Src>
 __global__ void __launch_bounds__(256)
-k_zero_scatter(pcl_geom g, const int32_t* __restrict__ plan, const int32_t* __restrict__ meta,
-               const float* __restrict__ dA, T* __restrict__ grad) {
+k_zero_scatter(pcl_geom g, const int32_t* __restrict__ plan, const int32_t* __restrict__ meta, Src src,
+               T* __restrict__ grad) {
   const int plane = blockIdx.x;
   const int D = g.D, ms = g.max_samples;
   const int b = plane / D, d = plane - b * D;
   const int64_t HW = (int64_t)g.h * g.w;
   T* dst = grad + (int64_t)plane * HW;
-  constexpr int E = 16 / sizeof(T);                // elements per 16-byte store
-  if (HW % E == 0) {
-    uint4* d4 = reinterpret_cast<uint4*>(dst);
-    const uint4 z = make_uint4(0u, 0u, 0u, 0u);
-    for (int64_t i = threadIdx.x; i < HW / E; i += blockDim.x) d4[i] = z;
-  } else {
-    for (int64_t i = threadIdx.x; i < HW; i += blockDim.x) dst[i] = from_f32<T>(0.f);
-  }
+  zero_plane(dst, HW);
   __syncthreads();
   const int A = min(plan[PCL_PLAN_A], ms);
+  const float scale = src.scale();
   for (int s = threadIdx.x; s < A; s += blockDim.x)
-    if (meta[ms + s] == b) dst[meta[s]] = from_f32<T>(dA[(int64_t)s * D + d]);
-}
-
-// Same, with the reduction of the backward sweep's per-split partial gradients folded in (step path: the (A, D)
-// gradient matrix is never written): value = scale * sum_p dpartials[p][s][d].
-template <typename T>
-__global__ void __launch_bounds__(256)
-k_zero_scatter_reduce(pcl_geom g, const int32_t* __restrict__ plan, const int32_t* __restrict__ meta,
-                      const float* __restrict__ dpartials, int splits, int a_pad, float inv_T,
-                      const float* __restrict__ grad_loss, T* __restrict__ grad) {
-  const int plane = blockIdx.x;
-  const int D = g.D, ms = g.max_samples;
-  const int b = plane / D, d = plane - b * D;
-  const int64_t HW = (int64_t)g.h * g.w;
-  T* dst = grad + (int64_t)plane * HW;
-  constexpr int E = 16 / sizeof(T);                // elements per 16-byte store
-  if (HW % E == 0) {
-    uint4* d4 = reinterpret_cast<uint4*>(dst);
-    const uint4 z = make_uint4(0u, 0u, 0u, 0u);
-    for (int64_t i = threadIdx.x; i < HW / E; i += blockDim.x) d4[i] = z;
-  } else {
-    for (int64_t i = threadIdx.x; i < HW; i += blockDim.x) dst[i] = from_f32<T>(0.f);
-  }
-  __syncthreads();
-  const int A = min(plan[PCL_PLAN_A], ms);
-  const float scale = inv_T * (grad_loss ? grad_loss[0] : 1.f);
-  for (int s = threadIdx.x; s < A; s += blockDim.x) {
-    if (meta[ms + s] == b) {
-      float v = 0.f;
-      for (int p = 0; p < splits; ++p) v += dpartials[((int64_t)p * a_pad + s) * D + d];    // fixed order
-      dst[meta[s]] = from_f32<T>(v * scale);
-    }
-  }
+    if (meta[ms + s] == b) dst[meta[s]] = from_f32<T>(src.at(s, d, D, scale));
 }
 
 // Scatter of the A gradient rows into an ALREADY zero-filled dense gradient, with the fixed-order sum of the per-split
@@ -536,10 +535,9 @@ k_zero_scatter_reduce(pcl_geom g, const int32_t* __restrict__ plan, const int32_
 // sequence (last kernel of the step).
 template <typename T>
 __global__ void __launch_bounds__(256)
-k_scatter_reduce(pcl_geom g, const int32_t* __restrict__ plan, const int32_t* __restrict__ meta,
-                 const float* __restrict__ dpartials, int splits, int split_cols, int a_pad, float inv_T,
-                 const float* __restrict__ grad_scale, T* __restrict__ grad, unsigned long long* step_counter,
-                 unsigned int* dbg, int32_t* __restrict__ prev_rows) {
+k_scatter_reduce(pcl_geom g, const int32_t* __restrict__ plan, const int32_t* __restrict__ meta, SplitRows src,
+                 int split_cols, T* __restrict__ grad, unsigned long long* step_counter, unsigned int* dbg,
+                 int32_t* __restrict__ prev_rows) {
   // one BLOCK per anchor row, one thread per channel: the sum over the splits (up to 18 for the bank sweeps) is a chain
   // of dependent adds per element, so the parallelism has to come from the elements (a warp per row leaves few warps
   // per SM)
@@ -551,12 +549,12 @@ k_scatter_reduce(pcl_geom g, const int32_t* __restrict__ plan, const int32_t* __
   if (prev_rows != nullptr && s == 0 && threadIdx.x == 0) prev_rows[0] = A;           // what the next step has to clear
   if (s >= A) return;
   // partial p covers the contrast columns [p * split_cols, (p+1) * split_cols): only the live ones were written
-  if (split_cols > 0) splits = min(splits, (A + split_cols - 1) / split_cols);
+  if (split_cols > 0) src.splits = min(src.splits, (A + split_cols - 1) / split_cols);
   const int ms = g.max_samples, D = g.D;
   const int64_t HW = (int64_t)g.h * g.w;
   const int pix = meta[s], b = meta[ms + s];
   if (prev_rows != nullptr && threadIdx.x == 0) { prev_rows[1 + s] = pix; prev_rows[1 + ms + s] = b; }
-  const float scale = inv_T * (grad_scale ? grad_scale[0] : 1.f);
+  const float scale = src.scale();
   // Whole 32-byte sectors: a store of 4 (2) bytes into a sector the fill left dirty in L2, or evicted, costs a
   // read-modify-write of the sector; the zeros around the anchor's pixel are written with it (measured on H100 after a
   // 268 MB fill: 1024 x 256 scattered 4-byte stores 26 us, the same stores as whole sectors 17 us).  Another sampled
@@ -581,32 +579,30 @@ k_scatter_reduce(pcl_geom g, const int32_t* __restrict__ plan, const int32_t* __
     if (s_skip) return;
     const int j = threadIdx.x % E, own = s_own[j];
     T* row = grad + (int64_t)b * D * HW + sec + j;
-    for (int d = threadIdx.x / E; d < D; d += blockDim.x / E) {
-      float v = 0.f;
-      for (int p = 0; own >= 0 && p < splits; ++p) v += dpartials[((int64_t)p * a_pad + own) * D + d];   // fixed order
-      row[(int64_t)d * HW] = from_f32<T>(own >= 0 ? v * scale : 0.f);    // +0 where no anchor, whatever the scale
-    }
+    for (int d = threadIdx.x / E; d < D; d += blockDim.x / E)
+      row[(int64_t)d * HW] = from_f32<T>(own >= 0 ? src.at(own, d, D, scale) : 0.f);   // +0 where no anchor, whatever the scale
     return;
   }
   T* dst = grad + (int64_t)b * D * HW + pix;
-  for (int d = threadIdx.x; d < D; d += blockDim.x) {
-    float v = 0.f;
-    for (int p = 0; p < splits; ++p) v += dpartials[((int64_t)p * a_pad + s) * D + d];      // fixed order
-    dst[(int64_t)d * HW] = from_f32<T>(v * scale);
-  }
+  for (int d = threadIdx.x; d < D; d += blockDim.x) dst[(int64_t)d * HW] = from_f32<T>(src.at(s, d, D, scale));
 }
 
-// Zero-fill with 16-byte stores (the dense gradient: B*D*h*w*4 bytes, the HBM floor of the step).  Small footprint
-// (256 threads, no shared memory) so that its CTAs share the SMs with the latency-bound kernels of the step.
-__global__ void __launch_bounds__(256)
-k_fill_zero(uint4* __restrict__ p, uint64_t n16, unsigned int* dbg) {
-  tl_begin(dbg, PCL_TL_FILL);
+// Zero-fill with 16-byte stores (the dense gradient: B*D*h*w*4 bytes, the HBM floor of the step), four independent
+// stores per iteration.
+__device__ __forceinline__ void fill_loop(uint4* __restrict__ p, uint64_t n16) {
   const uint4 z = make_uint4(0u, 0u, 0u, 0u);
   const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
   uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  // four independent stores per iteration
   for (; i + 3 * stride < n16; i += 4 * stride) { p[i] = z; p[i + stride] = z; p[i + 2 * stride] = z; p[i + 3 * stride] = z; }
   for (; i < n16; i += stride) p[i] = z;
+}
+
+// Small footprint (256 threads, no shared memory) so that its CTAs share the SMs with the latency-bound kernels of the
+// step.
+__global__ void __launch_bounds__(256)
+k_fill_zero(uint4* __restrict__ p, uint64_t n16, unsigned int* dbg) {
+  tl_begin(dbg, PCL_TL_FILL);
+  fill_loop(p, n16);
   tl_end(dbg, PCL_TL_FILL);
 }
 
@@ -617,11 +613,7 @@ __global__ void __launch_bounds__(1024, 1)
 k_fill_zero_excl(uint4* __restrict__ p, uint64_t n16, unsigned int* dbg) {
   extern __shared__ uint8_t fill_smem_unused[];
   tl_begin(dbg, PCL_TL_FILL);
-  const uint4 z = make_uint4(0u, 0u, 0u, 0u);
-  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
-  uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  for (; i + 3 * stride < n16; i += 4 * stride) { p[i] = z; p[i + stride] = z; p[i + 2 * stride] = z; p[i + 3 * stride] = z; }
-  for (; i < n16; i += stride) p[i] = z;
+  fill_loop(p, n16);
   tl_end(dbg, PCL_TL_FILL);
 }
 
@@ -636,73 +628,52 @@ int pcl::fill_zero(void* ptr, uint64_t bytes, void* stream, unsigned int* dbg, i
   PCL_REQUIRE(ptr && (bytes & 15) == 0 && ((uintptr_t)ptr & 15) == 0);
   if (bytes == 0) return PCL_OK;
   const uint64_t n16 = bytes >> 4;
-  uint64_t blocks = (n16 + 255) / 256;
-  // CTAs per SM: the fill is a long-running branch that shares the SMs with the latency-bound kernels of the step; a
-  // few resident warps per SM saturate the HBM write path (stores do not wait), more would only crowd the others out
-  // (the fill time does not depend on 1, 2, 4 or 8 CTAs per SM).
-  // PCL_FILL_CTAS_PER_SM overrides (tuning runs).
-  int per_sm = 1;
-  if (const char* e = getenv("PCL_FILL_CTAS_PER_SM")) { int v = atoi(e); if (v >= 1 && v <= 8) per_sm = v; }
-  int sms = num_sms() - reserve_sms;
-  if (sms < num_sms() / 2) sms = num_sms() / 2;
+  const int sms = num_sms(), free_sms = sms - reserve_sms;
   // reserve_sms > 0: the caller runs a kernel of `reserve_sms` big CTAs next to the fill -> fill CTAs that own their SMs
-  // (k_fill_zero_excl), on all SMs but the reserved ones.  PCL_FILL_EXCL = n overrides the CTA count (tuning runs).
-  int excl = (reserve_sms > 0 && num_sms() - reserve_sms >= num_sms() / 2) ? num_sms() - reserve_sms : 0;
-  if (const char* e = getenv("PCL_FILL_EXCL")) excl = atoi(e);
-  if (excl >= 1) {
+  // (k_fill_zero_excl), on all SMs but the reserved ones
+  if (reserve_sms > 0 && free_sms >= sms / 2 && free_sms >= 1) {
     // ALL of the SM's shared memory (227 KB + the 1 KB the system reserves per CTA): no other CTA fits next to it
     const size_t smem = 232448;
     PCL_SMEM_OPT_IN(k_fill_zero_excl, smem);
-    k_fill_zero_excl<<<(unsigned)excl, 1024, smem, (cudaStream_t)stream>>>((uint4*)ptr, n16, dbg);
+    k_fill_zero_excl<<<(unsigned)free_sms, 1024, smem, (cudaStream_t)stream>>>((uint4*)ptr, n16, dbg);
     PCL_LAUNCH_CHECK();
     return PCL_OK;
   }
-  uint64_t cap = (uint64_t)sms * per_sm;
-  // PCL_FILL_GRID (tuning runs): absolute CTA count — a fill throttled to a fraction of the HBM write rate
-  if (const char* e = getenv("PCL_FILL_GRID")) { int v = atoi(e); if (v >= 1) cap = (uint64_t)v; }
-  if (blocks > cap) blocks = cap;
+  // One CTA per SM, on at least half of them: the fill is a long-running branch that shares the SMs with the
+  // latency-bound kernels of the step; a few resident warps per SM saturate the HBM write path (stores do not wait),
+  // more would only crowd the others out (the fill time does not depend on 1, 2, 4 or 8 CTAs per SM).
+  uint64_t blocks = (n16 + 255) / 256;
+  if (blocks > (uint64_t)max(free_sms, sms / 2)) blocks = max(free_sms, sms / 2);
   k_fill_zero<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>((uint4*)ptr, n16, dbg);
   PCL_LAUNCH_CHECK();
   return PCL_OK;
 }
 
-int pcl::scatter_reduce_rows(const pcl_geom* g, const int32_t* plan, const int32_t* anchor_meta, const float* dpartials,
-                             int splits, int split_cols, int a_pad, float inv_T, const float* grad_scale, void* grad_embed,
-                             unsigned long long* step_counter, void* stream, unsigned int* dbg, int32_t* prev_rows,
-                             int grad_dtype) {
-  if (!g || !plan || !anchor_meta || !dpartials || !grad_embed || splits < 1 || !dtype_ok(grad_dtype)) return PCL_ERR_ARG;
-  PCL_DT_SWITCH(grad_dtype, T,
-    k_scatter_reduce<T><<<g->max_samples, g->D <= 128 ? 128 : 256, 0, (cudaStream_t)stream>>>(
-        *g, plan, anchor_meta, dpartials, splits, split_cols, a_pad, inv_T, grad_scale, (T*)grad_embed, step_counter, dbg,
-        prev_rows);)
-  PCL_LAUNCH_CHECK();
-  return PCL_OK;
-}
-
-int pcl::zero_scatter_reduce(const pcl_geom* g, const int32_t* plan, const int32_t* anchor_meta, const float* dpartials,
-                             int splits, int a_pad, float inv_T, const float* grad_loss, void* grad_embed, void* stream,
-                             int grad_dtype) {
-  if (!g || !plan || !anchor_meta || !dpartials || !grad_embed || !dtype_ok(grad_dtype)) return PCL_ERR_ARG;
-  PCL_DT_SWITCH(grad_dtype, T,
-    k_zero_scatter_reduce<T><<<(unsigned)(g->B * g->D), 256, 0, (cudaStream_t)stream>>>(*g, plan, anchor_meta, dpartials,
-                                                                                      splits, a_pad, inv_T, grad_loss,
-                                                                                      (T*)grad_embed);)
-  PCL_LAUNCH_CHECK();
-  return PCL_OK;
-}
-
-// Scatter-only variant for callers that zero-fill the dense gradient themselves (e.g. overlapped with the forward on a
-// second stream): drops the A gradient rows into an already-zero (B,D,h,w) buffer.
-int pcl::scatter_rows(const pcl_geom* g, const int32_t* plan, const int32_t* anchor_meta, const float* dA,
-                      const float* anchors_f32, const float* inv_norm, int normalize, void* grad_embed, void* stream,
-                      int grad_dtype) {
-  if (!g || !plan || !anchor_meta || !dA || !grad_embed || !dtype_ok(grad_dtype)) return PCL_ERR_ARG;
-  if (normalize && (!anchors_f32 || !inv_norm)) return PCL_ERR_ARG;
-  const int warps = 8;
-  PCL_DT_SWITCH(grad_dtype, T,
-    k_scatter<T><<<ceil_div(g->max_samples, warps), warps * 32, 0, (cudaStream_t)stream>>>(*g, plan, anchor_meta, dA,
-                                                                                          anchors_f32, inv_norm, normalize,
-                                                                                          (T*)grad_embed);)
+int pcl::dense_grad(const pcl_geom* g, const int32_t* plan, const int32_t* anchor_meta, const grad_rows& r, bool zeroed,
+                    void* grad_embed, int grad_dtype, void* stream, unsigned int* dbg, unsigned long long* step_counter,
+                    int32_t* prev_rows) {
+  if (!g || !plan || !anchor_meta || !grad_embed || !dtype_ok(grad_dtype)) return PCL_ERR_ARG;
+  const bool partial_rows = r.dpartials != nullptr;
+  if (partial_rows ? r.splits < 1 || r.normalize : !r.dA || (r.normalize && (!r.anchors_f32 || !r.inv_norm)))
+    return PCL_ERR_ARG;
+  cudaStream_t s = (cudaStream_t)stream;
+  const SplitRows sp{r.dpartials, r.splits, r.a_pad, r.inv_T, r.grad_scale};
+  if (!zeroed && !r.normalize) {                 // one pass: zero-fill and scatter per (image, channel) plane
+    const unsigned planes = (unsigned)(g->B * g->D);
+    PCL_DT_SWITCH(grad_dtype, T,
+      if (!partial_rows) k_zero_scatter<T, DaRows><<<planes, 256, 0, s>>>(*g, plan, anchor_meta, DaRows{r.dA}, (T*)grad_embed);
+      else               k_zero_scatter<T, SplitRows><<<planes, 256, 0, s>>>(*g, plan, anchor_meta, sp, (T*)grad_embed);)
+  } else if (partial_rows) {                     // into the zeroed buffer, one block per anchor row
+    PCL_DT_SWITCH(grad_dtype, T,
+      k_scatter_reduce<T><<<g->max_samples, g->D <= 128 ? 128 : 256, 0, s>>>(
+          *g, plan, anchor_meta, sp, r.split_cols, (T*)grad_embed, step_counter, dbg, prev_rows);)
+  } else {                                       // the normalise projection, or a zeroed buffer: one warp per anchor row
+    if (!zeroed) PCL_CUDA(cudaMemsetAsync(grad_embed, 0, (size_t)g->B * g->D * g->h * g->w * dtype_size(grad_dtype), s));
+    const int warps = 8;
+    PCL_DT_SWITCH(grad_dtype, T,
+      k_scatter<T><<<ceil_div(g->max_samples, warps), warps * 32, 0, s>>>(*g, plan, anchor_meta, r.dA, r.anchors_f32,
+                                                                         r.inv_norm, r.normalize, (T*)grad_embed);)
+  }
   PCL_LAUNCH_CHECK();
   return PCL_OK;
 }
@@ -737,39 +708,22 @@ extern "C" int pcl_select_sizes(const pcl_geom* g, pcl_select_sizes_t* out) {
 
 extern "C" int pcl_class_stats(const pcl_geom* g, const int64_t* labels, const float* seg, const int64_t* predict,
                                uint16_t* keys, int32_t* chunk_pref, int32_t* counts, void* stream) {
-  return pcl::class_stats(g, labels, seg, predict, keys, chunk_pref, counts, stream, PCL_DT_F32);
+  return pcl::class_stats(g, labels, seg, predict, keys, chunk_pref, counts, nullptr, nullptr, stream, PCL_DT_F32);
 }
 
+// done_ctr (one zeroed word; the step path): scan + totals + plan in ONE launch, the last block to finish runs the plan.
+// Without it the totals are atomics into the zeroed counts and the plan is left to k_plan.
 int pcl::class_stats(const pcl_geom* g, const int64_t* labels, const void* seg, const int64_t* predict, uint16_t* keys,
-                     int32_t* chunk_pref, int32_t* counts, void* stream, int seg_dtype) {
+                     int32_t* chunk_pref, int32_t* counts, int32_t* plan, unsigned int* done_ctr, void* stream,
+                     int seg_dtype) {
   int st = check_geom(g);
   if (st != PCL_OK) return st;
-  PCL_REQUIRE(labels && keys && chunk_pref && counts && (seg || predict) && dtype_ok(seg_dtype));
+  PCL_REQUIRE(labels && keys && chunk_pref && counts && (plan || !done_ctr) && (seg || predict) && dtype_ok(seg_dtype));
   cudaStream_t s = (cudaStream_t)stream;
   const int64_t HW = (int64_t)g->h * g->w;
   const int nchunk = (int)ceil_div64(HW, PCL_CHUNK);
   const float scale_h = (float)g->Himg / (float)g->h, scale_w = (float)g->Wimg / (float)g->w;
-  PCL_CUDA(cudaMemsetAsync(counts, 0, (size_t)g->B * 2 * g->K * sizeof(int32_t), s));
-  dim3 grid(nchunk, g->B);
-  size_t smem = (2 * g->K + 1) * sizeof(int);
-  PCL_DT_SWITCH(seg_dtype, T,
-    k_keys<T><<<grid, PCL_CHUNK, smem, s>>>(*g, nchunk, scale_h, scale_w, labels, (const T*)seg, predict, keys, chunk_pref,
-                                            counts, nullptr, nullptr);)
-  PCL_LAUNCH_CHECK();
-  return PCL_OK;
-}
-
-// Step path: scan + totals + plan in ONE launch (the last block to finish runs the plan; done_ctr: one zeroed word).
-int pcl::class_stats_plan(const pcl_geom* g, const int64_t* labels, const void* seg, const int64_t* predict, uint16_t* keys,
-                          int32_t* chunk_pref, int32_t* counts, int32_t* plan, unsigned int* done_ctr, void* stream,
-                          int seg_dtype) {
-  int st = check_geom(g);
-  if (st != PCL_OK) return st;
-  PCL_REQUIRE(labels && keys && chunk_pref && counts && plan && done_ctr && (seg || predict) && dtype_ok(seg_dtype));
-  cudaStream_t s = (cudaStream_t)stream;
-  const int64_t HW = (int64_t)g->h * g->w;
-  const int nchunk = (int)ceil_div64(HW, PCL_CHUNK);
-  const float scale_h = (float)g->Himg / (float)g->h, scale_w = (float)g->Wimg / (float)g->w;
+  if (!done_ctr) PCL_CUDA(cudaMemsetAsync(counts, 0, (size_t)g->B * 2 * g->K * sizeof(int32_t), s));
   dim3 grid(nchunk, g->B);
   size_t smem = (2 * g->K + 1) * sizeof(int);
   PCL_DT_SWITCH(seg_dtype, T,
@@ -790,29 +744,26 @@ extern "C" int pcl_plan_anchors(const pcl_geom* g, const int32_t* counts, int32_
   return PCL_OK;
 }
 
-int pcl::select_gather_ex(const pcl_geom* g, const void* embed, const uint16_t* keys, const int32_t* chunk_pref,
-                          const int32_t* plan, const int32_t* ranks, uint64_t seed, int normalize, int32_t* anchor_meta,
-                          float* anchors_f32, void* anchors_bf16, float* inv_norm, float* norm_max, float* row_m2,
-                          float m2_scale, float* partials, int64_t n_slot_rows, void* stream,
-                          const unsigned long long* seed_ctr, unsigned int* dbg, const int32_t* prev_rows, void* grad_clear,
-                          int embed_dtype) {
+int pcl::select_gather(const select_args& a, void* stream) {
+  const pcl_geom* g = a.g;
   int st = check_geom(g);
   if (st != PCL_OK) return st;
-  PCL_REQUIRE(embed && keys && chunk_pref && plan && anchor_meta && anchors_f32 && inv_norm && dtype_ok(embed_dtype));
+  PCL_REQUIRE(a.embed && a.keys && a.chunk_pref && a.plan && a.anchor_meta && a.anchors_f32 && a.inv_norm &&
+              dtype_ok(a.embed_dtype));
   cudaStream_t s = (cudaStream_t)stream;
   const int ms = g->max_samples;
   const int nchunk = (int)ceil_div64((int64_t)g->h * g->w, PCL_CHUNK);
-  if (norm_max) PCL_CUDA(cudaMemsetAsync(norm_max, 0, sizeof(float), s));     // optional output
+  if (a.norm_max) PCL_CUDA(cudaMemsetAsync(a.norm_max, 0, sizeof(float), s));     // optional output
   const int warps = 8;
   // rows in [A, max_samples) are zero-filled by the kernel itself (no separate memsets); the bf16 copy is padded to
   // a multiple of 128 rows: cover those too
-  const int rows = anchors_bf16 ? ceil_div(ms, 128) * 128 : ms;
-  PCL_DT_SWITCH(embed_dtype, T,
-    k_select<T><<<ceil_div(rows, warps), warps * 32, 0, s>>>(*g, nchunk, (const T*)embed, keys, chunk_pref, plan, ranks,
-                                                             seed, normalize, anchor_meta, anchors_f32,
-                                                             (__nv_bfloat16*)anchors_bf16, inv_norm, norm_max, row_m2,
-                                                             m2_scale, partials, n_slot_rows, seed_ctr, dbg, prev_rows,
-                                                             (T*)grad_clear);)
+  const int rows = a.anchors_bf16 ? ceil_div(ms, 128) * 128 : ms;
+  PCL_DT_SWITCH(a.embed_dtype, T,
+    k_select<T><<<ceil_div(rows, warps), warps * 32, 0, s>>>(*g, nchunk, (const T*)a.embed, a.keys, a.chunk_pref, a.plan,
+                                                             a.ranks, a.seed, a.normalize, a.anchor_meta, a.anchors_f32,
+                                                             (__nv_bfloat16*)a.anchors_bf16, a.inv_norm, a.norm_max,
+                                                             a.row_m2, a.m2_scale, a.partials, a.n_slot_rows, a.seed_ctr,
+                                                             a.dbg, a.prev_rows, (T*)a.grad_clear);)
   PCL_LAUNCH_CHECK();
   return PCL_OK;
 }
@@ -821,36 +772,19 @@ extern "C" int pcl_select_gather(const pcl_geom* g, const float* embed, const ui
                                  const int32_t* chunk_pref, const int32_t* plan, const int32_t* ranks,
                                  uint64_t seed, int normalize, int32_t* anchor_meta, float* anchors_f32,
                                  void* anchors_bf16, float* inv_norm, float* norm_max, void* stream) {
-  return pcl::select_gather_ex(g, embed, keys, chunk_pref, plan, ranks, seed, normalize, anchor_meta, anchors_f32,
-                               anchors_bf16, inv_norm, norm_max, nullptr, 0.f, nullptr, 0, stream);
+  pcl::select_args a = {};
+  a.g = g; a.embed = embed; a.embed_dtype = PCL_DT_F32; a.keys = keys; a.chunk_pref = chunk_pref; a.plan = plan;
+  a.ranks = ranks; a.seed = seed; a.normalize = normalize; a.anchor_meta = anchor_meta; a.anchors_f32 = anchors_f32;
+  a.anchors_bf16 = anchors_bf16; a.inv_norm = inv_norm; a.norm_max = norm_max;
+  return pcl::select_gather(a, stream);
 }
 
 extern "C" int pcl_scatter_grad(const pcl_geom* g, const int32_t* plan, const int32_t* anchor_meta, const float* dA,
                                 const float* anchors_f32, const float* inv_norm, int normalize, float* grad_embed,
                                 void* stream) {
-  return pcl::scatter_grad(g, plan, anchor_meta, dA, anchors_f32, inv_norm, normalize, grad_embed, stream, PCL_DT_F32);
-}
-
-int pcl::scatter_grad(const pcl_geom* g, const int32_t* plan, const int32_t* anchor_meta, const float* dA,
-                      const float* anchors_f32, const float* inv_norm, int normalize, void* grad_embed, void* stream,
-                      int grad_dtype) {
   int st = check_geom(g);
   if (st != PCL_OK) return st;
-  PCL_REQUIRE(plan && anchor_meta && dA && grad_embed && dtype_ok(grad_dtype));
-  if (normalize) PCL_REQUIRE(anchors_f32 && inv_norm);
-  cudaStream_t s = (cudaStream_t)stream;
-  if (!normalize) {
-    PCL_DT_SWITCH(grad_dtype, T,
-      k_zero_scatter<T><<<(unsigned)(g->B * g->D), 256, 0, s>>>(*g, plan, anchor_meta, dA, (T*)grad_embed);)
-    PCL_LAUNCH_CHECK();
-    return PCL_OK;
-  }
-  size_t bytes = (size_t)g->B * g->D * g->h * g->w * dtype_size(grad_dtype);
-  PCL_CUDA(cudaMemsetAsync(grad_embed, 0, bytes, s));
-  const int warps = 8;
-  PCL_DT_SWITCH(grad_dtype, T,
-    k_scatter<T><<<ceil_div(g->max_samples, warps), warps * 32, 0, s>>>(*g, plan, anchor_meta, dA, anchors_f32, inv_norm,
-                                                                       normalize, (T*)grad_embed);)
-  PCL_LAUNCH_CHECK();
-  return PCL_OK;
+  pcl::grad_rows r = {};
+  r.dA = dA; r.anchors_f32 = anchors_f32; r.inv_norm = inv_norm; r.normalize = normalize;
+  return pcl::dense_grad(g, plan, anchor_meta, r, false, grad_embed, PCL_DT_F32, stream);
 }

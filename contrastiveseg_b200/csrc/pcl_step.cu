@@ -1,6 +1,5 @@
 // One loss step chained on a stream behind a single descriptor (include/pcl.h: pcl_step_*).
 #include "pcl_common.cuh"
-#include <stdlib.h>
 
 static void fill_sweep(const pcl_step_desc* d, pcl_sweep_desc* w) {
   memset(w, 0, sizeof(*w));
@@ -42,17 +41,28 @@ static void fill_tc(const pcl_step_desc* d, pcl_tc_desc* t) {
 
 extern "C" int pcl_step_stats(const pcl_step_desc* d, void* stream) {
   if (!d) return PCL_ERR_ARG;
-  if (d->sync != nullptr)        // one launch: the scan's last block computes totals and plan (sync[4] = its counter)
-    return pcl::class_stats_plan(&d->g, d->labels, d->seg, d->predict, d->keys, d->chunk_pref, d->counts, d->plan,
-                                 d->sync + 4, stream, d->seg_dtype);
-  int st = pcl::class_stats(&d->g, d->labels, d->seg, d->predict, d->keys, d->chunk_pref, d->counts, stream, d->seg_dtype);
-  if (st != PCL_OK) return st;
+  // with the sync buffer: one launch, the scan's last block computes totals and plan (sync[4] = its counter)
+  unsigned int* done_ctr = d->sync != nullptr ? d->sync + 4 : nullptr;
+  int st = pcl::class_stats(&d->g, d->labels, d->seg, d->predict, d->keys, d->chunk_pref, d->counts, d->plan, done_ctr,
+                            stream, d->seg_dtype);
+  if (st != PCL_OK || done_ctr != nullptr) return st;
   return pcl_plan_anchors(&d->g, d->counts, d->plan, stream);
 }
 
 // a10: topk_negatives 0 = all negatives, k >= 1 needs the selection scratch, < 0 is refused
 static bool topk_ok(const pcl_step_desc* d) {
   return d->topk_negatives == 0 || (d->topk_negatives > 0 && d->topk_scratch != nullptr);
+}
+
+// The selection's arguments that come from the descriptor; ctr: captured sequences draw the anchors from the counter
+// instead of the injected ranks.  The caller sets the rest.
+static pcl::select_args select_args(const pcl_step_desc* d, const unsigned long long* ctr) {
+  pcl::select_args a = {};
+  a.g = &d->g; a.embed = d->embed; a.embed_dtype = d->embed_dtype;
+  a.keys = d->keys; a.chunk_pref = d->chunk_pref; a.plan = d->plan; a.ranks = ctr ? nullptr : d->ranks;
+  a.seed = d->seed; a.normalize = d->normalize; a.seed_ctr = ctr;
+  a.anchor_meta = d->anchor_meta; a.anchors_f32 = d->anchors_f32; a.anchors_bf16 = d->anchors_bf16; a.inv_norm = d->inv_norm;
+  return a;
 }
 
 static int step_forward(const pcl_step_desc* d, unsigned long long* ctr, void* stream);
@@ -70,24 +80,22 @@ extern "C" int pcl_step_forward_ctr(const pcl_step_desc* d, uint64_t* step_count
 static int step_forward(const pcl_step_desc* d, unsigned long long* ctr, void* stream) {
   if (!d || !topk_ok(d)) return PCL_ERR_ARG;
   const int k = d->topk_negatives;
+  pcl::select_args sel = select_args(d, ctr);
   if (d->precision == 1 && k == 0) {
     // tensor path: the selection kernel also writes the row stabilisers and initialises the partial slots
     if (!d->anchors_bf16 || !d->row_m2 || (d->mode == 1 && !d->shadow_bf16)) return PCL_ERR_ARG;
     pcl_tc_desc t;
     fill_tc(d, &t);
-    int64_t n_slot_rows = 0;
-    float m2_scale = 0.f;
-    int st = pcl::tc_query(&t, &n_slot_rows, &m2_scale);
+    int st = pcl::tc_query(&t, &sel.n_slot_rows, &sel.m2_scale);
     if (st != PCL_OK) return st;
-    st = pcl::select_gather_ex(&d->g, d->embed, d->keys, d->chunk_pref, d->plan, ctr ? nullptr : d->ranks, d->seed,
-                               d->normalize, d->anchor_meta, d->anchors_f32, d->anchors_bf16, d->inv_norm, nullptr, d->row_m2,
-                               m2_scale, d->partials, n_slot_rows, stream, ctr, nullptr, nullptr, nullptr, d->embed_dtype);
+    sel.row_m2 = d->row_m2;
+    sel.partials = d->partials;
+    st = pcl::select_gather(sel, stream);
     if (st != PCL_OK) return st;
     return pcl::tc_fwd_ex(&t, d->row_m2, d->partials, d->rowstats, d->loss, stream, true, ctr);
   }
-  int st = pcl::select_gather_ex(&d->g, d->embed, d->keys, d->chunk_pref, d->plan, ctr ? nullptr : d->ranks, d->seed,
-                                 d->normalize, d->anchor_meta, d->anchors_f32, d->anchors_bf16, d->inv_norm, d->norm_max,
-                                 nullptr, 0.f, nullptr, 0, stream, ctr, nullptr, nullptr, nullptr, d->embed_dtype);
+  sel.norm_max = d->norm_max;
+  int st = pcl::select_gather(sel, stream);
   if (st != PCL_OK) return st;
   if (d->precision == 1) {
     // top-k on the tensor path: the selection above leaves the stabilisers and the partial slots to the top-k forward's
@@ -102,60 +110,44 @@ static int step_forward(const pcl_step_desc* d, unsigned long long* ctr, void* s
   return pcl::simt_fwd_ex(&w, k, d->topk_scratch, d->partials, d->rowstats, d->loss, stream, ctr);
 }
 
-extern "C" int pcl_step_backward(const pcl_step_desc* d, const float* grad_loss, void* stream) {
-  if (!d || !topk_ok(d)) return PCL_ERR_ARG;
+// prezeroed: the caller has ALREADY zero-filled the dense gradient (the 268 MB fill is the HBM floor of the step; a
+// caller that starts it on a second stream at the beginning of the forward hides it behind the latency-bound selection
+// and sweep kernels), so only the anchor rows are scattered.
+static int step_backward(const pcl_step_desc* d, const float* grad_loss, void* stream, bool prezeroed) {
+  if (!d) return PCL_ERR_ARG;
+  if (prezeroed && d->topk_negatives != 0) return PCL_ERR_UNSUPPORTED;
+  if (!topk_ok(d)) return PCL_ERR_ARG;
   const int k = d->topk_negatives;
+  // tensor path without normalise and top-k: the sweep leaves its per-split partial rows and the dense-gradient writer
+  // sums them itself (fixed order), no (A, D) gradient round trip; otherwise the sweep reduces them to dA
+  const bool partial_rows = d->precision == 1 && !d->normalize && k == 0;
+  pcl::grad_rows r = {};
+  if (partial_rows) {
+    r.dpartials = d->dpartials; r.inv_T = 1.f / d->temperature; r.grad_scale = grad_loss;
+  } else {
+    r.dA = d->dA; r.anchors_f32 = d->anchors_f32; r.inv_norm = d->inv_norm; r.normalize = d->normalize;
+  }
   int st;
   if (d->precision == 1) {
     pcl_tc_desc t;
     fill_tc(d, &t);
-    if (!d->normalize && k == 0) {
-      // fused tail: the dense-gradient writer sums the per-split partials itself (no (A, D) gradient round trip)
-      int splits = 0, a_pad = 0;
-      st = pcl::tc_bwd_ex(&t, d->row_m2, d->rowstats, grad_loss, d->dpartials, nullptr, stream, &splits, &a_pad);
-      if (st != PCL_OK) return st;
-      return pcl::zero_scatter_reduce(&d->g, d->plan, d->anchor_meta, d->dpartials, splits, a_pad, 1.f / d->temperature,
-                                      grad_loss, d->grad_embed, stream, d->embed_dtype);
-    }
-    st = pcl::tc_bwd_ex(&t, d->row_m2, d->rowstats, grad_loss, d->dpartials, d->dA, stream, nullptr, nullptr,
-                        k > 0 ? d->topk_scratch : nullptr);
+    st = pcl::tc_bwd_ex(&t, d->row_m2, d->rowstats, grad_loss, d->dpartials, partial_rows ? nullptr : d->dA, stream,
+                        &r.splits, &r.a_pad, k > 0 ? d->topk_scratch : nullptr);
   } else {
     pcl_sweep_desc w;
     fill_sweep(d, &w);
     st = pcl::simt_bwd_ex(&w, k, d->topk_scratch, d->rowstats, grad_loss, d->dpartials, d->dA, stream);
   }
   if (st != PCL_OK) return st;
-  return pcl::scatter_grad(&d->g, d->plan, d->anchor_meta, d->dA, d->anchors_f32, d->inv_norm, d->normalize,
-                           d->grad_embed, stream, d->embed_dtype);
+  return pcl::dense_grad(&d->g, d->plan, d->anchor_meta, r, prezeroed, d->grad_embed, d->embed_dtype, stream, d->sync);
 }
 
-// Backward for a dense-gradient buffer the caller has ALREADY zero-filled (the 268 MB fill is the HBM floor of the
-// step; a caller that starts it on a second stream at the beginning of the forward hides it behind the latency-bound
-// selection and sweep kernels): backward sweep -> (A, D) gradient rows -> scatter of those rows only.
+extern "C" int pcl_step_backward(const pcl_step_desc* d, const float* grad_loss, void* stream) {
+  return step_backward(d, grad_loss, stream, false);
+}
+
 extern "C" int pcl_step_backward_prezeroed(const pcl_step_desc* d, const float* grad_loss, void* stream) {
-  if (!d) return PCL_ERR_ARG;
-  if (d->topk_negatives != 0) return PCL_ERR_UNSUPPORTED;
-  int st;
-  if (d->precision == 1) {
-    pcl_tc_desc t;
-    fill_tc(d, &t);
-    if (!d->normalize) {
-      // the scatter sums the per-split partial rows itself (fixed order): no (A, D) gradient round trip, one launch less
-      int splits = 0, a_pad = 0;
-      st = pcl::tc_bwd_ex(&t, d->row_m2, d->rowstats, grad_loss, d->dpartials, nullptr, stream, &splits, &a_pad);
-      if (st != PCL_OK) return st;
-      return pcl::scatter_reduce_rows(&d->g, d->plan, d->anchor_meta, d->dpartials, splits, 0, a_pad, 1.f / d->temperature,
-                                      grad_loss, d->grad_embed, nullptr, stream, d->sync, nullptr, d->embed_dtype);
-    }
-    st = pcl_infonce_tc_bwd(&t, d->row_m2, d->rowstats, grad_loss, d->dpartials, d->dA, stream);
-  } else {
-    pcl_sweep_desc w;
-    fill_sweep(d, &w);
-    st = pcl_infonce_bwd(&w, d->rowstats, grad_loss, d->dpartials, d->dA, stream);
-  }
-  if (st != PCL_OK) return st;
-  return pcl::scatter_rows(&d->g, d->plan, d->anchor_meta, d->dA, d->anchors_f32, d->inv_norm, d->normalize,
-                           d->grad_embed, stream, d->embed_dtype);
+  return step_backward(d, grad_loss, stream, true);
 }
 
 // ---- fused small-anchor step (include/pcl.h: pcl_step_fused_*) ----
@@ -172,15 +164,15 @@ extern "C" int pcl_step_fused_select(const pcl_step_desc* d, const uint64_t* ste
   if (!d->anchors_bf16 || !d->row_m2 || (prev_rows && !d->grad_embed)) return PCL_ERR_ARG;
   pcl_tc_desc t;
   fill_tc(d, &t);
-  int64_t n_slot_rows = 0;
-  float m2_scale = 0.f;
-  int st = pcl::tc_query(&t, &n_slot_rows, &m2_scale);
-  if (st != PCL_OK) return st;
   // selection + gather; the fused kernel writes every partial slot it reads: no slot initialisation
-  return pcl::select_gather_ex(&d->g, d->embed, d->keys, d->chunk_pref, d->plan, step_counter ? nullptr : d->ranks, d->seed,
-                               0, d->anchor_meta, d->anchors_f32, d->anchors_bf16, d->inv_norm, nullptr, d->row_m2, m2_scale,
-                               nullptr, 0, stream, reinterpret_cast<const unsigned long long*>(step_counter), d->sync,
-                               prev_rows, d->grad_embed, d->embed_dtype);
+  pcl::select_args sel = select_args(d, reinterpret_cast<const unsigned long long*>(step_counter));
+  int st = pcl::tc_query(&t, &sel.n_slot_rows, &sel.m2_scale);     // (no partials: the slot count goes unused)
+  if (st != PCL_OK) return st;
+  sel.row_m2 = d->row_m2;
+  sel.dbg = d->sync;
+  sel.prev_rows = prev_rows;
+  sel.grad_clear = d->grad_embed;
+  return pcl::select_gather(sel, stream);
 }
 
 extern "C" int pcl_step_fused_loss(const pcl_step_desc* d, void* stream) {
@@ -195,11 +187,13 @@ extern "C" int pcl_step_fused_scatter(const pcl_step_desc* d, const float* grad_
                                       int32_t* prev_rows, void* stream) {
   if (!pcl_step_fused_supported(d)) return PCL_ERR_UNSUPPORTED;
   if (!d->grad_embed) return PCL_ERR_ARG;
-  const int a_pad = ((d->g.max_samples + 127) / 128) * 128;
-  const int splits = (a_pad + 255) / 256;
-  return pcl::scatter_reduce_rows(&d->g, d->plan, d->anchor_meta, d->dpartials, splits, 256, a_pad, 1.f / d->temperature, grad_scale,
-                                  d->grad_embed, reinterpret_cast<unsigned long long*>(step_counter), stream, d->sync, prev_rows,
-                                  d->embed_dtype);
+  pcl::grad_rows r = {};
+  pcl::self_fused_splits(d->g.max_samples, &r.a_pad, &r.splits, &r.split_cols);
+  r.dpartials = d->dpartials;
+  r.inv_T = 1.f / d->temperature;
+  r.grad_scale = grad_scale;
+  return pcl::dense_grad(&d->g, d->plan, d->anchor_meta, r, true, d->grad_embed, d->embed_dtype, stream, d->sync,
+                         reinterpret_cast<unsigned long long*>(step_counter), prev_rows);
 }
 
 // zero-fill of the step's dense gradient on the engine's fill kernel (the caller picks the stream: a parallel branch)
@@ -212,9 +206,6 @@ extern "C" int pcl_step_fused_fill(const pcl_step_desc* d, void* stream) {
   // The fill forks right before the fused InfoNCE kernel (at most 8 x 4 = 32 CTAs, one per SM).  Its CTAs OWN their SMs
   // and leave 32 free: the InfoNCE kernel starts at once, next to the fill, instead of waiting for fill CTAs to retire
   // (its 384-thread, register-heavy CTAs fit on no SM that holds fill warps; measured in-graph on H100 with the
-  // shared-SM fill: the fused kernel starts 58 us later, step 0.164 -> 0.191 ms).  PCL_FILL_RESERVE_SMS overrides
-  // (tuning runs; 0 = the shared-SM fill).
-  int reserve = 32;
-  if (const char* e = getenv("PCL_FILL_RESERVE_SMS")) reserve = atoi(e);
-  return pcl::fill_zero(d->grad_embed, bytes, stream, d->sync, reserve);
+  // shared-SM fill: the fused kernel starts 58 us later, step 0.164 -> 0.191 ms).
+  return pcl::fill_zero(d->grad_embed, bytes, stream, d->sync, 32);
 }

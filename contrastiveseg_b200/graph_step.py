@@ -265,16 +265,13 @@ class GraphedContrastStep:
         if self.prologue is not None:
             self.prologue(stream)
         if self.fused:
-            early = bool(os.environ.get("PCL_FILL_FORK_EARLY")) and not self.sparse_reset      # tuning runs
-            if early:
-                self._fork_zero_fill()
             _abi.check(lib.pcl_step_stats(C.byref(d), stream), "pcl_step_stats")
             _abi.check(lib.pcl_step_fused_select(C.byref(d), self.counter.data_ptr(), _abi.ptr(self.prev_rows), stream),
                        "pcl_step_fused_select")
             # full-fill mode: the fill forks AFTER scan and selection — next to it their DRAM reads slow down (measured
             # in-graph on H100: scan 24 -> 91 us, selection 15 -> 22 us; step 0.164 -> 0.179 ms), only the L2-resident
             # InfoNCE kernel hides behind it
-            if not self.sparse_reset and not early:
+            if not self.sparse_reset:
                 self._fork_zero_fill()
             _abi.check(lib.pcl_step_fused_loss(C.byref(d), stream), "pcl_step_fused_loss")
             if not self.sparse_reset:

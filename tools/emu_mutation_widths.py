@@ -40,7 +40,8 @@ MUTANTS = [   # (name, source file, exact text, replacement, None or the reason 
      "g->D <= 128 ? 128 : 256", "g->D <= 128 ? 64 : 256",
      "the channel loop strides by blockDim.x, and only the tensor path (D = 256) launches k_scatter_reduce"),
     ("k_zero_scatter: grid of B * (D rounded down to a power of two) planes", SEL,
-     "k_zero_scatter<T><<<(unsigned)(g->B * g->D)", "k_zero_scatter<T><<<(unsigned)(g->B * (g->D & -g->D))", None),
+     "const unsigned planes = (unsigned)(g->B * g->D);", "const unsigned planes = (unsigned)(g->B * (g->D & -g->D));",
+     None),
     ("k_bank_segsum: channel groups D / 8 rounded down", BANK,
      "dim3(chunks, ceil_div(g->D, SEG_DG), g->B)", "dim3(chunks, g->D / SEG_DG, g->B)", None),
     ("k_bank_segsum: no early exit past the last channel", BANK,

@@ -1,4 +1,4 @@
-"""Timing probe of the fused small-anchor step (S1 shape): ms per graph replay for several fill occupancies."""
+"""Timing probe at the S1 shape: ms per graph replay of the fused, the sparse-reset and the unfused step."""
 import json
 import os
 import sys
@@ -16,22 +16,18 @@ inp = {k: v.to(dev) for k, v in bench.make_inputs(cfg, 304, None, False).items()
 crit = cs.PixelContrastLoss(bench.engine_configer(cfg, False, "bf16"))
 opts = crit.options(); opts.num_classes = cfg["K"]
 steps = int(os.environ.get("PROBE_STEPS", "200"))
-variants = [v for v in os.environ.get("PROBE_FILL", "1,2,3,4,8").split(",")]
 for fused in (True, "sparse", False):
-    for per_sm in (variants if fused is True else ["-"]):
-        if fused is True:
-            os.environ["PCL_FILL_CTAS_PER_SM"] = per_sm
-        st = cs.GraphedContrastStep(inp["embed"], inp["target"], seg=inp["seg"], options=opts, fused=bool(fused),
-                                    sparse_reset=(fused == "sparse"))
-        for _ in range(10):
-            st.replay()
-        torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(steps):
-            st.replay()
-        e1.record()
-        torch.cuda.synchronize()
-        print(json.dumps({"B": B, "fused": fused, "fill_ctas_per_sm": per_sm, "ms_per_step": e0.elapsed_time(e1) / steps,
-                          "loss": float(st.loss.item())}), flush=True)
-        del st
+    st = cs.GraphedContrastStep(inp["embed"], inp["target"], seg=inp["seg"], options=opts, fused=bool(fused),
+                                sparse_reset=(fused == "sparse"))
+    for _ in range(10):
+        st.replay()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(steps):
+        st.replay()
+    e1.record()
+    torch.cuda.synchronize()
+    print(json.dumps({"B": B, "fused": fused, "ms_per_step": e0.elapsed_time(e1) / steps, "loss": float(st.loss.item())}),
+          flush=True)
+    del st
