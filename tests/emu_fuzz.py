@@ -1,6 +1,7 @@
 """TEST INFRASTRUCTURE: differential fuzzing of the engine (real SIMT kernel sources on the host-fiber emulator,
 tests/emu) against the oracle over random geometries.  Used by tests/test_emu_fuzz.py (bounded) and
-tools/emu_fuzz.py (long runs).  Every fuzzer returns a list of failure descriptions (empty = clean).
+tools/emu_fuzz.py (long runs).  Every fuzzer returns a list of failure descriptions (empty = clean); fuzz_graphed_step
+also returns how many cases reached each of its coverage categories, so that a test can require all of them.
 
 It found the out-of-bounds wrap write for pixel_update_freq > memory_size (now refused, csrc/pcl_bank.cu: make_dims)."""
 import math
@@ -366,49 +367,329 @@ def tensor_case(A, N, ncls, T, mode, clustered, g, M=None, device="cpu", ref_dev
     return None
 
 
-def fuzz_graphed_step(seed: int, n: int):
-    """GraphedContrastStep's launch sequence (device-side rank draw, optional pre-zeroed scatter-only backward) against the
-    eager autograd step over random geometries: replay r must sample, and compute, exactly what eager step r+1 does."""
+GRAPH_CATEGORIES = ("fused full-fill", "fused sparse", "streaming bf16", "exact fp32", "bank", "bank + enqueue",
+                    "half embed", "A = 0 replay", "tile-edge crossing", "non-integer label ratio")
+# max_samples draws lean on the tile edges of the tensor path (128-row, 256-column tiles) and on the ends of the range
+_MS_EDGES = (1, 127, 128, 129, 255, 256, 257, 511, 513, 700, 1023, 1024)
+_BANK_NAMES = ("segment_queue", "pixel_queue", "segment_queue_ptr", "pixel_queue_ptr")
+
+
+def _sync(device):
+    if torch.device(device).type == "cuda":
+        torch.cuda.synchronize(device)
+
+
+def _same_bits(a, b):
+    """Bit-identical tensors (the sign of a zero counts; NaN equals NaN whatever its payload)."""
+    if a.shape != b.shape or a.dtype != b.dtype:
+        return False
+    na, nb = torch.isnan(a), torch.isnan(b)
+    if not torch.equal(na, nb):
+        return False
+    it = {2: torch.int16, 4: torch.int32}[a.element_size()]
+    z = torch.zeros((), dtype=a.dtype, device=a.device)
+    return torch.equal(torch.where(na, z, a).view(it), torch.where(nb, z, b).view(it))
+
+
+def _tiles(A):
+    return -(-A // 128), -(-A // 256)
+
+
+def graph_step_inputs(B, D, h, w, K, himg, wimg, block, ignore, seq, seed):
+    """draw(r): the CPU inputs of replay r (make_contrast_batch at himg x wimg, a fraction `ignore` of the labels set to
+    the ignore label).  seq "empty": replay 1 has one labelled pixel, so no class qualifies (A = 0); seq "edge": odd
+    replays keep one class of the label map, so A jumps between replays (across tile edges when max_samples allows)."""
+    def draw(r):
+        data = make_contrast_batch(B=B, D=D, h=h, w=w, num_classes=K, img_stride=1, block=block, seed=seed + 7919 * r,
+                                   himg=himg, wimg=wimg)
+        tgt = data["target"]
+        g = torch.Generator().manual_seed(seed + 31 * r + 1)
+        tgt[torch.rand(tgt.shape, generator=g) < ignore] = -1
+        if seq == "empty" and r == 1:
+            tgt.fill_(-1)
+            tgt[0, 0, 0] = 0
+        elif seq == "edge" and r % 2 == 1:
+            tgt[tgt != int(torch.randint(0, K, (1,), generator=g))] = -1
+        return data
+    return draw
+
+
+def _f64_reference(c, X, cls, refrow, queue):
+    """Loss and d loss / d embed rows of the drawn anchors in float64 (closed form), in the step's row order.
+    X: the drawn embed rows as stored (float64); queue: the (K, 2M, D) bank as the replay read it, or None.  The tensor
+    path computes on bf16 operands: the reference rounds them the same way.  None when the closed form cannot score the
+    draw (a bank step with more anchors than bank columns: the diagonal column of a row does not exist)."""
+    T, bT, A = c["T"], c["bT"], X.shape[0]
+    tensor = c["precision"] == "bf16"
+    y = F.normalize(X, dim=1) if c["normalize"] else X
+    a = _bf(y.float()).double() if tensor else y
+    if queue is None:
+        contrast, yc, diag, self_c = a, cls, None, True
+    else:
+        q = _bf(queue.float()).double() if tensor else queue
+        contrast, yc = P.flatten_queue(q)
+        yc, diag, self_c = yc.long(), refrow, False
+        if A > contrast.shape[0]:
+            return None
+    cf = P.infonce_closed_form(a, cls, contrast, yc, T, bT, self_contrast=self_c, diag_cols=diag)
+    loss, dA = cf["loss"], cf["dA"]
+    if c["nan_safe"]:            # rows without positives contribute 0 to the loss and nothing to the gradient
+        ok = cf["npos"] > 0
+        G = torch.where(ok[:, None], cf["G"], torch.zeros_like(cf["G"]))
+        dA = G @ contrast / T + ((G.t() @ a) / T if self_c else 0)
+        loss = torch.where(ok, cf["row_loss"], torch.zeros_like(cf["row_loss"])).sum() / A
+    if c["normalize"]:           # through the normalisation: (g - y (y . g)) / |x|
+        dA = (dA - y * (y * dA).sum(1, keepdim=True)) / X.norm(dim=1, keepdim=True)
+    return loss.item(), dA
+
+
+def graphed_step_case(c, draw, n_rep, device, check_sampling, cov, desc):
+    """One GraphedContrastStep (configuration `c`), `n_rep` replays, the static inputs refilled in place from draw(r)
+    before replay r.  Every replay: the anchors are a valid sample (check_sampling) and those of eager step r + 1,
+    loss and gradient match the eager step and the float64 closed form on the drawn rows, every gradient element at no
+    drawn anchor is +0 (the buffer is NaN before a full-fill replay), a bank written by the step equals the eager trainer
+    order.  Half embed: an fp32 twin step on the same values must give the same loss bits and the gradient rounded
+    once.  Adds the categories the case reached to `cov` (counted when a replay of the case was scored against float64;
+    cov["scored"] / cov["skipped"]: replays the closed form scored / could not score).
+    Returns the failures."""
+    from contrastiveseg_b200 import bank as bank_mod
+    dev = torch.device(device)
+    B, D, h, w, K, ms, mv, T, bT = (c[k] for k in ("B", "D", "h", "w", "K", "ms", "mv", "T", "bT"))
+    scale = c["grad_scale"]
+    tensor = c["precision"] == "bf16"
+    d0 = draw(0)
+    src = lambda d: d["embed_raw"] if c["normalize"] else d["embed"]        # noqa: E731
+    embed = src(d0).to(dev, c["embed_dtype"]).contiguous()
+    half = embed.dtype != torch.float32
+    embed32 = embed.float() if half else embed
+    labels = d0["target"].to(dev)
+    seg = d0["seg"].to(dev, c["seg_dtype"]) if c["seg_dtype"] is not None else None
+    pred = d0["seg"].argmax(1).to(dev) if seg is None else None
+    bank = bank_e = enq = None
+    kw, kw_e = {}, {}
+    if c["bank"] != "none":
+        b0 = make_bank(K, c["M"], D, c["seed"] + 1)
+
+        def new_bank():
+            mb = cs.MemoryBank(K, c["M"], D, with_shadow=tensor).to(dev)
+            for k in _BANK_NAMES:
+                getattr(mb, k).copy_(b0[k])
+            if tensor:
+                mb.sync_shadow()
+            return mb
+        bank = new_bank()
+        bank_e = new_bank() if c["bank"] == "enqueue" else bank
+        kw = dict(segment_queue=bank.segment_queue, pixel_queue=bank.pixel_queue, bank_shadow=bank.shadow)
+        kw_e = dict(segment_queue=bank_e.segment_queue, pixel_queue=bank_e.pixel_queue, bank_shadow=bank_e.shadow)
+        if c["bank"] == "enqueue":
+            enq = dict(network_stride=c["stride"], pixel_update_freq=c["freq"], seed=c["seed"] % 997)
+    opts = cs.ContrastOptions(temperature=T, base_temperature=bT, max_samples=ms, max_views=mv, seed=c["seed"] % 1000,
+                              num_classes=K, normalize=c["normalize"], nan_safe=c["nan_safe"], precision=c["precision"])
+    mk = lambda e, q: cs.GraphedContrastStep(e, labels, seg=seg, predict=pred, options=opts, grad_scale=scale,   # noqa: E731
+                                             overlap_zero_fill=c["overlap"], fused=c["fused"],
+                                             sparse_reset=c["sparse"], enqueue=q, **kw)
+    # the twin reads the bank before the step under test writes it (same state as the eager loss reads)
+    twin = mk(embed32, None) if half else None
+    step = mk(embed, dict(enq, bank=bank) if enq else None)
+    want_fused = tensor and c["bank"] == "none" and not c["normalize"] and c["fused"] is None
+    if step.fused != want_fused or (twin is not None and twin.fused != step.fused):
+        return [f"fused = {step.fused}, expected {want_fused}: {desc}"]
+    ref = twin if half else step                 # the fp32 step checked against the eager step and float64
+    steps = [s for s in (twin, step) if s is not None]
+    for s in steps:
+        if s.sparse_reset:                       # nothing else may write a sparse-reset buffer: poison, then reset
+            s.grad.fill_(float("nan"))
+            s.reset_grad()
+    reached = {"half embed": half, "bank": bank is not None, "bank + enqueue": enq is not None,
+               "fused full-fill": step.fused and not step.sparse_reset, "fused sparse": step.sparse_reset,
+               "streaming bf16": tensor and not step.fused, "exact fp32": not tensor,
+               "non-integer label ratio": c["himg"] % h != 0 or c["wimg"] % w != 0}
+    scored, prev_A = 0, None
+    for r in range(n_rep):
+        why = f"replay {r}: {desc}"
+        if r:
+            d = draw(r)
+            embed.copy_(src(d).to(embed.dtype))
+            if half:
+                embed32.copy_(embed.float())
+            labels.copy_(d["target"])
+            if seg is not None:
+                seg.copy_(d["seg"].to(seg.dtype))
+            else:
+                pred.copy_(d["seg"].argmax(1))
+        for s in steps:
+            if not s.sparse_reset:               # a full fill must cover the whole buffer
+                s.grad.fill_(float("nan"))
+        q_before = torch.cat((bank.segment_queue, bank.pixel_queue), 1).double().cpu() if bank is not None else None
+        for s in steps:
+            s.replay()
+        _sync(dev)
+        meta = ref.ws.anchor_meta.clone()
+        TC, V, A = ref.ws.plan_header()[:3]
+        # eager step with counter r + 1 (trainer order with an enqueue: loss -> enqueue -> backward)
+        Fn._step_counter[0] = r
+        bank_mod._enqueue_counter[0] = r
+        e = embed32.clone().requires_grad_(True)
+        l2 = cs.pixel_contrast_loss(e, labels, seg=seg, predict=pred, options=opts, **kw_e)
+        ws = Fn.last_workspace(e.device)
+        if enq:
+            bank_e.enqueue(e.detach(), labels, network_stride=enq["network_stride"],
+                           pixel_update_freq=enq["pixel_update_freq"], seed=enq["seed"])
+        l2.backward(torch.full((), scale, device=dev))
+        _sync(dev)
+        lv, gv = ref.loss.item(), ref.grad
+        if not torch.equal(ws.anchor_meta, meta):
+            return [f"anchors differ from the eager step: {why}"]
+        le = l2.item()
+        if step.fused:                           # the one-kernel InfoNCE against the streaming sweeps: summation order
+            ok_l = (math.isnan(le) and math.isnan(lv)) or abs(le - lv) <= 2e-6 * abs(le) + 1e-6
+            gfloor = abs(scale) * 1e-3 / (bT * max(A, 1))
+            ok_g = math.isnan(le) or (e.grad - gv).abs().max().item() <= 2e-3 * max(e.grad.abs().max().item(), gfloor)
+        else:
+            ok_l = _same_bits(l2.detach(), ref.loss)
+            ok_g = torch.allclose(e.grad, gv, rtol=3e-6, atol=0, equal_nan=True)
+        if not (ok_l and ok_g):
+            return [f"loss / gradient differ from the eager step (loss {lv} vs {le}): {why}"]
+        if half and not (_same_bits(step.loss, ref.loss) and _same_bits(step.grad, ref.grad.to(embed.dtype))):
+            return [f"half embed: loss or gradient differ from the fp32 twin's (rounded once): {why}"]
+        if enq:
+            for k in _BANK_NAMES:
+                if not torch.equal(getattr(bank, k), getattr(bank_e, k)):
+                    return [f"bank {k} differs from the eager trainer order: {why}"]
+            if tensor and not torch.equal(bank.shadow, bank_e.shadow):
+                return [f"bank shadow differs from the eager trainer order: {why}"]
+        # the drawn anchors: a valid sample of the replay's labels
+        lab = P.downsample_labels(labels.cpu(), h, w).reshape(B, -1)
+        prd = (seg.float().argmax(1) if seg is not None else pred).cpu().reshape(B, -1)
+        if TC == 0 or V == 0:
+            kept = sum(len(P.kept_classes(lab[b], -1, mv)) for b in range(B))
+            if A != 0 or kept != TC or step.loss.item() != 0.0:
+                return [f"no anchors: A = {A}, {kept} classes qualify for {TC}, loss {step.loss.item()}: {why}"]
+            reached["A = 0 replay"] = True
+            pix = img = torch.zeros(0, dtype=torch.long)
+        else:
+            try:
+                _, _, A, (pix, img, cls, refrow) = check_sampling(ref.ws, lab, prd, ms, mv)
+            except AssertionError as ex:
+                return [f"invalid sample set ({str(ex)[:120]}): {why}"]
+            if prev_A and _tiles(prev_A) != _tiles(A):
+                reached["tile-edge crossing"] = True
+            # float64 closed form on the drawn rows (the values embed holds)
+            X = embed32.permute(0, 2, 3, 1).reshape(B, h * w, D)[img.to(dev), pix.to(dev)].double().cpu()
+            out = _f64_reference(c, X, cls, refrow, q_before if bank is not None else None)
+            if out is None:
+                cov["skipped"] = cov.get("skipped", 0) + 1
+            else:
+                lo, dA = out
+                dA = scale * dA
+                g_rows = gv.float().permute(0, 2, 3, 1).reshape(B, h * w, D)[img.to(dev), pix.to(dev)].double().cpu()
+                if math.isnan(lo):
+                    if not math.isnan(lv):
+                        return [f"reference NaN, engine {lv}: {why}"]
+                else:
+                    # (a loss or gradient that is 0 in real arithmetic — one class, no negatives — comes out as rounding
+                    # noise: absolute floors next to the relative bounds, the gradient's at 1e-3 of its natural scale;
+                    # grad_scale 0 needs exact zeros)
+                    gmax = max(dA.abs().max().item(), abs(scale) * 1e-3 / (bT * A), 1e-300)
+                    gabs = (g_rows - dA).abs().max().item() / gmax
+                    gfro = ((g_rows - dA).norm() / max(dA.norm().item(), gmax)).item()
+                    if tensor:
+                        ok = abs(lv - lo) <= 5e-5 * abs(lo) + 1e-6 and gabs <= 6e-3 and gfro <= 5e-3
+                    else:
+                        ok = abs(lv - lo) <= 2e-6 * abs(lo) + 1e-6 and gabs <= 1e-5
+                    if not ok:
+                        return [f"float64: loss {lv} vs {lo}, gradient max-abs {gabs:.2e} Frobenius {gfro:.2e}: {why}"]
+                scored += 1
+                cov["scored"] = cov.get("scored", 0) + 1
+        prev_A = A
+        # every element at no drawn anchor is +0
+        z = step.grad.clone()
+        if A:
+            z.view(B, D, h * w)[img.to(dev), :, pix.to(dev)] = 0
+        if bool(((z != 0) | torch.signbit(z)).any()):
+            n_bad = int(((z != 0) | torch.signbit(z)).sum())
+            return [f"{n_bad} gradient elements at no drawn anchor are not +0: {why}"]
+    for s in steps:
+        if int(s.counter.item()) != n_rep:
+            return [f"step counter {int(s.counter.item())} after {n_rep} replays: {desc}"]
+        if s.fused and int(s.ws.sync.abs().sum().item()) != 0:
+            return [f"the fused kernels left their counters armed: {desc}"]
+    if scored:
+        for k, v in reached.items():
+            cov[k] = cov.get(k, 0) + int(bool(v))
+    return []
+
+
+def _draw_graph_case(rng, it, scale):
+    """Configuration of fuzz case `it`.  The step path cycles (fused full-fill, streaming bf16, exact fp32, fused
+    sparse, any) so that few cases reach all of them; the rest is drawn.  Caps: B <= 2 scale (<= 8), h, w <= 32 scale, max_samples <= 300 scale
+    (<= 1024, the fused kernel's limit)."""
+    path = ("fused", "streaming", "exact", "fused", "any")[it % 5]
+    seq = ("edge", "empty", "random")[it % 3]
+    precision = "fp32" if path == "exact" else ("bf16" if path in ("fused", "streaming") else rng.choice(["fp32", "bf16"]))
+    D = 256 if precision == "bf16" else rng.choice([32, 64, 128, 256])
+    bank = "none" if path == "fused" else rng.choice(["none", "shadow", "enqueue"])
+    normalize = path != "fused" and rng.random() < 0.25
+    fused = None if path == "fused" else rng.choice([None, False])
+    if path == "streaming" and bank == "none" and not normalize:
+        fused = False
+    ms_cap = min(1024, 300 * scale)
+    ms = rng.choice([m for m in _MS_EDGES if m <= ms_cap]) if rng.random() < 0.6 else rng.randint(1, ms_cap)
+    if seq == "edge" and ms < 129:               # room for A on both sides of a tile edge
+        ms = rng.choice([m for m in _MS_EDGES if 129 <= m <= ms_cap])
+    B = rng.randint(1, min(8, 2 * scale))
+    if seq == "edge":            # few classes of many pixels: max_views ~ max_samples / 4 still leaves classes in
+        h, w, K = rng.randint(20, 32 * scale), rng.randint(20, 32 * scale), rng.randint(2, 4)
+        mv = rng.randint(max(1, ms // 6), max(1, ms // 3))
+    else:
+        h, w, K = rng.randint(4, 32 * scale), rng.randint(4, 32 * scale), rng.randint(2, 7)
+        mv = rng.randint(1, 24 * scale)
+    if rng.random() < 0.5:
+        st = rng.choice([1, 2, 4])
+        himg, wimg = h * st, w * st
+    else:                                        # nearest down-sampling with a non-integer ratio
+        himg, wimg = rng.randint(h, 3 * h + 2), rng.randint(w, 3 * w + 2)
+    # bank rows: mostly enough columns for every anchor's diagonal column (2 M K >= max_samples), sometimes fewer
+    M = rng.randint(2, 24 * scale) if rng.random() < 0.25 else -(-ms // (2 * K)) + rng.randint(0, 8)
+    # enqueue: a label grid labels[:, ::s, ::s] with no more positions than feature columns, pixel_update_freq <= M
+    stride = next(s for s in range(1, 64) if -(-himg // s) * -(-wimg // s) <= h * w)
+    half = (torch.bfloat16, torch.float16)
+    return dict(path=path, seq=seq, precision=precision, D=D, bank=bank, normalize=normalize, fused=fused,
+                sparse=it % 5 == 3 or (it % 5 == 4 and rng.random() < 0.5), overlap=rng.random() < 0.5,
+                embed_dtype=rng.choice([torch.float32, *half]),
+                seg_dtype=None if rng.random() < 0.2 else rng.choice([torch.float32, *half]),
+                grad_scale=rng.choice([1.0, 1.0, 0.37, -0.5, -2.0, 0.0]), nan_safe=rng.random() < 0.3,
+                B=B, h=h, w=w, K=K, ms=ms, mv=mv, himg=himg, wimg=wimg, M=M, stride=stride, freq=rng.randint(1, M),
+                T=rng.choice([0.07, 0.1, 0.5]), bT=0.07, block=rng.choice([2, 4, 8]), ignore=rng.choice([0.0, 0.1, 0.3]),
+                n_rep=rng.randint(3, 4), seed=rng.randint(0, 10 ** 6))
+
+
+def fuzz_graphed_step(seed: int, n: int, check_sampling, device="cpu", scale: int = 1):
+    """GraphedContrastStep over random configurations (path, bank / enqueue, dtypes, grad_scale, nan_safe, sparse reset,
+    overlapped fill, normalise, non-integer label ratios, max_samples around the tile edges), several replays with the
+    static inputs refilled in place between them (graphed_step_case: eager step, float64 closed form, zeros outside the
+    anchors, bank).  On a CPU the emulated kernels run the launch sequence eagerly (no capture, the fill branch
+    inline); on a device nothing is patched: the replays are CUDA-graph replays.  Returns (failures, coverage): how many
+    cases reached each of GRAPH_CATEGORIES, "scored" and "skipped" (replays the closed form scored / could not score)."""
     from contrastiveseg_b200 import graph_step
     rng = random.Random(seed)
-    bad = []
-    saved = (graph_step.GraphedContrastStep._capture, graph_step.GraphedContrastStep._fork_zero_fill,
-             graph_step.GraphedContrastStep._join_zero_fill)
-    graph_step.GraphedContrastStep._capture = lambda self, warmup: None            # no CUDA graphs on a CPU: run eagerly
-    graph_step.GraphedContrastStep._fork_zero_fill = lambda self: self._side_branch(0)
-    graph_step.GraphedContrastStep._join_zero_fill = lambda self: None
+    bad, cov = [], {k: 0 for k in GRAPH_CATEGORIES + ("scored", "skipped")}
+    G = graph_step.GraphedContrastStep
+    saved = (G._capture, G._fork_zero_fill, G._join_zero_fill)
+    if torch.device(device).type == "cpu":
+        G._capture = lambda self, warmup: None                 # no CUDA graphs on a CPU: run eagerly
+        G._fork_zero_fill = lambda self: self._side_branch(0)
+        G._join_zero_fill = lambda self: None
     try:
         for it in range(n):
-            B, D, h, w = rng.randint(1, 3), rng.choice([32, 64]), rng.randint(4, 30), rng.randint(4, 30)
-            K, ms, mv = rng.randint(2, 9), rng.randint(4, 150), rng.randint(1, 12)
-            st, block, mem = rng.choice([1, 2, 4]), rng.choice([2, 4, 8]), rng.random() < 0.4
-            norm, overlap, sd = rng.random() < 0.3, rng.random() < 0.5, rng.randint(0, 10 ** 6)
-            desc = f"graph seed={seed} it={it} B={B} D={D} {h}x{w} K={K} ms={ms} mv={mv} mem={mem} norm={norm} overlap={overlap}"
-            data = make_contrast_batch(B=B, D=D, h=h, w=w, num_classes=K, img_stride=st, block=block, seed=sd)
-            bank = make_bank(K, rng.randint(4, 20), D, sd + 1)
-            kw = dict(segment_queue=bank["segment_queue"], pixel_queue=bank["pixel_queue"]) if mem else {}
-            opts = cs.ContrastOptions(temperature=0.1, base_temperature=0.07, max_samples=ms, max_views=mv, seed=sd % 1000,
-                                      num_classes=K, normalize=norm)
-            src = data["embed_raw"] if norm else data["embed"]
-            step = cs.GraphedContrastStep(src.clone(), data["target"], seg=data["seg"], options=opts,
-                                          overlap_zero_fill=overlap, **kw)
-            for r in range(2):
-                loss, grad = step.replay()
-                meta, lv, gv = step.ws.anchor_meta.clone(), loss.clone(), grad.clone()
-                Fn._step_counter[0] = r
-                e = src.clone().requires_grad_(True)
-                l2 = cs.pixel_contrast_loss(e, data["target"], seg=data["seg"], options=opts, **kw)
-                ws = Fn.last_workspace(e.device)
-                l2.backward()
-                same_l = torch.equal(l2.detach(), lv) or (torch.isnan(l2) and torch.isnan(lv))
-                ok_g = torch.allclose(e.grad, gv, rtol=3e-6, atol=0, equal_nan=True)
-                if not (torch.equal(ws.anchor_meta, meta) and same_l and ok_g):
-                    bad.append(f"replay {r} differs from the eager step: {desc}")
-                    break
+            c = _draw_graph_case(rng, it, scale)
+            desc = "graph seed={} it={} {}".format(seed, it, " ".join(f"{k}={v}" for k, v in c.items()))
+            draw = graph_step_inputs(c["B"], c["D"], c["h"], c["w"], c["K"], c["himg"], c["wimg"], c["block"],
+                                     c["ignore"], c["seq"], c["seed"])
+            bad += graphed_step_case(c, draw, c["n_rep"], device, check_sampling, cov, desc)
     finally:
-        (graph_step.GraphedContrastStep._capture, graph_step.GraphedContrastStep._fork_zero_fill,
-         graph_step.GraphedContrastStep._join_zero_fill) = saved
-    return bad
+        G._capture, G._fork_zero_fill, G._join_zero_fill = saved
+    return bad, cov
 
 
 def fuzz_trainer_hook(seed: int, n: int):

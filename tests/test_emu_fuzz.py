@@ -7,6 +7,8 @@ import emu_fuzz
 import emu_harness
 import test_gpu_parity as G
 
+NGRAPH = 24
+
 
 @pytest.fixture
 def emu(monkeypatch):
@@ -39,7 +41,10 @@ def test_fuzz_tensor_path(emu):
 
 
 def test_fuzz_graphed_step(emu):
-    assert emu_fuzz.fuzz_graphed_step(seed=17, n=15) == []
+    """The captured step's launch sequence (run eagerly): every path, bank and dtype reached, every replay scored."""
+    bad, cov = emu_fuzz.fuzz_graphed_step(seed=17, n=NGRAPH, check_sampling=G._check_device_sampling)
+    assert bad == []
+    assert all(cov[k] >= 1 for k in emu_fuzz.GRAPH_CATEGORIES), cov
 
 
 def test_fuzz_trainer_hook(emu):

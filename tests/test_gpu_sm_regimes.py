@@ -422,3 +422,40 @@ def test_fuzz_topk_on_the_device():
 def test_fuzz_device_sampling_on_the_device():
     assert emu_fuzz.fuzz_device_sampling(seed=14, n=25, check_sampling=G._check_device_sampling, device=DEV,
                                          scale=4) == []
+
+
+# The captured step (GraphedContrastStep) as real CUDA-graph replays, inputs refilled in place between replays: scale 4
+# draws max_samples up to 1024 (the one-kernel InfoNCE's 8 x 4 tiles), B up to 8 and feature maps up to 128 x 128.
+@pytest.mark.gpu
+@pytest.mark.timeout(1800)
+def test_fuzz_captured_steps_on_the_device():
+    bad, cov = emu_fuzz.fuzz_graphed_step(seed=17, n=30, check_sampling=G._check_device_sampling, device=DEV, scale=4)
+    assert bad == []
+    assert all(cov[k] >= 1 for k in emu_fuzz.GRAPH_CATEGORIES), cov
+
+
+# bench.py's S1 shape (Cityscapes crop 512 x 1024 at stride 4, 19 classes): a 268 MB fp32 gradient filled by
+# k_fill_zero_excl next to the one-kernel InfoNCE (or kept by the sparse reset), 1024 anchors scattered into sectors
+S1 = dict(B=8, D=256, h=128, w=256, K=19, himg=512, wimg=1024, ms=1024, mv=100, T=0.1, bT=0.07, block=32)
+_S1_DRAWS = {}
+
+
+@pytest.mark.gpu
+@pytest.mark.timeout(900)
+@pytest.mark.parametrize("embed_dtype", [torch.float32, BF], ids=["fp32", "bf16"])
+@pytest.mark.parametrize("sparse", [False, True], ids=["full_fill", "sparse_reset"])
+def test_captured_fused_step_at_the_s1_shape(sparse, embed_dtype):
+    c = dict(S1, precision="bf16", bank="none", normalize=False, fused=None, sparse=sparse, overlap=True,
+             embed_dtype=embed_dtype, seg_dtype=torch.float32, grad_scale=0.1, nan_safe=False, seed=304)
+    inputs = emu_fuzz.graph_step_inputs(c["B"], c["D"], c["h"], c["w"], c["K"], c["himg"], c["wimg"], c["block"], 0.0,
+                                        "random", c["seed"])
+
+    def draw(r):                 # the same inputs for every parameter set (embed_raw is not read: no normalise)
+        if r not in _S1_DRAWS:
+            _S1_DRAWS[r] = {k: v for k, v in inputs(r).items() if k != "embed_raw"}
+        return _S1_DRAWS[r]
+
+    cov = {}
+    bad = emu_fuzz.graphed_step_case(c, draw, 3, DEV, G._check_device_sampling, cov, f"S1 sparse={sparse} {embed_dtype}")
+    assert bad == []
+    assert cov["scored"] == 3 and cov["fused sparse" if sparse else "fused full-fill"] == 1, cov

@@ -28,7 +28,8 @@ if __name__ == "__main__":
                          ("segce", lambda s: emu_fuzz.fuzz_segce(s, n)), ("topk", lambda s: emu_fuzz.fuzz_topk(s, n)),
                          ("devrng", lambda s: emu_fuzz.fuzz_device_sampling(s, n, G._check_device_sampling)),
                          ("tensor", lambda s: emu_fuzz.fuzz_tensor_path(s, max(1, n // 5))),
-                         ("graph", lambda s: emu_fuzz.fuzz_graphed_step(s, max(1, n // 2))),
+                         ("graph", lambda s: emu_fuzz.fuzz_graphed_step(s, max(1, n // 2),
+                                                                        G._check_device_sampling)[0]),
                          ("hook", lambda s: emu_fuzz.fuzz_trainer_hook(s, max(1, n // 2))),
                          ("wrappers", lambda s: emu_fuzz.fuzz_wrappers(s, n))):
             bad = fn(1000 * r + base)
