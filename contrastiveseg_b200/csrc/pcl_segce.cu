@@ -378,7 +378,8 @@ k_segce_bwd_gather(SegCeArgs a, const float* __restrict__ lse, const float* __re
       acc += wy * wx * wc * (prob - (c == (int)t ? 1.f : 0.f));
     }
   }
-  dseg[((int64_t)b * a.K + c) * hw + e] = acc * scale;
+  // every pixel ignored (weight sum 0): acc is 0 and scale infinite; the gradient is 0, as the tile kernels leave it
+  dseg[((int64_t)b * a.K + c) * hw + e] = fin[1] == 0.f ? 0.f : acc * scale;
 }
 
 }  // namespace pcl

@@ -1,9 +1,12 @@
 """TEST INFRASTRUCTURE: differential fuzzing of the engine (real SIMT kernel sources on the host-fiber emulator,
 tests/emu) against the oracle over random geometries.  Used by tests/test_emu_fuzz.py (bounded) and
 tools/emu_fuzz.py (long runs).  Every fuzzer returns a list of failure descriptions (empty = clean); fuzz_graphed_step
-also returns how many cases reached each of its coverage categories, so that a test can require all of them.
+and fuzz_graphed_criterion also return how many cases reached each of their coverage categories, so that a test can
+require all of them.
 
-It found the out-of-bounds wrap write for pixel_update_freq > memory_size (now refused, csrc/pcl_bank.cu: make_dims)."""
+It found the out-of-bounds wrap write for pixel_update_freq > memory_size (now refused, csrc/pcl_bank.cu: make_dims)
+and the NaN gradient of the two-call seg CE with a label grid smaller than the logits and every pixel ignored (now 0,
+csrc/pcl_segce.cu: k_segce_bwd_gather)."""
 import math
 import random
 
@@ -443,6 +446,78 @@ def _f64_reference(c, X, cls, refrow, queue):
     return loss.item(), dA
 
 
+def score_step_replay(c, ref, step, embed32, labels, seg, pred, q_before, scale, check_sampling, cov, reached, prev_A,
+                      why):
+    """The float64 scoring of one replay of a captured contrast step: the drawn anchors are a valid sample of the
+    replay's labels (check_sampling), loss and gradient rows of `ref` (the fp32 step with the anchors of `step`: step
+    itself, or its fp32 twin when embed is half) match the closed form on the drawn rows (q_before: the bank as the
+    replay read it), and every element of step.grad at no drawn anchor is +0.  scale: the step's grad_scale.  Counts the
+    replay in cov["scored"] / cov["skipped"] and sets reached["A = 0 replay"] / ["tile-edge crossing"].
+    Returns (failure or None, A, whether the closed form scored the replay, the float64 contrast loss: 0 when A = 0,
+    None when unscored)."""
+    dev = labels.device
+    B, D, h, w, ms, mv, bT = (c[k] for k in ("B", "D", "h", "w", "ms", "mv", "bT"))
+    tensor = c["precision"] == "bf16"
+    TC, V, A = ref.ws.plan_header()[:3]
+    lv, gv = ref.loss.item(), ref.grad
+    scored, lo = False, None
+    # the drawn anchors: a valid sample of the replay's labels
+    lab = P.downsample_labels(labels.cpu(), h, w).reshape(B, -1)
+    lab[lab == c.get("ignore_label", -1)] = -1
+    prd = (seg.float().argmax(1) if seg is not None else pred).cpu().reshape(B, -1)
+    if TC == 0 or V == 0:
+        kept = sum(len(P.kept_classes(lab[b], -1, mv)) for b in range(B))
+        if A != 0 or kept != TC or step.loss.item() != 0.0:
+            return (f"no anchors: A = {A}, {kept} classes qualify for {TC}, loss {step.loss.item()}: {why}", A, False,
+                    None)
+        reached["A = 0 replay"] = True
+        pix = img = torch.zeros(0, dtype=torch.long)
+        lo = 0.0
+    else:
+        try:
+            _, _, A, (pix, img, cls, refrow) = check_sampling(ref.ws, lab, prd, ms, mv)
+        except AssertionError as ex:
+            return (f"invalid sample set ({str(ex)[:120]}): {why}", A, False, None)
+        if prev_A and _tiles(prev_A) != _tiles(A):
+            reached["tile-edge crossing"] = True
+        # float64 closed form on the drawn rows (the values embed holds)
+        X = embed32.permute(0, 2, 3, 1).reshape(B, h * w, D)[img.to(dev), pix.to(dev)].double().cpu()
+        out = _f64_reference(c, X, cls, refrow, q_before)
+        if out is None:
+            cov["skipped"] = cov.get("skipped", 0) + 1
+        else:
+            lo, dA = out
+            dA = scale * dA
+            g_rows = gv.float().permute(0, 2, 3, 1).reshape(B, h * w, D)[img.to(dev), pix.to(dev)].double().cpu()
+            if math.isnan(lo):
+                if not math.isnan(lv):
+                    return (f"reference NaN, engine {lv}: {why}", A, False, None)
+            else:
+                # (a loss or gradient that is 0 in real arithmetic — one class, no negatives — comes out as rounding
+                # noise: absolute floors next to the relative bounds, the gradient's at 1e-3 of its natural scale;
+                # grad_scale 0 needs exact zeros)
+                gmax = max(dA.abs().max().item(), abs(scale) * 1e-3 / (bT * A), 1e-300)
+                gabs = (g_rows - dA).abs().max().item() / gmax
+                gfro = ((g_rows - dA).norm() / max(dA.norm().item(), gmax)).item()
+                if tensor:
+                    ok = abs(lv - lo) <= 5e-5 * abs(lo) + 1e-6 and gabs <= 6e-3 and gfro <= 5e-3
+                else:
+                    ok = abs(lv - lo) <= 2e-6 * abs(lo) + 1e-6 and gabs <= 1e-5
+                if not ok:
+                    return (f"float64: loss {lv} vs {lo}, gradient max-abs {gabs:.2e} Frobenius {gfro:.2e}: {why}", A,
+                            False, None)
+            scored = True
+            cov["scored"] = cov.get("scored", 0) + 1
+    # every element at no drawn anchor is +0
+    z = step.grad.clone()
+    if A:
+        z.view(B, D, h * w)[img.to(dev), :, pix.to(dev)] = 0
+    if bool(((z != 0) | torch.signbit(z)).any()):
+        n_bad = int(((z != 0) | torch.signbit(z)).sum())
+        return (f"{n_bad} gradient elements at no drawn anchor are not +0: {why}", A, False, None)
+    return None, A, scored, lo
+
+
 def graphed_step_case(c, draw, n_rep, device, check_sampling, cov, desc):
     """One GraphedContrastStep (configuration `c`), `n_rep` replays, the static inputs refilled in place from draw(r)
     before replay r.  Every replay: the anchors are a valid sample (check_sampling) and those of eager step r + 1,
@@ -558,57 +633,12 @@ def graphed_step_case(c, draw, n_rep, device, check_sampling, cov, desc):
                     return [f"bank {k} differs from the eager trainer order: {why}"]
             if tensor and not torch.equal(bank.shadow, bank_e.shadow):
                 return [f"bank shadow differs from the eager trainer order: {why}"]
-        # the drawn anchors: a valid sample of the replay's labels
-        lab = P.downsample_labels(labels.cpu(), h, w).reshape(B, -1)
-        prd = (seg.float().argmax(1) if seg is not None else pred).cpu().reshape(B, -1)
-        if TC == 0 or V == 0:
-            kept = sum(len(P.kept_classes(lab[b], -1, mv)) for b in range(B))
-            if A != 0 or kept != TC or step.loss.item() != 0.0:
-                return [f"no anchors: A = {A}, {kept} classes qualify for {TC}, loss {step.loss.item()}: {why}"]
-            reached["A = 0 replay"] = True
-            pix = img = torch.zeros(0, dtype=torch.long)
-        else:
-            try:
-                _, _, A, (pix, img, cls, refrow) = check_sampling(ref.ws, lab, prd, ms, mv)
-            except AssertionError as ex:
-                return [f"invalid sample set ({str(ex)[:120]}): {why}"]
-            if prev_A and _tiles(prev_A) != _tiles(A):
-                reached["tile-edge crossing"] = True
-            # float64 closed form on the drawn rows (the values embed holds)
-            X = embed32.permute(0, 2, 3, 1).reshape(B, h * w, D)[img.to(dev), pix.to(dev)].double().cpu()
-            out = _f64_reference(c, X, cls, refrow, q_before if bank is not None else None)
-            if out is None:
-                cov["skipped"] = cov.get("skipped", 0) + 1
-            else:
-                lo, dA = out
-                dA = scale * dA
-                g_rows = gv.float().permute(0, 2, 3, 1).reshape(B, h * w, D)[img.to(dev), pix.to(dev)].double().cpu()
-                if math.isnan(lo):
-                    if not math.isnan(lv):
-                        return [f"reference NaN, engine {lv}: {why}"]
-                else:
-                    # (a loss or gradient that is 0 in real arithmetic — one class, no negatives — comes out as rounding
-                    # noise: absolute floors next to the relative bounds, the gradient's at 1e-3 of its natural scale;
-                    # grad_scale 0 needs exact zeros)
-                    gmax = max(dA.abs().max().item(), abs(scale) * 1e-3 / (bT * A), 1e-300)
-                    gabs = (g_rows - dA).abs().max().item() / gmax
-                    gfro = ((g_rows - dA).norm() / max(dA.norm().item(), gmax)).item()
-                    if tensor:
-                        ok = abs(lv - lo) <= 5e-5 * abs(lo) + 1e-6 and gabs <= 6e-3 and gfro <= 5e-3
-                    else:
-                        ok = abs(lv - lo) <= 2e-6 * abs(lo) + 1e-6 and gabs <= 1e-5
-                    if not ok:
-                        return [f"float64: loss {lv} vs {lo}, gradient max-abs {gabs:.2e} Frobenius {gfro:.2e}: {why}"]
-                scored += 1
-                cov["scored"] = cov.get("scored", 0) + 1
+        bad, A, ok, _ = score_step_replay(c, ref, step, embed32, labels, seg, pred, q_before, scale, check_sampling,
+                                          cov, reached, prev_A, why)
+        if bad is not None:
+            return [bad]
+        scored += ok
         prev_A = A
-        # every element at no drawn anchor is +0
-        z = step.grad.clone()
-        if A:
-            z.view(B, D, h * w)[img.to(dev), :, pix.to(dev)] = 0
-        if bool(((z != 0) | torch.signbit(z)).any()):
-            n_bad = int(((z != 0) | torch.signbit(z)).sum())
-            return [f"{n_bad} gradient elements at no drawn anchor are not +0: {why}"]
     for s in steps:
         if int(s.counter.item()) != n_rep:
             return [f"step counter {int(s.counter.item())} after {n_rep} replays: {desc}"]
@@ -689,6 +719,479 @@ def fuzz_graphed_step(seed: int, n: int, check_sampling, device="cpu", scale: in
             bad += graphed_step_case(c, draw, c["n_rep"], device, check_sampling, cov, desc)
     finally:
         G._capture, G._fork_zero_fill, G._join_zero_fill = saved
+    return bad, cov
+
+
+# ---- the captured criterion (GraphedContrastCriterion) ---------------------------------------------------------------
+CRIT_COMBOS = ("ce", "ce_lovasz", "ce_ohem", "aux_ce", "aux_rmi", "aux_ohem", "mem_ce", "mem_rmi", "mem_lovasz",
+               "mem_ohem")
+CRIT_CATEGORIES = CRIT_COMBOS + ("CE one-call", "CE one-call above 24 classes", "CE two-call", "fp16 head",
+                                 "bf16 head with two terms", "OHEM branch flip", "Lovasz present-set change",
+                                 "all-ignored replay", "A = 0 replay", "bank + enqueue", "negative grad_scale",
+                                 "set_grad_scale mid-case")
+_HALF_EPS = {torch.bfloat16: torch.finfo(torch.bfloat16).eps, torch.float16: torch.finfo(torch.float16).eps}
+
+
+def _pooled(n, s):
+    return n if s == 1 else (n + 2 * (s // 2) - s) // s + 1
+
+
+def _criterion_geometry(rng, c, mode, cap):
+    """h, w, H, W (and B) of geometry `mode` ("up": integer factor, "nonint", "identity", "down": a label grid smaller
+    than seg in one or both dimensions), B K H W within `cap`; c["refused"]: the terms refuse it (only the seg CE takes a
+    label grid smaller than seg; RMI needs a pooled map of at least radius x radius)."""
+    h, w = c["h0"], c["w0"]
+    while True:
+        if mode == "up":
+            st = rng.choice([2, 3, 4])
+            H, W = h * st, w * st
+        elif mode == "nonint":
+            H, W = rng.randint(h + 1, 3 * h + 2), rng.randint(w + 1, 3 * w + 2)
+            H, W = H + (H % h == 0), W + (W % w == 0)
+        elif mode == "identity":
+            H, W = h, w
+        else:
+            which = rng.choice(["H", "W", "both"])
+            H = rng.randint(max(1, h // 2), h - 1) if which != "W" else h * rng.choice([1, 2])
+            W = rng.randint(max(1, w // 2), w - 1) if which != "H" else w * rng.choice([1, 2])
+        if c["K"] * H * W <= cap or h <= 4 and w <= 4:
+            break
+        h, w = max(4, h * 3 // 4), max(4, w * 3 // 4)
+    B = max(1, min(c["B0"], cap // (c["K"] * H * W)))
+    refused = mode == "down" and c["name"] not in ("ce", "aux_ce", "mem_ce")
+    if c["name"].endswith("rmi"):
+        r, st = c["params"]["rmi_radius"], c["params"]["rmi_pool_stride"]
+        refused = refused or min(_pooled(H, st), _pooled(W, st)) < r
+    # enqueue: a label grid labels[:, ::s, ::s] with no more positions than feature columns
+    stride = next(s for s in range(1, 64) if -(-H // s) * -(-W // s) <= h * w)
+    c.update(mode=mode, h=h, w=w, H=H, W=W, B=B, refused=refused, stride=stride)
+    return c
+
+
+def _draw_criterion_case(rng, it, scale, device):
+    """Configuration of criterion fuzz case `it`: the wrapper x seg-term combination cycles through CRIT_COMBOS; case 0
+    draws K above 24 with integer up-sampling (the one-call seg CE of several class chunks), case 5 on a device K >= 150,
+    cases 3 and 4 a label grid smaller than seg (the two-call seg CE; RMI refuses it); cases 1 (bf16 seg: a bf16 head
+    with two terms), 6 (fp16 seg, bank with enqueue) and 2 (negative grad_scale) pin what the categories need, the rest
+    is drawn.  Caps: B <= 2 scale (<= 8), h, w <= 12 scale (<= 128), max_samples <= 96 scale (<= 1024); on a device
+    case 0 takes max_samples = 1024.  The aux weight is never 1 and the grad_scale set mid-case never 0, so a
+    coefficient lost on the way to a term shows."""
+    cuda = torch.device(device).type == "cuda"
+    name = CRIT_COMBOS[it % len(CRIT_COMBOS)]
+    K = rng.randint(25, 40) if it == 0 else (rng.randint(150, 171) if it == 5 and cuda else rng.randint(2, 24))
+    hw = min(128, 12 * scale) if K < 150 else 24
+    ms = min(1024, 96 * scale)
+    ms = rng.choice([m for m in _MS_EDGES if m <= ms]) if rng.random() < 0.5 else rng.randint(1, ms)
+    if cuda and it == 0:
+        ms = 1024
+    half = [torch.float32, torch.bfloat16, torch.float16]
+    ohem_sum = name in ("ce_ohem", "mem_ohem") and rng.random() < 0.5
+    params = dict(ce_ignore_index=rng.choice([-1, 255]), rmi_radius=rng.randint(1, 4), rmi_pool_way=rng.randint(0, 1),
+                  lambda_way=rng.randint(0, 1), ce_reduction="sum" if ohem_sum else "elementwise_mean")
+    params["rmi_pool_stride"] = params["rmi_pool_size"] = rng.randint(1, 4)
+    if rng.random() < 0.4:
+        params["ce_weight"] = [round(0.5 + rng.random(), 3) for _ in range(K)]
+    n_rep = rng.randint(3, 4)
+    all_ignored = it in (1, 2) or rng.random() < 0.3
+    c = dict(name=name, K=K, h0=rng.randint(4, hw), w0=rng.randint(4, hw), B0=rng.randint(1, min(8, 2 * scale)),
+             D=rng.choice([32, 64, 256]) if cuda else 32, ms=ms, mv=rng.randint(1, min(100, 16 * scale)),
+             seq=("edge", "empty", "random")[it % 3], block=rng.choice([2, 4, 8]), ignore=rng.choice([0.0, 0.1, 0.3]),
+             params=params, lw={"seg_loss": rng.choice([1.0, 0.7]), "aux_loss": rng.choice([0.4, 0.25, 1.5])},
+             seg_dtype=torch.bfloat16 if it == 1 else (torch.float16 if it == 6 else rng.choice(half)),
+             aux_dtype=rng.choice(half), embed_dtype=rng.choice([torch.float32, torch.bfloat16]),
+             bank=("enqueue" if it == 6 else rng.choice(["read", "enqueue"])) if name.startswith("mem") else "none",
+             grad_scale=-0.5 if it == 2 else rng.choice([1.0, 0.37, -0.5, -2.0, 0.0]),
+             scale2=rng.choice([2.0, -1.0, 0.5, -0.25]), n_rep=4 if all_ignored else n_rep,
+             all_ignored=all_ignored, seed=rng.randint(0, 10 ** 6), T=None, bT=None,
+             precision="fp32", normalize=False, nan_safe=False, ignore_label=params["ce_ignore_index"])
+    c["r_set"] = rng.randint(1, c["n_rep"] - 1)
+    c["M"] = -(-ms // (2 * K)) + rng.randint(0, 8)
+    c["freq"] = rng.randint(1, c["M"])
+    cap = (2 * 10 ** 6 if name.endswith("rmi") else 8 * 10 ** 6) if cuda else 8 * 10 ** 4
+    mode = "up" if it == 0 else ("down" if it in (3, 4) else rng.choice(["up", "nonint", "identity", "down"]))
+    return _criterion_geometry(rng, c, mode, cap), cap
+
+
+def criterion_inputs(c):
+    """inputs(r): the CPU (embed, target, seg, seg_aux) of replay r, on graph_step_inputs's label sequence (A = 0 on
+    replay 1 of "empty", one class on the odd replays of "edge") with: replay 1 of "random" without the first labelled
+    class of replay 0 (it comes back on replay 2), replay 3 with every label ignored when c["all_ignored"], and for
+    OHEM three quarters of replay 1's labels ignored: with min_kept at half the count under the threshold of replay 0,
+    too few pixels lie under it and the select branch runs, where the other replays take the threshold branch.  Ignored
+    labels are c's ignore index."""
+    ign = c["params"]["ce_ignore_index"]
+    base = graph_step_inputs(c["B"], c["D"], c["h"], c["w"], c["K"], c["H"], c["W"], c["block"], c["ignore"],
+                             c["seq"], c["seed"])
+    gone = []
+
+    def inputs(r):
+        d = base(r)
+        t = d["target"]
+        if r == 0 and bool((t >= 0).any()):
+            gone.append(int(t[t >= 0][0]))
+        if c["seq"] == "random" and r == 1 and gone:
+            t[t == gone[0]] = -1
+        if c["all_ignored"] and r == 3:
+            t.fill_(-1)
+        if "ohem" in c["name"] and r == 1:
+            t[torch.rand(t.shape, generator=torch.Generator().manual_seed(c["seed"] + 5)) < 0.75] = -1
+        seg = d["seg"]
+        if "ohem" in c["name"]:             # the logit range OHEM's bounds were measured on (test_gpu_ohem._inputs)
+            seg = (torch.rand(seg.shape, generator=torch.Generator().manual_seed(c["seed"] + 7 * r)) * 2 - 1) * 4
+        aux = seg * 0.5 + 0.3 * torch.randn(seg.shape, generator=torch.Generator().manual_seed(c["seed"] + r))
+        t[t == -1] = ign
+        return d["embed"], t, seg, aux
+    return inputs
+
+
+def _upsample_f64(s, H, W):
+    """s (B, K, h, w) float64 bilinearly (align_corners=True) up-sampled to H x W at the source coordinates the fp32
+    kernels sample (test_gpu_many_classes._bilinear_matrix): for non-integer ratios the exact coordinates differ by
+    more than OHEM's gradient bound allows."""
+    import test_gpu_many_classes as M
+    my, mx = M._bilinear_matrix(s.shape[2], H, s.device), M._bilinear_matrix(s.shape[3], W, s.device)
+    return torch.einsum("yh,bkhw,xw->bkyx", my, s, mx)
+
+
+def _score_seg_term(t, x, target, gs, gap_frac):
+    """One seg term of a replay against its float64 oracle on the values the head holds (x, fp32) and this replay's
+    labels, at the term's bounds (those of its standalone tests).  t.loss / t.dseg: the engine's loss and gradient
+    (times gs = grad_scale * coef).  Returns (failure or None, scored, loss_ref, gradient_ref * gs, gradient bound
+    (absolute), loss bound (absolute), (B, h, w) mask of the positions the gradient bound does not cover or None,
+    OHEM branch or None)."""
+    from oracle.lovasz_port import footprint_mask, lovasz_loss_and_grad
+    from oracle.ohem_port import ohem_loss
+    from oracle.rmi_port import rmi_loss_and_grad
+    import test_gpu_many_classes as M
+    B, K, h, w = x.shape
+    lv, d = t.loss.item(), t.dseg.double()
+    unscored = (None, False, None, None, None, None, None, None)
+    zero_ok = torch.count_nonzero(t.dseg).item() == 0
+    mask = branch = None
+    if t.kind == "ce":
+        s = x.double().requires_grad_(True)
+        wt = None if t.weight is None else t.weight.double()
+        ref = M.seg_ce_reference(s, target, wt, t.ignore)
+        lref = ref.item()
+        if not bool((target != t.ignore).any()):          # every pixel ignored: NaN, zero gradient
+            if not (math.isnan(lv) and zero_ok):
+                return (f"seg CE, every pixel ignored: loss {lv}, {torch.count_nonzero(t.dseg).item()} gradient "
+                        "elements not 0",) + unscored[1:]
+            return None, True, float("nan"), torch.zeros_like(d), 0.0, 0.0, None, None
+        if math.isnan(lref):
+            return unscored
+        ref.backward()
+        gref = s.grad * gs
+        gmax = gref.abs().max().item()
+        gbound, lbound = 1e-5 * gmax, 2e-6 * abs(lref)
+    elif t.kind == "lovasz":
+        lref, gref, near = lovasz_loss_and_grad(x, target, 1.0, ignore_index=t.ignore, near_tie_ulps=64)
+        lref, gref = lref.item(), gref * gs
+        gmax = gref.abs().max().item()
+        gbound, lbound = 1e-4 * gmax, 1e-5 * max(abs(lref), 1e-6)
+        mask = footprint_mask(near, h, w)
+        if gmax > 0:
+            if bool(mask.float().mean() > 0.5):           # near-tie footprints cover more than half the positions
+                return unscored
+            fro = ((d - gref).norm() / gref.norm()).item()
+            if fro > 1.7e-4:
+                return (f"Lovasz gradient: relative Frobenius error {fro:.2e}",) + unscored[1:]
+    elif t.kind == "ohem":
+        from contrastiveseg_b200.functional import ohem_selection
+        red = ("mean", "sum")[t.red]
+        kw = dict(weight=t.weight, ignore_index=t.ignore, thresh=t.thresh, min_kept=t.min_kept, reduction=red)
+        s = x.double().requires_grad_(True)
+        dd = ohem_loss(_upsample_f64(s, *target.shape[1:]), target, details=True, **kw)
+        dd["loss"].backward()
+        gref = s.grad
+        sel = ohem_selection(x, target, t.weight, t.ignore, t.thresh, t.min_kept, red)
+        branch = sel["branch"]
+        if not (sel["n"] == dd["n"] and sel["count"] == dd["count"] and torch.equal(sel["selected"], dd["selected"])):
+            return (f"OHEM selection: n {sel['n']} / {dd['n']}, count {sel['count']} / {dd['count']}",) + unscored[1:]
+        if gap_frac < 0.5:                                # the gap ignored more than half the counted pixels
+            return unscored
+        lref, gref = dd["loss"].item(), gref * gs
+        if math.isnan(lref):                              # mean of an empty selection: NaN, zero gradient
+            if dd["n"] == 0 or dd["count"] != 0 or red != "mean":
+                return unscored
+            if not (math.isnan(lv) and zero_ok):
+                return (f"OHEM, empty selection: loss {lv}, gradient not 0",) + unscored[1:]
+            return None, True, lref, torch.zeros_like(d), 0.0, 0.0, None, branch
+        gmax = gref.abs().max().item()
+        gbound, lbound = 3.8e-6 * gmax, 2.1e-7 * abs(lref)
+    else:                                                 # rmi
+        r_, way, st, lam, lway, lw = t.params
+        kw = dict(num_classes=K, radius=r_, pool_way=way, pool_stride=st, weight_lambda=lam, lambda_way=lway,
+                  loss_weight=lw)
+        try:
+            lref, gref = rmi_loss_and_grad(x, target, 1.0, **kw)
+            _, g32 = rmi_loss_and_grad(x, target, 1.0, front=torch.float32, **kw)
+        except RuntimeError:                              # a reference solve that is not positive definite
+            return unscored
+        lref = lref.item()
+        if not math.isfinite(lref):
+            return unscored
+        gmax0 = gref.abs().max().item()
+        if gmax0 > 0 and bool(((g32 - gref).abs() <= 1e-4 * gmax0).float().mean() < 0.5):
+            return unscored                               # the reference's own spread covers most elements
+        spread = (g32 - gref).abs().max().item() * abs(gs)
+        gref = gref * gs
+        gmax = gref.abs().max().item()
+        gbound, lbound = max(1e-4 * gmax, 4 * spread), 1e-5 * max(abs(lref), 1e-3)
+    if abs(lv - lref) > lbound or math.isnan(lv):
+        return (f"{t.kind} loss {lv} vs float64 {lref}",) + unscored[1:]
+    if gmax == 0:
+        if not zero_ok:
+            return (f"{t.kind}: the float64 gradient is 0, {torch.count_nonzero(t.dseg).item()} elements are not",) + \
+                unscored[1:]
+    else:
+        err = (d - gref).abs().amax(dim=1)                # (B, h, w): worst class plane
+        if mask is not None:
+            err = err[~mask]
+        if err.numel() and err.max().item() > gbound:
+            return (f"{t.kind} gradient: max error {err.max().item():.3e}, bound {gbound:.3e}",) + unscored[1:]
+    return None, True, lref, gref, gbound, lbound, mask, branch
+
+
+def graphed_criterion_case(c, device, check_sampling, cov, desc):
+    """One GraphedContrastCriterion (configuration `c`), c["n_rep"] replays, the target, every head and embed refilled
+    in place from criterion_inputs before each replay (OHEM's target gapped first, so fp32 and float64 select the same
+    pixels), grad_scale changed with set_grad_scale before replay c["r_set"].  Every replay: the loss equals the eager
+    seg terms plus loss_weight times a twin GraphedContrastStep to the bit, the embed gradient is the twin's (rounded once
+    for bf16 embed), each head within _close of the eager gradient, a bank written by the step equals the twin bank
+    after the eager enqueue; the contrast half is scored as fuzz_graphed_step's replays (score_step_replay), each seg
+    term against its float64 oracle (_score_seg_term), the total loss and each head's gradient against the float64 sums
+    within the terms' bounds combined.  A replay is scored when every part of it was.  Then apply() once.
+    Returns the failures, or None when the geometry is refused as expected (c["refused"]; PclError asserted)."""
+    from contrastiveseg_b200 import bank as bank_mod
+    from oracle.ohem_port import gap_labels
+    import test_gpu_graphed_criterion as TG
+    import test_gpu_ohem as TO
+    dev = torch.device(device)
+    name, K, D, h, w = c["name"], c["K"], c["D"], c["h"], c["w"]
+    aux, mem, ohem = name.startswith("aux"), name.startswith("mem"), "ohem" in name
+    heads = ["seg", "seg_aux"] if aux else ["seg"]
+    dtypes = {"seg": c["seg_dtype"], "seg_aux": c["aux_dtype"]}
+    ign = c["params"]["ce_ignore_index"]
+    inputs = criterion_inputs(c)
+    e0, t0, s0, a0 = inputs(0)
+    params = dict(c["params"])
+    if ohem:           # OHEM's thresh and min_kept from replay 0's logits as the head holds them: the threshold branch there
+        x0, tt = s0.to(dtypes["seg"]).float().to(dev), t0.to(dev)
+        thresh = TO.median_thresh(x0, tt, ign) if bool(((tt != ign)).any()) else 0.5
+        params.update(ohem_thresh=thresh, ohem_minkeep=TO.branch_min_kept(x0, tt, "threshold", thresh, ign))
+    crit = TG.make_criterion(name, ms=c["ms"], extra={"max_views": c["mv"]}, K=K, params=params,
+                             loss_weights=c["lw"]).to(dev)
+    cc = crit.contrast_criterion
+    c.update(T=cc.temperature, bT=cc.base_temperature)
+    lw = crit.loss_weight
+    ohem_mod = None
+    if ohem:
+        ohem_mod = crit.seg_criterion.ohem_ce_loss if aux else crit.seg_criterion
+    gap_frac = [1.0]
+
+    def gapped(t, seg):
+        """OHEM: the target with the pixels whose p_t lies near the threshold ignored (gap_labels)."""
+        if not ohem:
+            return t
+        x = _upsample_f64(seg.to(dtypes["seg"]).to(dev).double(), *t.shape[1:])
+        t = t.to(dev)
+        kw = dict(weight=ohem_mod.weight, thresh=ohem_mod.thresh, min_kept=ohem_mod.min_kept,
+                  reduction=ohem_mod.reduction)
+        g = gap_labels(x, t, ignore_index=ign, near_ulps=TO.NEAR_ULPS, **kw)
+        n0 = int(((t != ign) & (t >= 0) & (t < K)).sum())
+        gap_frac[0] = int(((g != ign) & (g >= 0) & (g < K)).sum()) / max(n0, 1) if n0 else 1.0
+        return g.cpu()
+
+    target = gapped(t0, s0).to(dev)
+    static = {k: v.to(dev, dtypes[k]).requires_grad_(True) for k, v in (("seg", s0), ("seg_aux", a0)) if k in heads}
+    static["embed"] = e0.to(dev, c["embed_dtype"]).requires_grad_(True)
+    half_e = c["embed_dtype"] != torch.float32
+    embed32 = static["embed"].detach().float() if half_e else static["embed"].detach()
+    bank = twin_bank = enq = None
+    if mem:
+        b0 = make_bank(K, c["M"], D, c["seed"] + 1)
+
+        def new_bank():
+            mb = cs.MemoryBank(K, c["M"], D).to(dev)
+            for k in _BANK_NAMES:
+                getattr(mb, k).copy_(b0[k])
+            return mb
+        bank, twin_bank = new_bank(), new_bank()
+        static["segment_queue"], static["pixel_queue"] = bank.segment_queue, bank.pixel_queue
+        if c["bank"] == "enqueue":
+            enq = dict(bank=bank, network_stride=c["stride"], pixel_update_freq=c["freq"], seed=c["seed"] % 997)
+    scale = c["grad_scale"]
+    try:
+        gc_ = cs.GraphedContrastCriterion(crit, static, target, grad_scale=scale, enqueue=enq)
+    except _abi.PclError as ex:
+        return None if c["refused"] else [f"refused ({str(ex)[:100]}): {desc}"]
+    if c["refused"]:
+        return [f"a geometry the terms refuse was accepted: {desc}"]
+    opts = cc.options()
+    opts.num_classes = K
+    twin = cs.GraphedContrastStep(embed32, target, seg=static["seg"].detach(), options=opts, grad_scale=scale * lw,
+                                  segment_queue=twin_bank.segment_queue if mem else None,
+                                  pixel_queue=twin_bank.pixel_queue if mem else None)
+    # each head's coefficient in the seg loss, from the configuration (not from the wrapper's seg_terms)
+    want = {"seg": c["lw"]["seg_loss"], "seg_aux": c["lw"]["aux_loss"]} if aux else {"seg": 1.0}
+    reached, branches, present, prev_A = set(), [], [], None
+    for r in range(c["n_rep"]):
+        why = f"replay {r}: {desc}"
+        if r:
+            e, t, s, a = inputs(r)
+            t = gapped(t, s)
+            with torch.no_grad():
+                static["embed"].copy_(e)
+                if half_e:
+                    embed32.copy_(static["embed"].float())
+                target.copy_(t)
+                for k, v in (("seg", s), ("seg_aux", a)):
+                    if k in heads:
+                        static[k].copy_(v.to(dtypes[k]))
+        if r == c["r_set"]:
+            scale = c["scale2"]
+            gc_.set_grad_scale(scale)
+            twin.set_grad_scale(scale * lw)
+        q_before = torch.cat((twin_bank.segment_queue, twin_bank.pixel_queue), 1).double().cpu() if mem else None
+        loss, grads = gc_.replay()
+        twin.replay()
+        _sync(dev)
+        # the exact checks: the eager seg terms, the twin step, the eager trainer order of a bank write
+        eager = {k: static[k].detach().clone().requires_grad_(True) for k in heads}
+        seg_loss = crit._seg_loss(eager, target)
+        seg_loss.backward(torch.full((), scale, device=dev))
+        if enq:
+            bank_mod._enqueue_counter[0] = r
+            twin_bank.enqueue(embed32, target, network_stride=enq["network_stride"],
+                              pixel_update_freq=enq["pixel_update_freq"], seed=enq["seed"])
+        _sync(dev)
+        if not _same_bits(loss, seg_loss.detach() + lw * twin.loss):
+            return [f"loss {loss.item()} is not the eager seg loss {seg_loss.item()} + loss_weight x the twin step's "
+                    f"{twin.loss.item()}: {why}"]
+        if not _same_bits(grads["embed"], twin.grad.to(grads["embed"].dtype)):
+            return [f"embed gradient differs from the twin step's: {why}"]
+        for k in heads:
+            parts = [t.dseg for t in gc_.terms if t.head == k]
+            if not (grads[k].dtype == dtypes[k] and TG._close(grads[k], eager[k].grad, parts)):
+                return [f"{k} gradient differs from the eager seg terms': {why}"]
+        if enq:
+            for k in _BANK_NAMES:
+                if not torch.equal(getattr(bank, k), getattr(twin_bank, k)):
+                    return [f"bank {k} differs from the eager trainer order: {why}"]
+        # the contrast half against float64
+        step_cov, step_reached = {}, {}
+        bad, A, ok, lo = score_step_replay(c, twin, gc_.step, embed32, target, static["seg"].detach(), None, q_before,
+                                           scale * lw, check_sampling, step_cov, step_reached, prev_A, why)
+        if bad is not None:
+            return [bad]
+        prev_A = A
+        scored = ok or A == 0
+        # each seg term against its float64 oracle
+        terms = []
+        for t in gc_.terms:
+            gs = scale * want[t.head]
+            out = _score_seg_term(t, static[t.head].detach().float(), target, gs, gap_frac[0])
+            if out[0] is not None:
+                return [f"{out[0]}: {why}"]
+            scored = scored and out[1]
+            terms.append((t,) + out[2:])
+        if not scored:
+            cov["skipped"] += 1
+            continue
+        # the whole criterion: total loss and each head's gradient against the float64 sums, bounds combined
+        coef = lambda t: want[t.head]                                       # noqa: E731
+        lref = sum(coef(t) * lr for t, lr, *_ in terms) + lw * lo
+        lbound = (sum(abs(coef(t)) * lb for t, _, _, _, lb, _, _ in terms) + abs(lw) * (2e-6 * abs(lo) + 1e-6) +
+                  1e-6 * (sum(abs(coef(t) * lr) for t, lr, *_ in terms if not math.isnan(lr)) + abs(lw * lo)))
+        lv = loss.item()
+        if not ((math.isnan(lref) and math.isnan(lv)) or abs(lv - lref) <= lbound):
+            return [f"total loss {lv} vs float64 {lref} (bound {lbound:.2e}): {why}"]
+        for k in heads:
+            mine = [tm for tm in terms if tm[0].head == k]
+            gsum = sum(tm[2] for tm in mine)
+            tol = sum(tm[3] for tm in mine)
+            if dtypes[k] != torch.float32:              # each term's gradient cast to the head's dtype, then added
+                eps, tiny = _HALF_EPS[dtypes[k]], torch.finfo(dtypes[k]).tiny
+                # one rounding per cast and per add: eps / 2 relative, and half a subnormal step below fp16's normal
+                # range (the gradients of a large label grid are small)
+                tol = tol * (1 + eps) + eps * sum(tm[2].abs() for tm in mine) + 2 * len(mine) * tiny * eps
+            err = (grads[k].double() - gsum).abs() - tol
+            for tm in mine:
+                if tm[5] is not None:                   # the Lovasz near-tie footprints
+                    err = err.masked_fill(tm[5][:, None], 0.0)
+            if bool((err > 0).any()):
+                return [f"{k} gradient vs the float64 sum of its terms: {int((err > 0).sum())} elements out of bounds: "
+                        f"{why}"]
+        cov["scored"] += 1
+        reached.add(name)
+        for t in gc_.terms:
+            if t.kind == "ce":
+                reached.add("CE one-call" if t.one_call else "CE two-call")
+                if t.one_call and K > 24:
+                    reached.add("CE one-call above 24 classes")
+        for k in heads:
+            if dtypes[k] == torch.float16:
+                reached.add("fp16 head")
+            if dtypes[k] == torch.bfloat16 and sum(t.head == k for t in gc_.terms) > 1:
+                reached.add("bf16 head with two terms")
+        if c["all_ignored"] and r == 3:
+            reached.add("all-ignored replay")
+        if A == 0:
+            reached.add("A = 0 replay")
+        if enq:
+            reached.add("bank + enqueue")
+        if scale < 0:
+            reached.add("negative grad_scale")
+        if r == c["r_set"]:
+            reached.add("set_grad_scale mid-case")
+        branches += [tm[6] for tm in terms if tm[6] is not None]
+        if any(t.kind == "lovasz" for t in gc_.terms):
+            present.append(set(target[(target != ign) & (target >= 0) & (target < K)].unique().tolist()))
+    # OHEM's branch flipped both ways: threshold -> select -> threshold over scored replays of the case
+    if any(branches[i:i + 3] == ["threshold", "select", "threshold"] for i in range(len(branches) - 2)):
+        reached.add("OHEM branch flip")
+    if any(cl in present[i] and cl not in present[j] and any(cl in p for p in present[j + 1:])
+           for i in range(len(present)) for j in range(i + 1, len(present)) for cl in present[i]):
+        reached.add("Lovasz present-set change")
+    # the autograd hand-off: apply() hands the heads and embed the buffers of its replay
+    gc_.set_grad_scale(1.0)
+    for k in heads + ["embed"]:
+        static[k].grad = None
+    gc_.apply(static).backward()
+    _sync(dev)
+    for k in heads + ["embed"]:
+        if not _same_bits(static[k].grad, grads[k]):
+            return [f"apply(): the {k} gradient is not the replay's: {desc}"]
+    for k in reached:
+        cov[k] += 1
+    return []
+
+
+def fuzz_graphed_criterion(seed: int, n: int, check_sampling, device="cpu", scale: int = 1):
+    """GraphedContrastCriterion over every wrapper x seg-term combination the wrappers capture, with drawn term
+    parameters, class counts, geometries, head / embed dtypes, bank, grad_scale (changed once per case), 3-4 replays per
+    case with the labels, the heads and embed refilled in place (a class gone and back, every label ignored, OHEM's
+    branch flipped, A = 0), each replay scored against float64 (graphed_criterion_case).  On a CPU the caller patches
+    the capture out (the launch sequence runs eagerly); on a device nothing is patched.  Returns (failures, coverage):
+    how many cases reached each of CRIT_CATEGORIES with a scored replay, "scored" / "skipped" replays and "refused"
+    geometries (refusal asserted, then drawn again)."""
+    import gc
+    rng = random.Random(seed)
+    bad, cov = [], {k: 0 for k in CRIT_CATEGORIES + ("scored", "skipped", "refused")}
+    for it in range(n):
+        c, cap = _draw_criterion_case(rng, it, scale, device)
+        while True:
+            desc = "criterion seed={} it={} {}".format(seed, it, " ".join(f"{k}={v}" for k, v in c.items()))
+            out = graphed_criterion_case(c, device, check_sampling, cov, desc)
+            if out is not None:
+                break
+            cov["refused"] += 1
+            c = _criterion_geometry(rng, c, rng.choice(["up", "nonint", "identity"]), cap)
+        bad += out
+        if torch.device(device).type == "cuda":        # the float64 references of a case go back to the shared GPU
+            gc.collect()
+            torch.cuda.empty_cache()
     return bad, cov
 
 

@@ -1,5 +1,7 @@
 """Bounded differential fuzzing of the real SIMT kernel sources (host-fiber emulation, tests/emu) against the oracle:
 random geometries per component, fixed seeds.  `python tools/emu_fuzz.py` runs the same fuzzers for as long as wanted."""
+import random
+
 import pytest
 import torch
 
@@ -8,12 +10,26 @@ import emu_harness
 import test_gpu_parity as G
 
 NGRAPH = 24
+NCRIT = 10
 
 
 @pytest.fixture
 def emu(monkeypatch):
     monkeypatch.setattr(torch.cuda, "synchronize", lambda *a, **k: None)
     return emu_harness.use_emulation(monkeypatch)
+
+
+@pytest.fixture
+def emu_fused(emu, monkeypatch):
+    """The criterion's launch sequence run eagerly (no CUDA graphs on a CPU, the fill branch inline) and the fused seg
+    CE taken for CPU tensors, as in test_emu_graphed_criterion.py."""
+    from contrastiveseg_b200 import graph_step, loss as loss_mod
+    G_ = graph_step.GraphedContrastStep
+    monkeypatch.setattr(G_, "_capture", lambda self, warmup: None)
+    monkeypatch.setattr(G_, "_fork_zero_fill", lambda self: self._side_branch(0))
+    monkeypatch.setattr(G_, "_join_zero_fill", lambda self: None)
+    monkeypatch.setattr(loss_mod.ContrastCELoss, "_can_fuse", lambda self, ce, s: self.fused_seg_ce)
+    return emu
 
 
 def test_fuzz_pixel_contrast_loss(emu):
@@ -62,3 +78,38 @@ def test_trainer_hook_fuzz_detects_an_early_bank_write(emu, monkeypatch):
 
 def test_fuzz_loss_wrappers(emu):
     assert emu_fuzz.fuzz_wrappers(seed=19, n=30) == []
+
+
+def test_fuzz_graphed_criterion(emu_fused):
+    """The captured criterion's launch sequence (run eagerly) with labels, heads and embed refilled between replays:
+    every wrapper x seg term, CE path, dtype, degenerate replay and grad_scale change reached on scored replays."""
+    bad, cov = emu_fuzz.fuzz_graphed_criterion(seed=21, n=NCRIT, check_sampling=G._check_device_sampling)
+    assert bad == []
+    assert all(cov[k] >= 1 for k in emu_fuzz.CRIT_CATEGORIES), cov
+    assert cov["scored"] >= 2 * cov["skipped"], cov
+
+
+def test_criterion_fuzz_detects_a_stale_label_map(emu_fused, monkeypatch):
+    """Negative control: seg terms that read a copy of the label map taken when the criterion was built (labels that
+    stop changing between replays) fail the fuzzer on a replay after the first, in most cases."""
+    from contrastiveseg_b200 import graph_criterion
+    init = graph_criterion._Term.__init__
+
+    def stale(self, lib, term, x, target, grad_scale):
+        init(self, lib, term, x, target.clone(), grad_scale)
+    monkeypatch.setattr(graph_criterion._Term, "__init__", stale)
+    bad, _ = emu_fuzz.fuzz_graphed_criterion(seed=21, n=6, check_sampling=G._check_device_sampling)
+    assert len(bad) >= 4, bad
+    assert not any(b.startswith("replay 0:") or "replay 0: " in b for b in bad), bad
+
+
+def test_criterion_fuzz_regression_two_call_ce_every_pixel_ignored(emu_fused):
+    """The criterion fuzzer's first finding, as a constructed case: case 3 of the fuzzer's draw (ContrastAuxCELoss with
+    a label grid smaller than the logits: the two-call seg CE) from a fixed stream, with replay 3 forced to ignore every
+    label.  Such a replay gave a NaN gradient in both heads (k_segce_bwd_gather: 0 times grad / 0); it is 0."""
+    c, _ = emu_fuzz._draw_criterion_case(random.Random(3), 3, 1, "cpu")
+    c.update(all_ignored=True, n_rep=4)
+    cov = {k: 0 for k in emu_fuzz.CRIT_CATEGORIES + ("scored", "skipped", "refused")}
+    assert c["name"] == "aux_ce" and c["mode"] == "down" and not c["refused"]
+    assert emu_fuzz.graphed_criterion_case(c, "cpu", G._check_device_sampling, cov, "regression") == []
+    assert cov["CE two-call"] == 1 and cov["all-ignored replay"] == 1, cov

@@ -36,6 +36,11 @@ def test_seg_ce_fwd_bwd_every_pixel_ignored_on_emulation(emu):
     T.check_fwd_bwd(1, 19, 5, 6, 13, 17, True, 255, all_ignored=True)
 
 
+@pytest.mark.parametrize("H,W", [(5, 11), (9, 6), (4, 5)])
+def test_seg_ce_two_call_every_pixel_ignored_below_the_logit_grid_on_emulation(emu, H, W):
+    T.check_two_call_every_pixel_ignored(H, W)
+
+
 def test_seg_ce_fwd_bwd_refuses_down_sampling_on_emulation(emu):
     T.test_seg_ce_fwd_bwd_refuses_down_sampling()
 

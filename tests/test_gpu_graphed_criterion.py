@@ -78,6 +78,23 @@ def test_seg_ce_fwd_bwd_every_pixel_ignored(ignore_index):
     check_fwd_bwd(2, 19, 9, 11, 37, 45, True, ignore_index, all_ignored=True)
 
 
+def check_two_call_every_pixel_ignored(H, W, ignore_index=255, B=2, K=5, h=9, w=11):
+    """A label grid smaller than seg (the two-call form's gather backward) with every pixel ignored: NaN loss and a zero
+    gradient, as with up-sampling and in torch (the gather divided by the zero weight sum: NaN everywhere)."""
+    seg, target, _ = M._seg_ce_inputs(B, K, h, w, H, W, False, ignore_index, seed=H * W)
+    target.fill_(ignore_index)
+    x = seg.to(DEV).requires_grad_(True)
+    loss = cs.upsample_cross_entropy(x, target.to(DEV), None, ignore_index)
+    loss.backward(torch.tensor(0.7, device=DEV))
+    assert torch.isnan(loss).item()
+    assert torch.count_nonzero(x.grad).item() == 0          # (NaN counts as non-zero)
+
+
+@pytest.mark.parametrize("H,W", [(5, 11), (9, 6), (4, 5)])
+def test_seg_ce_two_call_every_pixel_ignored_below_the_logit_grid(H, W):
+    check_two_call_every_pixel_ignored(H, W)
+
+
 def test_seg_ce_fwd_bwd_refuses_down_sampling():
     seg = torch.randn(2, 5, 40, 40, device=DEV)
     target = torch.zeros(2, 20, 50, dtype=torch.int64, device=DEV)
@@ -104,14 +121,17 @@ CRITERIA = {
 }
 
 
-def make_criterion(name, ms=256, extra=None):
+def make_criterion(name, ms=256, extra=None, K=K_CRIT, params=None, loss_weights=None):
+    """The criterion `name` with this file's configuration; K, `params` (loss.params entries) and `loss_weights`
+    (network.loss_weights) override it (the criterion fuzzer of tests/emu_fuzz.py draws them)."""
     wrapper, seg_cls, use_rmi = CRITERIA[name]
     d = cs.cityscapes_contrast_config(with_memory=wrapper is cs.MemContrastCELoss)
-    d["contrast"].update(max_samples=ms, max_views=8, use_rmi=use_rmi, **(extra or {}))
-    d["loss"]["params"].update(use_sigmoid=True, num_classes=K_CRIT, rmi_radius=3, rmi_pool_way=0, rmi_pool_size=3,
-                               rmi_pool_stride=3, loss_weight_lambda=0.5, loss_weight=1.0, lambda_way=1,
-                               ohem_thresh=0.7, ohem_minkeep=1000)
-    d["network"]["loss_weights"] = {"seg_loss": 1.0, "aux_loss": 0.4}
+    d["data"]["num_classes"] = K
+    d["contrast"].update(dict(max_samples=ms, max_views=8, use_rmi=use_rmi), **(extra or {}))
+    d["loss"]["params"].update(dict(use_sigmoid=True, num_classes=K, rmi_radius=3, rmi_pool_way=0, rmi_pool_size=3,
+                                    rmi_pool_stride=3, loss_weight_lambda=0.5, loss_weight=1.0, lambda_way=1,
+                                    ohem_thresh=0.7, ohem_minkeep=1000), **(params or {}))
+    d["network"]["loss_weights"] = dict(loss_weights or {"seg_loss": 1.0, "aux_loss": 0.4})
     cfg = cs.Configer(d)
     return wrapper(cfg, seg_criterion=seg_cls(cfg)) if seg_cls is not None else wrapper(cfg)
 
@@ -125,13 +145,21 @@ def _batch(seed, B, D, h, w, aux):
     return out, data["target"]
 
 
-def _close(g, ge):
+def _close(g, ge, parts=None):
     """Within 1e-6 max|g| of the eager gradient; a half gradient may also differ by one rounding of its dtype (the two
-    sides round fp32 gradients that agree to the last ulp or two)."""
+    sides round fp32 gradients that agree to the last ulp or two).  parts (the criterion fuzzer): the fp32 gradients of
+    the head's terms.  With them a half gradient may also differ by one subnormal step below its normal range (fp16
+    gradients of a large label grid are that small), and with several terms, each rounded to the head's dtype before
+    they are added, by three roundings on each side, which scale with the terms' magnitudes, not the sum's."""
     gmax = ge.float().abs().max().item()
     tol = 1e-6 * gmax
     if ge.dtype != torch.float32:
-        tol = tol + ge.float().abs() * torch.finfo(ge.dtype).eps
+        fi = torch.finfo(ge.dtype)
+        tol = tol + ge.float().abs() * fi.eps
+        if parts is not None:
+            if len(parts) > 1:
+                tol = 1e-6 * gmax * len(parts) + 2 * sum(p.abs() for p in parts) * fi.eps
+            tol = tol + fi.tiny * fi.eps
     return bool(((g.float() - ge.float()).abs() <= tol).all())
 
 
@@ -227,3 +255,39 @@ def check_refusals(B=2, D=64, h=16, w=16):
 
 def test_graphed_criterion_refusals():
     check_refusals()
+
+
+# ---------------------------------------------------------------------------------------------------
+# C. The captured criterion against float64 (tests/emu_fuzz.py: fuzz_graphed_criterion, graphed_criterion_case)
+# ---------------------------------------------------------------------------------------------------
+@pytest.mark.timeout(1800)
+def test_fuzz_captured_criteria_on_the_device():
+    """Real graph replays, nothing patched: every wrapper x seg term with drawn term parameters, K up to 40 and one
+    draw at 150-171 classes, B up to 8, h x w up to 120 x 120 (label grids within 8M B K H W elements), max_samples
+    up to 1024; labels, heads and embed refilled between replays; every coverage category reached on scored replays."""
+    import emu_fuzz
+    import test_gpu_parity as G
+    bad, cov = emu_fuzz.fuzz_graphed_criterion(seed=41, n=30, check_sampling=G._check_device_sampling, device=DEV,
+                                               scale=10)
+    assert bad == [], bad
+    assert all(cov[k] >= 1 for k in emu_fuzz.CRIT_CATEGORIES), cov
+    assert cov["scored"] >= 2 * cov["skipped"], cov
+
+
+@pytest.mark.timeout(900)
+@pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16], ids=["fp32", "bf16"])
+@pytest.mark.parametrize("name", ["ce", "aux_ce"])
+def test_captured_criterion_at_the_s1_shape(name, dtype):
+    """tools/criterion_bench.py's S1 shape (8 x 19 x 128 x 256 logits, 512 x 1024 labels, D 256, 1024 anchors), three
+    replays with refilled labels, heads and embed, grad_scale changed before the last, against float64 on the device."""
+    import emu_fuzz
+    import test_gpu_parity as G
+    c = dict(name=name, K=19, B=8, D=256, h=128, w=256, H=512, W=1024, ms=1024, mv=100, seq="random", block=32,
+             ignore=0.1, params={"ce_ignore_index": -1}, lw={"seg_loss": 1.0, "aux_loss": 0.4}, seg_dtype=dtype,
+             aux_dtype=dtype, embed_dtype=torch.float32, bank="none", grad_scale=1.0, scale2=2.0, n_rep=3, r_set=2, all_ignored=False,
+             seed=1234, T=None, bT=None, precision="fp32", normalize=False, nan_safe=False, ignore_label=-1,
+             refused=False, stride=1, M=None, freq=None)
+    cov = {k: 0 for k in emu_fuzz.CRIT_CATEGORIES + ("scored", "skipped", "refused")}
+    bad = emu_fuzz.graphed_criterion_case(c, DEV, G._check_device_sampling, cov, f"S1 {name} {dtype}")
+    assert bad == [], bad
+    assert cov["scored"] == 3 and cov[name] == 1, cov

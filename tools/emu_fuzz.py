@@ -22,6 +22,22 @@ if __name__ == "__main__":
     mp = pytest.MonkeyPatch()
     mp.setattr(torch.cuda, "synchronize", lambda *a, **k: None)
     emu_harness.use_emulation(mp)
+
+    def criterion(seed, k):
+        """fuzz_graphed_criterion with the criterion's launch sequence run eagerly (no CUDA graphs on a CPU) and the
+        fused seg CE taken for CPU tensors; the patches are undone afterwards (the other fuzzers run unpatched)."""
+        from contrastiveseg_b200 import graph_step, loss as loss_mod
+        cp = pytest.MonkeyPatch()
+        G_ = graph_step.GraphedContrastStep
+        cp.setattr(G_, "_capture", lambda self, warmup: None)
+        cp.setattr(G_, "_fork_zero_fill", lambda self: self._side_branch(0))
+        cp.setattr(G_, "_join_zero_fill", lambda self: None)
+        cp.setattr(loss_mod.ContrastCELoss, "_can_fuse", lambda self, ce, s: self.fused_seg_ce)
+        try:
+            return emu_fuzz.fuzz_graphed_criterion(seed, k, G._check_device_sampling)[0]
+        finally:
+            cp.undo()
+
     total = 0
     for r in range(rounds):
         for name, fn in (("loss", lambda s: emu_fuzz.fuzz_loss(s, n)), ("bank", lambda s: emu_fuzz.fuzz_bank(s, n)),
@@ -30,6 +46,7 @@ if __name__ == "__main__":
                          ("tensor", lambda s: emu_fuzz.fuzz_tensor_path(s, max(1, n // 5))),
                          ("graph", lambda s: emu_fuzz.fuzz_graphed_step(s, max(1, n // 2),
                                                                         G._check_device_sampling)[0]),
+                         ("criterion", lambda s: criterion(s, max(1, n // 4))),
                          ("hook", lambda s: emu_fuzz.fuzz_trainer_hook(s, max(1, n // 2))),
                          ("wrappers", lambda s: emu_fuzz.fuzz_wrappers(s, n))):
             bad = fn(1000 * r + base)
