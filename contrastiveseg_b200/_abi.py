@@ -115,6 +115,11 @@ SIGNATURES = {
     "pcl_proj_bn_bwd_dt": (c_i32, [c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_i64, c_vp, c_vp, c_vp,
                                    c_vp, c_vp, c_vp, c_vp, c_vp]),
     "pcl_proj_bn_input_grad_dt": (c_i32, [c_vp, c_i32, c_vp, c_vp, c_i32, c_i32, c_i64, c_i32, c_vp, c_vp]),
+    "pcl_proj_bn_cols_workspace_bytes": (c_i64, [c_i32, c_i32]),
+    "pcl_proj_bn_bwd_cols_dt": (c_i32, [c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_vp, c_i32, c_i32, c_i64,
+                                        c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "pcl_proj_bn_input_grad_cols_dt": (c_i32, [c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_i64, c_i32,
+                                               c_vp, c_vp]),
     "pcl_proj_conv1_workspace_bytes": (c_i64, [c_i32, c_i32, c_i64, c_i32]),
     "pcl_proj_conv1_pack": (c_i32, [c_vp, c_i32, c_vp, c_vp]),
     "pcl_proj_conv1_fwd_dt": (c_i32, [c_vp, c_i32, c_vp, c_vp, c_i32, c_i32, c_i64, c_vp, c_vp, c_vp, c_vp]),
@@ -155,6 +160,7 @@ SIGNATURES = {
     "pcl_step_forward": (c_i32, [C.POINTER(StepDesc), c_vp]),
     "pcl_step_backward": (c_i32, [C.POINTER(StepDesc), c_vp, c_vp]),
     "pcl_step_backward_prezeroed": (c_i32, [C.POINTER(StepDesc), c_vp, c_vp]),
+    "pcl_step_backward_cols": (c_i32, [C.POINTER(StepDesc), c_vp, c_vp, c_vp, c_vp]),
     "pcl_step_ranks": (c_i32, [C.POINTER(StepDesc), c_vp, c_vp, c_vp]),
     "pcl_step_forward_ctr": (c_i32, [C.POINTER(StepDesc), c_vp, c_vp]),
     "pcl_step_fused_supported": (c_i32, [C.POINTER(StepDesc)]),

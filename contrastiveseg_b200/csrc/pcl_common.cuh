@@ -115,6 +115,10 @@ struct grad_rows {
 int dense_grad(const pcl_geom* g, const int32_t* plan, const int32_t* anchor_meta, const grad_rows& r, bool zeroed,
                void* grad_embed, int grad_dtype, void* stream, unsigned int* dbg = nullptr,
                unsigned long long* step_counter = nullptr, int32_t* prev_rows = nullptr);
+// The same values as (max_samples, D) fp32 anchor columns: cols[s] and col_pix[s] = b h w + pix for s < A (A read on the
+// device), zeros and -1 beyond.  Bit-identical to what dense_grad stores for an fp32 gradient.
+int anchor_cols(const pcl_geom* g, const int32_t* plan, const int32_t* anchor_meta, const grad_rows& r, float* cols,
+                int32_t* col_pix, void* stream);
 
 // ---- per-device kernel attributes ----------------------------------------------------------------
 // cudaFuncAttributeMaxDynamicSharedMemorySize is a property of (function, device) and SETS the limit (a later call with

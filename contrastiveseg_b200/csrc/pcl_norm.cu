@@ -814,6 +814,179 @@ __global__ void __launch_bounds__(IG_NT) k_bn_input_grad(const T* __restrict__ y
 }
 
 // ------------------------------------------------------------------------------------------------------------------
+// (3b) The backward of (3) from the anchor columns of gzn alone (the contrast loss reads zn at no more than max_samples
+// pixels, so gzn is zero everywhere else).  n_cols columns: cols (n_cols, 256) fp32, col_pix = b HW + p or < 0 (dead).
+// Plain fp32 SIMT on the fp32 weight; every sum in a fixed order, no atomics.
+//   k_col_prep       per column: gz = (g - zn <zn, g>) inv, u = max(0, y scale + shift) (+ the constant-1 column of gb),
+//                    x_hat = (y - mean) invstd, gathered at the column's pixel.  Dead columns: all zero.
+//   k_col_gemm<0>    gW2 | gb2 = gz^T [u | 1]                      (256 x Cin + 1, sum over the columns)
+//   k_col_gemm<1>    gu = (gz W2) [u > 0], part = (gu, gu x_hat)   (n_cols x Cin, sum over the 256 channels)
+//   k_tile_sum<float> part -> gsum, gbeta, ggamma
+//   k_bn_input_grad_cols, k_bn_cols_scatter   g_y from y alone (gu = 0), then the anchor pixels with their gu
+struct ColLayout {
+  int64_t gz_off, u_off, xh_off, part_off, bytes;
+};
+static inline int64_t align256(int64_t v) { return (v + 255) & ~(int64_t)255; }
+static ColLayout col_layout(int n_cols, int Cin) {
+  ColLayout L;
+  L.gz_off = 0;
+  L.u_off = align256((int64_t)n_cols * DOUT * 4);
+  L.xh_off = L.u_off + align256((int64_t)n_cols * (Cin + 1) * 4);
+  L.part_off = L.xh_off + align256((int64_t)n_cols * Cin * 4);
+  L.bytes = L.part_off + align256((int64_t)n_cols * 2 * Cin * 4);
+  return L;
+}
+
+template <class T>
+__global__ void __launch_bounds__(DOUT) k_col_prep(const T* __restrict__ y, const T* __restrict__ zn,
+                                                   const float* __restrict__ inv_norm, const float* __restrict__ ss,
+                                                   const float* __restrict__ cols, const int32_t* __restrict__ col_pix,
+                                                   int B, int Cin, int64_t HW, int ldp, float* __restrict__ gz,
+                                                   float* __restrict__ u, float* __restrict__ xh) {
+  __shared__ float red[DOUT / 32];
+  const int a = blockIdx.x, t = threadIdx.x;
+  const int64_t q = col_pix[a];
+  float* ur = u + (int64_t)a * (Cin + 1);
+  float* xr = xh + (int64_t)a * Cin;
+  if (q < 0 || q >= (int64_t)B * HW) {
+    gz[(int64_t)a * DOUT + t] = 0.f;
+    for (int c = t; c <= Cin; c += DOUT) ur[c] = 0.f;
+    for (int c = t; c < Cin; c += DOUT) xr[c] = 0.f;
+    return;
+  }
+  const int64_t b = q / HW, p = q - b * HW;
+  const float g = cols[(int64_t)a * DOUT + t];
+  const float z = to_f32(zn[(b * DOUT + t) * HW + p]);
+  const float inv = inv_norm[q];
+  float dot = warp_sum(z * g);
+  if ((t & 31) == 0) red[t >> 5] = dot;
+  __syncthreads();
+  dot = 0.f;
+#pragma unroll
+  for (int w = 0; w < DOUT / 32; ++w) dot += red[w];                                    // fixed order
+  const float coef = inv < NORM_EPS_INV ? dot : 0.f;                                   // clamped rows: g inv
+  gz[(int64_t)a * DOUT + t] = (g - z * coef) * inv;
+  for (int c = t; c < Cin; c += DOUT) {
+    const float yv = to_f32(y[(b * Cin + c) * HW + p]);
+    ur[c] = fmaxf(fmaf(yv, ss[c], ss[ldp + c]), 0.f);                                   // the forward's BN + ReLU
+    xr[c] = (yv - ss[2 * ldp + c]) * ss[3 * ldp + c];
+  }
+  if (t == 0) ur[Cin] = 1.f;
+}
+
+// C (Mi x Nj) = A (Mi x K) B (K x Nj) with A[i][k] at a[i as_i + k as_k], B[k][j] at b[k ldb + j]: 64 x 64 tiles, 4 x 4
+// per thread, the k sum of every element in ascending order.
+// MODE 0: i = output channel n, j = input channel c (c == Cin: the bias column) -> gw (256, Cin), gb (may be null).
+// MODE 1: i = column, j = channel -> part[i][0][j] = gu = C [u > 0], part[i][1][j] = gu x_hat.
+constexpr int CG_T = 64, CG_K = 16, CG_NT = 256;
+struct ColGemmOut {
+  float *gw, *gb;                        // MODE 0
+  const float *u, *xh; float* part;      // MODE 1
+  int Cin;
+};
+template <int MODE>
+__global__ void __launch_bounds__(CG_NT) k_col_gemm(const float* __restrict__ a, int64_t as_i, int64_t as_k,
+                                                    const float* __restrict__ b, int64_t ldb, int Mi, int Nj, int K,
+                                                    ColGemmOut o) {
+  __shared__ float sa[CG_K][CG_T + 4];
+  __shared__ float sb[CG_K][CG_T + 4];
+  const int t = threadIdx.x, tx = t & 15, ty = t >> 4;
+  const int i0 = blockIdx.y * CG_T, j0 = blockIdx.x * CG_T;
+  float acc[4][4] = {};
+  for (int k0 = 0; k0 < K; k0 += CG_K) {
+#pragma unroll
+    for (int l = 0; l < CG_T * CG_K / CG_NT; ++l) {
+      const int idx = t + l * CG_NT;
+      // along the unit stride of A for coalesced loads
+      const int ii = as_k == 1 ? idx / CG_K : idx % CG_T, kk = as_k == 1 ? idx % CG_K : idx / CG_T;
+      const int i = i0 + ii, k = k0 + kk;
+      sa[kk][ii] = (i < Mi && k < K) ? a[(int64_t)i * as_i + (int64_t)k * as_k] : 0.f;
+      const int jj = idx % CG_T, kb = idx / CG_T, j = j0 + jj, k2 = k0 + kb;
+      sb[kb][jj] = (j < Nj && k2 < K) ? b[(int64_t)k2 * ldb + j] : 0.f;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int kk = 0; kk < CG_K; ++kk)
+#pragma unroll
+      for (int r = 0; r < 4; ++r)
+#pragma unroll
+        for (int c = 0; c < 4; ++c) acc[r][c] = fmaf(sa[kk][4 * ty + r], sb[kk][4 * tx + c], acc[r][c]);
+    __syncthreads();
+  }
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+      const int i = i0 + 4 * ty + r, j = j0 + 4 * tx + c;
+      if (i >= Mi || j >= Nj) continue;
+      if constexpr (MODE == 0) {
+        if (j < o.Cin) o.gw[(int64_t)i * o.Cin + j] = acc[r][c];
+        else if (o.gb) o.gb[i] = acc[r][c];
+      } else {
+        const float gu = o.u[(int64_t)i * (o.Cin + 1) + j] > 0.f ? acc[r][c] : 0.f;   // pre-ReLU > 0 <=> u > 0
+        o.part[(int64_t)i * 2 * o.Cin + j] = gu;
+        o.part[((int64_t)i * 2 + 1) * o.Cin + j] = gu * o.xh[(int64_t)i * o.Cin + j];
+      }
+    }
+}
+
+// k_bn_input_grad's per-channel terms: g_y = a (g_u - k1 - (y - mu) k2)
+struct BnIg { float a, mu, k2, k1; };
+__device__ __forceinline__ BnIg bn_ig(const float* __restrict__ st, const float* __restrict__ gsum, int C, int ldp,
+                                      int c, int training) {
+  BnIg r{st[c], st[2 * ldp + c], 0.f, 0.f};
+  if (training) {
+    const float invn = st[4 * ldp], is = st[3 * ldp + c];
+    r.k1 = gsum[c] * invn;
+    r.k2 = gsum[C + c] * invn * is;
+  }
+  return r;
+}
+
+// k_bn_input_grad with g_u = 0 everywhere (g is written, not read): training g_y = a (-k1 - x_hat k2), eval 0
+template <class T>
+__global__ void __launch_bounds__(IG_NT) k_bn_input_grad_cols(const T* __restrict__ y, T* __restrict__ g,
+                                                               const float* __restrict__ st,
+                                                               const float* __restrict__ gsum, int C, int ldp,
+                                                               int64_t HW, int training) {
+  const int64_t row = blockIdx.x;                       // b * C + c
+  const BnIg k = bn_ig(st, gsum, C, ldp, (int)(row % C), training);
+  const int64_t p0 = (int64_t)blockIdx.y * IG_NT * IG_UNROLL + threadIdx.x;
+  const T* yr = y + row * HW;
+  T* gr = g + row * HW;
+  float yv[IG_UNROLL];
+#pragma unroll
+  for (int i = 0; i < IG_UNROLL; ++i) {
+    const int64_t p = p0 + i * IG_NT;
+    yv[i] = p < HW ? to_f32(yr[p]) : 0.f;
+  }
+#pragma unroll
+  for (int i = 0; i < IG_UNROLL; ++i) {
+    const int64_t p = p0 + i * IG_NT;
+    if (p < HW) gr[p] = from_f32<T>(k.a * (0.f - k.k1 - (yv[i] - k.mu) * k.k2));
+  }
+}
+
+// The anchor pixels of g_y with their g_u (part[a][0][c]), after k_bn_input_grad_cols: one block per column
+template <class T>
+__global__ void __launch_bounds__(DOUT) k_bn_cols_scatter(const T* __restrict__ y, T* __restrict__ g,
+                                                          const float* __restrict__ st, const float* __restrict__ gsum,
+                                                          const float* __restrict__ part,
+                                                          const int32_t* __restrict__ col_pix, int B, int C, int ldp,
+                                                          int64_t HW, int training) {
+  const int a = blockIdx.x;
+  const int64_t q = col_pix[a];
+  if (q < 0 || q >= (int64_t)B * HW) return;
+  const int64_t b = q / HW, p = q - b * HW;
+  for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    const BnIg k = bn_ig(st, gsum, C, ldp, c, training);
+    const int64_t o = (b * C + c) * HW + p;
+    const float gu = part[(int64_t)a * 2 * C + c];
+    g[o] = from_f32<T>(k.a * (gu - k.k1 - (to_f32(y[o]) - k.mu) * k.k2));
+  }
+}
+
+// ------------------------------------------------------------------------------------------------------------------
 struct Layout {
   int cin64, cin256, ctiles, ldp;                // wgrad columns: Cin + 1 (the bias column) rounded up to 256
   int64_t HWp, wk_bytes, wt_off, pack_bytes;
@@ -1208,6 +1381,86 @@ extern "C" int pcl_proj_bn_input_grad_dt(const void* y, int32_t dtype, const voi
   else
     proj::k_bn_input_grad<__nv_bfloat16><<<grid, proj::IG_NT, 0, s>>>(
         (const __nv_bfloat16*)y, (__nv_bfloat16*)g, (const float*)bn_state, gsum, Cin, L.ldp, HW, training);
+  PCL_LAUNCH_CHECK();
+  return PCL_OK;
+}
+
+// (3b) the backward of (3) from the anchor columns (see the kernels above)
+extern "C" int64_t pcl_proj_bn_cols_workspace_bytes(int32_t n_cols, int32_t Cin) {
+  if (n_cols <= 0 || n_cols > (1 << 20) || Cin <= 0 || Cin > (1 << 20)) return PCL_ERR_ARG;
+  return proj::col_layout(n_cols, Cin).bytes;
+}
+
+template <class T>
+static void bn_cols_prep(const T* y, const T* zn, const float* inv_norm, const float* ss, const float* cols,
+                         const int32_t* col_pix, int32_t n_cols, int32_t B, int32_t Cin, int64_t HW, int ldp,
+                         uint8_t* sc, const proj::ColLayout& C, cudaStream_t s) {
+  proj::k_col_prep<T><<<(unsigned)n_cols, proj::DOUT, 0, s>>>(y, zn, inv_norm, ss, cols, col_pix, B, Cin, HW, ldp,
+                                                             (float*)(sc + C.gz_off), (float*)(sc + C.u_off),
+                                                             (float*)(sc + C.xh_off));
+}
+
+extern "C" int pcl_proj_bn_bwd_cols_dt(const void* y, int32_t dtype, const void* bn_state, const void* zn,
+                                       const float* inv_norm, const float* cols, const int32_t* col_pix,
+                                       int32_t n_cols, const float* w2, int32_t B, int32_t Cin, int64_t HW,
+                                       void* scratch, float* gw, float* gb, float* gsum, float* ggamma, float* gbeta,
+                                       void* stream) {
+  PCL_REQUIRE(y && bn_state && zn && inv_norm && cols && col_pix && w2 && scratch && gw && gsum &&
+              bn_dtype_ok(dtype) && bn_shape_ok(B, Cin, HW) && n_cols > 0 && n_cols <= (1 << 20));
+  const proj::Layout L = proj::layout(B, Cin, HW);
+  const proj::ColLayout CL = proj::col_layout(n_cols, Cin);
+  cudaStream_t s = (cudaStream_t)stream;
+  uint8_t* sc = (uint8_t*)scratch;
+  const float* ss = (const float*)bn_state;
+  if (dtype == PCL_DT_F32)
+    bn_cols_prep((const float*)y, (const float*)zn, inv_norm, ss, cols, col_pix, n_cols, B, Cin, HW, L.ldp, sc, CL, s);
+  else
+    bn_cols_prep((const __nv_bfloat16*)y, (const __nv_bfloat16*)zn, inv_norm, ss, cols, col_pix, n_cols, B, Cin, HW,
+                 L.ldp, sc, CL, s);
+  PCL_LAUNCH_CHECK();
+  const float* gz = (const float*)(sc + CL.gz_off);
+  float* part = (float*)(sc + CL.part_off);
+  proj::ColGemmOut o{gw, gb, (const float*)(sc + CL.u_off), (const float*)(sc + CL.xh_off), part, Cin};
+  using proj::CG_T;
+  // gW2 | gb2 (256 x Cin + 1) = gz^T (256 x n_cols) [u | 1] (n_cols x Cin + 1)
+  proj::k_col_gemm<0><<<dim3((unsigned)ceil_div(Cin + 1, CG_T), proj::DOUT / CG_T), proj::CG_NT, 0, s>>>(
+      gz, 1, proj::DOUT, o.u, Cin + 1, proj::DOUT, Cin + 1, n_cols, o);
+  PCL_LAUNCH_CHECK();
+  // gu (n_cols x Cin) = gz (n_cols x 256) W2 (256 x Cin), masked by the ReLU
+  proj::k_col_gemm<1><<<dim3((unsigned)ceil_div(Cin, CG_T), (unsigned)ceil_div(n_cols, CG_T)), proj::CG_NT, 0, s>>>(
+      gz, proj::DOUT, 1, w2, Cin, n_cols, Cin, proj::DOUT, o);
+  PCL_LAUNCH_CHECK();
+  proj::k_tile_sum<float><<<(unsigned)ceil_div(Cin, 32), proj::TS_NT, 0, s>>>(part, n_cols, Cin, Cin, gsum, gbeta,
+                                                                               ggamma, 0.);
+  PCL_LAUNCH_CHECK();
+  return PCL_OK;
+}
+
+template <class T>
+static void bn_input_grad_cols(const T* y, const float* st, const float* gsum, const float* part,
+                               const int32_t* col_pix, int32_t n_cols, int32_t B, int32_t Cin, int64_t HW, int ldp,
+                               int32_t training, T* g, cudaStream_t s) {
+  const dim3 grid((unsigned)((int64_t)B * Cin), (unsigned)ceil_div64(HW, (int64_t)proj::IG_NT * proj::IG_UNROLL));
+  proj::k_bn_input_grad_cols<T><<<grid, proj::IG_NT, 0, s>>>(y, g, st, gsum, Cin, ldp, HW, training);
+  proj::k_bn_cols_scatter<T><<<(unsigned)n_cols, proj::DOUT, 0, s>>>(y, g, st, gsum, part, col_pix, B, Cin, ldp, HW,
+                                                                    training);
+}
+
+extern "C" int pcl_proj_bn_input_grad_cols_dt(const void* y, int32_t dtype, const void* bn_state, const float* gsum,
+                                              const void* scratch, const int32_t* col_pix, int32_t n_cols, int32_t B,
+                                              int32_t Cin, int64_t HW, int32_t training, void* g, void* stream) {
+  PCL_REQUIRE(y && g && bn_state && scratch && col_pix && bn_dtype_ok(dtype) && bn_shape_ok(B, Cin, HW) &&
+              n_cols > 0 && n_cols <= (1 << 20));
+  PCL_REQUIRE(training == 0 || (training == 1 && gsum));
+  const proj::Layout L = proj::layout(B, Cin, HW);
+  const float* part = (const float*)((const uint8_t*)scratch + proj::col_layout(n_cols, Cin).part_off);
+  cudaStream_t s = (cudaStream_t)stream;
+  if (dtype == PCL_DT_F32)
+    bn_input_grad_cols((const float*)y, (const float*)bn_state, gsum, part, col_pix, n_cols, B, Cin, HW, L.ldp,
+                       training, (float*)g, s);
+  else
+    bn_input_grad_cols((const __nv_bfloat16*)y, (const float*)bn_state, gsum, part, col_pix, n_cols, B, Cin, HW, L.ldp,
+                       training, (__nv_bfloat16*)g, s);
   PCL_LAUNCH_CHECK();
   return PCL_OK;
 }

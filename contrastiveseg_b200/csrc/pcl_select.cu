@@ -8,6 +8,7 @@
 //   k_select  one warp per anchor: rank -> pixel (chunk prefix search + in-chunk ordered scan), gather
 //             of the pixel's D channels from NCHW, optional L2-normalise, fp32 + bf16 rows
 //   k_zero_scatter, k_scatter_reduce, k_scatter   the dense-gradient writers (dense_grad picks one)
+//   k_cols    the same values as the anchor columns alone, (max_samples, D) fp32 + their pixels (anchor_cols)
 #include "pcl_common.cuh"
 #include <math_constants.h>
 
@@ -442,6 +443,28 @@ k_select(pcl_geom g, int nchunk, const T* __restrict__ embed, const uint16_t* __
 // ------------------------------------------------------------------------------------------------
 // k_scatter: dA rows -> dense NCHW gradient (buffer is zeroed by a memset first)
 // ------------------------------------------------------------------------------------------------
+// Row s of dA as the dense gradient holds it, handed to put(d, value) channel by channel (lane d, d + 32, ...): with
+// `normalize` the projection of the L2 normalise, (dA - a <a, dA>) inv_norm, a = the normalised anchor row.  One warp
+// per row; k_scatter and k_cols share it, so their values are the same to the bit.
+template <class Put>
+__device__ __forceinline__ void da_row(int s, int lane, int D, const float* __restrict__ dA,
+                                       const float* __restrict__ anchors, const float* __restrict__ inv_norm,
+                                       int normalize, Put put) {
+  const float* ga = dA + (int64_t)s * D;
+  float dot = 0.f, inv = 1.f;
+  if (normalize) {
+    const float* y = anchors + (int64_t)s * D;
+    for (int d = lane; d < D; d += 32) dot += y[d] * ga[d];
+    dot = warp_sum(dot);
+    inv = inv_norm[s];
+  }
+  for (int d = lane; d < D; d += 32) {
+    float v = ga[d];
+    if (normalize) v = (v - anchors[(int64_t)s * D + d] * dot) * inv;
+    put(d, v);
+  }
+}
+
 template <typename T>       // element type of grad: the fp32 value is rounded once
 __global__ void __launch_bounds__(256)
 k_scatter(pcl_geom g, const int32_t* __restrict__ plan, const int32_t* __restrict__ meta,
@@ -454,20 +477,8 @@ k_scatter(pcl_geom g, const int32_t* __restrict__ plan, const int32_t* __restric
   const int ms = g.max_samples, D = g.D;
   const int64_t HW = (int64_t)g.h * g.w;
   const int pix = meta[s], b = meta[ms + s];
-  const float* ga = dA + (int64_t)s * D;
-  float dot = 0.f, inv = 1.f;
-  if (normalize) {
-    const float* y = anchors + (int64_t)s * D;
-    for (int d = lane; d < D; d += 32) dot += y[d] * ga[d];
-    dot = warp_sum(dot);
-    inv = inv_norm[s];
-  }
   T* dst = grad + (int64_t)b * D * HW + pix;
-  for (int d = lane; d < D; d += 32) {
-    float v = ga[d];
-    if (normalize) v = (v - anchors[(int64_t)s * D + d] * dot) * inv;
-    dst[(int64_t)d * HW] = from_f32<T>(v);
-  }
+  da_row(s, lane, D, dA, anchors, inv_norm, normalize, [&](int d, float v) { dst[(int64_t)d * HW] = from_f32<T>(v); });
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -528,6 +539,34 @@ k_zero_scatter(pcl_geom g, const int32_t* __restrict__ plan, const int32_t* __re
   const float scale = src.scale();
   for (int s = threadIdx.x; s < A; s += blockDim.x)
     if (meta[ms + s] == b) dst[meta[s]] = from_f32<T>(src.at(s, d, D, scale));
+}
+
+// k_cols: the anchor columns of the dense gradient instead of the dense tensor.  Row s < A: cols[s][0..D) = the fp32
+// values the dense writers store at the anchor's pixel (before their rounding to a half type) and col_pix[s] =
+// b h w + pix; rows s >= A: zeros and col_pix -1.  One warp per row (the lane order of da_row for dA sources).
+template <typename Src>
+__global__ void __launch_bounds__(256)
+k_cols(pcl_geom g, const int32_t* __restrict__ plan, const int32_t* __restrict__ meta, Src src,
+       const float* __restrict__ anchors, const float* __restrict__ inv_norm, int normalize, float* __restrict__ cols,
+       int32_t* __restrict__ col_pix) {
+  const int lane = threadIdx.x & 31;
+  const int s = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int ms = g.max_samples, D = g.D;
+  if (s >= ms) return;
+  const int A = min(plan[PCL_PLAN_A], ms);
+  float* row = cols + (int64_t)s * D;
+  if (s >= A) {
+    for (int d = lane; d < D; d += 32) row[d] = 0.f;
+    if (lane == 0) col_pix[s] = -1;
+    return;
+  }
+  if (lane == 0) col_pix[s] = (int32_t)((int64_t)meta[ms + s] * g.h * g.w + meta[s]);
+  if constexpr (std::is_same<Src, DaRows>::value) {
+    da_row(s, lane, D, src.dA, anchors, inv_norm, normalize, [&](int d, float v) { row[d] = v; });
+  } else {
+    const float scale = src.scale();
+    for (int d = lane; d < D; d += 32) row[d] = src.at(s, d, D, scale);
+  }
 }
 
 // Scatter of the A gradient rows into an ALREADY zero-filled dense gradient, with the fixed-order sum of the per-split
@@ -674,6 +713,26 @@ int pcl::dense_grad(const pcl_geom* g, const int32_t* plan, const int32_t* ancho
       k_scatter<T><<<ceil_div(g->max_samples, warps), warps * 32, 0, s>>>(*g, plan, anchor_meta, r.dA, r.anchors_f32,
                                                                          r.inv_norm, r.normalize, (T*)grad_embed);)
   }
+  PCL_LAUNCH_CHECK();
+  return PCL_OK;
+}
+
+int pcl::anchor_cols(const pcl_geom* g, const int32_t* plan, const int32_t* anchor_meta, const grad_rows& r, float* cols,
+                     int32_t* col_pix, void* stream) {
+  if (!g || !plan || !anchor_meta || !cols || !col_pix) return PCL_ERR_ARG;
+  const bool partial_rows = r.dpartials != nullptr;
+  if (partial_rows ? r.splits < 1 || r.normalize : !r.dA || (r.normalize && (!r.anchors_f32 || !r.inv_norm)))
+    return PCL_ERR_ARG;
+  cudaStream_t s = (cudaStream_t)stream;
+  const int warps = 8;
+  const unsigned blocks = (unsigned)ceil_div(g->max_samples, warps);
+  if (partial_rows)
+    k_cols<SplitRows><<<blocks, warps * 32, 0, s>>>(*g, plan, anchor_meta,
+                                                    SplitRows{r.dpartials, r.splits, r.a_pad, r.inv_T, r.grad_scale},
+                                                    nullptr, nullptr, 0, cols, col_pix);
+  else
+    k_cols<DaRows><<<blocks, warps * 32, 0, s>>>(*g, plan, anchor_meta, DaRows{r.dA}, r.anchors_f32, r.inv_norm,
+                                                 r.normalize, cols, col_pix);
   PCL_LAUNCH_CHECK();
   return PCL_OK;
 }

@@ -110,34 +110,38 @@ static int step_forward(const pcl_step_desc* d, unsigned long long* ctr, void* s
   return pcl::simt_fwd_ex(&w, k, d->topk_scratch, d->partials, d->rowstats, d->loss, stream, ctr);
 }
 
+// The backward sweep of the step (the top-k one with topk_negatives); *r = where the anchor rows of the gradient are.
+static int step_sweep_bwd(const pcl_step_desc* d, const float* grad_loss, void* stream, pcl::grad_rows* r) {
+  if (!topk_ok(d)) return PCL_ERR_ARG;
+  const int k = d->topk_negatives;
+  // tensor path without normalise and top-k: the sweep leaves its per-split partial rows and the gradient writer sums
+  // them itself (fixed order), no (A, D) gradient round trip; otherwise the sweep reduces them to dA
+  const bool partial_rows = d->precision == 1 && !d->normalize && k == 0;
+  *r = {};
+  if (partial_rows) {
+    r->dpartials = d->dpartials; r->inv_T = 1.f / d->temperature; r->grad_scale = grad_loss;
+  } else {
+    r->dA = d->dA; r->anchors_f32 = d->anchors_f32; r->inv_norm = d->inv_norm; r->normalize = d->normalize;
+  }
+  if (d->precision == 1) {
+    pcl_tc_desc t;
+    fill_tc(d, &t);
+    return pcl::tc_bwd_ex(&t, d->row_m2, d->rowstats, grad_loss, d->dpartials, partial_rows ? nullptr : d->dA, stream,
+                          &r->splits, &r->a_pad, k > 0 ? d->topk_scratch : nullptr);
+  }
+  pcl_sweep_desc w;
+  fill_sweep(d, &w);
+  return pcl::simt_bwd_ex(&w, k, d->topk_scratch, d->rowstats, grad_loss, d->dpartials, d->dA, stream);
+}
+
 // prezeroed: the caller has ALREADY zero-filled the dense gradient (the 268 MB fill is the HBM floor of the step; a
 // caller that starts it on a second stream at the beginning of the forward hides it behind the latency-bound selection
 // and sweep kernels), so only the anchor rows are scattered.
 static int step_backward(const pcl_step_desc* d, const float* grad_loss, void* stream, bool prezeroed) {
   if (!d) return PCL_ERR_ARG;
   if (prezeroed && d->topk_negatives != 0) return PCL_ERR_UNSUPPORTED;
-  if (!topk_ok(d)) return PCL_ERR_ARG;
-  const int k = d->topk_negatives;
-  // tensor path without normalise and top-k: the sweep leaves its per-split partial rows and the dense-gradient writer
-  // sums them itself (fixed order), no (A, D) gradient round trip; otherwise the sweep reduces them to dA
-  const bool partial_rows = d->precision == 1 && !d->normalize && k == 0;
-  pcl::grad_rows r = {};
-  if (partial_rows) {
-    r.dpartials = d->dpartials; r.inv_T = 1.f / d->temperature; r.grad_scale = grad_loss;
-  } else {
-    r.dA = d->dA; r.anchors_f32 = d->anchors_f32; r.inv_norm = d->inv_norm; r.normalize = d->normalize;
-  }
-  int st;
-  if (d->precision == 1) {
-    pcl_tc_desc t;
-    fill_tc(d, &t);
-    st = pcl::tc_bwd_ex(&t, d->row_m2, d->rowstats, grad_loss, d->dpartials, partial_rows ? nullptr : d->dA, stream,
-                        &r.splits, &r.a_pad, k > 0 ? d->topk_scratch : nullptr);
-  } else {
-    pcl_sweep_desc w;
-    fill_sweep(d, &w);
-    st = pcl::simt_bwd_ex(&w, k, d->topk_scratch, d->rowstats, grad_loss, d->dpartials, d->dA, stream);
-  }
+  pcl::grad_rows r;
+  int st = step_sweep_bwd(d, grad_loss, stream, &r);
   if (st != PCL_OK) return st;
   return pcl::dense_grad(&d->g, d->plan, d->anchor_meta, r, prezeroed, d->grad_embed, d->embed_dtype, stream, d->sync);
 }
@@ -148,6 +152,16 @@ extern "C" int pcl_step_backward(const pcl_step_desc* d, const float* grad_loss,
 
 extern "C" int pcl_step_backward_prezeroed(const pcl_step_desc* d, const float* grad_loss, void* stream) {
   return step_backward(d, grad_loss, stream, true);
+}
+
+// The backward with the anchor columns as its output instead of the dense gradient (grad_embed is not touched)
+extern "C" int pcl_step_backward_cols(const pcl_step_desc* d, const float* grad_loss, float* cols, int32_t* col_pix,
+                                      void* stream) {
+  if (!d || !cols || !col_pix) return PCL_ERR_ARG;
+  pcl::grad_rows r;
+  int st = step_sweep_bwd(d, grad_loss, stream, &r);
+  if (st != PCL_OK) return st;
+  return pcl::anchor_cols(&d->g, d->plan, d->anchor_meta, r, cols, col_pix, stream);
 }
 
 // ---- fused small-anchor step (include/pcl.h: pcl_step_fused_*) ----

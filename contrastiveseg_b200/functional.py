@@ -258,6 +258,74 @@ def _release_workspace(ws, token) -> None:
         ws.busy = False
 
 
+# ---- anchor-column hand-off (ProjectionHead(..., sparse_grad=True)) ----------------------------------------------
+# The contrast loss reads zn at no more than max_samples pixels, so d loss / d zn is zero elsewhere.  A fused BN head
+# built with sparse_grad=True registers its output zn here; an engine loss whose embed IS that zn (same tensor, same
+# version) deposits its anchor columns in the sink and hands autograd a zero placeholder that costs no memory.  The
+# head's backward takes the column path only when its incoming gradient is exactly that placeholder; anything else
+# (other consumers of zn, two losses) is the dense path on the gradient autograd summed, plus every deposit.
+class _ColumnSink:
+    __slots__ = ("ref", "version", "deposits", "zeros")
+
+    def __init__(self, zn: torch.Tensor):
+        self.ref = weakref.ref(zn)
+        self.version = zn._version
+        self.deposits = []                   # [(cols (max_samples, D) fp32, col_pix (max_samples,) int32)]
+        self.zeros = []                      # the placeholders' one-element storages
+
+    def accepts(self) -> bool:
+        """At the loss's backward: zn is alive and nobody reads its own gradient (retain_grad, tensor hooks)."""
+        zn = self.ref()
+        return zn is not None and not zn.retains_grad and not zn._backward_hooks
+
+    def deposit(self, cols, col_pix, shape):
+        zero = torch.zeros(1, dtype=self.ref().dtype, device=cols.device)
+        self.deposits.append((cols, col_pix))
+        self.zeros.append(zero)
+        return zero.expand(shape)
+
+    def is_placeholder(self, g: torch.Tensor) -> bool:
+        return (len(self.deposits) == 1 and len(self.zeros) == 1 and all(st == 0 for st in g.stride())
+                and g.data_ptr() == self.zeros[0].data_ptr())
+
+    def take(self):
+        deps, self.deposits, self.zeros = self.deposits, [], []
+        return deps
+
+
+_SINKS = {}                                  # id(zn) -> _ColumnSink (dropped with zn)
+
+
+def _register_sink(zn: torch.Tensor) -> _ColumnSink:
+    sink = _ColumnSink(zn)
+    key = id(zn)
+    _SINKS[key] = sink
+    weakref.finalize(zn, _SINKS.pop, key, None).atexit = False
+    return sink
+
+
+def _sink_of(embed: torch.Tensor) -> Optional[_ColumnSink]:
+    sink = _SINKS.get(id(embed))
+    if sink is None or sink.ref() is not embed or sink.version != embed._version:
+        return None
+    return sink
+
+
+def _with_deposits(gzn: torch.Tensor, deposits, dtype) -> torch.Tensor:
+    """gzn (as autograd summed it) plus every deposited column, each rounded to zn's dtype as the loss's dense gradient
+    would have been: the gradient the dense path would have received."""
+    g = gzn.to(dtype=dtype).contiguous().clone()
+    B, D = g.shape[0], g.shape[1]
+    gv = g.view(B, D, -1)
+    HW = gv.shape[2]
+    for cols, col_pix in deposits:
+        live = col_pix >= 0
+        q = col_pix[live].long()
+        b, p = q // HW, q % HW
+        gv[b, :, p] += cols[live].to(dtype)
+    return g
+
+
 class _PixelContrastFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, embed, labels, seg, predict, segq, pixq, shadow, opts: ContrastOptions):
@@ -377,6 +445,7 @@ class _PixelContrastFn(torch.autograd.Function):
                 raise _abi.PclError(f"unknown rng mode {opts.rng!r}")
             _abi.check(lib.pcl_step_forward(C.byref(d), stream), "pcl_step_forward")
         ctx.ws = ws
+        ctx.sink = _sink_of(embed)               # embed IS the zn of a sparse_grad head: hand it the anchor columns
         ctx.embed_shape, ctx.embed_dtype = tuple(embed_c.shape), embed_c.dtype
         ctx.keep = (embed_c, labels_c, seg_c, pred_c, segq_c, pixq_c, shadow_c)   # keep inputs alive until kernels ran
         if ctx.needs_input_grad[0]:          # (grad mode is always off inside forward: ask the ctx, not torch)
@@ -402,15 +471,25 @@ class _PixelContrastFn(torch.autograd.Function):
         if ctx.keep is None or ws.token != getattr(ctx, "token", None):
             raise _abi.PclError("pixel_contrast_loss: backward ran twice on the same graph (retain_graph=True is not "
                                 "supported: the engine keeps no copy of the forward's scratch); call the loss again")
-        grad = torch.empty(ctx.embed_shape, dtype=ctx.embed_dtype, device=device)     # written in embed's dtype
         go = grad_out
         if go.device != device or go.dtype != torch.float32 or not go.is_contiguous():
             go = go.detach().to(device=device, dtype=torch.float32).contiguous()
         d = ws.desc
-        d.grad_embed = grad.data_ptr()
         d.embed_dtype = DTYPE_CODES[ctx.embed_dtype]
-        with _on_device(device):
-            _abi.check(lib.pcl_step_backward(C.byref(d), go.data_ptr(), _stream_ptr(device)), "pcl_step_backward")
+        sink = ctx.sink if ctx.sink is not None and ctx.sink.accepts() else None
+        if sink is not None:                 # the anchor columns go to the head's backward, zn gets a zero placeholder
+            ms = ws.geom.max_samples
+            cols = torch.empty((ms, ws.geom.D), dtype=torch.float32, device=device)
+            col_pix = torch.empty(ms, dtype=torch.int32, device=device)
+            with _on_device(device):
+                _abi.check(lib.pcl_step_backward_cols(C.byref(d), go.data_ptr(), cols.data_ptr(), col_pix.data_ptr(),
+                                                      _stream_ptr(device)), "pcl_step_backward_cols")
+            grad = sink.deposit(cols, col_pix, ctx.embed_shape)
+        else:
+            grad = torch.empty(ctx.embed_shape, dtype=ctx.embed_dtype, device=device)     # written in embed's dtype
+            d.grad_embed = grad.data_ptr()
+            with _on_device(device):
+                _abi.check(lib.pcl_step_backward(C.byref(d), go.data_ptr(), _stream_ptr(device)), "pcl_step_backward")
         _release_workspace(ws, getattr(ctx, "token", ws.token))     # also applies bank writes held back for this backward
         ctx.keep = None
         return grad, None, None, None, None, None, None, None
@@ -596,14 +675,15 @@ def _conv1x1_f32(weight, bias, rows, cols, dev):
 
 
 def _proj_pack(lib, x, weight, bias, s):
-    """For the fused last conv on x (B, Cin, H, W): wpack (pcl_proj_pack), the fp32 bias or None, zn and inv_norm."""
+    """For the fused last conv on x (B, Cin, H, W): wpack (pcl_proj_pack), the fp32 (256, Cin) weight, the fp32 bias or
+    None, zn and inv_norm."""
     B, Cin, HW, dev = x.shape[0], x.shape[1], x[0, 0].numel(), x.device
     w, bc = _conv1x1_f32(weight, bias, PROJ_DIM, Cin, dev)
     wpack = torch.empty(lib.pcl_proj_workspace_bytes(B, Cin, HW, 0), dtype=torch.uint8, device=dev)
     zn = torch.empty((B, PROJ_DIM) + tuple(x.shape[2:]), dtype=x.dtype, device=dev)
     inv = torch.empty(B * HW, dtype=torch.float32, device=dev)
     _abi.check(lib.pcl_proj_pack(w.data_ptr(), Cin, wpack.data_ptr(), s), "pcl_proj_pack")
-    return wpack, bc, zn, inv
+    return wpack, w, bc, zn, inv
 
 
 def _proj_grad_buffers(x, zn, gzn, scratch_bytes, has_bias):
@@ -627,7 +707,7 @@ class _ProjNormFn(torch.autograd.Function):
         xc = x.contiguous()
         with _on_device(dev):
             s = _stream_ptr(dev)
-            wpack, bc, zn, inv = _proj_pack(lib, xc, weight, bias, s)
+            wpack, _, bc, zn, inv = _proj_pack(lib, xc, weight, bias, s)
             _abi.check(lib.pcl_proj_fwd_dt(xc.data_ptr(), dt, wpack.data_ptr(), _abi.ptr(bc), B, Cin, HW, zn.data_ptr(),
                                            inv.data_ptr(), s), "pcl_proj_fwd_dt")
         ctx.save_for_backward(xc, zn, inv, wpack)
@@ -692,7 +772,7 @@ def _check_bn_input(what, name, x, gamma, training) -> None:
 def _bn_head_forward(lib, yc, dt, bn, gamma, beta, weight, bias, sums, group, s):
     """From conv1's output y on: (training) the all-reduce of the statistics ``sums`` for a multi-rank SyncBatchNorm and
     the counter, the BN state (batch or running statistics, running buffers updated), the last conv's packed weight
-    and the fused GEMM.  Returns zn, inv_norm, wpack, bn_state."""
+    and the fused GEMM.  Returns zn, inv_norm, wpack, the fp32 weight, bn_state."""
     B, Cin, HW = yc.shape[0], yc.shape[1], yc[0, 0].numel()
     g32, b32 = gamma.detach().contiguous(), beta.detach().contiguous()
     state = torch.empty(lib.pcl_proj_bn_workspace_bytes(B, Cin, HW, 0), dtype=torch.uint8, device=yc.device)
@@ -704,15 +784,23 @@ def _bn_head_forward(lib, yc, dt, bn, gamma, beta, weight, bias, sums, group, s)
     _abi.check(lib.pcl_proj_bn_finalize(_abi.ptr(sums), g32.data_ptr(), b32.data_ptr(), bn.running_mean.data_ptr(),
                                         bn.running_var.data_ptr(), Cin, bn.eps, bn.momentum, int(training),
                                         state.data_ptr(), s), "pcl_proj_bn_finalize")
-    wpack, bc, zn, inv = _proj_pack(lib, yc, weight, bias, s)
+    wpack, w, bc, zn, inv = _proj_pack(lib, yc, weight, bias, s)
     _abi.check(lib.pcl_proj_bn_fwd_dt(yc.data_ptr(), dt, state.data_ptr(), wpack.data_ptr(), _abi.ptr(bc), B, Cin, HW,
                                       zn.data_ptr(), inv.data_ptr(), s), "pcl_proj_bn_fwd_dt")
-    return zn, inv, wpack, state
+    return zn, inv, wpack, w, state
 
 
-def _bn_head_backward(lib, yc, dt, zn, inv, wpack, state, gzn, has_bias, training, group, s):
+def _bn_head_backward(lib, yc, dt, zn, inv, wpack, w2, state, gzn, has_bias, training, group, sink, s):
     """The backward of _bn_head_forward: returns the gradients of y, gamma, beta (rank-local), weight (256, Cin) and
-    bias (or None)."""
+    bias (or None).  sink (sparse_grad): the column path when gzn is its placeholder, else the dense path on gzn plus
+    the sink's deposits."""
+    if sink is not None:
+        if sink.is_placeholder(gzn):
+            ((cols, col_pix),) = sink.take()
+            return _bn_head_backward_cols(lib, yc, dt, zn, inv, w2, state, cols, col_pix, has_bias, training, group, s)
+        deposits = sink.take()
+        if deposits:
+            gzn = _with_deposits(gzn, deposits, zn.dtype)
     B, Cin, HW = yc.shape[0], yc.shape[1], yc[0, 0].numel()
     dev = yc.device
     g, scratch, gy, gw, gb = _proj_grad_buffers(yc, zn, gzn, lib.pcl_proj_bn_workspace_bytes(B, Cin, HW, 1), has_bias)
@@ -730,9 +818,41 @@ def _bn_head_backward(lib, yc, dt, zn, inv, wpack, state, gzn, has_bias, trainin
     return gy, ggamma, gbeta, gw, gb
 
 
+def _bn_head_backward_cols(lib, yc, dt, zn, inv, w2, state, cols, col_pix, has_bias, training, group, s):
+    """_bn_head_backward from the anchor columns of gzn alone (zero elsewhere): the last conv's gradients and the BN
+    backward's sums over the columns, then the dense gradient of y from y and those sums."""
+    B, Cin, HW = yc.shape[0], yc.shape[1], yc[0, 0].numel()
+    dev = yc.device
+    n = col_pix.numel()
+    scratch = _byte_scratch(lib.pcl_proj_bn_cols_workspace_bytes(n, Cin), "pcl_proj_bn_cols_workspace_bytes", dev)
+    gw = torch.empty((PROJ_DIM, Cin), dtype=torch.float32, device=dev)
+    gb = torch.empty(PROJ_DIM, dtype=torch.float32, device=dev) if has_bias else None
+    gsum = torch.empty(2 * Cin, dtype=torch.float32, device=dev)
+    ggamma = torch.empty(Cin, dtype=torch.float32, device=dev)
+    gbeta = torch.empty(Cin, dtype=torch.float32, device=dev)
+    _abi.check(lib.pcl_proj_bn_bwd_cols_dt(yc.data_ptr(), dt, state.data_ptr(), zn.data_ptr(), inv.data_ptr(),
+                                           cols.data_ptr(), col_pix.data_ptr(), n, w2.data_ptr(), B, Cin, HW,
+                                           scratch.data_ptr(), gw.data_ptr(), _abi.ptr(gb), gsum.data_ptr(),
+                                           ggamma.data_ptr(), gbeta.data_ptr(), s), "pcl_proj_bn_bwd_cols_dt")
+    if training and group is not None:                   # gamma / beta gradients stay rank-local, as in torch
+        torch.distributed.all_reduce(gsum, group=group)
+    gy = torch.empty_like(yc)
+    _abi.check(lib.pcl_proj_bn_input_grad_cols_dt(yc.data_ptr(), dt, state.data_ptr(), gsum.data_ptr(),
+                                                  scratch.data_ptr(), col_pix.data_ptr(), n, B, Cin, HW, int(training),
+                                                  gy.data_ptr(), s), "pcl_proj_bn_input_grad_cols_dt")
+    return gy, ggamma, gbeta, gw, gb
+
+
+def _sparse_output(zn: torch.Tensor, sparse_grad: bool) -> torch.Tensor:
+    """A sparse_grad head's zn registered as the sink of the engine loss that reads it (when autograd records zn)."""
+    if sparse_grad and zn.grad_fn is not None:
+        zn.grad_fn.sink = _register_sink(zn)
+    return zn
+
+
 class _BnProjNormFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, y, gamma, beta, weight, bias, bn):
+    def forward(ctx, y, gamma, beta, weight, bias, bn, sparse_grad):
         lib = _abi.load()
         _require_cuda(y, "y")
         dt = proj_dtype_code(y.dtype, "bn_relu_project_normalize")
@@ -749,40 +869,44 @@ class _BnProjNormFn(torch.autograd.Function):
                 sums = torch.empty(2 * Cin + 1, dtype=torch.float64, device=dev)
                 _abi.check(lib.pcl_proj_bn_stats_dt(yc.data_ptr(), dt, B, Cin, HW, sums.data_ptr(), s),
                            "pcl_proj_bn_stats_dt")
-            zn, inv, wpack, state = _bn_head_forward(lib, yc, dt, bn, gamma, beta, weight, bias, sums, group, s)
-        ctx.save_for_backward(yc, zn, inv, wpack, state)
+            zn, inv, wpack, w2, state = _bn_head_forward(lib, yc, dt, bn, gamma, beta, weight, bias, sums, group, s)
+        ctx.save_for_backward(yc, zn, inv, wpack, w2 if sparse_grad else None, state)
         ctx.meta = (tuple(weight.shape), bias is not None, dt, training, group, gamma.dtype)
+        ctx.sink = None
         return zn
 
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, gzn):
         lib = _abi.load()
-        yc, zn, inv, wpack, state = ctx.saved_tensors
+        yc, zn, inv, wpack, w2, state = ctx.saved_tensors
         wshape, has_bias, dt, training, group, gdtype = ctx.meta
         dev = yc.device
         with _on_device(dev):
-            gy, ggamma, gbeta, gw, gb = _bn_head_backward(lib, yc, dt, zn, inv, wpack, state, gzn, has_bias, training,
-                                                          group, _stream_ptr(dev))
-        return gy, ggamma.to(gdtype), gbeta.to(gdtype), gw.view(wshape), gb, None
+            gy, ggamma, gbeta, gw, gb = _bn_head_backward(lib, yc, dt, zn, inv, wpack, w2, state, gzn, has_bias,
+                                                          training, group, ctx.sink, _stream_ptr(dev))
+        return gy, ggamma.to(gdtype), gbeta.to(gdtype), gw.view(wshape), gb, None, None
 
 
 def bn_relu_project_normalize(y: torch.Tensor, bn: torch.nn.Module, weight: torch.Tensor,
-                              bias: Optional[torch.Tensor] = None) -> torch.Tensor:
+                              bias: Optional[torch.Tensor] = None, *, sparse_grad: bool = False) -> torch.Tensor:
     """F.normalize(F.conv2d(relu(bn(y)), weight, bias), p=2, dim=1): the projection head from the output y of its
     first conv to zn, with bn a BatchNorm2d or SyncBatchNorm (affine, tracking running stats, numeric momentum).  In
     training mode the batch statistics (fp64 sums; over all ranks of a SyncBatchNorm's process group, one all_reduce
     each way) normalise y, and running_mean / running_var / num_batches_tracked are updated as nn.BatchNorm2d does; in
     eval mode the running statistics are used.  The BN output and the ReLU output are never written: the GEMMs apply
     max(0, y scale + shift) where they convert their activation tile.  y (B, Cin, H, W) fp32 or bf16 CUDA, as for
-    project_normalize; autograd reaches y, bn.weight, bn.bias, weight and bias (bn's gradients rank-local)."""
+    project_normalize; autograd reaches y, bn.weight, bn.bias, weight and bias (bn's gradients rank-local).
+    sparse_grad=True: an engine contrast loss whose embed is the returned zn hands this node its anchor columns instead
+    of a dense gradient, and zn itself receives a zero placeholder (INTEGRATION §1); the backward then runs over those
+    columns only."""
     _check_bn(bn)
-    return _BnProjNormFn.apply(y, bn.weight, bn.bias, weight, bias, bn)
+    return _sparse_output(_BnProjNormFn.apply(y, bn.weight, bn.bias, weight, bias, bn, bool(sparse_grad)), sparse_grad)
 
 
 class _ConvBnProjNormFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, w1, b1, gamma, beta, w2, b2, bn):
+    def forward(ctx, x, w1, b1, gamma, beta, w2, b2, bn, sparse_grad):
         lib = _abi.load()
         _require_cuda(x, "x")
         dt = proj_dtype_code(x.dtype, "conv_bn_relu_project_normalize")
@@ -809,8 +933,9 @@ class _ConvBnProjNormFn(torch.autograd.Function):
             _abi.check(lib.pcl_proj_conv1_fwd_dt(xc.data_ptr(), dt, pack.data_ptr(), _abi.ptr(bc), B, C, HW,
                                                  y.data_ptr(), _abi.ptr(sums), _abi.ptr(scratch), s),
                        "pcl_proj_conv1_fwd_dt")
-            zn, inv, wpack, state = _bn_head_forward(lib, y, dt, bn, gamma, beta, w2, b2, sums, group, s)
-        ctx.save_for_backward(xc, y, zn, inv, pack, wpack, state)
+            zn, inv, wpack, w2f, state = _bn_head_forward(lib, y, dt, bn, gamma, beta, w2, b2, sums, group, s)
+        ctx.save_for_backward(xc, y, zn, inv, pack, wpack, w2f if sparse_grad else None, state)
+        ctx.sink = None
         ctx.meta = (tuple(w1.shape), b1 is not None, tuple(w2.shape), b2 is not None, dt, training, group, gamma.dtype)
         return zn
 
@@ -818,7 +943,7 @@ class _ConvBnProjNormFn(torch.autograd.Function):
     @torch.autograd.function.once_differentiable
     def backward(ctx, gzn):
         lib = _abi.load()
-        xc, y, zn, inv, pack, wpack, state = ctx.saved_tensors
+        xc, y, zn, inv, pack, wpack, w2f, state = ctx.saved_tensors
         w1shape, has_b1, w2shape, has_b2, dt, training, group, gdtype = ctx.meta
         B, C, HW = xc.shape[0], xc.shape[1], xc[0, 0].numel()
         dev = xc.device
@@ -827,17 +952,18 @@ class _ConvBnProjNormFn(torch.autograd.Function):
         gb1 = torch.empty(C, dtype=torch.float32, device=dev) if has_b1 else None
         with _on_device(dev):
             s = _stream_ptr(dev)
-            gy, ggamma, gbeta, gw2, gb2 = _bn_head_backward(lib, y, dt, zn, inv, wpack, state, gzn, has_b2, training,
-                                                            group, s)
+            gy, ggamma, gbeta, gw2, gb2 = _bn_head_backward(lib, y, dt, zn, inv, wpack, w2f, state, gzn, has_b2,
+                                                            training, group, ctx.sink, s)
             scratch = torch.empty(lib.pcl_proj_conv1_workspace_bytes(B, C, HW, 2), dtype=torch.uint8, device=dev)
             _abi.check(lib.pcl_proj_conv1_bwd_dt(xc.data_ptr(), dt, gy.data_ptr(), pack.data_ptr(), B, C, HW,
                                                  scratch.data_ptr(), _abi.ptr(gx), gw1.data_ptr(), _abi.ptr(gb1), s),
                        "pcl_proj_conv1_bwd_dt")
-        return (gx, gw1.view(w1shape), gb1, ggamma.to(gdtype), gbeta.to(gdtype), gw2.view(w2shape), gb2, None)
+        return (gx, gw1.view(w1shape), gb1, ggamma.to(gdtype), gbeta.to(gdtype), gw2.view(w2shape), gb2, None, None)
 
 
 def conv_bn_relu_project_normalize(x: torch.Tensor, w1: torch.Tensor, b1: Optional[torch.Tensor], bn: torch.nn.Module,
-                                   w2: torch.Tensor, b2: Optional[torch.Tensor] = None) -> torch.Tensor:
+                                   w2: torch.Tensor, b2: Optional[torch.Tensor] = None, *,
+                                   sparse_grad: bool = False) -> torch.Tensor:
     """F.normalize(F.conv2d(relu(bn(F.conv2d(x, w1, b1))), w2, b2), p=2, dim=1): the whole ``convmlp`` projection head
     on the engine.  The first 1x1 convolution (w1 (C, C, 1, 1), b1 (C) or None) is a bf16 wgmma GEMM whose epilogue
     also sums the BatchNorm statistics of its output y; y then goes through bn_relu_project_normalize's kernels (same
@@ -845,9 +971,10 @@ def conv_bn_relu_project_normalize(x: torch.Tensor, w1: torch.Tensor, b1: Option
     reduced over its process group, running statistics in eval).  x (B, C, H, W) fp32 or bf16 CUDA decides y's and
     zn's dtype (fp32 x is rounded to the bf16 GEMM operand).  autograd reaches x, w1, b1, bn.weight, bn.bias, w2 and b2
     (bn's gradients rank-local); x's gradient is skipped when x needs none.  No cuDNN call: forward and backward are
-    capturable and bit-reproducible run to run."""
+    capturable and bit-reproducible run to run.  sparse_grad as for bn_relu_project_normalize."""
     _check_bn(bn)
-    return _ConvBnProjNormFn.apply(x, w1, b1, bn.weight, bn.bias, w2, b2, bn)
+    return _sparse_output(_ConvBnProjNormFn.apply(x, w1, b1, bn.weight, bn.bias, w2, b2, bn, bool(sparse_grad)),
+                          sparse_grad)
 
 
 # ------------------------------------------------------------------------------------------------

@@ -13,6 +13,9 @@ training, running ones in eval; SyncBatchNorm reduces over its process group) an
 (functional.conv_bn_relu_project_normalize): a bf16 wgmma GEMM that also sums the BatchNorm statistics of its output,
 so the whole head is one autograd node with no cuDNN call.  Under ``torch.autocast(dtype=torch.bfloat16)`` a float32
 input is cast to bfloat16 as autocast's conv would cast it (y and zn are then bf16); fp16 autocast is refused.
+``sparse_grad=True`` (with ``fuse_bn_relu=True``) lets an engine contrast loss that reads zn hand the head's backward
+its anchor columns instead of a dense gradient: the last conv's gradients and the BN backward's sums run over those
+columns, and zn itself receives a zero placeholder (INTEGRATION §1).
 ``normalize=False`` returns the raw projection for the fused loss path (PixelContrastLoss(..., normalize=True) then
 normalises only the sampled columns)."""
 from __future__ import annotations
@@ -38,8 +41,11 @@ def _autocast_input(x):
 
 class ProjectionHead(nn.Module):
     def __init__(self, dim_in, proj_dim=256, proj="convmlp", bn_type="torchsyncbn", normalize=True, fused=False,
-                 fuse_bn_relu=False, fuse_conv1=False):
+                 fuse_bn_relu=False, fuse_conv1=False, sparse_grad=False):
         super().__init__()
+        if sparse_grad and not fuse_bn_relu:
+            # without the BN inside the node the input gradient would be a dense zero tensor of Cin channels
+            raise PclError("ProjectionHead(sparse_grad=True) needs fused=True, fuse_bn_relu=True and proj='convmlp'")
         if fuse_conv1 and not fuse_bn_relu:
             raise PclError("ProjectionHead(fuse_conv1=True) needs fuse_bn_relu=True")
         if fuse_bn_relu and not fused:
@@ -62,6 +68,7 @@ class ProjectionHead(nn.Module):
         self.fused = fused
         self.fuse_bn_relu = fuse_bn_relu
         self.fuse_conv1 = fuse_conv1
+        self.sparse_grad = sparse_grad
 
     def forward(self, x):
         if self.fused:
@@ -70,10 +77,10 @@ class ProjectionHead(nn.Module):
             if self.fuse_conv1:
                 conv1, conv2 = self.proj[0], self.proj[2]
                 return conv_bn_relu_project_normalize(_autocast_input(x), conv1.weight, conv1.bias, self.proj[1][0],
-                                                      conv2.weight, conv2.bias)
+                                                      conv2.weight, conv2.bias, sparse_grad=self.sparse_grad)
             if self.fuse_bn_relu:
                 return bn_relu_project_normalize(self.proj[0](x), self.proj[1][0], self.proj[2].weight,
-                                                 self.proj[2].bias)
+                                                 self.proj[2].bias, sparse_grad=self.sparse_grad)
             if isinstance(self.proj, nn.Conv2d):
                 last, y = self.proj, x
             else:

@@ -260,6 +260,29 @@ int pcl_proj_bn_bwd_dt(const void* y, int32_t dtype, const void* bn_state, const
 int pcl_proj_bn_input_grad_dt(const void* y, int32_t dtype, const void* bn_state, const float* gsum, int32_t B,
                               int32_t Cin, int64_t HW, int32_t training, void* g, void* stream);
 
+/* The backward of the calls above when gzn is zero outside n_cols anchor columns (what pcl_step_backward_cols hands
+ * over): cols (n_cols, 256) fp32, col_pix[a] = b*HW + p, or < 0 for an unused column.  Replaces pcl_proj_bn_bwd_dt +
+ * pcl_proj_bn_input_grad_dt (csrc/pcl_norm.cu:1347, :1371) on the dense gzn built from the columns; no dense gzn, bf16
+ * gz or dense gu is written, and the last conv's GEMMs run over the columns only.  ReLU' and the BN backward of a
+ * gradient that is zero off the anchors leave g_y = gamma invstd (gu - sum gu / n - x_hat sum(gu x_hat) / n): the
+ * anchors' gu plus a per-channel affine function of x_hat.  Plain fp32 on w2, the fp32 (256, Cin) weight of the last
+ * conv; every sum runs in a fixed order (bit-reproducible).
+ *   pcl_proj_bn_cols_workspace_bytes  scratch bytes for (n_cols, Cin).
+ *   pcl_proj_bn_bwd_cols_dt       gw (256, Cin), gb (may be NULL), gsum (2*Cin) and gbeta / ggamma (may be NULL) as
+ *                                 pcl_proj_bn_bwd_dt defines them; the anchors' gu stay in scratch for the next call.
+ *   pcl_proj_bn_input_grad_cols_dt  writes the whole gradient g of y (B,Cin,HW, dtype) from y, bn_state, gsum (summed
+ *                                 over ranks for SyncBatchNorm) and the scratch of the call above; training 0 gives
+ *                                 gamma invstd gu at the anchors and 0 elsewhere.
+ * y, zn and g have element type `dtype` (PCL_DT_F32 or PCL_DT_BF16).  No call synchronises with the host. */
+int64_t pcl_proj_bn_cols_workspace_bytes(int32_t n_cols, int32_t Cin);
+int pcl_proj_bn_bwd_cols_dt(const void* y, int32_t dtype, const void* bn_state, const void* zn, const float* inv_norm,
+                            const float* cols, const int32_t* col_pix, int32_t n_cols, const float* w2, int32_t B,
+                            int32_t Cin, int64_t HW, void* scratch, float* gw, float* gb, float* gsum, float* ggamma,
+                            float* gbeta, void* stream);
+int pcl_proj_bn_input_grad_cols_dt(const void* y, int32_t dtype, const void* bn_state, const float* gsum,
+                                   const void* scratch, const int32_t* col_pix, int32_t n_cols, int32_t B, int32_t Cin,
+                                   int64_t HW, int32_t training, void* g, void* stream);
+
 /* The head's first 1x1 convolution (Conv2d(C, C, 1), lib/models/modules/projection.py:17-19) in front of the calls
  * above, as bf16 wgmma GEMMs (fp32 accumulate), forward and backward, with the BatchNorm statistics of its output in the
  * forward's epilogue.  x, y, gy and gx (B,C,HW) have element type `dtype` (PCL_DT_F32 or PCL_DT_BF16; anything else
@@ -552,6 +575,13 @@ int pcl_step_backward(const pcl_step_desc* d, const float* grad_loss, void* stre
  * the backward sweep and scatters only the sampled columns.  Nothing else of grad_embed is written.  Not for top-k
  * steps (PCL_ERR_UNSUPPORTED): their backward writes the dense gradient itself. */
 int pcl_step_backward_prezeroed(const pcl_step_desc* d, const float* grad_loss, void* stream);
+/* pcl_step_backward (csrc/pcl_step.cu:149) with the anchor columns as its output instead of the dense grad_embed, which
+ * is not touched: d loss / d embed is zero outside the A <= max_samples sampled pixels.  cols (max_samples, D) fp32:
+ * row s < A holds the values pcl_step_backward writes at the anchor's pixel (bit-identical for an fp32 embed; for a
+ * half embed, the fp32 values before its rounding), col_pix[s] = b*h*w + pix; rows s >= A are zero with col_pix -1.  A
+ * stays on the device (no host sync).  Every mode of pcl_step_backward: exact and tensor sweeps, top-k, normalize,
+ * bank. */
+int pcl_step_backward_cols(const pcl_step_desc* d, const float* grad_loss, float* cols, int32_t* col_pix, void* stream);
 
 /* CUDA-graph capture of a step (SURVEY §8f row 4).  The three calls above neither allocate nor synchronise, so a
  * stats -> forward -> backward sequence can be captured with cudaStreamBeginCapture / replayed with cudaGraphLaunch.
