@@ -285,7 +285,9 @@ class _ColumnSink:
         return zero.expand(shape)
 
     def is_placeholder(self, g: torch.Tensor) -> bool:
-        return (len(self.deposits) == 1 and len(self.zeros) == 1 and all(st == 0 for st in g.stride())
+        # expand() keeps the stride of a dimension of size 1 (W = 1, or HW = 1): only the others must be 0
+        return (len(self.deposits) == 1 and len(self.zeros) == 1
+                and all(st == 0 or n == 1 for st, n in zip(g.stride(), g.shape))
                 and g.data_ptr() == self.zeros[0].data_ptr())
 
     def take(self):

@@ -1,12 +1,13 @@
 """TEST INFRASTRUCTURE: differential fuzzing of the engine (real SIMT kernel sources on the host-fiber emulator,
 tests/emu) against the oracle over random geometries.  Used by tests/test_emu_fuzz.py (bounded) and
-tools/emu_fuzz.py (long runs).  Every fuzzer returns a list of failure descriptions (empty = clean); fuzz_graphed_step
-and fuzz_graphed_criterion also return how many cases reached each of their coverage categories, so that a test can
-require all of them.
+tools/emu_fuzz.py (long runs).  Every fuzzer returns a list of failure descriptions (empty = clean); fuzz_graphed_step,
+fuzz_graphed_criterion and fuzz_projection_head also return how many cases reached each of their coverage
+categories, so that a test can require all of them.
 
-It found the out-of-bounds wrap write for pixel_update_freq > memory_size (now refused, csrc/pcl_bank.cu: make_dims)
-and the NaN gradient of the two-call seg CE with a label grid smaller than the logits and every pixel ignored (now 0,
-csrc/pcl_segce.cu: k_segce_bwd_gather)."""
+It found the out-of-bounds wrap write for pixel_update_freq > memory_size (now refused, csrc/pcl_bank.cu: make_dims),
+the NaN gradient of the two-call seg CE with a label grid smaller than the logits and every pixel ignored (now 0,
+csrc/pcl_segce.cu: k_segce_bwd_gather), and the sparse head's silent dense fallback on a feature map one pixel wide
+(functional._ColumnSink.is_placeholder)."""
 import math
 import random
 
@@ -1320,3 +1321,710 @@ def fuzz_wrappers(seed: int, n: int):
     finally:
         loss_mod.ContrastCELoss._can_fuse = saved
     return bad
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# the fused projection head (csrc/pcl_norm.cu): every fusion level, the dense and the anchor-column backward
+# ------------------------------------------------------------------------------------------------------------------
+HEAD_CATEGORIES = ("plain", "bn_relu", "conv1", "fp32", "bf16", "autocast", "train", "eval", "SyncBatchNorm",
+                   "a bias None", "x without grad", "dense gzn", "column hand-off", "contrast loss", "fallback",
+                   "all-dead deposit", "first / last pixel column", "n_cols at a tile edge", "A = 0",
+                   "A = max_samples", "Cin at a 64 edge", "Cin 255-257", "HW = 1", "clamped pixel", "dead BN channel",
+                   "large-mean channel", "weights changed", "control replay")
+# Cin and H x W lean on the kernels' edges: 64-wide K-blocks and wgrad tiles, 256-channel bands (the column buffers'
+# Cin + 1 row, k_col_prep's c += 256 loop, conv1's one-row bands at 257 / 513), BM = 128 pixel tiles, WB = 64
+_HEAD_CIN = (16, 40, 63, 64, 65, 127, 128, 129, 191, 255, 256, 257, 300, 320)
+_HEAD_CIN_DEV = (511, 512, 513, 720, 1023, 1024, 2048)
+_HEAD_HW = (1, 2, 7, 63, 64, 65, 127, 128, 129, 191, 255, 256, 257)
+_HEAD_NCOLS = (1, 63, 64, 65, 127, 128, 129)
+_FALLBACK_PATTERNS = ("other_term", "two_losses", "retain_grad", "hook")
+
+# Per-element bound of |kernel - float64 reference| (_head_bound), built in float64 from the operand magnitudes along
+# the same chain, so that it scales with the shape instead of being measured at a few.  With u = 2^-24 and u_bf = 2^-8,
+# the unit roundoffs of fp32 and bf16 (24 and 8 significant bits: rounding to nearest is off by at most half an ulp, u
+# of the value), and gam(n) = n u / (1 - n u) (the classical bound of an n-term fp32 sum of products relative to the
+# sum of their magnitudes):
+#   * a GEMM product whose two operands the kernel rounds to bf16 and the reference may keep (u or W2 in fp32):
+#     _RB = (1 + u_bf)^2 - 1 of |a||b|;
+#   * a computed value that kernel and reference both round to bf16 (gz before the last conv's GEMMs, g_y before
+#     conv1's): their inputs differ by rounding, so the two results can land on neighbouring bf16 values, one ulp,
+#     _ULP = 2 u_bf = 2^-7 of the value;
+#   * a value only the kernel rounds to bf16 (the fp32 columns the reference takes rounded, the stored bf16 zn the
+#     backward reads): u_bf;
+#   * the forward error reaches the backward through zn and inv_norm (|d zn| <= (|dz| + |zn| <|zn|, |dz|>) inv), the
+#     BN terms through k1 = sum(g_u) / N and k2 = sum(g_u x_hat) / N;
+#   * an element within PB.KINK of the ReLU's kink may take the other branch: its g_u is bounded by its full magnitude;
+#   * the output's own rounding: u_bf of the value for bf16, 2u for fp32.
+# Every step adds the errors of its inputs through the magnitudes of the other operands.  That is first order: the
+# products of two errors it leaves out are below (2^-7)^2 of the terms, negligible next to the first-order ones.
+_U32 = 2. ** -24
+_UBF = 2. ** -8
+_RB = (1 + _UBF) ** 2 - 1
+_ULP = 2 * _UBF
+_OUT = {torch.float32: 2 * _U32, torch.bfloat16: _UBF}
+# The Frobenius norm of the error against that of the per-element bound: rounding errors of independent terms add up
+# like a random walk, the bound like a worst case, so the error stays a small fraction of it (DESIGN §4 lists the ratios
+# measured on an H100).
+HEAD_FROB_FRACTION = 0.25
+
+
+def _gam(n):
+    return n * _U32 / (1. - n * _U32)
+
+
+def _head_bound(c, x, w1, b1, bn0, w2, b2, g, y_stored, kink, out_dtype, n_rows):
+    """{name: float64 per-element bound} of the head's outputs (see the constants above) for one call.  bn0: (training,
+    gamma, beta, running_mean, running_var, eps) as the call saw them; y_stored: conv1's y as stored (conv1 level);
+    kink: the reference's ReLU-kink mask; n_rows: the length of the pixel sums (B HW, or the live column count)."""
+    d64 = lambda t: t.detach().double()                                             # noqa: E731
+    B, C = x.shape[:2]
+    P = x[0, 0].numel()
+    X = (d64(x.to(torch.bfloat16)) if c["level"] != "bn_relu" else d64(x)).reshape(B, C, P)
+    W2 = d64(w2).reshape(256, C)
+    aW2 = W2.abs()
+    absb2 = 0. if b2 is None else d64(b2).abs().view(1, 256, 1)
+    n = max(n_rows, 1)
+    out = {}
+    if c["level"] == "plain":
+        U, Eu = X, torch.zeros_like(X)
+    else:
+        training, gamma, beta, rm, rv, eps = bn0
+        Y = X if c["level"] == "bn_relu" else d64(y_stored).reshape(B, C, P)
+        if training:
+            mean, var = Y.mean((0, 2)), Y.var((0, 2), unbiased=False)
+        else:
+            mean, var = d64(rm), d64(rv)
+        invstd = 1. / torch.sqrt(var + eps)
+        sc = (d64(gamma) * invstd).view(1, C, 1)
+        sh = d64(beta).view(1, C, 1) - mean.view(1, C, 1) * sc
+        A = Y * sc + sh
+        mask = (A > 0).double()
+        U = A.clamp_min(0.)
+        Ea = 8 * _U32 * ((Y * sc).abs() + sh.abs())
+        Eu = Ea * (A > -Ea)                     # below -Ea the ReLU gives an exact 0 on both sides
+        XH = (Y - mean.view(1, C, 1)) * invstd.view(1, C, 1)
+        Exh = 8 * _U32 * (Y.abs() + mean.abs().view(1, C, 1)) * invstd.view(1, C, 1)
+        K = d64(kink).reshape(B, C, P).double()
+    Z = torch.einsum("nc,bcp->bnp", W2, U) + (0. if b2 is None else d64(b2).view(1, 256, 1))
+    Ez = (_RB + _gam(C + 1)) * (torch.einsum("nc,bcp->bnp", aW2, U.abs()) + absb2) + \
+        torch.einsum("nc,bcp->bnp", aW2, Eu)
+    nz = Z.norm(dim=1, keepdim=True)
+    inv = 1. / nz.clamp_min(1e-12)
+    ZN = Z * inv
+    aZN = ZN.abs()
+    rel_inv = (aZN * Ez).sum(1, keepdim=True) * inv                 # relative error of inv_norm
+    Ezn = (Ez + aZN * (aZN * Ez).sum(1, keepdim=True)) * inv + _gam(256) * aZN        # + the norm's own sum
+    out["zn"] = Ezn + _OUT[out_dtype] * aZN
+    Ezn_used = Ezn + (_UBF if out_dtype == torch.bfloat16 else 0.) * aZN      # the backward reads the stored zn
+    G = d64(g).reshape(B, 256, P)
+    aG = G.abs()
+    dot = (ZN * G).sum(1, keepdim=True)
+    GZ = torch.where(nz < 1e-12, G * inv, (G - ZN * dot) * inv)
+    MGZ = (aG + aZN * (aZN * aG).sum(1, keepdim=True)) * inv
+    # the column path takes the loss's fp32 columns, the reference their rounding to zn's dtype: one more u_bf of g
+    rg = _UBF if out_dtype == torch.bfloat16 else 0.
+    Egz = (_ULP + _gam(256) + rg) * MGZ + inv * (Ezn_used * dot.abs() + aZN * (Ezn_used * aG).sum(1, keepdim=True)) + \
+        GZ.abs() * rel_inv
+    aGZ = GZ.abs()
+    sum_p = lambda t: t.sum((0, 2)) if t.dim() == 3 else t                          # noqa: E731
+    out_w = lambda E, V: E + _OUT[torch.float32] * V.abs()                           # noqa: E731
+    GW2 = torch.einsum("bnp,bcp->nc", GZ, U)
+    Egw2 = (_RB + _gam(n)) * torch.einsum("bnp,bcp->nc", aGZ, U.abs()) + torch.einsum("bnp,bcp->nc", Egz, U.abs()) + \
+        torch.einsum("bnp,bcp->nc", aGZ, Eu)
+    Egb2 = _gam(n) * sum_p(aGZ) + sum_p(Egz)
+    wname, bname, xname = ("gw", "gb", "gx") if c["level"] == "plain" else \
+        (("gw", "gb", "gy") if c["level"] == "bn_relu" else ("gw2", "gb2", "gx"))
+    out[wname] = out_w(Egw2, GW2).view(256, C)
+    out[bname] = out_w(Egb2, sum_p(GZ))
+    MGU = torch.einsum("nc,bnp->bcp", aW2, aGZ)
+    Ed = (_RB + _gam(256)) * MGU + torch.einsum("nc,bnp->bcp", aW2, Egz)
+    if c["level"] == "plain":
+        GX = torch.einsum("nc,bnp->bcp", W2, GZ)
+        out["gx"] = (Ed + _OUT[out_dtype] * (GX.abs() + Ed)).reshape(x.shape)
+        return out
+    GU = torch.einsum("nc,bnp->bcp", W2, GZ) * mask
+    Egu = mask * Ed + K * MGU
+    aGU = GU.abs()
+    N = B * P
+    Egbeta = _gam(n) * sum_p(aGU) + sum_p(Egu)
+    Eggamma = (_gam(n) + 8 * _U32) * sum_p(aGU * XH.abs()) + sum_p(Egu * XH.abs()) + sum_p(aGU * Exh)
+    out["gbeta"] = out_w(Egbeta, sum_p(GU))
+    out["ggamma"] = out_w(Eggamma, sum_p(GU * XH))
+    if training:
+        k1, k2 = (sum_p(GU) / N).view(1, C, 1), (sum_p(GU * XH) / N).view(1, C, 1)
+        GY = sc * (GU - k1 - XH * k2)
+        Egy = sc.abs() * (Egu + (Egbeta / N).view(1, C, 1) + XH.abs() * (Eggamma / N).view(1, C, 1) +
+                          Exh * k2.abs() + 8 * _U32 * (aGU + k1.abs() + (XH * k2).abs()))
+    else:
+        GY = sc * GU
+        Egy = sc.abs() * (Egu + 4 * _U32 * aGU)
+    if c["level"] == "bn_relu":
+        out["gy"] = (Egy + _OUT[out_dtype] * (GY.abs() + Egy)).reshape(x.shape)
+        return out
+    W1 = d64(w1.to(torch.bfloat16)).reshape(C, C)
+    Egy_r = Egy + _ULP * GY.abs()                                   # g_y rounded to bf16 for conv1's GEMMs
+    aGY = GY.abs()
+    GX = torch.einsum("nc,bnp->bcp", W1, GY)
+    Egx = _gam(C) * torch.einsum("nc,bnp->bcp", W1.abs(), aGY) + torch.einsum("nc,bnp->bcp", W1.abs(), Egy_r)
+    out["gx"] = (Egx + _OUT[out_dtype] * (GX.abs() + Egx)).reshape(x.shape)
+    out["gw1"] = out_w(_gam(n) * torch.einsum("bnp,bcp->nc", aGY, X.abs()) +
+                       torch.einsum("bnp,bcp->nc", Egy_r, X.abs()),
+                       torch.einsum("bnp,bcp->nc", GY, X)).view(C, C, 1, 1)
+    out["gb1"] = out_w(_gam(n) * sum_p(aGY) + sum_p(Egy_r), sum_p(GY))
+    return out
+
+
+def _draw_head_case(rng, it, scale, device):
+    """One case of fuzz_projection_head: the head, the geometry, the incoming gradient and the adversarial value.  The
+    level, gradient source and adversarial value rotate with `it`, the rest is drawn."""
+    dev = torch.device(device).type == "cuda"
+    level = ("bn_relu", "conv1", "plain")[it % 3]
+    grad = "dense" if level == "plain" else ("cols", "loss", "fallback", "dense")[(it - (it + 1) // 3) % 4]
+    adv = (None, "clamped", "dead channel", "large mean", None)[(it // 2) % 5]
+    if level == "plain" and adv in ("dead channel", "large mean"):
+        adv = None
+    c = dict(level=level, grad=grad, adv=adv, seed=rng.randint(0, 10 ** 6))
+    c["act"] = ("fp32", "bf16", "autocast")[(it // 3) % 3] if level == "conv1" else rng.choice(["fp32", "bf16"])
+    c["train"] = level != "plain" and (adv == "large mean" or rng.random() < 0.7)
+    if adv == "clamped" and level == "conv1":
+        c["train"] = False          # conv1's y at an all-zero x column is b1: only the running statistics place it
+    c["sync"] = level != "plain" and rng.random() < 0.3
+    c["momentum"] = rng.choice([0.1, 0.01, 0.5, 1.0])
+    c["b1"] = level == "conv1" and rng.random() < 0.75
+    c["b2"] = rng.random() < 0.75 if adv != "clamped" else rng.choice([False, "tiny"])
+    c["x_grad"] = level != "conv1" or rng.random() < 0.75
+    cins = _HEAD_CIN + (_HEAD_CIN_DEV if dev else ())
+    if level == "conv1" and rng.random() < 0.3:
+        cins = (257, 513) if dev else (257,)                     # conv1's one-row bands
+    Cin = rng.choice(cins)
+    cap = 200 * scale * scale if Cin <= 320 else 30 * scale * scale
+    if not dev and it == 4:                                      # one wide case at a small image on the emulator
+        Cin, cap = 720, 12
+    if dev and it == 5:
+        Cin = 2048
+    hws = [h for h in _HEAD_HW if h <= cap and (h > 1 or not c["train"])]
+    HW = 1 if it == 2 else rng.choice(hws)
+    B = rng.randint(1, max(1, min(8, cap // HW)))
+    if c["train"] and B * HW < 2:
+        B = 2
+    divs = [d for d in range(1, HW + 1) if HW % d == 0]
+    H = rng.choice(divs)
+    c.update(B=B, Cin=Cin, H=H, W=HW // H)
+    if grad == "cols":
+        c["n_cols"] = rng.choice(_HEAD_NCOLS + (rng.randint(2, 300),))
+    if grad in ("loss", "fallback"):
+        K = rng.randint(2, 6)
+        c.update(K=K, precision=rng.choice(["fp32", "bf16"]), bank=rng.random() < 0.3,
+                 ms=rng.choice([B * K, B * K, 2 * B * K, rng.randint(2, 200)]), mv=rng.choice([2, 2, 4, 100]))
+    if grad == "fallback":
+        c["pattern"] = _FALLBACK_PATTERNS[(it // 12) % 4] if rng.random() < 0.5 else rng.choice(_FALLBACK_PATTERNS)
+    c["n_rep"] = rng.randint(2, 4)
+    c["actions"] = [rng.choice(["inputs", "weights", "both", "both", "control"]) for _ in range(c["n_rep"] - 1)]
+    return c
+
+
+class _Head:
+    """One copy of the fuzzed head: its leaves (w1, b1, gamma, beta, w2, b2), its BatchNorm and its call."""
+
+    def __init__(self, c, init, sparse, device):
+        import torch.nn as nn
+        self.c, self.sparse = c, sparse
+        C = c["Cin"]
+        self.bn = None
+        if c["level"] != "plain":
+            self.bn = (nn.SyncBatchNorm(C) if c["sync"] else nn.BatchNorm2d(C)).to(device)
+            self.bn.momentum = c["momentum"]
+            with torch.no_grad():
+                for k in ("weight", "bias", "running_mean", "running_var"):
+                    getattr(self.bn, k).copy_(init[k])
+            self.bn.train(c["train"])
+        if c["level"] == "conv1":
+            self.mod = cs.ProjectionHead(C, 256, "convmlp", bn_type="torchsyncbn" if c["sync"] else "torchbn",
+                                         fused=True, fuse_bn_relu=True, fuse_conv1=True, sparse_grad=sparse).to(device)
+            self.mod.proj[1][0] = self.bn
+            conv1, conv2 = self.mod.proj[0], self.mod.proj[2]
+            with torch.no_grad():
+                conv1.weight.copy_(init["w1"])
+                conv2.weight.copy_(init["w2"])
+                for conv, k in ((conv1, "b1"), (conv2, "b2")):
+                    if init[k] is None:
+                        conv.register_parameter("bias", None)
+                    else:
+                        conv.bias.copy_(init[k])
+            self.w1, self.b1, self.w2, self.b2 = conv1.weight, conv1.bias, conv2.weight, conv2.bias
+        else:
+            self.w1 = self.b1 = None
+            self.w2 = init["w2"].clone().to(device).requires_grad_(True)
+            self.b2 = None if init["b2"] is None else init["b2"].clone().to(device).requires_grad_(True)
+
+    def leaves(self):
+        ps = {"w1": self.w1, "b1": self.b1, "w2": self.w2, "b2": self.b2}
+        if self.bn is not None:
+            ps.update(gamma=self.bn.weight, beta=self.bn.bias)
+        return {k: v for k, v in ps.items() if v is not None}
+
+    def __call__(self, x):
+        c = self.c
+        if c["level"] == "plain":
+            return cs.project_normalize(x, self.w2, self.b2)
+        if c["level"] == "bn_relu":
+            return cs.bn_relu_project_normalize(x, self.bn, self.w2, self.b2, sparse_grad=self.sparse)
+        with torch.autocast(x.device.type, dtype=torch.bfloat16, enabled=c["act"] == "autocast"):
+            return self.mod(x)
+
+    def grads(self, x):
+        names = {"plain": {"w2": "gw", "b2": "gb"}, "bn_relu": {"w2": "gw", "b2": "gb"},
+                 "conv1": {"w1": "gw1", "b1": "gb1", "w2": "gw2", "b2": "gb2"}}[self.c["level"]]
+        out = {names[k]: p.grad for k, p in self.leaves().items() if k in names}
+        if self.bn is not None:
+            out.update(ggamma=self.bn.weight.grad, gbeta=self.bn.bias.grad)
+        if x.requires_grad:
+            out["gy" if self.c["level"] == "bn_relu" else "gx"] = x.grad
+        return out
+
+    def absent(self, x_grad):
+        """The outputs this head has none of: the gradient of a bias that is None, x's when x needs none."""
+        conv1 = self.c["level"] == "conv1"
+        out = set()
+        if self.b2 is None:
+            out.add("gb2" if conv1 else "gb")
+        if conv1 and self.b1 is None:
+            out.add("gb1")
+        if not x_grad:
+            out.add("gy" if self.c["level"] == "bn_relu" else "gx")
+        return out
+
+    def zero_grad(self, x):
+        for p in list(self.leaves().values()) + [x]:
+            p.grad = None
+
+    def buffers(self):
+        return {} if self.bn is None else {k: getattr(self.bn, k).clone() for k in ("running_mean", "running_var",
+                                                                                     "num_batches_tracked")}
+
+
+def _head_init(c, g):
+    C = c["Cin"]
+    init = {"w1": torch.randn(C, C, 1, 1, generator=g) / C ** 0.5, "b1": 0.5 * torch.randn(C, generator=g),
+            "weight": 1 + 0.2 * torch.randn(C, generator=g), "bias": 0.2 * torch.randn(C, generator=g),
+            "running_mean": 0.3 * torch.randn(C, generator=g), "running_var": 0.5 + torch.rand(C, generator=g),
+            "w2": torch.randn(256, C, 1, 1, generator=g) / C ** 0.5, "b2": 0.1 * torch.randn(256, generator=g)}
+    if not c["b1"]:
+        init["b1"] = None
+    if c["b2"] == "tiny":           # z = b2 at the clamped pixel: |z| = 0.95 eps, F.normalize's clamped branch with
+        b2 = torch.randn(256, generator=g)      # |zn| = 0.95, where projecting gzn would change its gradient
+        init["b2"] = b2 * (0.95e-12 / b2.norm())
+    elif not c["b2"]:
+        init["b2"] = None
+    if c["adv"] == "clamped":
+        init["weight"] = init["weight"].abs().clamp(0.9, 1.5)
+        init["bias"] = init["bias"].clamp(-0.3, 0.3)
+        if c["level"] == "conv1":   # y = b1 at the all-zero x column, 4 running standard deviations below the mean
+            init["b1"] = init["running_mean"] - 4 * torch.sqrt(init["running_var"] + 1e-5)
+    if c["adv"] == "dead channel":
+        init["bias"][0] = -1e3
+    if c["adv"] == "large mean" and c["level"] == "conv1":
+        if init["b1"] is None:
+            init["b1"] = torch.zeros(C)
+            c["b1"] = True
+        init["b1"][0] = 1000.
+    return init
+
+
+def _head_x(c, init_bn, g, pix):
+    """x for one replay (fp32, CPU), with the case's adversarial value; pix = (b, p) of the clamped pixel."""
+    B, C, H, W = c["B"], c["Cin"], c["H"], c["W"]
+    x = torch.randn(B, C, H, W, generator=g)
+    if c["level"] == "bn_relu":
+        x = x * (0.5 + torch.rand(1, C, 1, 1, generator=g)) + 0.5 * torch.randn(1, C, 1, 1, generator=g)
+    if c["adv"] == "large mean" and c["level"] == "bn_relu":
+        x[:, 0] += 1000.
+    if c["adv"] == "clamped":
+        b, p = pix
+        xv = x.view(B, C, H * W)
+        if c["level"] == "bn_relu":   # every BN output of the pixel below 0: 4 standard deviations under the others
+            if c["train"]:
+                others = torch.cat([xv[:b].transpose(0, 1).reshape(C, -1), xv[b, :, :p], xv[b, :, p + 1:],
+                                    xv[b + 1:].transpose(0, 1).reshape(C, -1)], 1)
+                xv[b, :, p] = others.min(1).values - 4 * (others.std(1, unbiased=False) + 1)
+            else:
+                xv[b, :, p] = init_bn[0] - 4 * torch.sqrt(init_bn[1] + 1e-5)
+        else:
+            xv[b, :, p] = 0.
+    return x
+
+
+def _head_cols(c, g, live, pix, n_px):
+    """Static column buffers of n_cols entries: `live` distinct pixels (the clamped pixel and, when there is room, the
+    first and last pixel of the batch among them) at shuffled slots, the rest dead (-1); bf16-exact values."""
+    n = c["n_cols"]
+    q = torch.randperm(n_px, generator=g)[:live]
+    if live:
+        forced = ([pix[0] * c["H"] * c["W"] + pix[1]] if c["adv"] == "clamped" else []) + [0, n_px - 1]
+        forced = torch.tensor(list(dict.fromkeys(forced)))
+        q = torch.cat([forced, q[~torch.isin(q, forced)]])[:live]
+    col_pix = torch.full((n,), -1, dtype=torch.int32)
+    slots = torch.randperm(n, generator=g)[:live]
+    col_pix[slots] = q.to(torch.int32)
+    cols = torch.randn(n, 256, generator=g).to(torch.bfloat16).float()
+    cols[col_pix < 0] = torch.randn(int((col_pix < 0).sum()), 256, generator=g).to(torch.bfloat16).float()
+    return cols, col_pix
+
+
+def _head_reference(c, x, h, gzn):
+    """The float64 chain of the case's level (test_gpu_projection*.py), with a bias that is None taken as zeros: the
+    outputs, the BN statistics (or None) and conv1's stored y (or None)."""
+    import test_gpu_projection as TP
+    import test_gpu_projection_bnrelu as TPB
+    import test_gpu_projection_conv1 as TPC
+    z = lambda b, n: torch.zeros(n, device=x.device) if b is None else b.detach()       # noqa: E731
+    w2, b2 = h.w2.detach(), z(h.b2, 256)
+    if c["level"] == "plain":
+        return TP._reference(x, w2, b2, gzn, True), None, None
+    if c["level"] == "bn_relu":
+        ref, st = TPB._reference(x, h.bn, w2, b2, gzn)
+        return ref, st, None
+    b1 = z(h.b1, c["Cin"])
+    ref, st = TPC.head_reference(x, h.w1.detach(), b1, h.bn, w2, b2, gzn)
+    return ref, st, TPC.conv1_abi(x, h.w1.detach(), b1)["y"]
+
+
+def _score_head(got, ref, bound, absent, worst, where):
+    """Every output within its per-element bound and the Frobenius fraction; worst[name] keeps the largest ratio.  Only
+    the outputs in `absent` (a bias that is None, x without a gradient) may be missing, and those must be."""
+    bad = []
+    for k, b in bound.items():
+        if (got.get(k) is None) != (k in absent):
+            bad.append(f"{where}: {k} {'missing' if k not in absent else 'written although the case has none'}")
+            continue
+        if k in absent:
+            continue
+        d = (got[k].double().reshape(-1) - ref[k].double().reshape(-1)).abs()
+        b = b.reshape(-1)
+        if not bool(torch.isfinite(d).all()):
+            bad.append(f"{where}: {k} not finite")
+            continue
+        ratio = (d / b.clamp_min(1e-300)).max().item()
+        frob = (d.norm() / b.norm().clamp_min(1e-300)).item()
+        worst[k] = max(worst.get(k, 0.), ratio)
+        worst["frob " + k] = max(worst.get("frob " + k, 0.), frob)
+        if ratio > 1. or frob > HEAD_FROB_FRACTION:
+            bad.append(f"{where}: {k} error/bound {ratio:.3g} (Frobenius {frob:.3g})")
+    return bad
+
+
+def _loss_options(c, r, k=0):
+    g = torch.Generator().manual_seed(c["seed"] + 1000 * r + k)
+    return cs.ContrastOptions(temperature=0.1, base_temperature=0.07, max_samples=c["ms"], max_views=c["mv"],
+                              precision=c["precision"], rng="torch_cpu", num_classes=c["K"], nan_safe=True,
+                              perm_fn=lambda n: torch.randperm(n, generator=g))
+
+
+def _head_loss(c, zn, lab, r):
+    """The contrast loss on zn (c), or the case's fallback consumer pattern (d)."""
+    target, seg, bank = lab
+    kw = dict(seg=seg, segment_queue=bank[0], pixel_queue=bank[1]) if bank else dict(seg=seg)
+    pat = c.get("pattern") if c["grad"] == "fallback" else None
+    if pat == "retain_grad":
+        zn.retain_grad()
+    if pat == "hook":
+        zn.register_hook(lambda g: g * 1.0)
+    loss = cs.pixel_contrast_loss(zn, target, options=_loss_options(c, r), **kw)
+    if pat == "other_term":
+        loss = loss + (zn.float() ** 2).mean()
+    if pat == "two_losses":
+        loss = loss + 0.5 * cs.pixel_contrast_loss(zn, target, options=_loss_options(c, r, 1), **kw)
+    return loss
+
+
+def head_case(c, device, cov, worst, desc, calls):
+    """One case of fuzz_projection_head: n_rep replays with inputs and weights changed in place between them, each
+    scored against float64 (_head_bound), the column path against the dense head fed the same gradient, the fallbacks
+    against the dense head bit for bit, and on a device the captured forward + backward of (a) / (b) against eager
+    calls bit for bit.  calls: the wrapper's record of _bn_head_backward_cols calls."""
+    dev = torch.device(device).type == "cuda"
+    g = torch.Generator().manual_seed(c["seed"])
+    init = _head_init(c, g)
+    B, C, H, W = c["B"], c["Cin"], c["H"], c["W"]
+    n_px = B * H * W
+    xdt = torch.bfloat16 if c["act"] == "bf16" else torch.float32
+    zdt = torch.float32 if c["act"] == "fp32" else torch.bfloat16
+    sparse = c["grad"] != "dense"
+    E = _Head(c, init, sparse, device)
+    D = _Head(c, init, False, device) if sparse else None
+    Gh = _Head(c, init, sparse, device) if dev and c["grad"] in ("dense", "cols") else None
+    pix = (int(torch.randint(B, (1,), generator=g)), int(torch.randint(H * W, (1,), generator=g)))
+    n_rep = c["n_rep"]
+    actions = ["inputs"] + list(c["actions"])
+    if c["grad"] in ("cols", "loss") and actions[-1] in ("weights", "control"):
+        actions[-1] = "both"                            # the last replay: every column dead / A = 0
+    bank = None
+    if c["grad"] in ("loss", "fallback") and c["bank"]:
+        bk = make_bank(c["K"], 12, 256, c["seed"] + 7)
+        bank = (bk["segment_queue"].to(device), bk["pixel_queue"].to(device))
+    heads = [h for h in (E, D, Gh) if h is not None]
+    graph = x_s = gzn_s = cols_s = pix_s = zn_g = None
+    lab = None
+    bad = []
+    reached = set()
+    for r in range(n_rep):
+        act = actions[r]
+        where = f"replay {r} ({act}): {desc}"
+        if act in ("inputs", "both"):
+            x_new = _head_x(c, (init["running_mean"], init["running_var"]), g, pix).to(device=device, dtype=xdt)
+            if c["grad"] == "dense":
+                gzn_new = torch.randn(B, 256, H, W, generator=g).to(device=device, dtype=zdt)
+            if c["grad"] == "cols":
+                last = r == n_rep - 1
+                live = 0 if last else int(torch.randint(1, min(c["n_cols"], n_px) + 1, (1,), generator=g))
+                cols_new, pix_new = _head_cols(c, g, live, pix, n_px)
+                cols_new, pix_new = cols_new.to(device), pix_new.to(device)
+            if c["grad"] in ("loss", "fallback"):
+                data = make_contrast_batch(B=B, D=8, h=H, w=W, num_classes=c["K"], img_stride=1,
+                                           block=int(torch.randint(1, 5, (1,), generator=g)), seed=c["seed"] + r)
+                target = data["target"].clone()
+                if c["grad"] == "loss" and r == n_rep - 1:
+                    target.fill_(-1)                            # no class qualifies: A = 0
+                lab = (target.to(device), data["seg"].to(device), bank)
+            if x_s is None:
+                x_s = x_new.clone().requires_grad_(c["x_grad"])
+                gzn_s = gzn_new.clone() if c["grad"] == "dense" else None
+                if c["grad"] == "cols":
+                    cols_s, pix_s = cols_new.clone(), pix_new.clone()
+            else:
+                with torch.no_grad():
+                    x_s.copy_(x_new)
+                    if c["grad"] == "dense":
+                        gzn_s.copy_(gzn_new)
+                    if c["grad"] == "cols":
+                        cols_s.copy_(cols_new)
+                        pix_s.copy_(pix_new)
+        if act in ("weights", "both"):
+            reached.add("weights changed")
+            with torch.no_grad():                               # an optimizer step, the same on every copy
+                for k, p in E.leaves().items():
+                    step = 0.05 * torch.randn(p.shape, generator=g).to(device) * p.detach().abs().mean()
+                    for h in heads:
+                        h.leaves()[k].add_(step)
+        if act == "control":
+            reached.add("control replay")
+        if Gh is not None and graph is None:                    # warm up on a side stream, then capture
+            s = torch.cuda.Stream()
+            s.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(s):
+                for h in (Gh, E):
+                    xw = x_s.detach().clone().requires_grad_(c["x_grad"])
+                    zw = h(xw)
+                    zw.backward(gzn_s if c["grad"] == "dense" else Fn._sink_of(zw).deposit(cols_s, pix_s, zw.shape))
+                    h.zero_grad(xw)
+            torch.cuda.current_stream().wait_stream(s)
+            torch.cuda.synchronize()
+            if D is not None and D.bn is not None:              # the dense twin starts from the warmed-up buffers
+                for k, v in E.buffers().items():
+                    getattr(D.bn, k).copy_(v)
+            Gh.zero_grad(x_s)
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph, capture_error_mode="thread_local"):
+                zn_g = Gh(x_s)
+                zn_g.backward(gzn_s if c["grad"] == "dense" else Fn._sink_of(zn_g).deposit(cols_s, pix_s, zn_g.shape))
+        # the eager call (and the reference, from the state the call starts from)
+        bn0 = None if E.bn is None else (E.bn.training, E.bn.weight.detach().clone(), E.bn.bias.detach().clone(),
+                                          E.bn.running_mean.clone(), E.bn.running_var.clone(), E.bn.eps)
+        nbt0 = None if E.bn is None else int(E.bn.num_batches_tracked.item())
+        x_ref = x_s.detach().to(torch.bfloat16) if c["act"] == "autocast" else x_s.detach()
+        xe = x_s.detach().clone().requires_grad_(c["x_grad"])
+        n_calls = len(calls)
+        zn = E(xe)
+        loss = None
+        if c["grad"] == "dense":
+            gref = gzn_s
+            zn.backward(gzn_s)
+        elif c["grad"] == "cols":
+            zn.backward(Fn._sink_of(zn).deposit(cols_s, pix_s, zn.shape))
+        else:
+            loss = _head_loss(c, zn, lab, r)
+            if c["grad"] == "loss":
+                A = int(Fn.last_workspace(zn.device).plan[_abi.PLAN_A].item())
+                reached.add("A = 0" if A == 0 else ("A = max_samples" if A == c["ms"] else "contrast loss"))
+            loss.backward()
+        _sync(device)
+        took_cols = len(calls) - n_calls
+        want = 1 if c["grad"] in ("cols", "loss") else 0
+        if took_cols != want:
+            bad.append(f"{where}: the column path ran {took_cols} times, expected {want}")
+            break
+        got = E.grads(xe)
+        got["zn"] = zn.detach()
+        if c["grad"] in ("cols", "loss"):
+            cols, cpix = calls[-1]
+            live = cpix[cpix >= 0].long()
+            if live.numel() == 0:
+                reached.add("all-dead deposit")
+            if live.numel() and (int(live.min()) == 0 or int(live.max()) == n_px - 1):
+                reached.add("first / last pixel column")
+            gref = Fn._with_deposits(torch.zeros(zn.shape, dtype=zdt, device=device), [(cols, cpix)], zdt)
+        if c["grad"] == "fallback":
+            gref = torch.zeros(zn.shape, dtype=zdt, device=device)      # the BN buffers only
+        ref, st, y_st = _head_reference(c, x_ref, _Snapshot(E, bn0), gref)
+        if c["grad"] != "fallback":
+            bound = _head_bound(c, x_ref, E.w1, E.b1, bn0, E.w2, E.b2, gref, y_st,
+                                None if st is None else st["kink"], zdt, n_px)
+            bad += _score_head(got, ref, bound, E.absent(c["x_grad"]), worst, where)
+        if E.bn is not None:
+            import test_gpu_projection_bnrelu as TPB
+            for k in ("running_mean", "running_var"):
+                rb = st[k]
+                if (getattr(E.bn, k).double() - rb).abs().max().item() > TPB.STATS_REL * rb.abs().max().item():
+                    bad.append(f"{where}: {k} off the float64 update")
+            if int(E.bn.num_batches_tracked.item()) != nbt0 + int(c["train"]):
+                bad.append(f"{where}: num_batches_tracked {int(E.bn.num_batches_tracked.item())}, expected "
+                           f"{nbt0 + int(c['train'])}")
+        if D is not None:                                       # the dense head, same inputs
+            xd = x_s.detach().clone().requires_grad_(c["x_grad"])
+            zd = D(xd)
+            if c["grad"] == "fallback":
+                ld = _head_loss(c, zd, lab, r)
+                ld.backward()
+            else:
+                if loss is not None:
+                    ld = cs.pixel_contrast_loss(zd.detach(), lab[0], seg=lab[1], options=_loss_options(c, r),
+                                                **(dict(segment_queue=bank[0], pixel_queue=bank[1]) if bank else {}))
+                zd.backward(gref)
+            _sync(device)
+            dg = D.grads(xd)
+            if not _same_bits(zd.detach(), got["zn"]):
+                bad.append(f"{where}: zn differs from the dense head's")
+            if loss is not None and not _same_bits(ld.detach(), loss.detach()):
+                bad.append(f"{where}: loss differs from the dense head's")
+            for k, v in E.buffers().items():
+                if not torch.equal(v, D.buffers()[k]):
+                    bad.append(f"{where}: {k} differs from the dense head's")
+            for k, v in dg.items():
+                if c["grad"] == "fallback":
+                    if not _same_bits(got[k], v):
+                        bad.append(f"{where}: {k} differs from the dense head's ({c['pattern']})")
+                elif k in bound:
+                    d = (got[k].double() - v.double()).abs().reshape(-1)
+                    if not bool((d <= 2 * bound[k].reshape(-1)).all()):
+                        bad.append(f"{where}: {k} of the column path off the dense head's by more than the bound")
+            if c.get("pattern") == "retain_grad" and not _same_bits(zn.grad, zd.grad):
+                bad.append(f"{where}: zn.grad differs from the dense head's")
+        if graph is not None:
+            graph.replay()
+            torch.cuda.synchronize()
+            gg = Gh.grads(x_s)
+            gg["zn"] = zn_g.detach()
+            for k, v in got.items():
+                if v is not None and not _same_bits(gg[k], v):
+                    bad.append(f"{where}: graph replay {k} differs from the eager call")
+        for h in heads:
+            if h is not Gh:
+                h.zero_grad(xe)
+        Fn.clear_workspaces()
+        if bad:
+            break
+    if graph is not None and not bad:
+        for k, v in E.buffers().items():
+            if not torch.equal(v, Gh.buffers()[k]):
+                bad.append(f"after the replays: {k} of the graph differs from the eager sequence: {desc}")
+    if not bad:
+        reached |= {c["level"], c["act"], "train" if c["train"] else "eval"}
+        reached |= {{"dense": "dense gzn", "cols": "column hand-off", "loss": "contrast loss",
+                     "fallback": "fallback"}[c["grad"]]}
+        if c["sync"]:
+            reached.add("SyncBatchNorm")
+        if (c["level"] == "conv1" and not c["b1"]) or not c["b2"]:
+            reached.add("a bias None")
+        if not c["x_grad"]:
+            reached.add("x without grad")
+        if c["grad"] == "cols" and c["n_cols"] in _HEAD_NCOLS:
+            reached.add("n_cols at a tile edge")
+        if C % 64 in (63, 0, 1):
+            reached.add("Cin at a 64 edge")
+        if 255 <= C <= 257:
+            reached.add("Cin 255-257")
+        if H * W == 1:
+            reached.add("HW = 1")
+        if c["adv"]:
+            reached.add({"clamped": "clamped pixel", "dead channel": "dead BN channel",
+                         "large mean": "large-mean channel"}[c["adv"]])
+        for k in reached & set(HEAD_CATEGORIES):
+            cov[k] += 1
+    return bad
+
+
+class _Snapshot:
+    """A head's leaves with its BatchNorm as it was before a call (bn0): what the float64 reference starts from."""
+
+    def __init__(self, h, bn0):
+        import copy
+        self.w1, self.b1, self.w2, self.b2 = h.w1, h.b1, h.w2, h.b2
+        self.bn = None
+        if bn0 is not None:
+            self.bn = copy.deepcopy(h.bn)
+            with torch.no_grad():
+                self.bn.weight.copy_(bn0[1])
+                self.bn.bias.copy_(bn0[2])
+                self.bn.running_mean.copy_(bn0[3])
+                self.bn.running_var.copy_(bn0[4])
+
+
+def fuzz_projection_head(seed: int, n: int, device="cpu", scale: int = 1):
+    """The fused projection head (project_normalize, bn_relu_project_normalize, conv_bn_relu_project_normalize /
+    ProjectionHead) over drawn fusion levels, activation dtypes (autocast included), BatchNorm modes, biases and
+    geometries at the kernels' edges, with a dense gzn, a column hand-off, the real contrast loss or a fallback consumer
+    pattern, and adversarial values (a clamped pixel, a dead BN channel, a large-mean channel).  Each case runs 2-4
+    replays with x, the gradient or the columns, and the weights changed in place between them (head_case).  On a
+    device (a) and (b) are captured as one CUDA graph and replayed for real.  Returns (failures, coverage): how many
+    clean cases reached each of HEAD_CATEGORIES, and coverage["worst"], the largest error / bound ratio per output."""
+    rng = random.Random(seed)
+    return run_head_cases([_draw_head_case(rng, it, scale, device) for it in range(n)], device, f"seed={seed}")
+
+
+def run_head_cases(cases, device="cpu", tag=""):
+    """head_case over `cases` with _bn_head_backward_cols wrapped to record its calls; (failures, coverage)."""
+    import gc
+    bad, cov = [], {k: 0 for k in HEAD_CATEGORIES}
+    cov["worst"] = {}
+    calls = []
+    orig = Fn._bn_head_backward_cols
+
+    def counted(lib, yc, dt, zn, inv, w2, state, cols, col_pix, *a):
+        calls.append((cols.clone(), col_pix.clone()))
+        return orig(lib, yc, dt, zn, inv, w2, state, cols, col_pix, *a)
+    Fn._bn_head_backward_cols = counted
+    try:
+        for it, c in enumerate(cases):
+            desc = "head {} it={} {}".format(tag, it, " ".join(f"{k}={v}" for k, v in c.items()))
+            bad += head_case(c, device, cov, cov["worst"], desc, calls)
+            calls.clear()
+            if torch.device(device).type == "cuda":
+                gc.collect()
+                torch.cuda.empty_cache()
+    finally:
+        Fn._bn_head_backward_cols = orig
+    return bad, cov
+
+
+def edge_cases():
+    """Constructed cases for what a short random draw may miss: the column path at Cin = 300 (k_col_prep's channel loop
+    past 256) with a clamped anchor whose |z| is just under eps, and bf16 fallbacks whose deposits add to another
+    gradient term (each deposit rounded to zn's dtype before the sum, as the loss's dense gradient would be)."""
+    base = dict(adv=None, seed=9, act="fp32", train=True, sync=False, momentum=0.1, b1=False, b2=True, x_grad=True,
+                B=2, Cin=40, H=5, W=4, n_rep=2, actions=["both"])
+    cols = dict(base, level="bn_relu", grad="cols", adv="clamped", b2="tiny", Cin=300, n_cols=65)
+    fb = [dict(base, level="bn_relu", grad="fallback", act="bf16", pattern=p, K=3, precision="fp32", bank=False,
+               ms=12, mv=2) for p in ("other_term", "two_losses")]
+    return [cols] + fb
+
+
+def width_one_case(grad, Cin=64, B=2, H=9):
+    """The constructed case of the fuzzer's finding: a feature map one pixel wide, the gradient a column hand-off or the
+    contrast loss.  The placeholder's last dimension (W = 1) keeps stride 1 under expand(); the column path must run."""
+    c = dict(level="bn_relu", grad=grad, adv=None, seed=5, act="fp32", train=True, sync=False, momentum=0.1, b1=False,
+             b2=True, x_grad=True, B=B, Cin=Cin, H=H, W=1, n_rep=2, actions=["both"])
+    if grad == "cols":
+        c["n_cols"] = 7
+    else:
+        c.update(K=3, precision="fp32", bank=False, ms=6, mv=2)
+    return c

@@ -11,6 +11,8 @@ import test_gpu_parity as G
 
 NGRAPH = 24
 NCRIT = 10
+NHEAD = 10
+HEAD_SEED = 24
 
 
 @pytest.fixture
@@ -113,3 +115,43 @@ def test_criterion_fuzz_regression_two_call_ce_every_pixel_ignored(emu_fused):
     assert c["name"] == "aux_ce" and c["mode"] == "down" and not c["refused"]
     assert emu_fuzz.graphed_criterion_case(c, "cpu", G._check_device_sampling, cov, "regression") == []
     assert cov["CE two-call"] == 1 and cov["all-ignored replay"] == 1, cov
+
+
+def test_fuzz_projection_head(emu):
+    """The fused projection head at every fusion level with the dense, column, loss and fallback backward, inputs and
+    weights changed between replays, scored against float64 with a per-element bound: every category reached."""
+    bad, cov = emu_fuzz.fuzz_projection_head(seed=HEAD_SEED, n=NHEAD)
+    assert bad == []
+    assert all(cov[k] >= 1 for k in emu_fuzz.HEAD_CATEGORIES), cov
+
+
+def test_head_fuzz_detects_a_weight_packed_once(emu, monkeypatch):
+    """Negative control: a head that packs the last conv's weight on its first call and reuses that pack (weights that
+    stop changing between replays, as a pack captured once would) fails the fuzzer on a replay after the first."""
+    from contrastiveseg_b200 import functional as Fn
+    orig, packs = Fn._proj_pack, {}
+
+    def packed_once(lib, x, weight, bias, s):
+        out = orig(lib, x, weight, bias, s)
+        key = (id(weight), weight.data_ptr(), tuple(weight.shape), tuple(x.shape))
+        return (packs.setdefault(key, out[0]),) + out[1:]
+    monkeypatch.setattr(Fn, "_proj_pack", packed_once)
+    bad, _ = emu_fuzz.fuzz_projection_head(seed=HEAD_SEED, n=3)
+    assert len(bad) >= 2, bad
+    assert not any(b.startswith("replay 0 ") for b in bad), bad
+
+
+@pytest.mark.parametrize("grad", ["cols", "loss"])
+def test_head_fuzz_regression_column_path_at_width_one(emu, grad):
+    """The head fuzzer's finding, as a constructed case: a feature map one pixel wide (W = 1).  expand() keeps the
+    stride of a size-1 dimension, so the loss's zero placeholder failed _ColumnSink.is_placeholder's stride check and
+    the head silently took the dense path.  head_case asserts that the column path ran, on every replay."""
+    bad, cov = emu_fuzz.run_head_cases([emu_fuzz.width_one_case(grad)], "cpu")
+    assert bad == [] and cov["column hand-off" if grad == "cols" else "contrast loss"] == 1, (bad, cov)
+
+
+def test_head_fuzz_edge_cases(emu):
+    """Constructed head cases: the column path past 256 channels with a clamped anchor just under eps, and bf16
+    fallbacks whose deposits add to another gradient term."""
+    bad, cov = emu_fuzz.run_head_cases(emu_fuzz.edge_cases(), "cpu", "edge")
+    assert bad == [] and cov["clamped pixel"] == 1 and cov["fallback"] == 2, (bad, cov)

@@ -48,6 +48,7 @@ if __name__ == "__main__":
                                                                         G._check_device_sampling)[0]),
                          ("criterion", lambda s: criterion(s, max(1, n // 4))),
                          ("hook", lambda s: emu_fuzz.fuzz_trainer_hook(s, max(1, n // 2))),
+                         ("head", lambda s: emu_fuzz.fuzz_projection_head(s, max(1, n // 10))[0]),
                          ("wrappers", lambda s: emu_fuzz.fuzz_wrappers(s, n))):
             bad = fn(1000 * r + base)
             total += len(bad)
