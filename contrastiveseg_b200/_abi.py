@@ -167,6 +167,7 @@ SIGNATURES = {
     "pcl_step_fused_select": (c_i32, [C.POINTER(StepDesc), c_vp, c_vp, c_vp]),
     "pcl_step_fused_loss": (c_i32, [C.POINTER(StepDesc), c_vp]),
     "pcl_step_fused_scatter": (c_i32, [C.POINTER(StepDesc), c_vp, c_vp, c_vp, c_vp]),
+    "pcl_step_fused_cols": (c_i32, [C.POINTER(StepDesc), c_vp, c_vp, c_vp, c_vp, c_vp]),
     "pcl_step_fused_fill": (c_i32, [C.POINTER(StepDesc), c_vp]),
     "pcl_fill_zero": (c_i32, [c_vp, c_u64, c_vp]),
 }

@@ -116,9 +116,10 @@ int dense_grad(const pcl_geom* g, const int32_t* plan, const int32_t* anchor_met
                void* grad_embed, int grad_dtype, void* stream, unsigned int* dbg = nullptr,
                unsigned long long* step_counter = nullptr, int32_t* prev_rows = nullptr);
 // The same values as (max_samples, D) fp32 anchor columns: cols[s] and col_pix[s] = b h w + pix for s < A (A read on the
-// device), zeros and -1 beyond.  Bit-identical to what dense_grad stores for an fp32 gradient.
+// device), zeros and -1 beyond.  Bit-identical to what dense_grad stores for an fp32 gradient.  step_counter: advanced
+// (the captured fused step's last kernel).
 int anchor_cols(const pcl_geom* g, const int32_t* plan, const int32_t* anchor_meta, const grad_rows& r, float* cols,
-                int32_t* col_pix, void* stream);
+                int32_t* col_pix, void* stream, unsigned long long* step_counter = nullptr);
 
 // ---- per-device kernel attributes ----------------------------------------------------------------
 // cudaFuncAttributeMaxDynamicSharedMemorySize is a property of (function, device) and SETS the limit (a later call with

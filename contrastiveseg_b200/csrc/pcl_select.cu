@@ -543,14 +543,18 @@ k_zero_scatter(pcl_geom g, const int32_t* __restrict__ plan, const int32_t* __re
 
 // k_cols: the anchor columns of the dense gradient instead of the dense tensor.  Row s < A: cols[s][0..D) = the fp32
 // values the dense writers store at the anchor's pixel (before their rounding to a half type) and col_pix[s] =
-// b h w + pix; rows s >= A: zeros and col_pix -1.  One warp per row (the lane order of da_row for dA sources).
+// b h w + pix; rows s >= A: zeros and col_pix -1, so every row is written on every call.  One warp per row (the lane
+// order of da_row for dA sources).  The fused small-anchor step's column writer (split_cols > 0, in place of
+// k_scatter_reduce) sums only the live partials as that kernel does and advances the step counter of a captured
+// sequence.
 template <typename Src>
 __global__ void __launch_bounds__(256)
 k_cols(pcl_geom g, const int32_t* __restrict__ plan, const int32_t* __restrict__ meta, Src src,
        const float* __restrict__ anchors, const float* __restrict__ inv_norm, int normalize, float* __restrict__ cols,
-       int32_t* __restrict__ col_pix) {
+       int32_t* __restrict__ col_pix, int split_cols, unsigned long long* step_counter) {
   const int lane = threadIdx.x & 31;
   const int s = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (step_counter != nullptr && s == 0 && lane == 0) *step_counter += 1ull;
   const int ms = g.max_samples, D = g.D;
   if (s >= ms) return;
   const int A = min(plan[PCL_PLAN_A], ms);
@@ -564,6 +568,10 @@ k_cols(pcl_geom g, const int32_t* __restrict__ plan, const int32_t* __restrict__
   if constexpr (std::is_same<Src, DaRows>::value) {
     da_row(s, lane, D, src.dA, anchors, inv_norm, normalize, [&](int d, float v) { row[d] = v; });
   } else {
+    if constexpr (std::is_same<Src, SplitRows>::value) {
+      // partial p covers the contrast columns [p * split_cols, (p+1) * split_cols): only the live ones were written
+      if (split_cols > 0) src.splits = min(src.splits, (A + split_cols - 1) / split_cols);
+    }
     const float scale = src.scale();
     for (int d = lane; d < D; d += 32) row[d] = src.at(s, d, D, scale);
   }
@@ -718,7 +726,7 @@ int pcl::dense_grad(const pcl_geom* g, const int32_t* plan, const int32_t* ancho
 }
 
 int pcl::anchor_cols(const pcl_geom* g, const int32_t* plan, const int32_t* anchor_meta, const grad_rows& r, float* cols,
-                     int32_t* col_pix, void* stream) {
+                     int32_t* col_pix, void* stream, unsigned long long* step_counter) {
   if (!g || !plan || !anchor_meta || !cols || !col_pix) return PCL_ERR_ARG;
   const bool partial_rows = r.dpartials != nullptr;
   if (partial_rows ? r.splits < 1 || r.normalize : !r.dA || (r.normalize && (!r.anchors_f32 || !r.inv_norm)))
@@ -729,10 +737,10 @@ int pcl::anchor_cols(const pcl_geom* g, const int32_t* plan, const int32_t* anch
   if (partial_rows)
     k_cols<SplitRows><<<blocks, warps * 32, 0, s>>>(*g, plan, anchor_meta,
                                                     SplitRows{r.dpartials, r.splits, r.a_pad, r.inv_T, r.grad_scale},
-                                                    nullptr, nullptr, 0, cols, col_pix);
+                                                    nullptr, nullptr, 0, cols, col_pix, r.split_cols, step_counter);
   else
     k_cols<DaRows><<<blocks, warps * 32, 0, s>>>(*g, plan, anchor_meta, DaRows{r.dA}, r.anchors_f32, r.inv_norm,
-                                                 r.normalize, cols, col_pix);
+                                                 r.normalize, cols, col_pix, 0, step_counter);
   PCL_LAUNCH_CHECK();
   return PCL_OK;
 }

@@ -210,6 +210,20 @@ extern "C" int pcl_step_fused_scatter(const pcl_step_desc* d, const float* grad_
                          reinterpret_cast<unsigned long long*>(step_counter), prev_rows);
 }
 
+// The fused step's anchor columns in place of the scatter: the same partial sums, no dense gradient
+extern "C" int pcl_step_fused_cols(const pcl_step_desc* d, const float* grad_scale, uint64_t* step_counter, float* cols,
+                                   int32_t* col_pix, void* stream) {
+  if (!pcl_step_fused_supported(d)) return PCL_ERR_UNSUPPORTED;
+  if (!cols || !col_pix) return PCL_ERR_ARG;
+  pcl::grad_rows r = {};
+  pcl::self_fused_splits(d->g.max_samples, &r.a_pad, &r.splits, &r.split_cols);
+  r.dpartials = d->dpartials;
+  r.inv_T = 1.f / d->temperature;
+  r.grad_scale = grad_scale;
+  return pcl::anchor_cols(&d->g, d->plan, d->anchor_meta, r, cols, col_pix, stream,
+                          reinterpret_cast<unsigned long long*>(step_counter));
+}
+
 // zero-fill of the step's dense gradient on the engine's fill kernel (the caller picks the stream: a parallel branch)
 extern "C" int pcl_step_fused_fill(const pcl_step_desc* d, void* stream) {
   if (!d || !d->grad_embed || !pcl::dtype_ok(d->embed_dtype)) return PCL_ERR_ARG;

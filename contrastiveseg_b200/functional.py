@@ -328,6 +328,28 @@ def _with_deposits(gzn: torch.Tensor, deposits, dtype) -> torch.Tensor:
     return g
 
 
+def cols_to_dense(cols: torch.Tensor, col_pix: torch.Tensor, shape, dtype: torch.dtype) -> torch.Tensor:
+    """The dense (B, D, h, w) gradient of ``dtype`` that holds the anchor columns (cols (n, D) fp32, col_pix[s] =
+    b*h*w + pix or < 0 for an unused row) and +0 elsewhere: each column rounded once to ``dtype`` and stored, not
+    added, so the result equals the loss step's dense gradient to the bit (a -0 entry included).  No host
+    synchronisation: every row is stored, an unused row into D scratch elements past the end of the tensor (its values
+    are zero, so the rows that share them store the same bits)."""
+    B, D = shape[0], shape[1]
+    n = 1
+    for e in shape:
+        n *= e
+    HW = n // (B * D)
+    flat = torch.zeros(n + D, dtype=dtype, device=cols.device)
+    q = col_pix.long()
+    live = q >= 0
+    q = q.clamp(min=0)
+    base = torch.where(live, (q // HW) * (D * HW) + q % HW, torch.full_like(q, n))        # (rows,)
+    step = torch.where(live, torch.full_like(q, HW), torch.ones_like(q))                  # channel stride
+    idx = base[:, None] + step[:, None] * torch.arange(D, device=cols.device)[None, :]    # (rows, D)
+    flat.index_put_((idx.reshape(-1),), cols.to(dtype).reshape(-1))
+    return flat[:n].view(shape)
+
+
 class _PixelContrastFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, embed, labels, seg, predict, segq, pixq, shadow, opts: ContrastOptions):
@@ -678,14 +700,32 @@ def _conv1x1_f32(weight, bias, rows, cols, dev):
 
 def _proj_pack(lib, x, weight, bias, s):
     """For the fused last conv on x (B, Cin, H, W): wpack (pcl_proj_pack), the fp32 (256, Cin) weight, the fp32 bias or
-    None, zn and inv_norm."""
+    None and inv_norm."""
     B, Cin, HW, dev = x.shape[0], x.shape[1], x[0, 0].numel(), x.device
     w, bc = _conv1x1_f32(weight, bias, PROJ_DIM, Cin, dev)
     wpack = torch.empty(lib.pcl_proj_workspace_bytes(B, Cin, HW, 0), dtype=torch.uint8, device=dev)
-    zn = torch.empty((B, PROJ_DIM) + tuple(x.shape[2:]), dtype=x.dtype, device=dev)
     inv = torch.empty(B * HW, dtype=torch.float32, device=dev)
     _abi.check(lib.pcl_proj_pack(w.data_ptr(), Cin, wpack.data_ptr(), s), "pcl_proj_pack")
-    return wpack, w, bc, zn, inv
+    return wpack, w, bc, inv
+
+
+def _zn_buffer(x: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """zn (B, 256, H, W) of x's dtype for the fused last conv on x: ``out`` when given (checked by _check_zn_out)."""
+    if out is not None:
+        return out
+    return torch.empty((x.shape[0], PROJ_DIM) + tuple(x.shape[2:]), dtype=x.dtype, device=x.device)
+
+
+def _check_zn_out(name: str, x: torch.Tensor, out: Optional[torch.Tensor]) -> None:
+    """out= of the fused BN heads: a contiguous (B, 256, H, W) tensor of zn's dtype (x's) on x's device that nobody
+    differentiates through, e.g. the static embed of a captured contrast step (zn written in place, no copy)."""
+    if out is None:
+        return
+    shape = (x.shape[0], PROJ_DIM) + tuple(x.shape[2:])
+    if (tuple(out.shape) != shape or out.dtype != x.dtype or out.device != x.device or not out.is_contiguous()
+            or out.requires_grad):
+        raise _abi.PclError(f"{name}: out must be a contiguous {x.dtype} tensor of shape {shape} on {x.device} that "
+                            f"does not require grad, got {out.dtype} {tuple(out.shape)} on {out.device}")
 
 
 def _proj_grad_buffers(x, zn, gzn, scratch_bytes, has_bias):
@@ -709,7 +749,8 @@ class _ProjNormFn(torch.autograd.Function):
         xc = x.contiguous()
         with _on_device(dev):
             s = _stream_ptr(dev)
-            wpack, _, bc, zn, inv = _proj_pack(lib, xc, weight, bias, s)
+            wpack, _, bc, inv = _proj_pack(lib, xc, weight, bias, s)
+            zn = _zn_buffer(xc)
             _abi.check(lib.pcl_proj_fwd_dt(xc.data_ptr(), dt, wpack.data_ptr(), _abi.ptr(bc), B, Cin, HW, zn.data_ptr(),
                                            inv.data_ptr(), s), "pcl_proj_fwd_dt")
         ctx.save_for_backward(xc, zn, inv, wpack)
@@ -771,10 +812,10 @@ def _check_bn_input(what, name, x, gamma, training) -> None:
         raise ValueError(f"Expected more than 1 value per channel when training, got input size {tuple(x.shape)}")
 
 
-def _bn_head_forward(lib, yc, dt, bn, gamma, beta, weight, bias, sums, group, s):
+def _bn_head_forward(lib, yc, dt, bn, gamma, beta, weight, bias, sums, group, s, out=None):
     """From conv1's output y on: (training) the all-reduce of the statistics ``sums`` for a multi-rank SyncBatchNorm and
     the counter, the BN state (batch or running statistics, running buffers updated), the last conv's packed weight
-    and the fused GEMM.  Returns zn, inv_norm, wpack, the fp32 weight, bn_state."""
+    and the fused GEMM.  Returns zn (``out`` when given), inv_norm, wpack, the fp32 weight, bn_state."""
     B, Cin, HW = yc.shape[0], yc.shape[1], yc[0, 0].numel()
     g32, b32 = gamma.detach().contiguous(), beta.detach().contiguous()
     state = torch.empty(lib.pcl_proj_bn_workspace_bytes(B, Cin, HW, 0), dtype=torch.uint8, device=yc.device)
@@ -786,7 +827,8 @@ def _bn_head_forward(lib, yc, dt, bn, gamma, beta, weight, bias, sums, group, s)
     _abi.check(lib.pcl_proj_bn_finalize(_abi.ptr(sums), g32.data_ptr(), b32.data_ptr(), bn.running_mean.data_ptr(),
                                         bn.running_var.data_ptr(), Cin, bn.eps, bn.momentum, int(training),
                                         state.data_ptr(), s), "pcl_proj_bn_finalize")
-    wpack, w, bc, zn, inv = _proj_pack(lib, yc, weight, bias, s)
+    wpack, w, bc, inv = _proj_pack(lib, yc, weight, bias, s)
+    zn = _zn_buffer(yc, out)
     _abi.check(lib.pcl_proj_bn_fwd_dt(yc.data_ptr(), dt, state.data_ptr(), wpack.data_ptr(), _abi.ptr(bc), B, Cin, HW,
                                       zn.data_ptr(), inv.data_ptr(), s), "pcl_proj_bn_fwd_dt")
     return zn, inv, wpack, w, state
@@ -854,11 +896,12 @@ def _sparse_output(zn: torch.Tensor, sparse_grad: bool) -> torch.Tensor:
 
 class _BnProjNormFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, y, gamma, beta, weight, bias, bn, sparse_grad):
+    def forward(ctx, y, gamma, beta, weight, bias, bn, sparse_grad, out):
         lib = _abi.load()
         _require_cuda(y, "y")
         dt = proj_dtype_code(y.dtype, "bn_relu_project_normalize")
         B, Cin, HW = _proj_dims(y, weight)
+        _check_zn_out("bn_relu_project_normalize", y, out)
         training = bn.training
         _check_bn_input("bn_relu_project_normalize", "y", y, gamma, training)
         group = _bn_sync_group(bn)
@@ -871,7 +914,10 @@ class _BnProjNormFn(torch.autograd.Function):
                 sums = torch.empty(2 * Cin + 1, dtype=torch.float64, device=dev)
                 _abi.check(lib.pcl_proj_bn_stats_dt(yc.data_ptr(), dt, B, Cin, HW, sums.data_ptr(), s),
                            "pcl_proj_bn_stats_dt")
-            zn, inv, wpack, w2, state = _bn_head_forward(lib, yc, dt, bn, gamma, beta, weight, bias, sums, group, s)
+            zn, inv, wpack, w2, state = _bn_head_forward(lib, yc, dt, bn, gamma, beta, weight, bias, sums, group, s,
+                                                         out)
+        if out is not None:                  # a fresh alias: autograd's history goes on it, not on the caller's buffer
+            zn = out.view_as(out)
         ctx.save_for_backward(yc, zn, inv, wpack, w2 if sparse_grad else None, state)
         ctx.meta = (tuple(weight.shape), bias is not None, dt, training, group, gamma.dtype)
         ctx.sink = None
@@ -887,11 +933,12 @@ class _BnProjNormFn(torch.autograd.Function):
         with _on_device(dev):
             gy, ggamma, gbeta, gw, gb = _bn_head_backward(lib, yc, dt, zn, inv, wpack, w2, state, gzn, has_bias,
                                                           training, group, ctx.sink, _stream_ptr(dev))
-        return gy, ggamma.to(gdtype), gbeta.to(gdtype), gw.view(wshape), gb, None, None
+        return gy, ggamma.to(gdtype), gbeta.to(gdtype), gw.view(wshape), gb, None, None, None
 
 
 def bn_relu_project_normalize(y: torch.Tensor, bn: torch.nn.Module, weight: torch.Tensor,
-                              bias: Optional[torch.Tensor] = None, *, sparse_grad: bool = False) -> torch.Tensor:
+                              bias: Optional[torch.Tensor] = None, *, sparse_grad: bool = False,
+                              out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """F.normalize(F.conv2d(relu(bn(y)), weight, bias), p=2, dim=1): the projection head from the output y of its
     first conv to zn, with bn a BatchNorm2d or SyncBatchNorm (affine, tracking running stats, numeric momentum).  In
     training mode the batch statistics (fp64 sums; over all ranks of a SyncBatchNorm's process group, one all_reduce
@@ -901,18 +948,22 @@ def bn_relu_project_normalize(y: torch.Tensor, bn: torch.nn.Module, weight: torc
     project_normalize; autograd reaches y, bn.weight, bn.bias, weight and bias (bn's gradients rank-local).
     sparse_grad=True: an engine contrast loss whose embed is the returned zn hands this node its anchor columns instead
     of a dense gradient, and zn itself receives a zero placeholder (INTEGRATION §1); the backward then runs over those
-    columns only."""
+    columns only.
+    out: zn is written into this (B, 256, H, W) tensor of y's dtype (contiguous, not requiring grad) and the result
+    shares its storage, e.g. the static embed of a GraphedContrastStep, whose apply() and column hand-off accept it."""
     _check_bn(bn)
-    return _sparse_output(_BnProjNormFn.apply(y, bn.weight, bn.bias, weight, bias, bn, bool(sparse_grad)), sparse_grad)
+    return _sparse_output(_BnProjNormFn.apply(y, bn.weight, bn.bias, weight, bias, bn, bool(sparse_grad), out),
+                          sparse_grad)
 
 
 class _ConvBnProjNormFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, w1, b1, gamma, beta, w2, b2, bn, sparse_grad):
+    def forward(ctx, x, w1, b1, gamma, beta, w2, b2, bn, sparse_grad, out):
         lib = _abi.load()
         _require_cuda(x, "x")
         dt = proj_dtype_code(x.dtype, "conv_bn_relu_project_normalize")
         B, C, HW = _proj_dims(x, w2)
+        _check_zn_out("conv_bn_relu_project_normalize", x, out)
         if w1.shape[0] != C or w1.numel() != C * C:
             raise _abi.PclError(f"conv_bn_relu_project_normalize: w1 must be ({C}, {C}, 1, 1), got {tuple(w1.shape)}")
         if b1 is not None and b1.numel() != C:
@@ -935,7 +986,9 @@ class _ConvBnProjNormFn(torch.autograd.Function):
             _abi.check(lib.pcl_proj_conv1_fwd_dt(xc.data_ptr(), dt, pack.data_ptr(), _abi.ptr(bc), B, C, HW,
                                                  y.data_ptr(), _abi.ptr(sums), _abi.ptr(scratch), s),
                        "pcl_proj_conv1_fwd_dt")
-            zn, inv, wpack, w2f, state = _bn_head_forward(lib, y, dt, bn, gamma, beta, w2, b2, sums, group, s)
+            zn, inv, wpack, w2f, state = _bn_head_forward(lib, y, dt, bn, gamma, beta, w2, b2, sums, group, s, out)
+        if out is not None:                  # a fresh alias: autograd's history goes on it, not on the caller's buffer
+            zn = out.view_as(out)
         ctx.save_for_backward(xc, y, zn, inv, pack, wpack, w2f if sparse_grad else None, state)
         ctx.sink = None
         ctx.meta = (tuple(w1.shape), b1 is not None, tuple(w2.shape), b2 is not None, dt, training, group, gamma.dtype)
@@ -960,12 +1013,13 @@ class _ConvBnProjNormFn(torch.autograd.Function):
             _abi.check(lib.pcl_proj_conv1_bwd_dt(xc.data_ptr(), dt, gy.data_ptr(), pack.data_ptr(), B, C, HW,
                                                  scratch.data_ptr(), _abi.ptr(gx), gw1.data_ptr(), _abi.ptr(gb1), s),
                        "pcl_proj_conv1_bwd_dt")
-        return (gx, gw1.view(w1shape), gb1, ggamma.to(gdtype), gbeta.to(gdtype), gw2.view(w2shape), gb2, None, None)
+        return (gx, gw1.view(w1shape), gb1, ggamma.to(gdtype), gbeta.to(gdtype), gw2.view(w2shape), gb2, None, None,
+                None)
 
 
 def conv_bn_relu_project_normalize(x: torch.Tensor, w1: torch.Tensor, b1: Optional[torch.Tensor], bn: torch.nn.Module,
                                    w2: torch.Tensor, b2: Optional[torch.Tensor] = None, *,
-                                   sparse_grad: bool = False) -> torch.Tensor:
+                                   sparse_grad: bool = False, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """F.normalize(F.conv2d(relu(bn(F.conv2d(x, w1, b1))), w2, b2), p=2, dim=1): the whole ``convmlp`` projection head
     on the engine.  The first 1x1 convolution (w1 (C, C, 1, 1), b1 (C) or None) is a bf16 wgmma GEMM whose epilogue
     also sums the BatchNorm statistics of its output y; y then goes through bn_relu_project_normalize's kernels (same
@@ -973,9 +1027,10 @@ def conv_bn_relu_project_normalize(x: torch.Tensor, w1: torch.Tensor, b1: Option
     reduced over its process group, running statistics in eval).  x (B, C, H, W) fp32 or bf16 CUDA decides y's and
     zn's dtype (fp32 x is rounded to the bf16 GEMM operand).  autograd reaches x, w1, b1, bn.weight, bn.bias, w2 and b2
     (bn's gradients rank-local); x's gradient is skipped when x needs none.  No cuDNN call: forward and backward are
-    capturable and bit-reproducible run to run.  sparse_grad as for bn_relu_project_normalize."""
+    capturable and bit-reproducible run to run.  sparse_grad and out as for bn_relu_project_normalize (out has x's
+    dtype)."""
     _check_bn(bn)
-    return _sparse_output(_ConvBnProjNormFn.apply(x, w1, b1, bn.weight, bn.bias, w2, b2, bn, bool(sparse_grad)),
+    return _sparse_output(_ConvBnProjNormFn.apply(x, w1, b1, bn.weight, bn.bias, w2, b2, bn, bool(sparse_grad), out),
                           sparse_grad)
 
 

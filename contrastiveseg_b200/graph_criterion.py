@@ -19,7 +19,7 @@ import torch
 
 from . import _abi
 from . import functional as _fn
-from .graph_step import GraphedContrastStep, _canonical, _canonical_float
+from .graph_step import GraphedContrastStep, _canonical, _canonical_float, _cols_backward, _keep_cols
 from .loss import ContrastAuxCELoss, ContrastCELoss
 
 
@@ -94,6 +94,8 @@ class GraphedContrastCriterion:
 
     >>> gc = GraphedContrastCriterion(crit, preds, target, grad_scale=1.0)
     >>> loss, grads = gc.replay()       # grads: {'seg', 'embed'[, 'seg_aux']}, static buffers, times grad_scale
+    >>> gc = GraphedContrastCriterion(crit, preds, target, embed_grad="cols")
+    >>> loss, grads = gc.replay()       # grads['embed'] = (cols, col_pix): the anchor columns (GraphedContrastStep)
 
     ``preds`` holds the tensors the graph reads in place on every replay (refill them, do not replace them): 'seg',
     'embed', and 'seg_aux' (ContrastAuxCELoss) or 'segment_queue' / 'pixel_queue' [/ 'bank_shadow']
@@ -101,10 +103,13 @@ class GraphedContrastCriterion:
     phase is captured: during the warm-up epochs, call the eager criterion.  Raises PclError, before anything is
     captured or written, for a criterion whose seg loss runs partly in torch (contrast.fused_seg_ce off, a CE the kernels do not
     fuse, a custom seg_criterion), rng other than 'device', tensors that are not contiguous or of the wrong dtype, and a
-    MemContrastCELoss without queues."""
+    MemContrastCELoss without queues.  embed_grad="cols": the embedding's gradient as the contrast step's anchor
+    columns (GraphedContrastStep(grad="cols")): no dense embedding gradient and no fill in the graph, and apply() hands
+    the columns to a sparse_grad projection head; the seg heads' gradients stay dense."""
 
     def __init__(self, crit: ContrastCELoss, preds: Dict[str, torch.Tensor], target: torch.Tensor,
-                 grad_scale: float = 1.0, enqueue: Optional[dict] = None, capture: bool = True):
+                 grad_scale: float = 1.0, enqueue: Optional[dict] = None, capture: bool = True,
+                 embed_grad: str = "dense"):
         if not isinstance(crit, ContrastCELoss):
             raise _abi.PclError("crit must be a ContrastCELoss, ContrastAuxCELoss or MemContrastCELoss")
         cc = crit.contrast_criterion
@@ -149,7 +154,8 @@ class GraphedContrastCriterion:
         self.step = GraphedContrastStep(embed, target, seg=xs["seg"], segment_queue=segq, pixel_queue=pixq,
                                         bank_shadow=preds.get("bank_shadow"), options=opts,
                                         grad_scale=float(grad_scale) * self.loss_weight, capture=False,
-                                        enqueue=enqueue, prologue=self._seg_half, epilogue=self._total)
+                                        enqueue=enqueue, prologue=self._seg_half, epilogue=self._total,
+                                        grad=embed_grad)
         if capture:                            # the hooks read self.step: capture once it is set
             self.step._capture(2)
 
@@ -185,14 +191,16 @@ class GraphedContrastCriterion:
         self.step.set_grad_scale(float(value) * self.loss_weight)
 
     def replay(self) -> Tuple[torch.Tensor, Dict[str, torch.Tensor]]:
-        """One criterion step on the current stream: (loss, grads), static buffers overwritten by the next replay."""
+        """One criterion step on the current stream: (loss, grads), static buffers overwritten by the next replay
+        (grads['embed'] = (cols, col_pix) with embed_grad="cols")."""
         self.step.replay()
-        return self.loss, dict(self.grads, embed=self.step.grad)
+        return self.loss, dict(self.grads, embed=self.step.grad_out)
 
     def apply(self, preds: Dict[str, torch.Tensor]) -> torch.Tensor:
         """Autograd hand-off: replays the graph and returns the loss connected to preds' heads and embedding (the
         tensors the graph was captured on); its backward hands them the replay's gradients.  Valid when backward starts
-        from gradient 1 (fold weights into grad_scale), as GraphedContrastStep.apply."""
+        from gradient 1 (fold weights into grad_scale), as GraphedContrastStep.apply.  embed_grad="cols": the embedding
+        receives its gradient as GraphedContrastStep.apply() gives it in column mode."""
         ins = [preds[k] for k in self.heads] + [preds["embed"]]
         for k, t in zip(self.heads + ["embed"], ins):
             mine = self.step.embed if k == "embed" else self.xs[k]
@@ -206,6 +214,8 @@ class _GraphedCriterionFn(torch.autograd.Function):
     def forward(ctx, gc: GraphedContrastCriterion, *ins):
         loss, _ = gc.replay()
         ctx.gc = gc
+        if gc.step.cols is not None:
+            _keep_cols(ctx, gc.step, ins[-1])
         return loss.view(())
 
     @staticmethod
@@ -214,4 +224,6 @@ class _GraphedCriterionFn(torch.autograd.Function):
         torch._assert_async((grad_out == 1).all(),
                             "GraphedContrastCriterion.apply(): upstream gradient != 1; fold the factor into grad_scale")
         gc = ctx.gc
-        return (None,) + tuple(gc.grads[k] for k in gc.heads) + (gc.step.grad,)
+        step = gc.step
+        g_embed = step.grad if step.cols is None else _cols_backward(ctx, step.embed.shape, step.embed.dtype)
+        return (None,) + tuple(gc.grads[k] for k in gc.heads) + (g_embed,)

@@ -17,6 +17,13 @@ selection and sweep kernels; the backward then scatters only the sampled columns
 * the upstream gradient is a device scalar (``grad_scale``, default 1) folded into the dense gradient by the
   backward kernels, not an autograd input: use it for the loss weight (``contrast.loss_weight``).
 
+Column mode (``grad="cols"``): the step writes no dense gradient at all.  The loss reads embed at no more than
+max_samples pixels, so its gradient is those anchor columns and zero elsewhere; the backward writes them as
+``cols`` (max_samples, D) fp32 and ``col_pix`` (max_samples,) int32 (b*h*w + pixel, -1 for a row the replay did not use),
+every row on every replay.  No dense buffer and no zero-fill branch exist (268 MB at the Cityscapes shape).  ``apply()``
+hands the columns to a ``sparse_grad`` projection head (INTEGRATION §1), or builds the dense gradient from them for any
+other consumer.
+
 The reference RNG stream (``rng='torch_cpu'`` / injected permutations) needs a host round trip and is not capturable.
 
 Memory-bank steps (``enqueue=``): the trainer's order loss -> enqueue -> backward (trainer_contrastive.py:241-255) is part
@@ -64,7 +71,10 @@ class GraphedContrastStep:
 
     >>> step = GraphedContrastStep(embed, labels, seg=seg, options=opts, grad_scale=loss_weight)
     >>> loss, grad = step.replay()          # 0-dim loss and (B,D,h,w) gradient, both static buffers
+    >>> step = GraphedContrastStep(zn_buf, labels, seg=seg, options=opts, grad="cols")
+    >>> loss, (cols, col_pix) = step.replay()    # anchor columns instead of the dense gradient
     """
+    cols = col_pix = None                  # column mode's static buffers (dense mode: none)
 
     def __init__(self, embed: torch.Tensor, labels: torch.Tensor, *, seg: Optional[torch.Tensor] = None,
                  predict: Optional[torch.Tensor] = None, segment_queue: Optional[torch.Tensor] = None,
@@ -72,13 +82,20 @@ class GraphedContrastStep:
                  options: Optional[ContrastOptions] = None, grad_scale: float = 1.0, capture: bool = True,
                  warmup: int = 2, overlap_zero_fill: bool = True, enqueue: Optional[dict] = None,
                  fused: Optional[bool] = None, sparse_reset: bool = False,
-                 prologue: Optional[Callable[[int], None]] = None, epilogue: Optional[Callable[[int], None]] = None):
+                 prologue: Optional[Callable[[int], None]] = None, epilogue: Optional[Callable[[int], None]] = None,
+                 grad: str = "dense"):
         """embed and seg may be fp32, bf16 or fp16 (each independently); ``grad`` has embed's dtype.
         enqueue (bank steps): dict(bank=MemoryBank, keys=(B,D,h,w) fp32/bf16/fp16 [default: embed], labels=(B,Himg,Wimg) int64
         [default: labels], network_stride=int, pixel_update_freq=int, seed=int, group=process group or None).
         prologue / epilogue: work of the caller launched on the step's stream (its handle is the argument) before the
         step's first kernel and after its last, captured into the first and the last graph (GraphedContrastCriterion's
-        seg half and total loss)."""
+        seg half and total loss).
+        grad: "dense" (the (B, D, h, w) gradient) or "cols" (the anchor columns, see the module docstring; refuses
+        sparse_reset, which only manages a dense buffer)."""
+        if grad not in ("dense", "cols"):
+            raise _abi.PclError(f"grad must be 'dense' or 'cols', got {grad!r}")
+        if grad == "cols" and sparse_reset:
+            raise _abi.PclError("sparse_reset=True clears a dense gradient buffer: grad='cols' has none")
         self.lib = _abi.load()
         self.prologue, self.epilogue = prologue, epilogue
         opts = options or ContrastOptions()
@@ -114,7 +131,12 @@ class GraphedContrastStep:
         self.ws = ContrastWorkspace(device, geom, mode, bank_K, M0, M1)        # owned by this object, never shared
         self.device = device
         self.loss = torch.zeros((), dtype=torch.float32, device=device)
-        self.grad = torch.empty_like(self.embed)
+        self.grad = self.cols = self.col_pix = None
+        if grad == "dense":
+            self.grad = torch.empty_like(self.embed)
+        else:
+            self.cols = torch.zeros((opts.max_samples, D), dtype=torch.float32, device=device)
+            self.col_pix = torch.full((opts.max_samples,), -1, dtype=torch.int32, device=device)
         self.counter = torch.zeros(1, dtype=torch.int64, device=device)         # replay index, lives on the device
         self.scale = torch.full((1,), float(grad_scale), dtype=torch.float32, device=device)
         d = self.ws.desc
@@ -144,7 +166,7 @@ class GraphedContrastStep:
         elif opts.precision != "fp32":
             raise _abi.PclError(f"unknown precision {opts.precision!r}")
         d.seed = int(opts.seed) & 0xFFFFFFFFFFFFFFFF          # base seed; the per-replay part is the device counter
-        d.loss, d.grad_embed = self.loss.data_ptr(), self.grad.data_ptr()
+        d.loss, d.grad_embed = self.loss.data_ptr(), _abi.ptr(self.grad)
         # Small-anchor shape (no bank, tensor path, D = 256, max_samples <= 1024: BASELINE configs[1]): four launches
         # instead of eleven — scan+plan, selection, ONE kernel for the InfoNCE forward and backward (logits stay in tensor
         # memory), scatter — with the engine's own zero-fill of the dense gradient on a parallel branch.
@@ -173,7 +195,7 @@ class GraphedContrastStep:
         # the step computes: run it on a second stream from the start of the step, behind the latency-bound selection
         # and sweep kernels, and let the backward scatter only the sampled columns (pcl_step_backward_prezeroed).  Not for
         # top-k steps: their backward writes the dense gradient itself (zero-fill + scatter).
-        self.overlap_zero_fill = bool(overlap_zero_fill) and not opts.topk_negatives
+        self.overlap_zero_fill = bool(overlap_zero_fill) and not opts.topk_negatives and self.cols is None
         self.side = None
         if capture:
             self._capture(max(1, int(warmup)))
@@ -270,11 +292,12 @@ class GraphedContrastStep:
                        "pcl_step_fused_select")
             # full-fill mode: the fill forks AFTER scan and selection — next to it their DRAM reads slow down (measured
             # in-graph on H100: scan 24 -> 91 us, selection 15 -> 22 us; step 0.164 -> 0.179 ms), only the L2-resident
-            # InfoNCE kernel hides behind it
-            if not self.sparse_reset:
+            # InfoNCE kernel hides behind it.  Column mode: nothing to fill.
+            fill = not self.sparse_reset and self.cols is None
+            if fill:
                 self._fork_zero_fill()
             _abi.check(lib.pcl_step_fused_loss(C.byref(d), stream), "pcl_step_fused_loss")
-            if not self.sparse_reset:
+            if fill:
                 self._join_zero_fill()
             return
         side = self.overlap_zero_fill or self.enq is not None
@@ -287,13 +310,22 @@ class GraphedContrastStep:
             self._join_zero_fill()
 
     def _enqueue_b(self, stream: int) -> None:
-        """Second half: backward -> dense gradient -> (after the sweep that re-reads the bank) the bank write."""
+        """Second half: backward -> dense gradient or anchor columns -> (after the sweep that re-reads the bank) the bank
+        write."""
         lib, d = self.lib, self.ws.desc
         if self.fused:
-            _abi.check(lib.pcl_step_fused_scatter(C.byref(d), self.scale.data_ptr(), self.counter.data_ptr(),
-                                                  _abi.ptr(self.prev_rows), stream), "pcl_step_fused_scatter")
+            if self.cols is not None:
+                _abi.check(lib.pcl_step_fused_cols(C.byref(d), self.scale.data_ptr(), self.counter.data_ptr(),
+                                                   self.cols.data_ptr(), self.col_pix.data_ptr(), stream),
+                           "pcl_step_fused_cols")
+            else:
+                _abi.check(lib.pcl_step_fused_scatter(C.byref(d), self.scale.data_ptr(), self.counter.data_ptr(),
+                                                      _abi.ptr(self.prev_rows), stream), "pcl_step_fused_scatter")
             return
-        if self.overlap_zero_fill:
+        if self.cols is not None:
+            _abi.check(lib.pcl_step_backward_cols(C.byref(d), self.scale.data_ptr(), self.cols.data_ptr(),
+                                                  self.col_pix.data_ptr(), stream), "pcl_step_backward_cols")
+        elif self.overlap_zero_fill:
             _abi.check(lib.pcl_step_backward_prezeroed(C.byref(d), self.scale.data_ptr(), stream),
                        "pcl_step_backward_prezeroed")
         else:
@@ -385,9 +417,22 @@ class GraphedContrastStep:
     def set_grad_scale(self, value: float) -> None:
         self.scale.fill_(float(value))
 
-    def replay(self) -> Tuple[torch.Tensor, torch.Tensor]:
+    @property
+    def grad_out(self):
+        """What replay() hands out beside the loss: the dense gradient, or (cols, col_pix) in column mode."""
+        return self.grad if self.cols is None else (self.cols, self.col_pix)
+
+    def dense_grad(self) -> torch.Tensor:
+        """The dense gradient of the last replay: the static buffer, or (column mode) a new tensor built from the
+        columns, equal to the dense mode's gradient to the bit."""
+        if self.cols is None:
+            return self.grad
+        return _fn.cols_to_dense(self.cols, self.col_pix, self.embed.shape, self.embed.dtype)
+
+    def replay(self):
         """Run one step on the current stream.  Returns (loss, grad_embed): static buffers, overwritten by the next
-        replay; grad_embed = grad_scale * d loss / d embed."""
+        replay; grad_embed = grad_scale * d loss / d embed.  Column mode: (loss, (cols, col_pix)), the anchor columns
+        of grad_scale * d loss / d embed."""
         if self.graph is not None:
             self.graph.replay()
             if self.graph_c is not None:
@@ -407,25 +452,53 @@ class GraphedContrastStep:
             with _fn._on_device(self.device):
                 self._enqueue(_fn._stream_ptr(self.device))
         self.replays += 1
-        return self.loss, self.grad
+        return self.loss, self.grad_out
 
     def apply(self, embed: torch.Tensor) -> torch.Tensor:
         """Autograd hand-off: replays the graph and returns the loss connected to ``embed`` (which must be the tensor
         the graph was captured on); its backward returns the pre-computed static gradient.  Valid when the returned
         loss enters the total loss with coefficient 1 and ``backward`` starts from gradient 1 (fold weights into
         ``grad_scale``): the upstream gradient is NOT multiplied in (that would cost another pass over the dense
-        gradient)."""
+        gradient).
+        Column mode: when ``embed`` is the output of a sparse_grad projection head (e.g. written into the step's embed
+        with ``out=``) and nobody reads its own gradient, the backward hands the head the replay's anchor columns and
+        embed receives a zero placeholder; otherwise the dense gradient is built from the columns (dense_grad()).  The
+        columns are copied (max_samples x D fp32) when the replay runs, so the backward sees this replay's columns even
+        if the step is replayed again before it."""
         if embed.data_ptr() != self.embed.data_ptr():
             raise _abi.PclError("apply() must receive the tensor the step was captured on")
         return _GraphedFn.apply(embed, self)
 
 
+def _cols_backward(ctx, shape, dtype):
+    """The embed gradient of an apply() in column mode, from the columns kept at its forward (ctx.cols): the sink's
+    placeholder, or the dense gradient built from the columns."""
+    if ctx.cols is None:
+        raise _abi.PclError("apply() in column mode: backward ran twice on the same graph (retain_graph=True is not "
+                            "supported: the columns are handed over once); call apply() again")
+    cols, col_pix = ctx.cols
+    ctx.cols = None
+    sink = ctx.sink if ctx.sink is not None and ctx.sink.accepts() else None
+    if sink is not None:
+        return sink.deposit(cols, col_pix, shape)
+    return _fn.cols_to_dense(cols, col_pix, shape, dtype)
+
+
+def _keep_cols(ctx, step: GraphedContrastStep, embed: torch.Tensor) -> None:
+    """Column mode, at apply()'s forward: the head's sink (if embed is a sparse_grad head's zn) and a copy of the
+    replay's columns for the backward."""
+    ctx.sink = _fn._sink_of(embed)
+    ctx.cols = (step.cols.clone(), step.col_pix.clone())
+
+
 class _GraphedFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, embed, step: GraphedContrastStep):
-        loss, _ = step.replay()
+        step.replay()
         ctx.step = step
-        return loss.view(())
+        if step.cols is not None:
+            _keep_cols(ctx, step, embed)
+        return step.loss.view(())
 
     @staticmethod
     @torch.autograd.function.once_differentiable
@@ -434,4 +507,7 @@ class _GraphedFn(torch.autograd.Function):
         # AMP loss scaling) would be silently dropped -> asynchronous device-side assertion (no host sync, one tiny kernel)
         torch._assert_async((grad_out == 1).all(),
                             "GraphedContrastStep.apply(): upstream gradient != 1; fold the factor into grad_scale")
-        return ctx.step.grad, None
+        step = ctx.step
+        if step.cols is not None:
+            return _cols_backward(ctx, step.embed.shape, step.embed.dtype), None
+        return step.grad, None

@@ -70,17 +70,21 @@ class ProjectionHead(nn.Module):
         self.fuse_conv1 = fuse_conv1
         self.sparse_grad = sparse_grad
 
-    def forward(self, x):
+    def forward(self, x, out=None):
+        """out (fuse_bn_relu heads): a (B, proj_dim, H, W) tensor of zn's dtype that zn is written into, e.g. the static
+        embed of a GraphedContrastStep (bn_relu_project_normalize)."""
+        if out is not None and not self.fuse_bn_relu:
+            raise PclError("ProjectionHead.forward(out=...) needs fuse_bn_relu=True (the fused BN heads write zn in place)")
         if self.fused:
             _fn._require_cuda(x, "x")
             _fn.proj_dtype_code(x.dtype, "ProjectionHead(fused=True)")
             if self.fuse_conv1:
                 conv1, conv2 = self.proj[0], self.proj[2]
                 return conv_bn_relu_project_normalize(_autocast_input(x), conv1.weight, conv1.bias, self.proj[1][0],
-                                                      conv2.weight, conv2.bias, sparse_grad=self.sparse_grad)
+                                                      conv2.weight, conv2.bias, sparse_grad=self.sparse_grad, out=out)
             if self.fuse_bn_relu:
                 return bn_relu_project_normalize(self.proj[0](x), self.proj[1][0], self.proj[2].weight,
-                                                 self.proj[2].bias, sparse_grad=self.sparse_grad)
+                                                 self.proj[2].bias, sparse_grad=self.sparse_grad, out=out)
             if isinstance(self.proj, nn.Conv2d):
                 last, y = self.proj, x
             else:

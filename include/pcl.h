@@ -620,6 +620,14 @@ int pcl_step_fused_select(const pcl_step_desc* d, const uint64_t* step_counter, 
 int pcl_step_fused_loss(const pcl_step_desc* d, void* stream);
 int pcl_step_fused_scatter(const pcl_step_desc* d, const float* grad_scale, uint64_t* step_counter, int32_t* prev_rows,
                            void* stream);
+/* pcl_step_fused_scatter (csrc/pcl_step.cu:200) with the anchor columns as its output, in the layout of
+ * pcl_step_backward_cols: cols (max_samples, 256) fp32, row s < A = the values the scatter writes at the anchor's pixel
+ * (the same fixed-order sum of the live per-column-tile partials, times *grad_scale: bit-identical for an fp32 embed, the
+ * fp32 values before the rounding for a half embed), col_pix[s] = b*h*w + pix; rows s >= A are zero with col_pix -1, so
+ * every row is written on every call.  d->grad_embed is not read or written: no fill is needed.  Advances *step_counter
+ * (may be NULL).  sparse reset has no meaning here (no dense buffer). */
+int pcl_step_fused_cols(const pcl_step_desc* d, const float* grad_scale, uint64_t* step_counter, float* cols,
+                        int32_t* col_pix, void* stream);
 int pcl_step_fused_fill(const pcl_step_desc* d, void* stream);   /* zero-fill of d->grad_embed (B*D*h*w elements of
                                                                     d->embed_dtype) */
 /* Zero-fill `bytes` (multiple of 16, 16-byte aligned) with 16-byte stores on the engine's own fill kernel. */
